@@ -3,6 +3,7 @@
 
     python bench.py --gpus N --steps K --warmup W            # this repo's CUDA backend
     python bench.py --impl reference --steps K --warmup W    # the reference algorithm on the host CPU
+    python bench.py ... --dump-outputs DIR                   # + what the timed loop's last step returned, as DIR/<name>.npy
 
 metric  : frame-pairs/sec, RAFT, 1024x436, 12 refinement iterations, f16 storage, batch 8 per GPU
           (BASELINE.json configs[1]); weak scaling over N GPUs (frame pairs shard, no collective on
@@ -58,7 +59,8 @@ def host_cores() -> int:
     return max(1, n)
 
 
-FALLBACK_PEAKS = {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}
+# NVIDIA's H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 dense BF16 TFLOP/s -- nominal, not measured
+FALLBACK_PEAKS = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}
 
 
 def parse_args():
@@ -73,7 +75,7 @@ def parse_args():
     ap.add_argument("--width", type=int, default=1024)
     ap.add_argument("--iters", type=int, default=12)
     ap.add_argument("--dtype", default="fp16", choices=["fp16", "bf16", "fp32"])
-    ap.add_argument("--kernel-impl", type=int, default=0, help="0 auto, 1 SIMT, 2 tcgen05")
+    ap.add_argument("--kernel-impl", type=int, default=0, help="0 auto, 1 SIMT, 2 tensor cores (wgmma)")
     ap.add_argument("--inflight", type=int, default=1, help="frame-pair batches in flight per GPU (ptlflow_b200.pipeline.FramePipeline); 1 = one stream")
     ap.add_argument("--cuda-graph", type=int, default=1, help="1: one CUDA graph launch per forward (default); 0: eager launches")
     ap.add_argument("--fp32-context", action="store_true", help="accuracy mode: context encoder in fp32 (RAFT.enable_fp32_context)")
@@ -84,7 +86,31 @@ def parse_args():
     ap.add_argument("--no-comparators", action="store_true")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--cpu-baseline-seconds", type=float, default=12.0)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the outputs of the last timed step as DIR/<name>.npy (float32, <= 64 MB in all)")
     return ap.parse_args()
+
+
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, outputs: dict) -> None:
+    """Every floating-point tensor a caller of the forward receives -> out_dir/<name>.npy in float32 (float64 stays float64).
+    An array larger than its share of DUMP_LIMIT_BYTES is replaced by a fixed, seeded sample of its flattened elements (the
+    same positions for the same shape), so that two builds can be compared output for output."""
+    import numpy as np
+
+    arrays = {k: v for k, v in outputs.items() if torch.is_tensor(v) and v.is_floating_point()}
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_LIMIT_BYTES // max(1, len(arrays))
+    for name, t in sorted(arrays.items()):
+        a = t.detach().to("cpu", torch.float64 if t.dtype == torch.float64 else torch.float32).numpy()
+        if a.nbytes > share:
+            flat = a.reshape(-1)
+            idx = np.sort(np.random.default_rng(0).choice(flat.size, share // a.itemsize, replace=False))
+            a = flat[idx]
+        np.save(os.path.join(out_dir, name + ".npy"), a)
+    log(f"dumped {sorted(arrays)} to {out_dir}")
 
 
 def load_peaks():
@@ -95,7 +121,7 @@ def load_peaks():
         p["_source"] = "measured (MEASURED_PEAKS.json)"
         return p
     p = dict(FALLBACK_PEAKS)
-    p["_source"] = "fallback (B200_PROFILING.md)"
+    p["_source"] = "fallback (H100 SXM data sheet, nominal)"
     return p
 
 
@@ -182,7 +208,7 @@ def algorithmic_work(model, B, H8, W8, iters, esize):
     ref_layers = (_lib.L_CONVC1, _lib.L_CONVC2, _lib.L_CONVF2, _lib.L_CONV, _lib.L_GRU_ZR1, _lib.L_GRU_Q1, _lib.L_GRU_ZR2, _lib.L_GRU_Q2,
                   _lib.L_FLOW1, _lib.L_FLOW2, _lib.L_MASK1, _lib.L_MASK2, _lib.L_AGG_V)
     if eng.layers[_lib.L_CONVF1].weight_k is None:
-        ref_layers += (_lib.L_CONVF1,)  # (on tcgen05 convf1 runs in its own kernel class, "flowconv")
+        ref_layers += (_lib.L_CONVF1,)  # (on the tensor cores convf1 runs in its own kernel class, "flowconv")
     for lid in ref_layers:  # the reference's layers (update.py:94-153): the ALGORITHMIC work
         pk = eng.layers.get(lid)
         if pk is None:
@@ -275,8 +301,12 @@ def run_ours(args):
     def launches_now():
         return int(lib.pfb_launch_count(-1)) + int(model.graph_launches_replayed)
 
+    last_out = {}
+
     def step_resident(i):
-        return model({"images": devin[i % pool]})
+        out = model({"images": devin[i % pool]})
+        last_out["out"] = out
+        return out
 
     # e2e: what a caller feeding frames from host memory runs.  Two device input slots; the H2D copy of step i+1 and the
     # D2H copy of step i's flow ride a side stream while step i / i+1 computes (PCIe is full duplex).  Every step's input
@@ -381,6 +411,10 @@ def run_ours(args):
         # ---- value: device-resident inputs, exactly K steps ----
         ms_value, _, launches = timed(run_value, args.steps)
         log(f"resident: {ms_value / args.steps:.3f} ms/step")
+        if args.dump_outputs and rank == 0:  # before any other forward reuses the (graph-owned) output buffers
+            if pipe is not None:
+                raise SystemExit("--dump-outputs needs --inflight 1")
+            dump_outputs(args.dump_outputs, last_out["out"])
         # ---- e2e: pinned host inputs, H2D + forward + D2H of the flow every step ----
         ms_e2e_ev, ms_e2e_wall, _ = timed(run_e2e_any, args.steps)
         ms_e2e = max(ms_e2e_ev, ms_e2e_wall)
@@ -519,7 +553,7 @@ def run_ours(args):
                     traffic = round(json.load(f)["dram_bytes_per_launch"])
                 break
         # the timed region is a burst (~0.1 s at ~1.9 GHz), so the burst bf16 peak is the matching denominator
-        roofline = {"kernel": "update-block conv (implicit GEMM, tcgen05)", "bound": "tensor", "achieved": e["tflops"],
+        roofline = {"kernel": "update-block conv (implicit GEMM, wgmma)", "bound": "tensor", "achieved": e["tflops"],
                     "peak": peaks["bf16_tflops"], "unit": "TFLOP/s", "frac": e["frac_of_bf16_burst_peak"],
                     "frac_of_sustained_peak": e["frac_of_bf16_sustained_peak"],
                     "traffic": traffic, "peak_source": peaks["_source"] + ", burst bf16 GEMM",
@@ -590,7 +624,7 @@ def parity_check(args, model, sd_fp32, frames, dev):
 
 
 def same_gpu_comparators(args, dev):
-    """The reference's algorithm as plain PyTorch-CUDA ops (the oracle port) on the same B200, same workload, timed with the
+    """The reference's algorithm as plain PyTorch-CUDA ops (the oracle port) on the same GPU, same workload, timed with the
     model_benchmark.py protocol: fp32 with TF32 off, and half precision like ``model.half()``.  Reported baselines."""
     from oracle import raft_oracle as O
     from oracle import synth

@@ -1,5 +1,5 @@
 /*
- * ptlflow_b200 -- C ABI of the B200-native RAFT-family inference hot path.
+ * ptlflow_b200 -- C ABI of the H100-native (sm_90a) RAFT-family inference hot path.
  *
  * This is the drop-in boundary: a plain C interface (device pointers, sizes, a CUDA
  * stream) that replaces, for the RAFT hot path, what the reference reaches through
@@ -67,8 +67,8 @@ PFB_API int pfb_stream_destroy(pfb_stream stream);
  *   replaces CorrBlock.corr + CorrBlock.__init__     ptlflow/models/raft/corr.py:13-27, 56-64
  * fmap1, fmap2 : [B, H, W, C] dtype.   pyramid[l] : [B*H*W, H>>l, W>>l] dtype (floor sizes),
  * level 0 = <f1, f2> / sqrt(C); level l = 2x2 mean of level l-1.
- * impl: 0 = auto (tcgen05 tensor-core GEMM for f16/bf16 when the shape allows, else SIMT),
- *       1 = force the SIMT fp32-accumulate kernel, 2 = force tcgen05.
+ * impl: 0 = auto (wgmma tensor-core GEMM for f16/bf16 when the shape allows, else SIMT),
+ *       1 = force the SIMT fp32-accumulate kernel, 2 = force wgmma.
  * ---------------------------------------------------------------------------------- */
 PFB_API int pfb_corr_volume_build(const void* fmap1, const void* fmap2, void* const* pyramid, int B, int H, int W,
                           int C, int levels, pfb_dtype dtype, int impl, pfb_stream stream);
@@ -127,7 +127,7 @@ PFB_API int pfb_corr_lookup_onthefly(const void* fmap1, void* const* fmap2_pyram
                              pfb_dtype out_dtype, int out_nchw, int out_stride, pfb_stream stream);
 
 /* a4 on the tensor cores (f16 / bf16, radius 4, C % 64 == 0, C <= 256, pixel-major output): every 8 x 16 tile of neighbouring queries
- * multiplies its query vectors with the region of fmap2_pyramid[l] that holds all its windows (tcgen05 GEMM, TMA-fed, out-of-map
+ * multiplies its query vectors with the region of fmap2_pyramid[l] that holds all its windows (wgmma GEMM, TMA-fed, out-of-map
  * targets zero-filled by the TMA unit) and blends its windows out of the accumulator; queries whose window does not fit the region
  * (rough flow inside a tile) are recomputed by the SIMT kernel of pfb_corr_lookup_onthefly, so the values never depend on the flow.
  * workspace: pfb_corr_lookup_onthefly_tc_workspace_bytes(B, H, W) bytes (one flag per query).  Same output as
@@ -198,7 +198,7 @@ typedef struct {
   float* coords;       /* PFB_EPI_FLOW: coords1 [B,H,W,2] fp32 in/out */
   const float* flow;   /* PFB_EPI_RELU_APPEND_FLOW: [B,H,W,2] fp32 */
   pfb_dtype dtype;
-  int impl;            /* 0 auto, 1 SIMT, 2 tcgen05 */
+  int impl;            /* 0 auto, 1 SIMT, 2 wgmma */
   /* tensor-core operand (f16/bf16 only, may be NULL -> SIMT path): the same weights packed K-major
    * by pfb_pack_conv_weight_kmajor: [KH*KW][Cout_pad_k][Cin_pad], every source padded to 64 channels */
   const void* weight_k;
@@ -208,7 +208,7 @@ typedef struct {
    * update.py:60-63 split by linearity).  addend_stride >= Cout_pad_k, % 8 == 0.  NULL = use bias. */
   const void* addend;
   int addend_stride;
-  /* > 0 (1x1 layers, tcgen05 path): sample b multiplies with ITS OWN weight matrix, rows [b * w_rows_per_sample, + Cout_pad_k)
+  /* > 0 (1x1 layers, wgmma path): sample b multiplies with ITS OWN weight matrix, rows [b * w_rows_per_sample, + Cout_pad_k)
    * of weight_k [B * w_rows_per_sample][Cin_pad] -- one launch for all samples of "attention @ v" (gma_utils.py:101-113),
    * where the "weights" are the sample's transposed v.  0 = one weight matrix for all samples. */
   int w_rows_per_sample;
@@ -223,7 +223,7 @@ PFB_API int pfb_pack_conv_weight(const void* src, void* dst, int Cout, int Cin, 
                          int col_offset, pfb_dtype src_dtype, pfb_dtype dst_dtype, pfb_stream stream);
 /* dst[offset + i] = (float) src[i] */
 PFB_API int pfb_pack_bias(const void* src, float* dst, int n, int offset, pfb_dtype src_dtype, pfb_stream stream);
-/* torch-layout weight -> K-major packing for the tcgen05 path: dst[tap][row_offset + co][kpos(ci)] where the
+/* torch-layout weight -> K-major packing for the wgmma path: dst[tap][row_offset + co][kpos(ci)] where the
  * input channels are the concatenation of `nsrc` sources of src_channels[i] channels and each source is
  * padded to a multiple of 64 in dst (kpos skips the pad).  dst is [KH*KW][Cout_pad_k][Cin_pad]; zero it first. */
 PFB_API int pfb_pack_conv_weight_kmajor(const void* src, void* dst, int Cout, int Cin, int KH, int KW, int Cout_pad_k,
@@ -292,7 +292,7 @@ typedef struct {
   const void* weight; /* packed, see pfb_pack_conv_weight */
   const float* bias;
   int Cout, Cout_pad, Cin, KH, KW;
-  const void* weight_k; /* K-major packing (tcgen05), NULL if not packed */
+  const void* weight_k; /* K-major packing (wgmma), NULL if not packed */
   int Cin_pad, Cout_pad_k;
 } pfb_layer;
 
@@ -308,7 +308,7 @@ typedef struct {
   int iters;
   int alternate_corr; /* 0: look up the materialised pyramid; 1: on-the-fly (a4) */
   int out_h, out_w, pad_top, pad_left; /* full-resolution output window */
-  int impl;           /* 0 auto, 1 SIMT everywhere, 2 tcgen05 where available */
+  int impl;           /* 0 auto, 1 SIMT everywhere, 2 wgmma where available */
   int volume_layout;  /* 0: dense pyramid (pfb_corr_volume_build); 1: tiled pyramid (pfb_corr_volume_build_tiled) */
   int fork_flow;      /* 1: the flow branch of the motion encoder (convf1, convf2) and the once-per-forward context terms run on a second
                          stream of the calling host thread, forked / joined with events (parallel branches when the caller captures a
@@ -365,21 +365,21 @@ PFB_API int pfb_instance_norm_act(const void* x, void* y, const void* residual, 
 PFB_API int pfb_instance_norm_apply(const void* x, void* y, const void* residual, void* workspace, int B, int H, int W, int C,
                                     float eps, int relu, pfb_dtype dtype, pfb_stream stream);
 /* First encoder convolution: nn.Conv2d(3, 64, 7, stride=2, padding=3) of BasicEncoder (extractor.py:136,171-178)
- * on tcgen05 without an im2col buffer (overlapping-window operand descriptors, see csrc/first_conv.cu).
+ * on wgmma without an im2col buffer (overlapping-window operand descriptors, see csrc/first_conv.cu).
  *   x      [N,H,W,4]  f16/bf16 pixel-major frames from pfb_preprocess_frames(out_channels = 4); H, W even
  *   wpack  9 x 8192 B: for input-row offset j = 0..8 a [128][32] K-major tile, row p*64+co, column 4*t+c =
- *          W[co][c][j-2p][t-1] (zero where j-2p or t-1 fall outside 0..6, or c = 3), stored as non-swizzled UMMA
+ *          W[co][c][j-2p][t-1] (zero where j-2p or t-1 fall outside 0..6, or c = 3), stored as non-swizzled wgmma
  *          core matrices [16 row groups][4 K groups][8 rows][8 elements]   (ptlflow_b200.ops.pack_first_conv)
  *   bias   fp32 [64] or NULL (folded batch norm + conv bias);  relu: apply max(.,0) after the bias
  *   stats  NULL, or B*64*2 doubles that receive per (image, channel) sum / sum of squares of the fp32 result
  *          (instance norm: follow with pfb_instance_norm_apply)
  *   out    [N,H/2,W/2,64] */
 /* convf1 of the motion encoder, nn.Conv2d(2, 128, 7, padding=3) + ReLU on the fp32 flow (update.py:84,96), on
- * tcgen05 with the same overlapping-window operand (csrc/first_conv.cu).  The flow is split into hi + lo halves of
+ * wgmma with the same overlapping-window operand (csrc/first_conv.cu).  The flow is split into hi + lo halves of
  * the storage type inside the kernel, so the arithmetic equals fp32 flow x f16/bf16 weights, fp32 accumulate.
  *   flow   fp32 [B,H,W,2];   bias fp32 [128]
  *   wpack  7 x 16384 B: for filter row ky a [128][64] K-major tile, column 8*t+c = W[co][c & 1][ky][t-1] for
- *          c < 4 (hi and lo halves see the same weight), zero for t = 0 or c >= 4; non-swizzled UMMA core-matrix
+ *          c < 4 (hi and lo halves see the same weight), zero for t = 0 or c >= 4; non-swizzled wgmma core-matrix
  *          order [16 row groups][8 K groups][8 rows][8 elements]   (ptlflow_b200.ops.pack_flow_conv)
  *   out    [B,H,W,out_stride] storage type, channels out_offset .. out_offset+127 written */
 PFB_API int pfb_flow_conv7x7(const float* flow, const void* wpack, const float* bias, void* out, int out_stride, int out_offset,
@@ -393,9 +393,9 @@ PFB_API int pfb_bias_act(const void* x, const float* bias, const void* residual,
 
 /* ------------------------------------------------------------------------------------
  * Measurement hooks (bench.py): launch accounting and live per-kernel-class timing.
- * kernel_class: 0 volume, 1 pool, 2 lookup, 3 on-the-fly lookup, 4 update-block conv (tcgen05 / SIMT), 5 upsample,
+ * kernel_class: 0 volume, 1 pool, 2 lookup, 3 on-the-fly lookup, 4 update-block conv (wgmma / SIMT), 5 upsample,
  * 6 misc (packing, coords, softmax, transposes), 7 encoder normalise / bias / activation passes, 8 encoder instance-norm
- * statistics, 9 first encoder convolution (tcgen05), 10 convf1 (7x7 on the flow, tcgen05), 11 flow-head tap gather;
+ * statistics, 9 first encoder convolution (wgmma), 10 convf1 (7x7 on the flow, wgmma), 11 flow-head tap gather;
  * -1 = all.  pfb_profile_collect synchronises the device, writes summed milliseconds and span
  * counts per class (arrays of >= PFB_KERNEL_CLASSES entries) and clears the recorded spans.
  * ---------------------------------------------------------------------------------- */

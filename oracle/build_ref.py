@@ -3,13 +3,13 @@
 
 The two source files are compiled where they lie under /root/reference (ptlflow/utils/external/alt_cuda_corr/
 correlation.cpp + correlation_kernel.cu: plain CUDA C + a pybind11 shim, nothing arch specific) with
-``torch.utils.cpp_extension`` for sm_100; only the resulting ``oracle/_ref/alt_cuda_corr.so`` is kept (git-ignored, it
-travels to the GPU box with the snapshot like this repo's own .so).  No reference source is copied.
+``torch.utils.cpp_extension`` for sm_90; only the resulting ``oracle/_ref/alt_cuda_corr.so`` is kept (git-ignored, it
+sits next to the library build products).  No reference source is copied.
 
 Uses: (1) the parity tests check ``ptlflow_b200.alt_cuda_corr.forward`` against the real reference kernel
 (tests/test_gpu_ref_plugin.py), (2) tools/time_config4.py times it beside this library's on-the-fly kernel
-(SURVEY.md section 8(d): "the reference alt_cuda_corr built for sm_100 as the existing native kernel comparator").
-The reference checkout does not exist on the GPU box: nothing there builds, it only loads the prebuilt file.
+(SURVEY.md section 8(d): the reference alt_cuda_corr as the existing native kernel comparator).
+Where the reference checkout is absent nothing builds; a prebuilt file is only loaded.
 
     python oracle/build_ref.py            # -> oracle/_ref/alt_cuda_corr.so (a no-op when /root/reference is absent)
 """
@@ -33,7 +33,7 @@ def build(verbose: bool = False) -> str | None:
     if os.path.exists(TARGET) and all(os.path.getmtime(TARGET) >= os.path.getmtime(s) for s in srcs):
         return TARGET
     os.makedirs(OUT, exist_ok=True)
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0")
     os.environ.setdefault("MAX_JOBS", "4")
     from torch.utils import cpp_extension
 

@@ -175,6 +175,95 @@ def make_ops() -> None:
         print("state_shapes", variant, len(shapes), sum(int(np.prod(s)) for k, s in shapes.items() if "running" not in k and "num_batches" not in k))
 
 
+# (b, c, h1, w1, h2, w2, radius) of tests/test_gpu_ref_plugin.py; the reference kernel's output is stored as a fixed, seeded
+# sample of at most REF_PLUGIN_SAMPLES elements per case (the largest case is 2.3 MB in full)
+REF_PLUGIN_CASES = [(1, 256, 16, 24, 16, 24, 4), (2, 128, 17, 29, 8, 14, 4), (1, 64, 9, 12, 9, 12, 3), (1, 256, 55, 128, 27, 64, 4)]
+REF_PLUGIN_SAMPLES = 8192
+
+
+def ref_plugin_inputs(b, c, h1, w1, h2, w2):
+    """(fmap1, fmap2, coords) of one REF_PLUGIN_CASES entry, on the CPU."""
+    f1 = torch.from_numpy(synth.synth_normal("rp/f1", (b, h1, w1, c), 21))
+    f2 = torch.from_numpy(synth.synth_normal("rp/f2", (b, h2, w2, c), 21))
+    grid = torch.stack(torch.meshgrid(torch.arange(w1, dtype=torch.float32), torch.arange(h1, dtype=torch.float32), indexing="xy"), dim=-1)
+    coords = (grid[None, None] * (w2 / w1) + torch.from_numpy(synth.synth_normal("rp/c", (b, 1, h1, w1, 2), 21, scale=3.0))).contiguous()
+    return f1, f2, coords
+
+
+def ref_plugin_sample(numel: int) -> np.ndarray:
+    return np.sort(np.random.default_rng(0).choice(numel, min(numel, REF_PLUGIN_SAMPLES), replace=False))
+
+
+def make_ref_plugin(out_dir: str = GOLDEN_DIR) -> None:
+    """The reference's own alt_cuda_corr kernel (oracle/_ref, built by oracle/build_ref.py) on a CUDA device."""
+    from . import build_ref
+
+    mod = build_ref.load()
+    assert mod is not None and torch.cuda.is_available(), "needs oracle/_ref/alt_cuda_corr.so and a CUDA device"
+    arrays = {}
+    for i, (b, c, h1, w1, h2, w2, r) in enumerate(REF_PLUGIN_CASES):
+        f1, f2, coords = (t.cuda() for t in ref_plugin_inputs(b, c, h1, w1, h2, w2))
+        (ref,) = mod.forward(f1, f2, coords, r)
+        flat = ref.float().cpu().numpy().reshape(-1)
+        idx = ref_plugin_sample(flat.size)
+        arrays[f"shape{i}"] = np.array(ref.shape, dtype=np.int64)
+        arrays[f"idx{i}"] = idx
+        arrays[f"val{i}"] = flat[idx]
+    np.savez_compressed(os.path.join(out_dir, "ref_plugin_alt_corr.npz"), **arrays)
+
+
+# SURVEY.md appendix E: the sibling corr.py copies of the zoo (tests/test_oracle_golden.py).  Outputs stored as a fixed,
+# seeded sample of SIBLING_SAMPLES elements per (family, levels, radius).
+SIBLING_SAME_AS_RAFT = ["gma", "gmflownet", "rapidflow", "rpknet", "skflow", "ms_raft_plus"]
+SIBLING_PER_LEVEL_GEMM = ["sea_raft", "memfof", "flow_anything", "flowseek", "recover"]
+SIBLING_SETTINGS = {"same": ((4, 4), (2, 3)), "per_level": ((3, 3),)}
+SIBLING_SAMPLES = 4096
+
+
+def sibling_inputs():
+    b, c, h, w = 2, 32, 17, 24  # 17x24 -> 8x12 -> 4x6 -> 2x3: no 1-pixel level (the reference's sampler divides by W - 1)
+    f1 = torch.from_numpy(synth.synth_normal("sib/f1", (b, c, h, w), 61))
+    f2 = torch.from_numpy(synth.synth_normal("sib/f2", (b, c, h, w), 61))
+    coords = O.coords_grid(b, h, w) + torch.from_numpy(synth.synth_normal("sib/c", (b, 2, h, w), 61, scale=3.0))
+    return f1, f2, coords
+
+
+def sibling_sample(numel: int) -> np.ndarray:
+    return np.sort(np.random.default_rng(1).choice(numel, min(numel, SIBLING_SAMPLES), replace=False))
+
+
+def make_sibling_corr() -> None:
+    import importlib
+
+    ref_shim.load_raft()
+    f1, f2, coords = sibling_inputs()
+    arrays = {}
+    for kind, families in (("same", SIBLING_SAME_AS_RAFT), ("per_level", SIBLING_PER_LEVEL_GEMM)):
+        for family in families:
+            mod = importlib.import_module(f"ptlflow.models.{family}.corr")
+            for levels, radius in SIBLING_SETTINGS[kind]:
+                out = mod.CorrBlock(f1, f2, levels, radius)(coords).numpy()
+                key = f"{family}_{levels}_{radius}"
+                arrays[key + "_shape"] = np.array(out.shape, dtype=np.int64)
+                arrays[key] = out.reshape(-1)[sibling_sample(out.size)]
+    np.savez_compressed(os.path.join(GOLDEN_DIR, "sibling_corr.npz"), **arrays)
+
+
+def make_flo_file() -> None:
+    """A .flo file written by the reference's own flow_write (utils/flow_utils.py), NaN included."""
+    import sys
+    import types
+
+    ref_shim.load_raft()
+    for absent in ("png", "h5py"):  # only the .flo branch is exercised
+        sys.modules.setdefault(absent, types.ModuleType(absent))
+    import ptlflow.utils.flow_utils as ref_io
+
+    flow = (np.random.default_rng(4).standard_normal((9, 11, 2)) * 7).astype(np.float32)
+    flow[1, 1] = np.nan
+    ref_io.flow_write(os.path.join(GOLDEN_DIR, "ref_flow_write.flo"), flow)
+
+
 def main() -> None:
     os.makedirs(GOLDEN_DIR, exist_ok=True)
     torch.set_num_threads(max(1, os.cpu_count() or 1))
@@ -182,9 +271,16 @@ def main() -> None:
     make_e2e()
     make_warm_start()
     make_gma_ops()
+    make_sibling_corr()
+    make_flo_file()
     total = sum(os.path.getsize(os.path.join(GOLDEN_DIR, f)) for f in os.listdir(GOLDEN_DIR))
     print("golden bytes:", total)
 
 
 if __name__ == "__main__":
-    main()
+    import sys
+
+    if sys.argv[1:2] == ["ref_plugin"]:  # python -m oracle.make_golden ref_plugin [OUT_DIR]
+        make_ref_plugin(*sys.argv[2:3])
+    else:
+        main()

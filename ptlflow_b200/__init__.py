@@ -1,4 +1,4 @@
-"""ptlflow_b200 -- B200-native backend for ptlflow's RAFT-family inference hot path.
+"""ptlflow_b200 -- H100-native (sm_90a) backend for ptlflow's RAFT-family inference hot path.
 
 Public surface mirrors ptlflow/__init__.py:65-285 for the models this backend covers:
 ``get_model``, ``get_model_reference``, ``get_model_names``, ``get_trainable_model_names``,

@@ -1,4 +1,4 @@
-// Shared helpers for the ptlflow_b200 CUDA library (sm_100a only).
+// Shared helpers for the ptlflow_b200 CUDA library (sm_90a only).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -118,7 +118,7 @@ class ProfScope {
 // ---- kernel families implemented in the other translation units ---------------------
 // conv_simt.cu
 int conv2d_simt(const pfb_conv_params* p, cudaStream_t s);
-// conv_umma.cu (tcgen05); returns PFB_ERR_UNSUPPORTED when the shape does not fit
+// conv_umma.cu (wgmma); returns PFB_ERR_UNSUPPORTED when the shape does not fit
 int conv2d_umma(const pfb_conv_params* p, cudaStream_t s);
 bool conv2d_umma_supported(const pfb_conv_params* p);
 // conv_special.cu

@@ -1,6 +1,6 @@
 // Generic stride-1 "same" convolution as an implicit GEMM on the CUDA cores, fp32 accumulate.
 // This is the reference-precision path (fp32 parity <= 1e-3, raft_small, odd channel counts);
-// the f16/bf16 production path is conv_umma.cu (tcgen05).  It evaluates the reference's
+// the f16/bf16 production path is conv_umma.cu (wgmma).  It evaluates the reference's
 // nn.Conv2d + activation (+ GRU gate arithmetic) of ptlflow/models/raft/update.py:6-153
 // without materialising any torch.cat: the K loop walks (tap, source, channel-chunk).
 #include "common.cuh"
@@ -296,12 +296,12 @@ extern "C" PFB_API int pfb_conv2d(const pfb_conv_params* p, pfb_stream stream) {
     if (conv_flow7x7_supported(p)) return conv_flow7x7(p, s);
     if (conv2d_umma_supported(p)) return conv2d_umma(p, s);
     if (p->impl == 2) {
-      set_error("conv2d: tcgen05 path does not support this shape/dtype");
+      set_error("conv2d: wgmma path does not support this shape/dtype");
       return PFB_ERR_UNSUPPORTED;
     }
   }
   if (p->addend || p->w_rows_per_sample) {
-    set_error("conv2d: per-pixel addend / per-sample weights are implemented by the tcgen05 path only (shape / dtype / impl not eligible)");
+    set_error("conv2d: per-pixel addend / per-sample weights are implemented by the wgmma path only (shape / dtype / impl not eligible)");
     return PFB_ERR_UNSUPPORTED;
   }
   return conv2d_simt(p, s);

@@ -1,5 +1,5 @@
 // Two small convolutions of the update block that do not fit the tensor-core tile economically, plus
-// the K-major weight packing used by the tcgen05 path.
+// the K-major weight packing used by the wgmma path.
 //   * flow-head conv2 (3x3, 256 -> 2, update.py:9) fused with the coordinate update of raft.py:174-178:
 //     one warp per pixel, lanes split the input channels with 128-bit loads, shuffle reduction.
 //   * motion-encoder convf1 (7x7, 2 -> 128/64, update.py:99,:81): one thread per output channel keeps its

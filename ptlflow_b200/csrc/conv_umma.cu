@@ -1,38 +1,35 @@
-// Implicit-GEMM convolution on the 5th-gen tensor cores (f16 / bf16 storage, fp32 accumulate in TMEM).
+// Implicit-GEMM convolution on the Hopper tensor cores (wgmma; f16 / bf16 storage, fp32 accumulate).
 //
 //   out[p, n] = epilogue( bias[n] + sum_{tap, src, c} X_src[p + tap, c] * Wk[tap][n][kpos(src, c)] )
 //
-//   M tile : 128 pixels = TW x TH of one image, chosen per shape for the least padding (one image row, 128 x 1, for
-//            W = 128: 440 tiles = 2.97 waves of 148 SMs).  The A operand of a tap is a TMA box of the pixel-major
-//            activation tensor: out-of-image elements are zero-filled by the TMA unit, which is exactly "same"
-//            zero padding -- no im2col, no torch.cat (each concatenated source has its own tensor map).
-//            Halo reuse: with row tiles one patch of TW + KW - 1 pixels serves all KW horizontal taps (tap kx =
-//            the same patch read through a descriptor advanced by kx * 128 B); vertical kernels with N < 256 use
-//            (TH + KH - 1) x TW patches the same way (advance TW * 128 B, a multiple of the 1024-byte swizzle period).
-//   N tile : all (<= 256) output channels of the layer in one TMEM accumulator (z|r of the GRU = 256).
+//   M tile : 128 pixels = TW x TH of one image, chosen per shape for the least padding.  The A operand of a tap is a TMA
+//            box of the pixel-major activation tensor: out-of-image elements are zero-filled by the TMA unit, which is
+//            exactly "same" zero padding -- no im2col, no torch.cat (each concatenated source has its own tensor map).
+//            Halo reuse: with row tiles one patch of TW + KW - 1 pixels serves all KW horizontal taps (tap kx = the same
+//            patch read through a descriptor advanced by kx * 128 B); vertical kernels use (TH + KH - 1) x TW patches the
+//            same way (advance TW * 128 B, a multiple of the 1024-byte swizzle period).
+//   N tile : up to 128 output channels (equal tiles, multiples of 32): the two MMA warpgroups hold 64 x N fp32 each in
+//            registers.
 //   K loop : (64-channel chunk of a source, ky, kx).  Two rings: activation patches and weight tiles; a weight stage
-//            holds one tap (N = 256) or all taps of a patch (N <= 192, "b_group").
-//   CG = 2 : CTA pairs (cta_group::2): the pair shares every weight tile, the leader issues M = 256 MMAs.
+//            holds one tap or all taps of a patch ("b_group").
 //
-// Persistent CTAs (one per SM, 10 warps: 4 = TMA producer, 5 = MMA issuer / TMEM owner, 0-3 and 6-9 = two
-// epilogue groups that split the accumulator columns) walk the output tiles round-robin.  The rings run continuously
-// across tiles and the accumulator is double-buffered in TMEM (2 x <= 256 columns): the epilogue of tile i overlaps
-// the MMAs of tile i+1.  The epilogue fuses bias + ReLU / sigmoid / tanh + the GRU gate arithmetic of
+// Persistent CTAs (one per SM) walk the output tiles round-robin.  The rings run continuously across tiles; at the end of
+// a tile the MMA warpgroups park their fragments in a shared-memory accumulator tile and go on with the next tile while
+// the epilogue warps read it.  The epilogue fuses bias + ReLU / sigmoid / tanh + the GRU gate arithmetic of
 // ptlflow/models/raft/update.py:58-73 and writes pixel-major f16/bf16 with 16-byte stores; its h / z / residual
 // operands are requested before the accumulator wait.  Launched with programmatic stream serialization: the
-// prologue (barriers, TMEM, tensor-map prefetch) overlaps the previous kernel's drain (pdl_wait below).
+// prologue (barriers, bias, tensor-map prefetch) overlaps the previous kernel's drain (pdl_wait below).
 // PFB_CONV_TRACE=<file> records a per-CTA timeline of every launch (tools/conv_trace_report.py).
-// What bounds it (DESIGN.md section 4, findings 6-7): ~9 us of fixed cost per launch and a floor of ~135 clk per
-// tcgen05.mma (A-operand fetch), so only the N = 256 layers approach the nominal tensor rate.
 #include <stdio.h>
 #include <stdlib.h>
 
 #include <atomic>
+#include <type_traits>
 
 #include "umma.cuh"
 
 namespace pfb {
-using namespace sm100;
+using namespace sm90;
 
 constexpr int kATileBytes = 128 * 128;
 constexpr int kMaxBias = 1024;  // output channels per layer whose bias is kept in shared memory (Cout_pad_k <= 1024)
@@ -43,9 +40,8 @@ struct __align__(8) ConvBars {
   uint64_t a_empty[kMaxAStages];
   uint64_t b_full[kMaxBStages];
   uint64_t b_empty[kMaxBStages];
-  uint64_t acc_full[2];
-  uint64_t acc_empty[2];
-  uint32_t tmem_base;
+  uint64_t acc_full;
+  uint64_t acc_empty;
 };
 
 struct ConvUmmaArgs {
@@ -53,16 +49,15 @@ struct ConvUmmaArgs {
   int src_chunks[PFB_MAX_SRC];   // 64-channel chunks per source
   int src_coff[PFB_MAX_SRC];     // first channel inside the source tensor
   int B, H, W, KH, KW;
-  int NT;                        // N tile (multiple of 32, <= 256)
+  int NT;                        // N tile (multiple of 32, <= 128)
   int n_tiles;                   // N tiles per M tile
   int TW, TH, tw_shift;          // M tile = TW x TH pixels (TW * TH = 128, powers of two)
   int tiles_x, tiles_y, n_work;  // work items = tiles_x * tiles_y * B * n_tiles
-  int acc_stride;                // TMEM column offset between the two accumulators
   int Cout, Cout_pad_k;
   // Two rings: activation patches (A) and weight tiles (B).  With row tiles (TH == 1, "halo" mode) one A patch of
   // TW + KW - 1 pixels serves all KW horizontal taps of a (chunk, ky): tap kx reads it through a descriptor whose
   // start address is advanced by kx pixel rows (128 B each) -- the swizzle is a function of the absolute shared-memory
-  // address, so TMA writes and UMMA reads stay consistent.  Otherwise every tap loads its own patch.
+  // address, so TMA writes and wgmma reads stay consistent.  Otherwise every tap loads its own patch.
   int halo;
   int a_stages, a_slot_bytes, a_tx_bytes, b_stages, b_slot_bytes;
   int b_group, b_tap_bytes;      // weight stage = b_group consecutive taps of one activation patch (1, or all of them)
@@ -136,30 +131,80 @@ __device__ __forceinline__ void load32(const T* src, float (&v)[32]) {
   }
 }
 
-// G taps x 4 K-steps of one pipeline step, straight-line (descriptor words advance by constants)
-template <int CG, int G>
-__device__ __forceinline__ void issue_taps(uint32_t d, uint32_t a_lo, uint32_t a_tap16, uint32_t b_lo, uint32_t b_tap16, uint32_t desc_hi,
-                                           uint32_t idesc, uint32_t acc) {
+// The MMA role: two warpgroups, rows 0-63 and 64-127 of the M tile, each m64nNT per 16-channel K step with the
+// accumulator in registers.  A pipeline step (b_group taps x 4 K steps) is committed as one wgmma group; its ring slots are
+// released when the group has completed.  At the end of a tile the fragments go to the shared-memory accumulator tile
+// (once the epilogue has released it), so the epilogue of tile i overlaps the MMAs of tile i + 1.
+template <int NT, bool BF16, int G>
+__device__ __forceinline__ void issue_taps(float (&d)[NT / 2], uint32_t a_lo, uint32_t a_tap16, uint32_t b_lo, uint32_t b_tap16, uint32_t acc) {
 #pragma unroll
   for (int g = 0; g < G; ++g) {
 #pragma unroll
     for (int kk = 0; kk < 4; ++kk) {
       const uint32_t en = (g == 0 && kk == 0) ? acc : 1u;
-      if (CG == 2) umma_f16_lohi_2cta(d, a_lo + g * a_tap16 + 2 * kk, b_lo + g * b_tap16 + 2 * kk, desc_hi, idesc, en);
-      else umma_f16_lohi(d, a_lo + g * a_tap16 + 2 * kk, b_lo + g * b_tap16 + 2 * kk, desc_hi, idesc, en);
+      wgmma<NT, BF16>(d, gdesc(a_lo + g * a_tap16 + 2 * kk, kDescHiSw128), gdesc(b_lo + g * b_tap16 + 2 * kk, kDescHiSw128), en);
     }
   }
 }
 
-// CG = 1: one CTA per MMA (M = 128).  CG = 2: CTA pairs (cta_group::2, M = 256): the pair shares every weight
-// tile -- each CTA stages only half of its rows and the tensor cores of both SMs read both halves -- which
-// halves the shared-memory traffic per MMA, the limiter of the single-CTA version (see DESIGN.md).
+template <int NT, bool BF16>
+__device__ __forceinline__ void conv_mma_role(const ConvUmmaArgs& a, ConvBars* bars, uint8_t* smemA, uint8_t* smemB, float* sacc,
+                                              int chunks, int group0, int group_stride) {
+  const int wg = (threadIdx.x >> 7) - 2, tid = threadIdx.x & 127, lane = threadIdx.x & 31;
+  const uint32_t a_slot16 = (uint32_t)a.a_slot_bytes >> 4, b_slot16 = (uint32_t)a.b_slot_bytes >> 4;
+  const uint32_t a_lo0 = gdesc_lo(smem_u32(smemA) + wg * 64 * 128, 16);  // this warpgroup's 64 pixel rows
+  const uint32_t b_lo0 = gdesc_lo(smem_u32(smemB), 16);
+  const uint32_t bar_a_full = smem_u32(&bars->a_full[0]);
+  const uint32_t bar_b_full = smem_u32(&bars->b_full[0]);
+  const int kw_halo = a.halo == 1 ? a.KW : (a.halo == 2 ? a.KH : 1);  // taps served by one activation patch
+  const int groups = chunks * (a.halo == 1 ? a.KH : (a.halo == 2 ? 1 : a.KH * a.KW));  // patches per tile
+  const uint32_t tap_step16 = a.halo == 2 ? (uint32_t)a.TW * 8u : 8u;  // descriptor advance per tap (16-B units)
+  const uint32_t b_tap16 = (uint32_t)a.b_tap_bytes >> 4;
+  int sa = 0, sb = 0, i = 0;
+  uint32_t pha = 0, phb = 0;
+  uint32_t a_lo = a_lo0, b_lo = b_lo0;
+  float d[NT / 2];
+  for (int w = group0; w < a.n_work; w += group_stride, ++i) {
+    uint32_t acc = 0;  // first MMA of the tile overwrites the accumulator
+    for (int g = 0; g < groups; ++g) {
+      mbar_wait_uniform(bar_a_full + 8 * sa, pha);
+      for (int kx = 0; kx < kw_halo; kx += a.b_group) {
+        mbar_wait_uniform(bar_b_full + 8 * sb, phb);
+        const uint32_t al = a_lo + tap_step16 * kx;  // x halo: +1 pixel row (128 B) per tap; y halo: +TW rows
+        wgmma_fence();
+        switch (a.b_group) {
+          case 5: issue_taps<NT, BF16, 5>(d, al, tap_step16, b_lo, b_tap16, acc); break;
+          case 3: issue_taps<NT, BF16, 3>(d, al, tap_step16, b_lo, b_tap16, acc); break;
+          default: issue_taps<NT, BF16, 1>(d, al, tap_step16, b_lo, b_tap16, acc); break;
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence(d);
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(&bars->b_empty[sb]);
+          if (kx + a.b_group >= kw_halo) mbar_arrive(&bars->a_empty[sa]);
+        }
+        acc = 1;
+        b_lo += b_slot16;
+        if (++sb == a.b_stages) { sb = 0; phb ^= 1; b_lo = b_lo0; }
+      }
+      a_lo += a_slot16;
+      if (++sa == a.a_stages) { sa = 0; pha ^= 1; a_lo = a_lo0; }
+    }
+    mbar_wait(&bars->acc_empty, (i & 1) ^ 1);
+    acc_store<NT>(sacc, d, wg * 64, tid);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&bars->acc_full);
+  }
+}
+
+// 17 warps: 0-7 epilogue (two groups of four that split the accumulator columns), 8-15 the two MMA warpgroups, 16 TMA producer.
 // EPI (the pfb_epilogue) is a template parameter: with a run-time switch the register allocation of every epilogue was the
 // union of all of them (h, z, addend and bias operands live together), and the staged-store version spilled.
-template <typename T, int CG, int EPI>
-// 10 warps = 3 + 3 + 2 + 2 per SM sub-partition, each with 16 K registers: 168 registers per thread is the hardware ceiling
-// (ptxas picks it under __launch_bounds__(320, 1); __maxnreg__(192 / 200) compiles but does not launch).
-__global__ void __launch_bounds__(320, 1)
+constexpr int kConvThreads = 17 * 32;
+template <typename T, int EPI>
+__global__ void __launch_bounds__(kConvThreads, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
                  const __grid_constant__ CUtensorMap tm2, const __grid_constant__ CUtensorMap tmW,
                  const __grid_constant__ CUtensorMap tmO0, const __grid_constant__ CUtensorMap tmO1, const ConvUmmaArgs a) {
@@ -170,13 +215,12 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smemA = smem;
   uint8_t* smemB = smem + a.a_stages * a.a_slot_bytes;
-  // output staging: [128 pixels][64 channels] (16 KB), 128-byte swizzled like an operand tile, followed by the bias vector.  The epilogue's
-  // thread <-> pixel mapping makes every direct global access a 16-byte piece per lane at a 256..768-byte stride (32 sectors
-  // per instruction, half of each used): the per-CTA timelines had the N = 256 epilogues at 4.5-8.4 us per tile, longer
-  // than the tile's MMAs once the GRU lost its context third.  Staged, the stores are conflict-free 16-byte shared-memory
-  // writes and the global side is the TMA unit writing whole 128-byte rows.
+  // output staging: [128 pixels][64 channels] (16 KB), 128-byte swizzled like an operand tile.  The epilogue's thread <-> pixel
+  // mapping makes every direct global access a 16-byte piece per lane at a 256..768-byte stride; staged, the stores are
+  // conflict-free 16-byte shared-memory writes and the global side is the TMA unit writing whole 128-byte rows.
   uint8_t* smemO = smemB + a.b_stages * a.b_slot_bytes;
-  float* sbias = reinterpret_cast<float*>(smemO + (tma_out ? kATileBytes : 0));  // n_tiles * NT <= kMaxBias floats
+  float* sacc = reinterpret_cast<float*>(smemO + (tma_out ? kATileBytes : 0));  // fp32 accumulator tile, NT columns
+  float* sbias = sacc + a.NT * kAccPitch;  // n_tiles * NT <= kMaxBias floats
   ConvBars* bars = reinterpret_cast<ConvBars*>(reinterpret_cast<uint8_t*>(sbias) + kMaxBias * sizeof(float));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -187,54 +231,40 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
   int chunks = 0;
   for (int s = 0; s < a.nsrc; ++s) chunks += a.src_chunks[s];
   const int tiles_m = a.tiles_x * a.tiles_y * a.B;
-  const int rank = CG == 2 ? (int)cluster_ctarank() : 0;  // 0 = MMA leader
-  const int group0 = blockIdx.x / CG, group_stride = gridDim.x / CG;
-  const int pairs_m = (tiles_m + CG - 1) / CG;              // work items per N tile (an item = CG adjacent M tiles)
+  const int group0 = blockIdx.x, group_stride = gridDim.x;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < a.a_stages; ++s) {
       mbar_init(&bars->a_full[s], 1);
-      mbar_init(&bars->a_empty[s], 1);
+      mbar_init(&bars->a_empty[s], 8);  // one arrival per MMA warp
     }
     for (int s = 0; s < a.b_stages; ++s) {
       mbar_init(&bars->b_full[s], 1);
-      mbar_init(&bars->b_empty[s], 1);
+      mbar_init(&bars->b_empty[s], 8);
     }
-    for (int t = 0; t < 2; ++t) {
-      mbar_init(&bars->acc_full[t], 1);
-      mbar_init(&bars->acc_empty[t], 8 * CG);  // one arrival per epilogue warp (of both CTAs in pair mode)
-    }
+    mbar_init(&bars->acc_full, 8);
+    mbar_init(&bars->acc_empty, 8);  // one arrival per epilogue warp
     fence_barrier_init();
   }
   // the bias vector is read by every epilogue thread for every 32-column chunk: one copy in shared memory instead of 8
-  // dependent global loads per chunk (11.6 % + 10.1 % of the convc1 launch's stall samples sat on them, ncu r02c)
+  // dependent global loads per chunk
   for (int k = threadIdx.x; k < a.n_tiles * a.NT && k < kMaxBias; k += blockDim.x) sbias[k] = a.bias ? a.bias[k] : 0.f;
-  if (warp == 5) {
-    if (CG == 2) tmem_alloc_2cta<512>(&bars->tmem_base);
-    else tmem_alloc<512>(&bars->tmem_base);
-  }
-  if (warp == 4 && lane == 0) {
+  if (warp == 16 && lane == 0) {
     prefetch_tmap(&tm0);
     prefetch_tmap(&tmW);
     if (tma_out) prefetch_tmap(&tmO0);
   }
-  tc_fence_before();
   __syncthreads();
-  if (CG == 2) cluster_sync_all();  // the peer's barriers must be initialised before anything signals them
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
-  // PDL: everything above (barriers, TMEM, tensor-map prefetch) overlapped the previous kernel's drain
+  // PDL: everything above (barriers, bias, tensor-map prefetch) overlapped the previous kernel's drain
   pdl_wait();
   pdl_trigger();
   if (warp == 0) PFB_TR(2);
 
   // work item j -> (n tile, image, tile row, tile col) of THIS CTA; n-tile major so concurrent CTAs share the weight
-  // tile in L2.  In pair mode the two CTAs take adjacent M tiles; a missing partner tile decodes to b == B
-  // (all its TMA loads fall outside the tensor and are zero-filled, its stores are masked).
+  // tile in L2
   auto decode = [&](int j, int& n0, int& b, int& y0, int& x0) {
-    const int nt = j / pairs_m;
-    int m = (j - nt * pairs_m) * CG + rank;
-    if (m >= tiles_m) m = tiles_m;  // -> b == B
+    const int nt = j / tiles_m;
+    int m = j - nt * tiles_m;
     const int px = m % a.tiles_x;
     m /= a.tiles_x;
     const int py = m % a.tiles_y;
@@ -244,153 +274,78 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
     x0 = px * a.TW;
   };
 
-  if (warp == 4) {
+  if (warp == 16) {
     // ================= TMA producer (warp-uniform loop, one elected lane issues) =================
-    {
-      const int ph2 = a.KH >> 1, pw2 = a.KW >> 1;
-      const uint32_t btx = a.NT * 128;  // bytes of the whole weight tile (both halves in pair mode)
-      const int brow = rank * (a.NT / CG);  // this CTA stages rows [brow, brow + NT / CG) of the weight tile
-      // ring positions advance incrementally (stage index + phase bit): no integer division on the issue path
-      int sta = 0, stb = 0, bg = 0;
-      uint32_t pha = 0, phb = 0;
-      PFB_TR(3);
-      for (int w = group0; w < a.n_work; w += group_stride) {
-        int n0, b, y0, x0;
-        decode(w, n0, b, y0, x0);
-        int kidx = 0;
-        const int wrow0 = (b < a.B ? b : 0) * a.w_rows_per_sample;  // per-sample weights (GMA aggregate: the sample's v^T)
-        for (int s = 0; s < a.nsrc; ++s) {
-          const CUtensorMap* tm = s == 0 ? &tm0 : (s == 1 ? &tm1 : &tm2);
-          for (int c = 0; c < a.src_chunks[s]; ++c, ++kidx) {
-            int wrow = wrow0;  // + (ky * KW + kx) * Cout_pad_k
-            for (int ky = 0; ky < a.KH; ++ky) {
-              for (int kx = 0; kx < a.KW; ++kx) {
-                // activation patch: once per (chunk, ky) with the x halo, once per chunk with the y halo, else per tap
-                if (a.halo == 0 || (a.halo == 1 && kx == 0) || (a.halo == 2 && ky == 0)) {
-                  mbar_wait(&bars->a_empty[sta], pha ^ 1);
-                  if (elect_one()) {
-                    // the leader's barrier collects the bytes of both CTAs; only the leader posts the expectation
-                    if (rank == 0) mbar_arrive_expect_tx(&bars->a_full[sta], a.a_tx_bytes * CG);
-                    if (CG == 2)
-                      tma_load_4d_2cta(smemA + sta * a.a_slot_bytes, tm, &bars->a_full[sta], a.src_coff[s] + c * 64,
-                                       x0 - pw2 + (a.halo ? 0 : kx), y0 + ky - ph2, b);
-                    else
-                      tma_load_4d(smemA + sta * a.a_slot_bytes, tm, &bars->a_full[sta], a.src_coff[s] + c * 64,
-                                  x0 - pw2 + (a.halo ? 0 : kx), y0 + ky - ph2, b);
-                  }
-                  __syncwarp();
-                  if (++sta == a.a_stages) { sta = 0; pha ^= 1; }
-                }
-                // weight stage: b_group consecutive taps of this patch share one barrier (fewer, larger pipeline steps)
-                if (bg == 0) mbar_wait(&bars->b_empty[stb], phb ^ 1);
+    const int ph2 = a.KH >> 1, pw2 = a.KW >> 1;
+    const uint32_t btx = a.NT * 128;  // bytes of one weight tap
+    // ring positions advance incrementally (stage index + phase bit): no integer division on the issue path
+    int sta = 0, stb = 0, bg = 0;
+    uint32_t pha = 0, phb = 0;
+    PFB_TR(3);
+    for (int w = group0; w < a.n_work; w += group_stride) {
+      int n0, b, y0, x0;
+      decode(w, n0, b, y0, x0);
+      int kidx = 0;
+      const int wrow0 = b * a.w_rows_per_sample;  // per-sample weights (GMA aggregate: the sample's v^T)
+      for (int s = 0; s < a.nsrc; ++s) {
+        const CUtensorMap* tm = s == 0 ? &tm0 : (s == 1 ? &tm1 : &tm2);
+        for (int c = 0; c < a.src_chunks[s]; ++c, ++kidx) {
+          int wrow = wrow0;  // + (ky * KW + kx) * Cout_pad_k
+          for (int ky = 0; ky < a.KH; ++ky) {
+            for (int kx = 0; kx < a.KW; ++kx) {
+              // activation patch: once per (chunk, ky) with the x halo, once per chunk with the y halo, else per tap
+              if (a.halo == 0 || (a.halo == 1 && kx == 0) || (a.halo == 2 && ky == 0)) {
+                mbar_wait(&bars->a_empty[sta], pha ^ 1);
                 if (elect_one()) {
-                  if (rank == 0 && bg == 0) mbar_arrive_expect_tx(&bars->b_full[stb], btx * a.b_group);
-                  uint8_t* dstB = smemB + stb * a.b_slot_bytes + bg * a.b_tap_bytes;
-                  if (CG == 2) tma_load_2d_2cta(dstB, &tmW, &bars->b_full[stb], kidx * 64, wrow + n0 + brow);
-                  else tma_load_2d(dstB, &tmW, &bars->b_full[stb], kidx * 64, wrow + n0);
+                  mbar_arrive_expect_tx(&bars->a_full[sta], a.a_tx_bytes);
+                  tma_load_4d(smemA + sta * a.a_slot_bytes, tm, &bars->a_full[sta], a.src_coff[s] + c * 64,
+                              x0 - pw2 + (a.halo ? 0 : kx), y0 + ky - ph2, b);
                 }
                 __syncwarp();
-                wrow += a.Cout_pad_k;
-                if (++bg == a.b_group) {
-                  bg = 0;
-                  if (++stb == a.b_stages) { stb = 0; phb ^= 1; }
-                }
+                if (++sta == a.a_stages) { sta = 0; pha ^= 1; }
+              }
+              // weight stage: b_group consecutive taps of this patch share one barrier (fewer, larger pipeline steps)
+              if (bg == 0) mbar_wait(&bars->b_empty[stb], phb ^ 1);
+              if (elect_one()) {
+                if (bg == 0) mbar_arrive_expect_tx(&bars->b_full[stb], btx * a.b_group);
+                tma_load_2d(smemB + stb * a.b_slot_bytes + bg * a.b_tap_bytes, &tmW, &bars->b_full[stb], kidx * 64, wrow + n0);
+              }
+              __syncwarp();
+              wrow += a.Cout_pad_k;
+              if (++bg == a.b_group) {
+                bg = 0;
+                if (++stb == a.b_stages) { stb = 0; phb ^= 1; }
               }
             }
           }
         }
       }
-      PFB_TR(4);
     }
-  } else if (warp == 5) {
-    // ================= MMA issuer =================
-    // One thread issues everything, so its instruction count per tap IS the pacing of the tensor pipe when the
-    // tile is small (ncu: ~130 SASS instructions/tap at ~8 clk each paced the first version).  Everything that can
-    // be precomputed is: 32-bit shared addresses of barriers and slots, descriptor words updated by adds only.
-    // The WHOLE warp walks the loop (warp-uniform control flow, all lanes poll the barriers) and one elected lane
-    // issues the MMAs / commits: under a divergent `lane == 0` branch ptxas wraps every tcgen05 instruction in its
-    // own ELECT / vote / branch sequence, which showed up as most of the issue thread's time in the ncu source view.
-    if (rank == 0) {
-      const uint32_t idesc = make_idesc_f16(128 * CG, a.NT, a.ab_fmt);
-      // descriptor = {lo: (addr >> 4) | LBO(1) << 16, hi: SBO(1024 >> 4) | version 1 << 14 | SWIZZLE_128B 2 << 29}
-      const uint32_t desc_hi = (1024u >> 4) | (1u << 14) | (2u << 29);
-      const uint32_t a_slot16 = (uint32_t)a.a_slot_bytes >> 4, b_slot16 = (uint32_t)a.b_slot_bytes >> 4;
-      const uint32_t a_lo0 = ((smem_u32(smemA) & 0x3FFFF) >> 4) | (1u << 16);
-      const uint32_t b_lo0 = ((smem_u32(smemB) & 0x3FFFF) >> 4) | (1u << 16);
-      const uint32_t bar_a_full = smem_u32(&bars->a_full[0]), bar_a_empty = smem_u32(&bars->a_empty[0]);
-      const uint32_t bar_b_full = smem_u32(&bars->b_full[0]), bar_b_empty = smem_u32(&bars->b_empty[0]);
-      const int kw_halo = a.halo == 1 ? a.KW : (a.halo == 2 ? a.KH : 1);  // taps served by one activation patch
-      const int groups = chunks * (a.halo == 1 ? a.KH : (a.halo == 2 ? 1 : a.KH * a.KW));  // patches per tile
-      const uint32_t tap_step16 = a.halo == 2 ? (uint32_t)a.TW * 8u : 8u;  // descriptor advance per tap (16-B units)
-      const uint32_t b_tap16 = (uint32_t)a.b_tap_bytes >> 4;
-      int sa = 0, sb = 0, i = 0;
-      uint32_t pha = 0, phb = 0;
-      uint32_t a_lo = a_lo0, b_lo = b_lo0;
-      for (int w = group0; w < a.n_work; w += group_stride, ++i) {
-        const int t = i & 1;
-        mbar_wait(&bars->acc_empty[t], ((i >> 1) & 1) ^ 1);
-        tc_fence_after();
-        if (i < 3) PFB_TR(9 + i);
-        const uint32_t d = tmem_base + t * a.acc_stride;
-        uint32_t acc = 0;  // first MMA of the tile overwrites the accumulator
-        for (int g = 0; g < groups; ++g) {
-          mbar_wait_uniform(bar_a_full + 8 * sa, pha);
-          if (i == 0 && g == 0) PFB_TR(5);
-          for (int kx = 0; kx < kw_halo; kx += a.b_group) {
-            mbar_wait_uniform(bar_b_full + 8 * sb, phb);
-            tc_fence_after();
-            const uint32_t al = a_lo + tap_step16 * kx;  // x halo: +1 pixel row (128 B) per tap; y halo: +TW rows
-            if (elect_one()) {
-              // straight-line issue of the whole group: the per-step overhead of this single thread (barrier poll,
-              // election, R->UR moves, ring bookkeeping: ~65 SASS instructions, ~500 clk) is what paced the N <= 192
-              // layers at 4 MMAs per step (PFB_CONV_TRACE timelines); 12-20 MMAs per step amortise it.
-              switch (a.b_group) {
-                case 5: issue_taps<CG, 5>(d, al, tap_step16, b_lo, b_tap16, desc_hi, idesc, acc); break;
-                case 3: issue_taps<CG, 3>(d, al, tap_step16, b_lo, b_tap16, desc_hi, idesc, acc); break;
-                default: issue_taps<CG, 1>(d, al, tap_step16, b_lo, b_tap16, desc_hi, idesc, acc); break;
-              }
-              if (CG == 2) umma_commit_addr_2cta(bar_b_empty + 8 * sb);
-              else umma_commit_addr(bar_b_empty + 8 * sb);
-              if (kx + a.b_group >= kw_halo) {
-                if (CG == 2) umma_commit_addr_2cta(bar_a_empty + 8 * sa);
-                else umma_commit_addr(bar_a_empty + 8 * sa);
-              }
-            }
-            __syncwarp();
-            acc = 1;
-            b_lo += b_slot16;
-            if (++sb == a.b_stages) { sb = 0; phb ^= 1; b_lo = b_lo0; }
-          }
-          a_lo += a_slot16;
-          if (++sa == a.a_stages) { sa = 0; pha ^= 1; a_lo = a_lo0; }
-        }
-        if (elect_one()) {
-          if (CG == 2) umma_commit_addr_2cta(smem_u32(&bars->acc_full[t]));
-          else umma_commit(&bars->acc_full[t]);
-        }
-        __syncwarp();
-        if (i < 3) PFB_TR(6 + i);
-      }
+    PFB_TR(4);
+  } else if (warp >= 8) {
+    // ================= MMA warpgroups =================
+    switch (a.NT) {
+      case 32: conv_mma_role<32, std::is_same<T, __nv_bfloat16>::value>(a, bars, smemA, smemB, sacc, chunks, group0, group_stride); break;
+      case 64: conv_mma_role<64, std::is_same<T, __nv_bfloat16>::value>(a, bars, smemA, smemB, sacc, chunks, group0, group_stride); break;
+      case 96: conv_mma_role<96, std::is_same<T, __nv_bfloat16>::value>(a, bars, smemA, smemB, sacc, chunks, group0, group_stride); break;
+      default: conv_mma_role<128, std::is_same<T, __nv_bfloat16>::value>(a, bars, smemA, smemB, sacc, chunks, group0, group_stride); break;
     }
   } else {
     // ================= epilogue: thread <-> pixel, 32 output channels at a time =================
-    // warps 0-3 take the even 32-column chunks, warps 6-9 the odd ones; a warp may only touch the TMEM
-    // lane quarter (warp id % 4)
-    const int quarter = warp & 3, group = warp < 4 ? 0 : 1;
+    // warps 0-3 take the even 32-column chunks, warps 4-7 the odd ones
+    const int quarter = warp & 3, group = warp >> 2;
     const int row = quarter * 32 + lane;
     const int hd = a.hidden;
     int i = 0;
     for (int w = group0; w < a.n_work; w += group_stride, ++i) {
       int n0, b, y0, x0;
       decode(w, n0, b, y0, x0);
-      const int t = i & 1, tuse = i >> 1;
       const int y = y0 + (row >> a.tw_shift), x = x0 + (row & (a.TW - 1));
       const bool ok = (y < a.H) && (x < a.W) && (b < a.B);
       const size_t p = ((size_t)b * a.H + (ok ? y : 0)) * a.W + (ok ? x : 0);
       // Operands that do not depend on the accumulator (h, z, residual) are requested BEFORE waiting for the MMAs
-      // of this tile, and the next chunk's while the current one is processed: the ncu source view of the first
-      // version had the epilogue warps parked on these loads (exposed L2 latency, 25 % of their time), which made
-      // the GRU layers epilogue-bound (3 tiles per CTA, each epilogue ~2x the tile's MMA time).
+      // of this tile, and the next chunk's while the current one is processed (exposed L2 latency otherwise makes the
+      // GRU layers epilogue-bound).
       const bool aux_h_any = EPI == PFB_EPI_GRU_ZR || EPI == PFB_EPI_GRU_Q || EPI == PFB_EPI_AXPY;
       auto issue_h = [&](int c, uint4 (&hq)[4]) {
         const int n = n0 + c;
@@ -433,14 +388,11 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
       if (aux_h_any) issue_h(group * 32, hnext);
       issue_z(group * 32, znext);
       issue_add(group * 32, anext);
-      mbar_wait(&bars->acc_full[t], tuse & 1);
-      tc_fence_after();
+      mbar_wait(&bars->acc_full, i & 1);
       if (warp == 0 && i < 3) PFB_TR(12 + i);
-      const uint32_t taddr = tmem_base + t * a.acc_stride + ((uint32_t)(quarter * 32) << 16);
-      // TMEM reads are software-pipelined too: the load of chunk c + 64 is issued as soon as chunk c has been moved
-      // to v[], and completes under the arithmetic and the stores of chunk c.
+      // accumulator reads are software-pipelined too: chunk c + 64 is loaded as soon as chunk c has been moved to v[]
       uint32_t r[32];
-      if (group * 32 < a.NT) tmem_ld_32x32(taddr + group * 32, r);
+      if (group * 32 < a.NT) acc_ld32(sacc, row, group * 32, r);
       // 32 packed values -> this thread's half (group) of its pixel's 128-byte row in the staging buffer
       auto stage32 = [&](const uint4 (&pk)[4]) {
         uint8_t* sb = smemO + row * 128;
@@ -460,7 +412,6 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
           uint4 araw[4];
 #pragma unroll
           for (int q = 0; q < 4; ++q) araw[q] = anext[q];
-          tmem_ld_wait();
 #pragma unroll
           for (int q = 0; q < 4; ++q) {
             float f[8];
@@ -472,7 +423,6 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
           float4 bb[8];
 #pragma unroll
           for (int q = 0; q < 8; ++q) bb[q] = reinterpret_cast<const float4*>(sbias + n)[q];
-          tmem_ld_wait();
 #pragma unroll
           for (int q = 0; q < 8; ++q) {
             v[4 * q + 0] = __uint_as_float(r[4 * q + 0]) + bb[q].x;
@@ -482,7 +432,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
           }
         }
         if (!kLate && c + 64 < a.NT) {  // warp-uniform
-          tmem_ld_32x32(taddr + c + 64, r);
+          acc_ld32(sacc, row, c + 64, r);
           if (aux_h_any) issue_h(c + 64, hnext);
           issue_z(c + 64, znext);
           issue_add(c + 64, anext);
@@ -588,7 +538,7 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
           }
         }
         if (kLate && c + 64 < a.NT) {  // warp-uniform
-          tmem_ld_32x32(taddr + c + 64, r);
+          acc_ld32(sacc, row, c + 64, r);
           if (aux_h_any) issue_h(c + 64, hnext);
           issue_z(c + 64, znext);
           issue_add(c + 64, anext);
@@ -610,31 +560,27 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
          }
        }
       }
-      tc_fence_before();
       __syncwarp();
       if (warp == 0 && i < 3) PFB_TR(15 + i);
-      if (warp == 6 && i < 3) PFB_TR(21 + i);
-      if (lane == 0) {
-        if (CG == 2) mbar_arrive_leader_relaxed(&bars->acc_empty[t]);  // the leader's MMA thread owns the accumulator hand-off
-        else mbar_arrive(&bars->acc_empty[t]);
-      }
+      if (warp == 4 && i < 3) PFB_TR(21 + i);
+      if (lane == 0) mbar_arrive(&bars->acc_empty);
     }
   }
   if (tma_out && threadIdx.x == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // stores complete (not only read)
-  tc_fence_before();
   __syncthreads();
   if (warp == 0) PFB_TR(18);
-  if (CG == 2) cluster_sync_all();  // the leader's MMAs read the peer's shared memory: nobody leaves early
-  if (warp == 0) PFB_TR(19);
   if (a.trace && threadIdx.x == 0) a.trace[blockIdx.x * 32 + 20] = global_timer_ns();
-  if (warp == 5) {
-    if (CG == 2) tmem_dealloc_2cta<512>(tmem_base);
-    else tmem_dealloc<512>(tmem_base);
-  }
 }
 
 // ------------------------------------------------------------------------------------------------
 static int eff_channels(const pfb_conv_src& s) { return (int)align_up((size_t)s.channels, 64); }
+
+// N tiling: the fewest equal tiles of <= 128 columns that are multiples of 32 (epilogue chunk); 0 if there is none
+static int conv_n_tiles(int cout_pad) {
+  for (int n = ceil_div(cout_pad, 128); n <= cout_pad / 32; ++n)
+    if (cout_pad % n == 0 && (cout_pad / n) % 32 == 0) return n;
+  return 0;
+}
 
 bool conv2d_umma_supported(const pfb_conv_params* p) {
   if (p->dtype != PFB_F16 && p->dtype != PFB_BF16) return false;
@@ -668,15 +614,10 @@ bool conv2d_umma_supported(const pfb_conv_params* p) {
   if (p->out_stride % 8 || p->out_offset % 8) return false;
   if (p->w_rows_per_sample && (p->KH != 1 || p->KW != 1 || p->w_rows_per_sample < p->Cout_pad_k)) return false;
   if (p->addend && (p->addend_stride % 8 || (reinterpret_cast<uintptr_t>(p->addend) & 15) || p->addend_stride < p->Cout_pad_k)) return false;
-  // N tiling: equal tiles of <= 256 columns, multiple of 32 (epilogue chunk) unless a single small tile
-  int n_tiles = ceil_div(p->Cout_pad_k, 256);
-  if (p->Cout_pad_k % n_tiles) return false;
-  int NT = p->Cout_pad_k / n_tiles;
-  if (NT % 32) return false;
-  return true;
+  return conv_n_tiles(p->Cout_pad_k) > 0;
 }
 
-template <typename T, int CG, int EPI>
+template <typename T, int EPI>
 static int launch_conv_umma_e(const CUtensorMap* tms, const CUtensorMap& tmW, const CUtensorMap* tmO, const ConvUmmaArgs& a, int grid,
                               size_t smem, cudaStream_t s) {
   // once per (instantiation, device): correct when one process drives several devices, and off the per-launch path
@@ -684,38 +625,34 @@ static int launch_conv_umma_e(const CUtensorMap* tms, const CUtensorMap& tmW, co
   int dev = 0;
   PFB_CUDA(cudaGetDevice(&dev));
   if (!(attr_done.load(std::memory_order_acquire) & (1ull << (dev & 63)))) {
-    PFB_CUDA(cudaFuncSetAttribute(conv_umma_kernel<T, CG, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    PFB_CUDA(cudaFuncSetAttribute(conv_umma_kernel<T, EPI>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
     attr_done.fetch_or(1ull << (dev & 63), std::memory_order_release);
   }
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(320);
+  cfg.blockDim = dim3(kConvThreads);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = s;
-  cudaLaunchAttribute attr[2];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = CG;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  attr[1].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attr[1].val.programmaticStreamSerializationAllowed = pdl_enabled();
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled();
   cfg.attrs = attr;
-  cfg.numAttrs = 2;
-  PFB_CUDA(cudaLaunchKernelEx(&cfg, conv_umma_kernel<T, CG, EPI>, tms[0], tms[1], tms[2], tmW, tmO[0], tmO[1], a));
+  cfg.numAttrs = 1;
+  PFB_CUDA(cudaLaunchKernelEx(&cfg, conv_umma_kernel<T, EPI>, tms[0], tms[1], tms[2], tmW, tmO[0], tmO[1], a));
   return PFB_OK;
 }
 
-template <typename T, int CG>
+template <typename T>
 static int launch_conv_umma(const CUtensorMap* tms, const CUtensorMap& tmW, const CUtensorMap* tmO, const ConvUmmaArgs& a, int grid,
                             size_t smem, cudaStream_t s) {
   switch (a.epilogue) {
-    case PFB_EPI_LINEAR: return launch_conv_umma_e<T, CG, PFB_EPI_LINEAR>(tms, tmW, tmO, a, grid, smem, s);
-    case PFB_EPI_RELU: return launch_conv_umma_e<T, CG, PFB_EPI_RELU>(tms, tmW, tmO, a, grid, smem, s);
-    case PFB_EPI_GRU_ZR: return launch_conv_umma_e<T, CG, PFB_EPI_GRU_ZR>(tms, tmW, tmO, a, grid, smem, s);
-    case PFB_EPI_GRU_Q: return launch_conv_umma_e<T, CG, PFB_EPI_GRU_Q>(tms, tmW, tmO, a, grid, smem, s);
-    case PFB_EPI_RELU_APPEND_FLOW: return launch_conv_umma_e<T, CG, PFB_EPI_RELU_APPEND_FLOW>(tms, tmW, tmO, a, grid, smem, s);
-    case PFB_EPI_AXPY: return launch_conv_umma_e<T, CG, PFB_EPI_AXPY>(tms, tmW, tmO, a, grid, smem, s);
-    case PFB_EPI_LINEAR_F32: return launch_conv_umma_e<T, CG, PFB_EPI_LINEAR_F32>(tms, tmW, tmO, a, grid, smem, s);
+    case PFB_EPI_LINEAR: return launch_conv_umma_e<T, PFB_EPI_LINEAR>(tms, tmW, tmO, a, grid, smem, s);
+    case PFB_EPI_RELU: return launch_conv_umma_e<T, PFB_EPI_RELU>(tms, tmW, tmO, a, grid, smem, s);
+    case PFB_EPI_GRU_ZR: return launch_conv_umma_e<T, PFB_EPI_GRU_ZR>(tms, tmW, tmO, a, grid, smem, s);
+    case PFB_EPI_GRU_Q: return launch_conv_umma_e<T, PFB_EPI_GRU_Q>(tms, tmW, tmO, a, grid, smem, s);
+    case PFB_EPI_RELU_APPEND_FLOW: return launch_conv_umma_e<T, PFB_EPI_RELU_APPEND_FLOW>(tms, tmW, tmO, a, grid, smem, s);
+    case PFB_EPI_AXPY: return launch_conv_umma_e<T, PFB_EPI_AXPY>(tms, tmW, tmO, a, grid, smem, s);
+    case PFB_EPI_LINEAR_F32: return launch_conv_umma_e<T, PFB_EPI_LINEAR_F32>(tms, tmW, tmO, a, grid, smem, s);
     default: break;
   }
   set_error("conv_umma: epilogue %d has no tensor-core instantiation", a.epilogue);
@@ -737,12 +674,9 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
   CUtensorMap tms[3];
   pick_tile(p->H, p->W, a.TW, a.TH);
   static const int env_halo = getenv("PFB_CONV_HALO") ? atoi(getenv("PFB_CONV_HALO")) : 1;
-  static const int env_cg = getenv("PFB_CONV_CTA_PAIR") ? atoi(getenv("PFB_CONV_CTA_PAIR")) : 1;
   static const int env_vhalo = getenv("PFB_CONV_VHALO") ? atoi(getenv("PFB_CONV_VHALO")) : 1;
   a.halo = (env_halo && a.TH == 1 && p->KW > 1) ? 1 : 0;
-  // (with all 256 output channels in one tile the 448-tile grid of the 8x16 patches costs a fourth round that the
-  //  smaller activation traffic does not pay back: 61.5 vs 57.8 us on the z|r layer, launch lists v13-v15)
-  if (env_vhalo && p->KW == 1 && p->KH > 1 && p->Cout_pad_k / ceil_div(p->Cout_pad_k, 256) < 256) {
+  if (env_vhalo && p->KW == 1 && p->KH > 1) {
     // vertical taps: a (TH + KH - 1) x TW patch serves all KH taps of a chunk when the per-tap offset TW * 128 B keeps
     // the 1024-byte swizzle phase (TW % 8 == 0).  Fewest tiles first, then the smallest patch.
     long best_tiles = -1, best_patch = 0;
@@ -772,40 +706,41 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
     if (rc) return rc;
   }
   for (int i = p->nsrc; i < 3; ++i) tms[i] = tms[0];
-  a.n_tiles = ceil_div(p->Cout_pad_k, 256);
+  a.n_tiles = conv_n_tiles(p->Cout_pad_k);
+  if (a.n_tiles == 0) return PFB_ERR_UNSUPPORTED;
   a.NT = p->Cout_pad_k / a.n_tiles;
-  // CTA pairs split the weight tile in two: needs an even row count per half (UMMA N % 16) -> NT % 32, always true here
-  // (per-sample weights: a CTA pair shares one weight tile, and adjacent M tiles may belong to different samples -> single CTAs)
-  const int CG = (env_cg && (sm_count() % 2) == 0 && p->w_rows_per_sample == 0) ? 2 : 1;
-  a.acc_stride = a.NT > 128 ? 256 : 128;
   CUtensorMap tmW;
   {
     uint64_t dims[2] = {(uint64_t)p->Cin_pad, p->w_rows_per_sample > 0 ? (uint64_t)p->B * p->w_rows_per_sample : (uint64_t)p->KH * p->KW * p->Cout_pad_k};
     uint64_t str[1] = {(uint64_t)p->Cin_pad * 2};
-    uint32_t box[2] = {64, (uint32_t)(a.NT / CG)};
+    uint32_t box[2] = {64, (uint32_t)a.NT};
     int rc = make_tensor_map(&tmW, p->weight_k, p->dtype, 2, dims, str, box);
     if (rc) return rc;
   }
   a.B = p->B; a.H = p->H; a.W = p->W; a.KH = p->KH; a.KW = p->KW;
   a.tiles_x = ceil_div(p->W, a.TW);
   a.tiles_y = ceil_div(p->H, a.TH);
-  a.n_work = ceil_div(a.tiles_x * a.tiles_y * p->B, CG) * a.n_tiles;  // items of CG adjacent M tiles
+  a.n_work = a.tiles_x * a.tiles_y * p->B * a.n_tiles;
   a.Cout = p->Cout; a.Cout_pad_k = p->Cout_pad_k;
   a.a_tx_bytes = patch_w * patch_h * 128;
   a.a_slot_bytes = (int)align_up((size_t)a.a_tx_bytes, 1024);
-  a.b_tap_bytes = (a.NT / CG) * 128;
+  a.b_tap_bytes = a.NT * 128;
   {
     static const int env_tma_out = getenv("PFB_CONV_TMA_STORE") ? atoi(getenv("PFB_CONV_TMA_STORE")) : 1;
     const bool plain = p->epilogue == PFB_EPI_LINEAR || p->epilogue == PFB_EPI_RELU || p->epilogue == PFB_EPI_RELU_APPEND_FLOW;
-    a.tma_out = env_tma_out && plain && (reinterpret_cast<uintptr_t>(p->out) & 15) == 0;
+    // a staged store writes whole 64-channel blocks: with several N tiles of NT % 64 == 32 the last block of a tile would
+    // overwrite the first 32 channels of the next one (a single tile is clipped at the layer's last channel by the tensor map)
+    a.tma_out = env_tma_out && plain && (reinterpret_cast<uintptr_t>(p->out) & 15) == 0 && (a.NT % 64 == 0 || a.n_tiles == 1);
   }
-  const int ring_budget = (a.tma_out ? 192 : 208) * 1024;  // 16 KB of output staging + 4 KB of bias come out of the rings' share
+  // 227 KB less the accumulator tile, the output staging, the bias, the barriers and the alignment slack
+  const int ring_budget = 227 * 1024 - acc_tile_bytes(a.NT) - (a.tma_out ? kATileBytes : 0) - kMaxBias * (int)sizeof(float) -
+                          (int)sizeof(ConvBars) - 1024;
   {
     static const int env_group = getenv("PFB_CONV_TAP_GROUP") ? atoi(getenv("PFB_CONV_TAP_GROUP")) : 1;
     const int taps = a.halo == 1 ? p->KW : (a.halo == 2 ? p->KH : 1);
     a.b_group = 1;
     // all taps of a patch in one weight stage when at least 3 such stages fit next to 3 activation patches
-    if (env_group && (taps == 3 || taps == 5) && 3 * taps * a.b_tap_bytes + 3 * a.a_slot_bytes <= ring_budget && a.NT <= 192) a.b_group = taps;
+    if (env_group && (taps == 3 || taps == 5) && 3 * taps * a.b_tap_bytes + 3 * a.a_slot_bytes <= ring_budget) a.b_group = taps;
   }
   a.b_slot_bytes = a.b_group * a.b_tap_bytes;
   // ---- outputs through staging + TMA bulk stores (everything but the fp32 tap products) ----
@@ -830,10 +765,9 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
     }
   }
   {
-    // Split ~212 KB between the rings.  The per-CTA timelines (PFB_CONV_TRACE, profiles/r01_conv_trace_*.txt) show a
-    // slot is reused only once per ~2.2 us (commit -> producer wake-up -> TMA round trip -> issue), so the number of
-    // K steps in flight, not the bytes, sets the pace of the small-N layers: maximise min(steps covered by the
-    // activation ring, weight stages).
+    // Split the rest between the rings.  A slot is reused only once per round trip (release -> producer wake-up -> TMA ->
+    // MMA), so the number of K steps in flight, not the bytes, sets the pace of the small-N layers: maximise min(steps
+    // covered by the activation ring, weight stages).
     const int budget = ring_budget;
     const int taps_per_patch = a.halo == 1 ? p->KW : (a.halo == 2 ? p->KH : 1);
     int best = -1;
@@ -853,10 +787,9 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
   a.w_rows_per_sample = p->w_rows_per_sample;
   a.ab_fmt = p->dtype == PFB_F16 ? 0 : 1;
   const size_t smem = (size_t)a.a_stages * a.a_slot_bytes + (size_t)a.b_stages * a.b_slot_bytes + (a.tma_out ? kATileBytes : 0) +
-                      kMaxBias * sizeof(float) + sizeof(ConvBars) + 1024;
-  int groups = sm_count() / CG;
-  if (groups > a.n_work) groups = a.n_work;
-  const int grid = groups * CG;
+                      acc_tile_bytes(a.NT) + kMaxBias * sizeof(float) + sizeof(ConvBars) + 1024;
+  int grid = sm_count();
+  if (grid > a.n_work) grid = a.n_work;
   static const char* env_trace = getenv("PFB_CONV_TRACE");  // debug: per-CTA timeline of every launch -> JSON lines
   if (env_trace) {
     static unsigned long long* dbuf = nullptr;
@@ -864,8 +797,7 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
     PFB_CUDA(cudaMemsetAsync(dbuf, 0, 256 * 32 * 8, s));
     a.trace = dbuf;
     int rc;
-    if (CG == 2) rc = p->dtype == PFB_F16 ? launch_conv_umma<__half, 2>(tms, tmW, tmO, a, grid, smem, s) : launch_conv_umma<__nv_bfloat16, 2>(tms, tmW, tmO, a, grid, smem, s);
-    else rc = p->dtype == PFB_F16 ? launch_conv_umma<__half, 1>(tms, tmW, tmO, a, grid, smem, s) : launch_conv_umma<__nv_bfloat16, 1>(tms, tmW, tmO, a, grid, smem, s);
+    rc = p->dtype == PFB_F16 ? launch_conv_umma<__half>(tms, tmW, tmO, a, grid, smem, s) : launch_conv_umma<__nv_bfloat16>(tms, tmW, tmO, a, grid, smem, s);
     if (rc) return rc;
     PFB_CUDA(cudaStreamSynchronize(s));
     static unsigned long long host[256 * 32];
@@ -880,12 +812,8 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
     return PFB_OK;
   }
   ProfScope prof(KC_CONV, s);
-  if (CG == 2) {
-    if (p->dtype == PFB_F16) return launch_conv_umma<__half, 2>(tms, tmW, tmO, a, grid, smem, s);
-    return launch_conv_umma<__nv_bfloat16, 2>(tms, tmW, tmO, a, grid, smem, s);
-  }
-  if (p->dtype == PFB_F16) return launch_conv_umma<__half, 1>(tms, tmW, tmO, a, grid, smem, s);
-  return launch_conv_umma<__nv_bfloat16, 1>(tms, tmW, tmO, a, grid, smem, s);
+  if (p->dtype == PFB_F16) return launch_conv_umma<__half>(tms, tmW, tmO, a, grid, smem, s);
+  return launch_conv_umma<__nv_bfloat16>(tms, tmW, tmO, a, grid, smem, s);
 }
 
 }  // namespace pfb

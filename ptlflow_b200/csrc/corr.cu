@@ -404,7 +404,7 @@ extern "C" PFB_API int pfb_corr_volume_build_ex(const void* fmap1, const void* f
   cudaStream_t s = as_stream(stream);
   bool can_umma = corr_volume_umma_supported(B, H, W, C, levels, dtype);
   if (impl == 2 && !can_umma) {
-    set_error("corr_volume_build: tcgen05 path does not support B=%d H=%d W=%d C=%d dtype=%d", B, H, W, C, (int)dtype);
+    set_error("corr_volume_build: wgmma path does not support B=%d H=%d W=%d C=%d dtype=%d", B, H, W, C, (int)dtype);
     return PFB_ERR_UNSUPPORTED;
   }
   if ((impl == 0 && can_umma) || impl == 2) return corr_volume_umma(fmap1, fmap2, pyramid, B, N1, H, W, C, levels, scale, dtype, s);

@@ -8,10 +8,10 @@
 // completely when the flow is locally smooth, so the item multiplies the tile's 128 query vectors with a REGION of the
 // level's feature map that contains all their windows -- anchored at the tile's smallest window origin, 32 targets wide, in
 // bands of 8 rows (band stride 7, so that every vertical tap pair lies inside one band):
-//     D[128 queries][256 targets] = F1_tile[128][C] . F2_band[256][C]^T        (tcgen05, M = 128, N = 256, fp32 in TMEM)
+//     D[128 queries][256 targets] = F1_tile[128][C] . F2_band[256][C]^T        (wgmma: two warpgroups of m64n128 per band half)
 // Both operands are TMA boxes of the pixel-major feature maps (out-of-map targets are zero-filled by the TMA unit: the
-// zero padding of raft/utils.py:71-75 for free).  Each epilogue thread owns one query: it dumps its accumulator row to
-// shared memory (scaled, storage type -- the same rounding the materialised volume has), then blends the window rows that
+// zero padding of raft/utils.py:71-75 for free).  The MMA warpgroups dump the accumulator rows to shared memory (storage
+// type -- the same rounding the materialised volume has); each epilogue thread owns one query and blends the window rows that
 // fall into this band (x-major order of corr.py:43-47) and stages the level's 81 outputs for a coalesced store.
 // Queries whose window does not fit the region (rough flow inside a tile) are flagged and recomputed by the SIMT kernel
 // (exact same values, one warp per flagged query), so the result never depends on the smoothness of the flow.
@@ -20,19 +20,19 @@
 #include <algorithm>
 #include <vector>
 #include <stdio.h>
+#include <type_traits>
 
 #include "umma.cuh"
 
 namespace pfb {
-using namespace sm100;
+using namespace sm90;
 
 constexpr int kOtfTileBytes = 128 * 128;       // 128 rows x 64 channels
-constexpr int kOtfBandRows = 256;              // targets per band: 8 rows x 32 columns
 constexpr int kOtfMaxBands = 8;                // 7 * 8 + 1 = 57 region rows at most
 constexpr int kOtfRW = 32;
 constexpr int kOtfDumpPitch = 520;             // bytes per accumulator-dump row: 256 targets x 2 bytes + 8 (130 words: 8-byte stores of a
                                                // half-warp and the gather's 4-byte loads of a warp spread over the banks)
-constexpr int kOtfMaxStages = 4;               // B-operand ring: 64-channel chunks of one band (32 KB each)
+constexpr int kOtfMaxStages = 6;               // B-operand ring: 64-channel chunks of one band half (4 rows x 32 columns, 16 KB each)
 
 struct OtfArgs {
   const float* coords;
@@ -41,7 +41,6 @@ struct OtfArgs {
   int B, H, W, kchunks, levels, out_stride;
   int lh[4], lw[4];
   float scale;
-  int ab_fmt;
   int tiles_x, tiles_y, n_tiles;
   int b_stages;
   unsigned long long* trace;  // PFB_OTF_TRACE: [CTA][64] clock64 stamps of the CTA's second work item (phase timeline), else null
@@ -50,9 +49,8 @@ struct OtfArgs {
 struct __align__(8) OtfBars {
   uint64_t a_full, a_empty;
   uint64_t b_full[kOtfMaxStages], b_empty[kOtfMaxStages];
-  uint64_t acc_full[2], acc_empty[2];
+  uint64_t dump_full, dump_empty;
   uint64_t reg_full[2], reg_empty[2];
-  uint32_t tmem_base;
   int region[2][4];  // per item parity: bx0, by0, number of bands
   int red[4][3];
 };
@@ -82,20 +80,20 @@ __device__ __forceinline__ unsigned short otf_f32_to_bits<__half>(float v) { ret
 template <>
 __device__ __forceinline__ unsigned short otf_f32_to_bits<__nv_bfloat16>(float v) { return __bfloat16_as_ushort(__float2bfloat16_rn(v)); }
 
-// Roles: warps 0-7 = epilogue (two threads per query of the tile: warps w and w + 4 share a TMEM lane quarter and split the
-// accumulator columns / window rows), warp 8 = TMA producer, warp 9 = MMA issuer.  The three walk the
-// same list of work items (tile, level) and are coupled only through mbarriers:
+// Roles: warps 0-7 = epilogue (two threads per query of the tile: warps w and w + 4 hold the same queries and split the
+// window rows), warps 8-15 = two MMA warpgroups (query halves; the band's two target halves one after the other),
+// warp 16 = TMA producer.  The three
+// walk the same list of work items (tile, level) and are coupled only through mbarriers:
 //   reg_full / reg_empty [item parity]  the epilogue publishes the item's region (anchor, bands) one item AHEAD, so the
 //                                       producer streams the next item's operands while the epilogue still blends this one
 //   a_full / a_empty                    the tile's query vectors (kchunks x 16 KB), loaded once per item
-//   b_full / b_empty [stage]            ring of 64-channel chunks of a band (32 KB each): a band's chunks are consumed once,
+//   b_full / b_empty [stage]            ring of 64-channel chunks of a band half (16 KB each): consumed once,
 //                                       so the band is never resident as a whole
-//   acc_full / acc_empty [2]            two 256-column accumulators in TMEM: band k+1 is multiplied while band k is dumped
-// (The first version ran TMA -> MMA -> dump -> gather in lock step per band with the dump aliasing the operand buffer:
-// per-CTA timelines, PFB_OTF_TRACE, showed 1.7 k + 2.3 k + 1.2 k + 2.6 k clk per band and 9.6 k clk of output loop per item; the
-// pipelined version with four epilogue warps was bound by them: 1.2 k dump + 2.4 k gather per band against 2.3 k of MMAs.)
+//   dump_full / dump_empty              the band's accumulator dump: band k+1 is multiplied (into registers) while the
+//                                       epilogue blends band k out of the dump
+constexpr int kOtfThreads = 17 * 32;
 template <typename T, int R>
-__global__ void __launch_bounds__(320, 1)
+__global__ void __launch_bounds__(kOtfThreads, 1)
 corr_onthefly_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB0,
                           const __grid_constant__ CUtensorMap tmB1, const __grid_constant__ CUtensorMap tmB2,
                           const __grid_constant__ CUtensorMap tmB3, const OtfArgs a) {
@@ -104,40 +102,36 @@ corr_onthefly_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;                                       // kchunks x 16 KB
-  uint8_t* sB = sA + a.kchunks * kOtfTileBytes;             // b_stages x 32 KB
-  uint8_t* sD = sB + a.b_stages * 2 * kOtfTileBytes;        // accumulator dump [128 queries][256 targets] (storage type), pitch 520 B
+  uint8_t* sB = sA + a.kchunks * kOtfTileBytes;             // b_stages x 16 KB
+  uint8_t* sD = sB + a.b_stages * kOtfTileBytes;            // accumulator dump [128 queries][256 targets] (storage type), pitch 520 B
   unsigned short* sOut = reinterpret_cast<unsigned short*>(sD + 128 * kOtfDumpPitch);  // [128][SP] staged outputs of one level
   OtfBars* bars = reinterpret_cast<OtfBars*>(reinterpret_cast<uint8_t*>(sOut) + ((128 * SP * 2 + 15) & ~15));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) {
     mbar_init(&bars->a_full, 1);
-    mbar_init(&bars->a_empty, 1);
+    mbar_init(&bars->a_empty, 8);  // one arrival per MMA warp
     for (int s = 0; s < kOtfMaxStages; ++s) {
       mbar_init(&bars->b_full[s], 1);
-      mbar_init(&bars->b_empty[s], 1);
+      mbar_init(&bars->b_empty[s], 8);
     }
+    mbar_init(&bars->dump_full, 8);  // one arrival per MMA warp
+    mbar_init(&bars->dump_empty, 8);  // one arrival per epilogue warp
     for (int s = 0; s < 2; ++s) {
-      mbar_init(&bars->acc_full[s], 1);
-      mbar_init(&bars->acc_empty[s], 8);  // one arrival per epilogue warp
       mbar_init(&bars->reg_full[s], 1);
-      mbar_init(&bars->reg_empty[s], 2);  // producer + MMA issuer have read the slot
+      mbar_init(&bars->reg_empty[s], 9);  // producer + the 8 MMA warps have read the slot
     }
     fence_barrier_init();
   }
-  if (warp == 9) tmem_alloc<512>(&bars->tmem_base);
-  if (warp == 8 && lane == 0) {
+  if (warp == 16 && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB0);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
   const int n_items = a.n_tiles * a.levels;
 #define OTF_TR(slot) do { if (a.trace && n == 1 && (slot) < 64) a.trace[blockIdx.x * 64 + (slot)] = clock64(); } while (0)
 
-  if (warp == 8) {
+  if (warp == 16) {
     // ================= TMA producer =================
     if (lane == 0) {
       int sb = 0;
@@ -156,49 +150,66 @@ corr_onthefly_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
         for (int k = 0; k < a.kchunks; ++k) tma_load_4d(sA + k * kOtfTileBytes, &tmA, &bars->a_full, k * 64, tx * 16, ty * 8, b);
         for (int kb = 0; kb < nb; ++kb) {
           OTF_TR(8 + kb * 6 + 0);
-          for (int k = 0; k < a.kchunks; ++k) {
-            mbar_wait(&bars->b_empty[sb], phb ^ 1);
-            mbar_arrive_expect_tx(&bars->b_full[sb], 2 * kOtfTileBytes);
-            tma_load_4d(sB + sb * 2 * kOtfTileBytes, tmB, &bars->b_full[sb], k * 64, bx0, by0 + 7 * kb, b);
-            if (++sb == a.b_stages) { sb = 0; phb ^= 1; }
+          for (int nh = 0; nh < 2; ++nh) {
+            for (int k = 0; k < a.kchunks; ++k) {
+              mbar_wait(&bars->b_empty[sb], phb ^ 1);
+              mbar_arrive_expect_tx(&bars->b_full[sb], kOtfTileBytes);
+              tma_load_4d(sB + sb * kOtfTileBytes, tmB, &bars->b_full[sb], k * 64, bx0, by0 + 7 * kb + 4 * nh, b);
+              if (++sb == a.b_stages) { sb = 0; phb ^= 1; }
+            }
           }
         }
       }
     }
-  } else if (warp == 9) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_f16(128, 256, a.ab_fmt);
-      int sb = 0, g = 0;
-      uint32_t phb = 0;
-      int n = 0;
-      for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++n) {
-        const int slot = n & 1;
-        mbar_wait(&bars->reg_full[slot], (n >> 1) & 1);
-        const int nb = bars->region[slot][2];
-        mbar_arrive(&bars->reg_empty[slot]);
-        mbar_wait(&bars->a_full, n & 1);
-        tc_fence_after();
-        for (int kb = 0; kb < nb; ++kb, ++g) {
-          const int t = g & 1;
-          mbar_wait(&bars->acc_empty[t], ((g >> 1) & 1) ^ 1);
-          tc_fence_after();
-          const uint32_t d = tmem_base + t * 256;
-          for (int k = 0; k < a.kchunks; ++k) {
-            mbar_wait(&bars->b_full[sb], phb);
-            tc_fence_after();
-            const uint64_t da = make_desc_k_sw128(smem_u32(sA + k * kOtfTileBytes));
-            const uint64_t db = make_desc_k_sw128(smem_u32(sB + sb * 2 * kOtfTileBytes));
+  } else if (warp >= 8) {
+    // ================= MMA warpgroups: query half mh, m64n128 per target half nh of the band =================
+    const int mh = (threadIdx.x >> 7) - 2, tid = threadIdx.x & 127;
+    float d[64];
+    int sb = 0, g = 0;
+    uint32_t phb = 0;
+    int n = 0;
+    for (int item = blockIdx.x; item < n_items; item += gridDim.x, ++n) {
+      const int slot = n & 1;
+      mbar_wait(&bars->reg_full[slot], (n >> 1) & 1);
+      const int nb = bars->region[slot][2];
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars->reg_empty[slot]);
+      mbar_wait(&bars->a_full, n & 1);
+      for (int kb = 0; kb < nb; ++kb, ++g) {
+       for (int nh = 0; nh < 2; ++nh) {
+        for (int k = 0; k < a.kchunks; ++k) {
+          mbar_wait(&bars->b_full[sb], phb);
+          const uint32_t al = gdesc_lo(smem_u32(sA + k * kOtfTileBytes) + mh * 64 * 128, 16);
+          const uint32_t bl = gdesc_lo(smem_u32(sB + sb * kOtfTileBytes), 16);
+          wgmma_fence();
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk) umma_f16(d, desc_advance(da, kk * 32), desc_advance(db, kk * 32), idesc, (k | kk) != 0);
-            umma_commit(&bars->b_empty[sb]);
-            if (++sb == a.b_stages) { sb = 0; phb ^= 1; }
-          }
-          OTF_TR(8 + kb * 6 + 1);
-          umma_commit(&bars->acc_full[t]);
+          for (int kk = 0; kk < 4; ++kk)
+            wgmma<128, std::is_same<T, __nv_bfloat16>::value>(d, gdesc(al + 2 * kk, kDescHiSw128), gdesc(bl + 2 * kk, kDescHiSw128), (k | kk) != 0);
+          wgmma_commit();
+          wgmma_wait<0>();
+          reg_fence(d);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&bars->b_empty[sb]);
+          if (++sb == a.b_stages) { sb = 0; phb ^= 1; }
         }
-        umma_commit(&bars->a_empty);  // arrives once every MMA issued so far has read its operands
+        if (threadIdx.x == 256) OTF_TR(8 + kb * 6 + 1);
+        // ---- accumulator -> dump rows (storage-type rounding, the rounding the materialised volume has) ----
+        if (nh == 0) mbar_wait(&bars->dump_empty, (g & 1) ^ 1);  // the epilogue is done with band g - 1
+        {
+          const int r0 = mh * 64 + 16 * (tid >> 5) + ((tid & 31) >> 2), c0 = nh * 128 + 2 * (tid & 3);
+          uint8_t* d0 = sD + r0 * kOtfDumpPitch + c0 * 2;
+#pragma unroll
+          for (int j = 0; j < 16; ++j) {
+            *reinterpret_cast<uint32_t*>(d0 + 16 * j) = otf_pack2<T>(d[4 * j + 0], d[4 * j + 1]);
+            *reinterpret_cast<uint32_t*>(d0 + 8 * kOtfDumpPitch + 16 * j) = otf_pack2<T>(d[4 * j + 2], d[4 * j + 3]);
+          }
+        }
+       }
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars->dump_full);
       }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars->a_empty);  // every MMA of this warp has read its operands
     }
   } else {
     // ================= epilogue: region, accumulator dump, window blend, output =================
@@ -310,29 +321,7 @@ corr_onthefly_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
       const float w00 = cur.w00, w10 = cur.w10, w01 = cur.w01, w11 = cur.w11;
       uint8_t* drow = sD + q_local * kOtfDumpPitch;
       for (int kb = 0; kb < nb; ++kb, ++g) {
-        const int t = g & 1;
-        // ---- accumulator row -> shared memory (storage-type rounding, the rounding the materialised volume has) ----
-        mbar_wait(&bars->acc_full[t], (g >> 1) & 1);
-        if (threadIdx.x == 0) OTF_TR(8 + kb * 6 + 2);
-        tc_fence_after();
-        const uint32_t taddr = tmem_base + t * 256 + ((uint32_t)((warp & 3) * 32) << 16);
-#pragma unroll 1
-        for (int c = 4 * half; c < 4 * half + 4; ++c) {  // this thread's half of the band: region rows 4 half .. 4 half + 3
-          uint32_t r[32];
-          tmem_ld_32x32(taddr + c * 32, r);
-          tmem_ld_wait();
-#pragma unroll
-          for (int e = 0; e < 8; ++e) {
-            uint2 u;
-            u.x = otf_pack2<T>(__uint_as_float(r[4 * e + 0]), __uint_as_float(r[4 * e + 1]));
-            u.y = otf_pack2<T>(__uint_as_float(r[4 * e + 2]), __uint_as_float(r[4 * e + 3]));
-            *reinterpret_cast<uint2*>(drow + (((c << 3) | e) << 3)) = u;
-          }
-        }
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&bars->acc_empty[t]);  // the issuer may overwrite this accumulator (band kb + 2)
-        named_barrier_sync(2, 256);  // the other half of this query's dump row is written
+        mbar_wait(&bars->dump_full, g & 1);  // band kb's dump rows are written
         if (threadIdx.x == 0) OTF_TR(8 + kb * 6 + 3);
         // ---- gather: the window rows j (of this thread's parity) whose tap pair (region rows ryo + j, ryo + j + 1) lies in
         // this band.  4-byte loads of the aligned words that cover the 2r+2 taps, realigned by a funnel shift ----
@@ -365,7 +354,8 @@ corr_onthefly_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
           }
         }
         if (threadIdx.x == 0) OTF_TR(8 + kb * 6 + 4);
-        if (kb + 1 < nb) named_barrier_sync(2, 256);  // both threads of a query are done with its dump row before the next band lands in it
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars->dump_empty);  // this warp's queries are done with their dump rows: the next band may land
       }
       // ---- the level's 81 outputs of the 128 queries: coalesced 2-byte runs (81 consecutive channels per query), four rows
       // per round so that a warp has 12 loads, then 12 stores in flight ----
@@ -404,9 +394,6 @@ corr_onthefly_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
     }
   }
 #undef OTF_TR
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) tmem_dealloc<512>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -427,7 +414,6 @@ int corr_onthefly_umma(const void* fmap1, void* const* pyr, const float* coords,
   a.coords = coords; a.out = out; a.flags = flags;
   a.B = B; a.H = H; a.W = W; a.kchunks = C / 64; a.levels = levels; a.out_stride = out_stride;
   a.scale = 1.0f / sqrtf((float)C);
-  a.ab_fmt = dt == PFB_F16 ? 0 : 1;
   a.tiles_x = ceil_div(W, 16); a.tiles_y = ceil_div(H, 8); a.n_tiles = a.tiles_x * a.tiles_y * B;
   CUtensorMap tmA, tmB[4];
   {
@@ -442,21 +428,21 @@ int corr_onthefly_umma(const void* fmap1, void* const* pyr, const float* coords,
     a.lh[l] = H >> ll; a.lw[l] = W >> ll;
     uint64_t dims[4] = {(uint64_t)C, (uint64_t)a.lw[l], (uint64_t)a.lh[l], (uint64_t)B};
     uint64_t str[3] = {(uint64_t)C * 2, (uint64_t)a.lw[l] * C * 2, (uint64_t)a.lh[l] * a.lw[l] * C * 2};
-    uint32_t box[4] = {64, (uint32_t)kOtfRW, 8, 1};
+    uint32_t box[4] = {64, (uint32_t)kOtfRW, 4, 1};  // one band half
     int rc = make_tensor_map(&tmB[l], pyr[ll], dt, 4, dims, str, box);
     if (rc) return rc;
   }
   PFB_CUDA(cudaMemsetAsync(flags, 0, (size_t)B * H * W, s));
-  // shared memory: query tile + operand ring + accumulator dump + output staging; the ring takes what is left (2 stages at C = 256)
+  // shared memory: query tile + operand ring + accumulator dump + output staging; the ring takes what is left (4 stages at C = 256)
   const size_t fixed = (size_t)a.kchunks * kOtfTileBytes + 128 * kOtfDumpPitch + ((128 * 82 * 2 + 15) & ~15) + sizeof(OtfBars) + 1024;
-  int stages = (int)((227 * 1024 - fixed) / (2 * kOtfTileBytes));
+  int stages = (int)((227 * 1024 - fixed) / kOtfTileBytes);
   if (stages > kOtfMaxStages) stages = kOtfMaxStages;
   if (stages < 2) {
     set_error("corr_lookup_onthefly_tc: no room for the operand ring (C=%d)", C);
     return PFB_ERR_UNSUPPORTED;
   }
   a.b_stages = stages;
-  const size_t smem = fixed + (size_t)stages * 2 * kOtfTileBytes;
+  const size_t smem = fixed + (size_t)stages * kOtfTileBytes;
   int grid = sm_count();
   if (grid > a.n_tiles) grid = a.n_tiles;
   // PFB_OTF_TRACE=<file>: per-CTA phase timeline of the second work item (clock64 at the role hand-overs), appended as JSON lines
@@ -469,10 +455,10 @@ int corr_onthefly_umma(const void* fmap1, void* const* pyr, const float* coords,
     ProfScope prof(KC_ONTHEFLY, s);
     if (dt == PFB_F16) {
       PFB_CUDA(cudaFuncSetAttribute(corr_onthefly_umma_kernel<__half, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      corr_onthefly_umma_kernel<__half, 4><<<grid, 320, smem, s>>>(tmA, tmB[0], tmB[1], tmB[2], tmB[3], a);
+      corr_onthefly_umma_kernel<__half, 4><<<grid, kOtfThreads, smem, s>>>(tmA, tmB[0], tmB[1], tmB[2], tmB[3], a);
     } else {
       PFB_CUDA(cudaFuncSetAttribute(corr_onthefly_umma_kernel<__nv_bfloat16, 4>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-      corr_onthefly_umma_kernel<__nv_bfloat16, 4><<<grid, 320, smem, s>>>(tmA, tmB[0], tmB[1], tmB[2], tmB[3], a);
+      corr_onthefly_umma_kernel<__nv_bfloat16, 4><<<grid, kOtfThreads, smem, s>>>(tmA, tmB[0], tmB[1], tmB[2], tmB[3], a);
     }
     PFB_LAUNCH_CHECK();
   }

@@ -1,4 +1,4 @@
-// a1 + a2 on the 5th-gen tensor cores: all-pairs correlation as a TMA-fed tcgen05 GEMM whose epilogue
+// a1 + a2 on the Hopper tensor cores: all-pairs correlation as a TMA-fed wgmma GEMM whose epilogue
 // also emits the 2x2 / 4x4 / 8x8 pooled pyramid levels, so the 4D volume is written once and never
 // re-read (the reference does matmul -> divide -> 3x avg_pool2d, ptlflow/models/raft/corr.py:13-27,56-64).
 //
@@ -8,15 +8,18 @@
 //             level of that patch is an intra-thread reduction in the epilogue
 //   K       = C (<= 256), whole-K tiles resident in shared memory, 128-byte swizzle
 //
-// CTA = 6 warps: 0-3 epilogue (TMEM lane quarter = warp id), 4 = TMA producer, 5 = MMA issuer / TMEM owner.
-// A (this CTA's 128 queries) is loaded once; B patches stream through a 2-deep ring; two 128-column TMEM
-// accumulators let the epilogue of patch i overlap the MMAs of patch i+1.
+// CTA = 13 warps: 0-3 epilogue (thread = query row), 4-11 two MMA warpgroups (64 query rows each), 12 TMA producer.
+// A (this CTA's 128 queries) is loaded once; B patches stream through a 1- or 2-deep ring (whatever fits next to the
+// fp32 accumulator tile in shared memory); the MMA warpgroups hand each patch's accumulators over through that tile,
+// so the epilogue of patch i overlaps the MMAs of patch i+1.
 #include <stdlib.h>
+
+#include <type_traits>
 
 #include "umma.cuh"
 
 namespace pfb {
-using namespace sm100;
+using namespace sm90;
 
 struct PyrOut {
   void* ptr[4];
@@ -29,10 +32,33 @@ struct __align__(8) CorrBars {
   uint64_t a_full;
   uint64_t b_full[2];
   uint64_t b_empty[2];
-  uint64_t acc_full[2];
-  uint64_t acc_empty[2];
-  uint32_t tmem_base;
+  uint64_t acc_full;
+  uint64_t acc_empty;
 };
+
+constexpr int kCorrThreads = 13 * 32;
+
+// The MMA warpgroups of both volume kernels: D[128 queries][128 targets] of one patch, rows 64 * wg .. 64 * wg + 63 per
+// warpgroup.  `stage_of(i, k)` gives the ring stage holding chunk k of item i; the ring slot is released per item
+// (whole-K B stages, single_chunk = false) or per chunk (single_chunk = true).
+template <bool BF16>
+__device__ __forceinline__ void corr_mma_k(float (&d)[64], uint32_t a_base, uint32_t b_base, int kchunks_here, bool first) {
+  const int wg = (threadIdx.x >> 7) - 1;
+#pragma unroll 1
+  for (int k = 0; k < kchunks_here; ++k) {
+    const uint32_t al = gdesc_lo(a_base + k * kTileBytes + wg * 64 * 128, 16), bl = gdesc_lo(b_base + k * kTileBytes, 16);
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk)
+      wgmma<128, BF16>(d, gdesc(al + 2 * kk, kDescHiSw128), gdesc(bl + 2 * kk, kDescHiSw128), (first && k == 0 && kk == 0) ? 0u : 1u);
+  }
+}
+__device__ __forceinline__ void corr_acc_handoff(float (&d)[64], float* sacc, uint64_t* acc_empty, uint64_t* acc_full, int i) {
+  const int wg = (threadIdx.x >> 7) - 1;
+  mbar_wait(acc_empty, (i & 1) ^ 1);
+  acc_store<128>(sacc, d, wg * 64, threadIdx.x & 127);
+  __syncwarp();
+  if ((threadIdx.x & 31) == 0) mbar_arrive(acc_full);
+}
 
 template <typename T>
 __device__ __forceinline__ float rt(float v) { return to_f32(from_f32<T>(v)); }
@@ -75,18 +101,19 @@ __device__ __forceinline__ void store_row(T* dst, const float (&v)[N], int valid
 }
 
 template <typename T>
-__global__ void __launch_bounds__(192, 1)
+__global__ void __launch_bounds__(kCorrThreads, 1)
 corr_volume_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                         const __grid_constant__ CUtensorMap tmO, PyrOut out, int H, int W, int N, int kchunks, int levels,
-                        float scale, int n_groups, int ab_fmt, int tma_store) {
+                        float scale, int n_groups, int b_stages, int tma_store) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024-byte alignment for the 128B-swizzle atoms
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;                                     // kchunks tiles
-  uint8_t* sB = smem + kchunks * kTileBytes;              // 2 stages x kchunks tiles
+  uint8_t* sB = smem + kchunks * kTileBytes;              // b_stages x kchunks tiles
+  float* sacc = reinterpret_cast<float*>(sB + b_stages * kchunks * kTileBytes);  // fp32 accumulator tile, 128 columns
   // level-0 staging for the TMA store: [8 patch rows][128 queries][16 cols] (32 KB); a thread writes its query's
   // 32-byte row segments at (hh * 128 + row) * 32 -> consecutive lanes on consecutive segments, no bank conflicts
-  uint8_t* sC = sB + 2 * kchunks * kTileBytes;
+  uint8_t* sC = reinterpret_cast<uint8_t*>(sacc) + acc_tile_bytes(128);
   CorrBars* bars = reinterpret_cast<CorrBars*>(sC + (tma_store ? 8 * 128 * 32 : 0));
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -99,29 +126,25 @@ corr_volume_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
     mbar_init(&bars->a_full, 1);
     for (int s = 0; s < 2; ++s) {
       mbar_init(&bars->b_full[s], 1);
-      mbar_init(&bars->b_empty[s], 1);
-      mbar_init(&bars->acc_full[s], 1);
-      mbar_init(&bars->acc_empty[s], 4);  // one arrival per epilogue warp
+      mbar_init(&bars->b_empty[s], 8);  // one arrival per MMA warp
     }
+    mbar_init(&bars->acc_full, 8);
+    mbar_init(&bars->acc_empty, 4);  // one arrival per epilogue warp
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc<256>(&bars->tmem_base);
-  if (warp == 4 && lane == 0) {
+  if (warp == 12 && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
 
-  if (warp == 4) {
+  if (warp == 12) {
     // ================= TMA producer =================
     if (lane == 0) {
       mbar_arrive_expect_tx(&bars->a_full, kchunks * kTileBytes);
       for (int k = 0; k < kchunks; ++k) tma_load_3d(sA + k * kTileBytes, &tmA, &bars->a_full, k * 64, m_tile * 128, b);
       for (int i = 0; i < my_tiles; ++i) {
-        const int s = i & 1, use = i >> 1;
+        const int s = i % b_stages, use = i / b_stages;
         const int tile = group + i * n_groups;
         const int ph = tile / PW, pw = tile - ph * PW;
         mbar_wait(&bars->b_empty[s], (use & 1) ^ 1);
@@ -130,26 +153,21 @@ corr_volume_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
           tma_load_4d(sB + (s * kchunks + k) * kTileBytes, &tmB, &bars->b_full[s], k * 64, pw * 16, ph * 8, b);
       }
     }
-  } else if (warp == 5) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_f16(128, 128, ab_fmt);
-      mbar_wait(&bars->a_full, 0);
-      for (int i = 0; i < my_tiles; ++i) {
-        const int s = i & 1, use = i >> 1;
-        mbar_wait(&bars->acc_empty[s], (use & 1) ^ 1);
-        mbar_wait(&bars->b_full[s], use & 1);
-        tc_fence_after();
-        const uint32_t d = tmem_base + s * 128;
-        for (int k = 0; k < kchunks; ++k) {
-          const uint64_t da = make_desc_k_sw128(smem_u32(sA + k * kTileBytes));
-          const uint64_t db = make_desc_k_sw128(smem_u32(sB + (s * kchunks + k) * kTileBytes));
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) umma_f16(d, desc_advance(da, kk * 32), desc_advance(db, kk * 32), idesc, (k | kk) != 0);
-        }
-        umma_commit(&bars->b_empty[s]);   // smem stage free once these MMAs retire
-        umma_commit(&bars->acc_full[s]);  // accumulator ready for the epilogue
-      }
+  } else if (warp >= 4) {
+    // ================= MMA warpgroups =================
+    float d[64];
+    mbar_wait(&bars->a_full, 0);
+    for (int i = 0; i < my_tiles; ++i) {
+      const int s = i % b_stages, use = i / b_stages;
+      mbar_wait(&bars->b_full[s], use & 1);
+      wgmma_fence();
+      corr_mma_k<std::is_same<T, __nv_bfloat16>::value>(d, smem_u32(sA), smem_u32(sB + s * kchunks * kTileBytes), kchunks, true);
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(d);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars->b_empty[s]);  // smem stage free once these MMAs retired
+      corr_acc_handoff(d, sacc, &bars->acc_empty, &bars->acc_full, i);
     }
   } else {
     // ================= epilogue (warps 0-3, 128 threads = 128 query rows) =================
@@ -165,22 +183,18 @@ corr_volume_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
     // vector stores need every row start 16-byte (level 0/1), 8-byte (2), 4-byte (3) aligned
     const bool vec0 = (W % 8) == 0, vec1 = (W1 % 8) == 0, vec2 = (W2 % 4) == 0, vec3 = (W3 % 2) == 0;
     for (int i = 0; i < my_tiles; ++i) {
-      const int s = i & 1, use = i >> 1;
       const int tile = group + i * n_groups;
       const int ph = tile / PW, pw = tile - ph * PW;
-      mbar_wait(&bars->acc_full[s], use & 1);
-      tc_fence_after();
+      mbar_wait(&bars->acc_full, i & 1);
       if (tma_store && i > 0) {  // the previous tile's bulk store must have drained the staging buffer
         if (threadIdx.x == 0) tma_store_wait_read();
         named_barrier_sync(1, 128);
       }
-      const uint32_t taddr = tmem_base + s * 128 + ((uint32_t)(warp * 32) << 16);
       float l1prev[8], l2prev[4];
 #pragma unroll
       for (int c = 0; c < 4; ++c) {  // 32 columns = patch rows 2c, 2c+1
         uint32_t r[32];
-        tmem_ld_32x32(taddr + c * 32, r);
-        tmem_ld_wait();
+        acc_ld32(sacc, row, c * 32, r);
         float v[2][16];
 #pragma unroll
         for (int e = 0; e < 32; ++e) v[e >> 4][e & 15] = rt<T>(__uint_as_float(r[e]) * scale);
@@ -226,9 +240,8 @@ corr_volume_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
           }
         }
       }
-      tc_fence_before();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&bars->acc_empty[s]);
+      if (lane == 0) mbar_arrive(&bars->acc_empty);
       if (tma_store) {
         fence_proxy_async();         // generic-proxy writes -> visible to the async (TMA) proxy
         named_barrier_sync(1, 128);  // the four epilogue warps
@@ -240,31 +253,25 @@ corr_volume_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_co
     }
     if (tma_store && threadIdx.x == 0) tma_store_wait_read();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc<256>(tmem_base);
 }
 
 // =====================================================================================================================
 // Tiled-pyramid variant (round 2): same GEMM, output in the T84 layout of csrc/corr_tiled.cu (4 x 8 tiles of 64 bytes).
 //
-//   * N = 256: two target patches per accumulator (tcgen05 runs M = 128 at the nominal rate only for N = 256; the
-//     N = 128 version above spends 128 clk per MMA on 64 clk of math), 2 x 256 TMEM columns double-buffered.
-//   * 8 epilogue warps: warps 0-3 take the first patch of the pair, warps 4-7 the second (TMEM lane quarter = warp % 4).
-//     ncu (r01) had the 4-warp epilogue at ~7000 clk per patch against ~1900 clk of HBM time.
+//   * one target patch per item (N = 128): the MMA warpgroups of the kernel above, accumulators handed over through the
+//     shared-memory tile; 4 epilogue warps, thread <-> query row.
 //   * pooled levels are means of the fp32 accumulators, rounded once (closer to the fp32 reference than re-rounding
 //     every level like the reference's half path does; also 2 conversions fewer per element), packed conversions.
 //   * level 0 leaves through one TMA bulk store per patch: box [2 tile rows][128 queries][128 bytes] (the two tiles a
 //     patch owns in a tile row are contiguous), 128-byte swizzled staging; level 1 is one full 64-byte tile per
 //     (query, patch) written with 16-byte stores.
-//   B operand ring: 3 stages of one 64-channel chunk of BOTH patches (32 KB).  224 KB of shared memory, one CTA per SM.
+//   B operand ring: 3 stages of one 64-channel chunk of the patch (16 KB).  One CTA per SM.
 struct __align__(8) CorrTBars {
   uint64_t a_full;
   uint64_t b_full[3];
   uint64_t b_empty[3];
-  uint64_t acc_full[2];
-  uint64_t acc_empty[2];
-  uint32_t tmem_base;
+  uint64_t acc_full;
+  uint64_t acc_empty;
 };
 
 struct TiledOut {
@@ -293,47 +300,42 @@ __device__ __forceinline__ uint32_t cvt_pack2<__nv_bfloat16>(float lo, float hi)
 }
 
 template <typename T>
-__global__ void __launch_bounds__(320, 1)
+__global__ void __launch_bounds__(kCorrThreads, 1)
 corr_volume_tiled_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                          const __grid_constant__ CUtensorMap tmO, TiledOut out, int H, int W, int N1, int kchunks, int levels,
                          float scale, int ab_fmt) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* sA = smem;                                   // kchunks x 16 KB
-  uint8_t* sB = sA + kchunks * kTileBytes;              // 3 stages x 32 KB
-  uint8_t* sC = sB + 3 * 2 * kTileBytes;                // 2 groups x 32 KB: [tile row 2][chunk 8][query 128][16 B]
-  CorrTBars* bars = reinterpret_cast<CorrTBars*>(sC + 2 * 2 * kTileBytes);
+  uint8_t* sB = sA + kchunks * kTileBytes;              // 3 stages x 16 KB
+  float* sacc = reinterpret_cast<float*>(sB + 3 * kTileBytes);  // fp32 accumulator tile, 128 columns
+  uint8_t* sC = reinterpret_cast<uint8_t*>(sacc) + acc_tile_bytes(128);  // 32 KB: [tile row 2][chunk 8][query 128][16 B]
+  CorrTBars* bars = reinterpret_cast<CorrTBars*>(sC + 2 * kTileBytes);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_tile = blockIdx.x, b = blockIdx.z;
   const int PW = (W + 15) / 16, PH = (H + 7) / 8;
   const int n_patches = PW * PH;
-  const int n_items = (n_patches + 1) >> 1;
+  const int n_items = n_patches;
 
   if (threadIdx.x == 0) {
     mbar_init(&bars->a_full, 1);
     for (int s = 0; s < 3; ++s) {
       mbar_init(&bars->b_full[s], 1);
-      mbar_init(&bars->b_empty[s], 1);
+      mbar_init(&bars->b_empty[s], 8);  // one arrival per MMA warp
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&bars->acc_full[s], 1);
-      mbar_init(&bars->acc_empty[s], 8);  // one arrival per epilogue warp
-    }
+    mbar_init(&bars->acc_full, 8);
+    mbar_init(&bars->acc_empty, 4);  // one arrival per epilogue warp
     fence_barrier_init();
   }
-  if (warp == 9) tmem_alloc<512>(&bars->tmem_base);
-  if (warp == 8 && lane == 0) {
+  if (warp == 12 && lane == 0) {
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
     prefetch_tmap(&tmO);
   }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
 
-  if (warp == 8) {
+  if (warp == 12) {
     // ================= TMA producer =================
     if (lane == 0) {
       mbar_arrive_expect_tx(&bars->a_full, kchunks * kTileBytes);
@@ -341,70 +343,58 @@ corr_volume_tiled_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
       int st = 0;
       uint32_t phs = 0;
       for (int i = 0; i < n_items; ++i) {
-        const int p0 = 2 * i, p1 = 2 * i + 1;
-        const int ph0 = p0 / PW, pw0 = p0 - ph0 * PW;
-        const int ph1 = p1 / PW, pw1 = p1 - ph1 * PW;  // p1 == n_patches decodes to ph1 == PH: every row out of range -> zero fill
+        const int ph0 = i / PW, pw0 = i - ph0 * PW;
         for (int k = 0; k < kchunks; ++k) {
           mbar_wait(&bars->b_empty[st], phs ^ 1);
-          mbar_arrive_expect_tx(&bars->b_full[st], 2 * kTileBytes);
-          tma_load_4d(sB + st * 2 * kTileBytes, &tmB, &bars->b_full[st], k * 64, pw0 * 16, ph0 * 8, b);
-          tma_load_4d(sB + st * 2 * kTileBytes + kTileBytes, &tmB, &bars->b_full[st], k * 64, pw1 * 16, ph1 * 8, b);
+          mbar_arrive_expect_tx(&bars->b_full[st], kTileBytes);
+          tma_load_4d(sB + st * kTileBytes, &tmB, &bars->b_full[st], k * 64, pw0 * 16, ph0 * 8, b);
           if (++st == 3) { st = 0; phs ^= 1; }
         }
       }
     }
-  } else if (warp == 9) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_f16(128, 256, ab_fmt);
-      mbar_wait(&bars->a_full, 0);
-      int st = 0;
-      uint32_t phs = 0;
-      for (int i = 0; i < n_items; ++i) {
-        const int t = i & 1;
-        mbar_wait(&bars->acc_empty[t], ((i >> 1) & 1) ^ 1);
-        tc_fence_after();
-        const uint32_t d = tmem_base + t * 256;
-        for (int k = 0; k < kchunks; ++k) {
-          mbar_wait(&bars->b_full[st], phs);
-          tc_fence_after();
-          const uint64_t da = make_desc_k_sw128(smem_u32(sA + k * kTileBytes));
-          const uint64_t db = make_desc_k_sw128(smem_u32(sB + st * 2 * kTileBytes));
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) umma_f16(d, desc_advance(da, kk * 32), desc_advance(db, kk * 32), idesc, (k | kk) != 0);
-          umma_commit(&bars->b_empty[st]);
-          if (++st == 3) { st = 0; phs ^= 1; }
-        }
-        umma_commit(&bars->acc_full[t]);
+  } else if (warp >= 4) {
+    // ================= MMA warpgroups =================
+    float d[64];
+    mbar_wait(&bars->a_full, 0);
+    int st = 0;
+    uint32_t phs = 0;
+    for (int i = 0; i < n_items; ++i) {
+      for (int k = 0; k < kchunks; ++k) {
+        mbar_wait(&bars->b_full[st], phs);
+        wgmma_fence();
+        corr_mma_k<std::is_same<T, __nv_bfloat16>::value>(d, smem_u32(sA + k * kTileBytes), smem_u32(sB + st * kTileBytes), 1, k == 0);
+        wgmma_commit();
+        wgmma_wait<0>();
+        reg_fence(d);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(&bars->b_empty[st]);
+        if (++st == 3) { st = 0; phs ^= 1; }
       }
+      corr_acc_handoff(d, sacc, &bars->acc_empty, &bars->acc_full, i);
     }
   } else {
-    // ================= epilogue: 2 groups of 4 warps, thread <-> query row =================
-    const int quarter = warp & 3, grp = warp >> 2;
+    // ================= epilogue: 4 warps, thread <-> query row =================
+    const int quarter = warp & 3, grp = 0;
     const int row = quarter * 32 + lane;
     const int n1 = m_tile * 128 + row;
     const bool row_ok = n1 < N1;
     const size_t q = (size_t)b * N1 + (row_ok ? n1 : 0);
-    uint8_t* sCg = sC + grp * 2 * kTileBytes;
+    uint8_t* sCg = sC;
     T* o1 = levels > 1 ? reinterpret_cast<T*>(out.ptr[1]) + q * out.map_elems[1] : nullptr;
     T* o2 = levels > 2 ? reinterpret_cast<T*>(out.ptr[2]) + q * out.map_elems[2] : nullptr;
     T* o3 = levels > 3 ? reinterpret_cast<T*>(out.ptr[3]) + q * out.map_elems[3] : nullptr;
     const float s1 = 0.25f * scale, s2 = 0.0625f * scale, s3 = 0.015625f * scale;
     const bool leader = (row == 0);
     for (int i = 0; i < n_items; ++i) {
-      const int t = i & 1;
-      const int p = 2 * i + grp;
+      const int p = i;
       const bool p_ok = p < n_patches;
       const int ph = p / PW, pw = p - ph * PW;
-      mbar_wait(&bars->acc_full[t], (i >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + t * 256 + grp * 128 + ((uint32_t)(quarter * 32) << 16);
+      mbar_wait(&bars->acc_full, i & 1);
       float l2acc[4], l3acc[2];
 #pragma unroll
       for (int c = 0; c < 4; ++c) {  // 32 accumulator columns = patch rows 2c, 2c+1 (16 columns each)
         uint32_t r[32];
-        tmem_ld_32x32(taddr + c * 32, r);
-        tmem_ld_wait();
+        acc_ld32(sacc, row, c * 32, r);
         if (c == 0 && i > 0) {  // the previous bulk store of this group must have drained the staging buffer
           if (leader) tma_store_wait_read();
           named_barrier_sync(1 + grp, 128);
@@ -476,9 +466,8 @@ corr_volume_tiled_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
           }
         }
       }
-      tc_fence_before();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&bars->acc_empty[t]);
+      if (lane == 0) mbar_arrive(&bars->acc_empty);
       fence_proxy_async();               // generic-proxy writes -> visible to the async (TMA) proxy
       named_barrier_sync(1 + grp, 128);  // the four warps of this group
       if (leader && p_ok) {
@@ -489,9 +478,6 @@ corr_volume_tiled_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
     }
     if (leader) tma_store_wait_read();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 9) tmem_dealloc<512>(tmem_base);
 }
 
 bool corr_volume_umma_supported(int B, int H, int W, int C, int L, pfb_dtype dt) {
@@ -526,7 +512,13 @@ int corr_volume_umma(const void* f1, const void* f2, void* const* pyr, int B, in
   // level 0 leaves through TMA bulk stores (full-sector writes issued by the copy engine instead of 16-byte
   // per-thread stores to 128 different query maps); needs 16-byte aligned target rows
   static const int env_tma = getenv("PFB_VOLUME_TMA_STORE") ? atoi(getenv("PFB_VOLUME_TMA_STORE")) : 1;
-  const int tma_store = (env_tma && (W % 8) == 0) ? 1 : 0;
+  // shared memory: A (kchunks tiles) + accumulator tile + B ring (2 stages where they fit, else 1) + level-0 staging where
+  // it fits
+  const size_t smem_cap = 227 * 1024 - sizeof(CorrBars) - 1024;
+  const size_t fixed = (size_t)kchunks * kTileBytes + acc_tile_bytes(128), stage = (size_t)kchunks * kTileBytes, staging = 8 * 128 * 32;
+  int tma_store = (env_tma && (W % 8) == 0) ? 1 : 0;
+  if (fixed + stage + (tma_store ? staging : 0) > smem_cap) tma_store = 0;
+  const int b_stages = fixed + 2 * stage + (tma_store ? staging : 0) <= smem_cap ? 2 : 1;
   CUtensorMap tmO = tmA;
   if (tma_store) {
     // dims ordered (w, query, h, b) so that the shared-memory box is [h][query][w]
@@ -542,15 +534,15 @@ int corr_volume_umma(const void* f1, const void* f2, void* const* pyr, int B, in
   int groups = ceil_div(2 * sm_count(), m_tiles * B);
   if (groups < 1) groups = 1;
   if (groups > n_tiles) groups = n_tiles;
-  const size_t smem = (size_t)3 * kchunks * kTileBytes + (tma_store ? 8 * 128 * 32 : 0) + sizeof(CorrBars) + 1024;
+  const size_t smem = fixed + b_stages * stage + (tma_store ? staging : 0) + sizeof(CorrBars) + 1024;
   dim3 grid(m_tiles, groups, B);
   ProfScope prof(KC_VOLUME, s);
   if (dt == PFB_F16) {
     PFB_CUDA(cudaFuncSetAttribute(corr_volume_umma_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    corr_volume_umma_kernel<__half><<<grid, 192, smem, s>>>(tmA, tmB, tmO, out, H, W, N, kchunks, L, scale, groups, 0, tma_store);
+    corr_volume_umma_kernel<__half><<<grid, kCorrThreads, smem, s>>>(tmA, tmB, tmO, out, H, W, N, kchunks, L, scale, groups, b_stages, tma_store);
   } else {
     PFB_CUDA(cudaFuncSetAttribute(corr_volume_umma_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    corr_volume_umma_kernel<__nv_bfloat16><<<grid, 192, smem, s>>>(tmA, tmB, tmO, out, H, W, N, kchunks, L, scale, groups, 1, tma_store);
+    corr_volume_umma_kernel<__nv_bfloat16><<<grid, kCorrThreads, smem, s>>>(tmA, tmB, tmO, out, H, W, N, kchunks, L, scale, groups, b_stages, tma_store);
   }
   PFB_LAUNCH_CHECK();
   return PFB_OK;
@@ -607,15 +599,15 @@ int corr_volume_tiled(const void* f1, const void* f2, void* const* pyr, int B, i
     if (rc) return rc;
   }
   const int m_tiles = ceil_div(N1, 128);
-  const size_t smem = (size_t)kchunks * kTileBytes + 3 * 2 * kTileBytes + 2 * 2 * kTileBytes + sizeof(CorrTBars) + 1024;
+  const size_t smem = (size_t)kchunks * kTileBytes + 3 * kTileBytes + acc_tile_bytes(128) + 2 * kTileBytes + sizeof(CorrTBars) + 1024;
   dim3 grid(m_tiles, 1, B);
   ProfScope prof(KC_VOLUME, s);
   if (dt == PFB_F16) {
     PFB_CUDA(cudaFuncSetAttribute(corr_volume_tiled_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    corr_volume_tiled_kernel<__half><<<grid, 320, smem, s>>>(tmA, tmB, tmO, out, H, W, N1, kchunks, L, scale, 0);
+    corr_volume_tiled_kernel<__half><<<grid, kCorrThreads, smem, s>>>(tmA, tmB, tmO, out, H, W, N1, kchunks, L, scale, 0);
   } else {
     PFB_CUDA(cudaFuncSetAttribute(corr_volume_tiled_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    corr_volume_tiled_kernel<__nv_bfloat16><<<grid, 320, smem, s>>>(tmA, tmB, tmO, out, H, W, N1, kchunks, L, scale, 1);
+    corr_volume_tiled_kernel<__nv_bfloat16><<<grid, kCorrThreads, smem, s>>>(tmA, tmB, tmO, out, H, W, N1, kchunks, L, scale, 1);
   }
   PFB_LAUNCH_CHECK();
   return PFB_OK;

@@ -407,7 +407,6 @@ extern "C" PFB_API int pfb_instance_norm_act(const void* x, void* y, const void*
   // plenty of blocks, few global atomics (fewer, fatter blocks were measured slower: r01 launch list v19)
   const int threads = 256;
   static const int env_ppb = getenv("PFB_STATS_PPB") ? atoi(getenv("PFB_STATS_PPB")) : 0;  // tuning knob
-  // measured on B200 (launch lists, 16 frames): 1536 px/block for the 220x512 maps, 768 for 110x256 (53 / 27 us vs 57 / 31 at 1024)
   const int ppb = env_ppb > 0 && HW >= 8192 ? env_ppb : (HW >= 65536 ? 1536 : (HW >= 8192 ? 768 : (HW >= 1024 ? 256 : 64)));
   dim3 grid(ceil_div(HW, ppb), B);
   {

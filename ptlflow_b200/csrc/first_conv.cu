@@ -1,43 +1,47 @@
 // First encoder convolution (7x7, stride 2, 3 -> 64 channels; ptlflow/models/raft/extractor.py:136,171-178) on the
-// 5th-gen tensor cores WITHOUT an im2col buffer.
+// Hopper tensor cores (wgmma) WITHOUT an im2col buffer.
 //
 //   out[n, y, x, co] = sum_{ky, kx, c} X[n, 2y + ky - 3, 2x + kx - 3, c] * W[co, c, ky, kx]        (zero padding 3)
 //
 // The frames arrive pixel-major with 4 channels (RGB + a zero channel: 8-byte pixels).  For one input row r the
 // 8-pixel window of output pixel x, input pixels 2x-4 .. 2x+3, is 64 contiguous bytes that start 16 bytes after
-// the window of pixel x-1.  That is exactly the geometry of a NON-swizzled K-major UMMA operand whose "core
+// the window of pixel x-1.  That is exactly the geometry of a NON-swizzled K-major wgmma operand whose "core
 // matrices" (8 rows x 16 bytes, rows 16 bytes apart) overlap: leading-dimension (K) byte offset 16, stride (N)
-// byte offset 128.  So the B operand of tcgen05.mma is the raw input row in shared memory, read through an
-// overlapping-window descriptor: N = 256 output pixels, K = 32 (8 pixels x 4 channels) per input row.
+// byte offset 128.  So the B operand of wgmma is the raw input row in shared memory, read through an
+// overlapping-window descriptor: N = 128 output pixels, K = 32 (8 pixels x 4 channels) per input row.
 // The weights are the A operand: M = 128 = 64 output channels x 2 output rows (rows y and y+1 of a pair see input
 // row r through filter rows ky and ky-2), packed per input-row offset j = r - (2y - 3), j = 0..8, as canonical
-// non-swizzled K-major tiles [16 row groups][4 K groups][8 rows][16 B] by the host (models/raft/extractor.py).
-// The accumulator is TRANSPOSED (TMEM lane = (row phase, channel), column = pixel), which makes the per-channel
+// non-swizzled K-major tiles [16 row groups][4 K groups][8 rows][16 B] by the host (models/raft/extractor.py); two
+// warpgroups take the two row phases (M = 64 each).
+// The accumulator is TRANSPOSED (row = (row phase, channel), column = pixel), which makes the per-channel
 // instance-norm statistics a per-thread reduction: they are accumulated from the fp32 accumulators in the
 // epilogue, so the separate statistics pass over the 230 MB activation tensor disappears, and for the
 // batch-norm (folded) encoder bias + ReLU are applied here and nothing else touches the tensor.
 //
-// 18 MMAs (128 x 256 x 16) per work item (= 2 output rows x 256 pixels), 37 KB of input rows per item.
+// 18 K steps (128 x 128 x 16) per work item (= 2 output rows x 128 pixels), 19 KB of input rows per item.  The item
+// width is what lets the fp32 accumulator tile (64 KB) sit in shared memory next to the weights and two input slots.
 #include <stdlib.h>
+
+#include <type_traits>
 
 #include "umma.cuh"
 
 namespace pfb {
-using namespace sm100;
+using namespace sm90;
 
-constexpr int kFcRowBytes = 4224;  // (2 * 256 + 8) pixels * 8 B = 4160, + zero tail, 128-byte multiple
+constexpr int kFcPix = 128;        // output pixels per work item (the N of the MMA)
+constexpr int kFcRowBytes = 2176;  // (2 * 128 + 8) pixels * 8 B = 2112, + zero tail, 128-byte multiple
 constexpr int kFcRows = 9;
 constexpr int kFcSlotBytes = kFcRows * kFcRowBytes;
 constexpr int kFcABytes = 9 * 8192;
-constexpr int kFcSlots = 3;
+constexpr int kFcSlots = 2;
 
 struct __align__(8) FcBars {
   uint64_t full[kFcSlots];
   uint64_t empty[kFcSlots];
-  uint64_t acc_full[2];
-  uint64_t acc_empty[2];
+  uint64_t acc_full;
+  uint64_t acc_empty;
   uint64_t a_full;
-  uint32_t tmem_base;
 };
 
 struct FcArgs {
@@ -77,33 +81,30 @@ __device__ __forceinline__ void store_chunk_transposed(uint8_t* stage, const flo
   __syncwarp();
 }
 
+// 17 warps: 0-7 epilogue, 8-15 the two MMA warpgroups (row phase 0 / 1), 16 producer
+constexpr int kFcThreads = 17 * 32;
 template <typename T>
-__global__ void __launch_bounds__(576, 1) first_conv_umma_kernel(const FcArgs a) {
+__global__ void __launch_bounds__(kFcThreads, 1) first_conv_umma_kernel(const FcArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smemA = smem;
   uint8_t* smemX = smem + kFcABytes;
-  uint8_t* smemStage = smemX + kFcSlots * kFcSlotBytes;  // 16 epilogue warps x 2 KB
-  FcBars* bars = reinterpret_cast<FcBars*>(smemStage + 16 * 2048);
+  float* sacc = reinterpret_cast<float*>(smemX + kFcSlots * kFcSlotBytes);  // fp32 accumulator tile, kFcPix columns
+  uint8_t* smemStage = reinterpret_cast<uint8_t*>(sacc) + acc_tile_bytes(kFcPix);  // 8 epilogue warps x 2 KB
+  FcBars* bars = reinterpret_cast<FcBars*>(smemStage + 8 * 2048);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < kFcSlots; ++s) {
       mbar_init(&bars->full[s], 1);
-      mbar_init(&bars->empty[s], 1);
+      mbar_init(&bars->empty[s], 8);  // one arrival per MMA warp
     }
-    for (int s = 0; s < 2; ++s) {
-      mbar_init(&bars->acc_full[s], 1);
-      mbar_init(&bars->acc_empty[s], 16);
-    }
+    mbar_init(&bars->acc_full, 8);
+    mbar_init(&bars->acc_empty, 8);  // one arrival per epilogue warp
     mbar_init(&bars->a_full, 1);
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc<512>(&bars->tmem_base);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
   pdl_wait();
   pdl_trigger();
 
@@ -115,10 +116,10 @@ __global__ void __launch_bounds__(576, 1) first_conv_umma_kernel(const FcArgs a)
     const int r = w - n * per_img;
     const int q = r / a.nseg;
     y = 2 * q;
-    x0 = (r - q * a.nseg) * 256;
+    x0 = (r - q * a.nseg) * kFcPix;
   };
 
-  if (warp == 4) {
+  if (warp == 16) {
     // ================= producer: weights once, then 9 input rows per item (1-D bulk copies) =================
     if (lane == 0) {
       mbar_arrive_expect_tx(&bars->a_full, kFcABytes);
@@ -135,7 +136,7 @@ __global__ void __launch_bounds__(576, 1) first_conv_umma_kernel(const FcArgs a)
       // valid outputs can touch outside the image is zeroed (generic-proxy stores, fenced before the hand-off)
       const int pstart = 2 * x0 - 4;
       const int plo = pstart < 0 ? 0 : pstart;
-      int phi = 2 * x0 + 2 * 256 + 2;
+      int phi = 2 * x0 + 2 * kFcPix + 2;
       if (phi > a.W) phi = a.W;
       const uint32_t bytes = (uint32_t)(phi - plo) * 8u;
       const uint32_t doff = (uint32_t)(plo - pstart) * 8u;
@@ -164,62 +165,53 @@ __global__ void __launch_bounds__(576, 1) first_conv_umma_kernel(const FcArgs a)
       }
       __syncwarp();
     }
-  } else if (warp == 5) {
-    // ================= MMA issuer =================
-    const uint32_t idesc = make_idesc_f16(128, 256, a.ab_fmt);
-    // non-swizzled K-major descriptors: {addr >> 4, LBO >> 4 at bit 16} , {SBO >> 4, version 1 at bit 14}
-    // LBO = byte distance between core matrices along K, SBO = along M / N (the reading that
-    // tests/test_gpu_ops.py::test_first_conv7x7s2_vs_torch confirms on B200)
-    const uint32_t a_lbo = 128 >> 4, a_sbo = 512 >> 4, b_lbo = 16 >> 4, b_sbo = 128 >> 4;
-    const uint32_t a_hi = a_sbo | (1u << 14), b_hi = b_sbo | (1u << 14);
-    const uint32_t a_lo0 = ((smem_u32(smemA) & 0x3FFFF) >> 4) | (a_lbo << 16);
+  } else if (warp >= 8) {
+    // ================= MMA warpgroups: rows 0-63 (output row y) and 64-127 (row y + 1) =================
+    // non-swizzled K-major descriptors: LBO = byte distance between core matrices along K, SBO = along M / N
+    // (tests/test_gpu_ops.py::test_first_conv7x7s2_vs_torch checks the reading)
+    const int wg = (threadIdx.x >> 7) - 2, tid = threadIdx.x & 127;
+    const uint32_t a_hi = gdesc_hi(512, 0), b_hi = gdesc_hi(128, 0);
+    const uint32_t a_lo0 = gdesc_lo(smem_u32(smemA) + wg * 4096, 128);
     mbar_wait(&bars->a_full, 0);
+    float d[kFcPix / 2];
     int i = 0;
     for (int w = w0; w < w1; ++w, ++i) {
       int n, y, x0;
       decode(w, n, y, x0);
-      const int slot = i % kFcSlots, acc_slot = i & 1;  // 3 input-row slots in flight (one was load-latency bound), 2 accumulators
-      mbar_wait(&bars->acc_empty[acc_slot], ((i >> 1) & 1) ^ 1);
+      const int slot = i % kFcSlots;
       mbar_wait(&bars->full[slot], (i / kFcSlots) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t d = tmem_base + acc_slot * 256;
-        const uint32_t b_lo0 = ((smem_u32(smemX + slot * kFcSlotBytes) & 0x3FFFF) >> 4) | (b_lbo << 16);
-        const int r0 = 2 * y - 3;
-        uint32_t acc = 0;
-        for (int j = 0; j < kFcRows; ++j) {
-          if (r0 + j < 0 || r0 + j >= a.H) continue;  // rows outside the image contribute zero
+      const uint32_t b_lo0 = gdesc_lo(smem_u32(smemX + slot * kFcSlotBytes), 16);
+      const int r0 = 2 * y - 3;
+      uint32_t acc = 0;
+      wgmma_fence();
+      for (int j = 0; j < kFcRows; ++j) {
+        if (r0 + j < 0 || r0 + j >= a.H) continue;  // rows outside the image contribute zero
 #pragma unroll
-          for (int s = 0; s < 2; ++s) {
-            const uint32_t al = a_lo0 + ((j * 8192 + s * 256) >> 4);
-            const uint32_t bl = b_lo0 + ((j * kFcRowBytes + s * 32) >> 4);
-            asm volatile(
-                "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-                "mov.b64 da, {%1, %3};\n\t"
-                "mov.b64 db, {%2, %4};\n\t"
-                "setp.ne.b32 p, %6, 0;\n\t"
-                "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}" ::"r"(d),
-                "r"(al), "r"(bl), "r"(a_hi), "r"(b_hi), "r"(idesc), "r"(acc)
-                : "memory");
-            acc = 1;
-          }
+        for (int s = 0; s < 2; ++s) {
+          wgmma<kFcPix, std::is_same<T, __nv_bfloat16>::value>(d, gdesc(a_lo0 + ((j * 8192 + s * 256) >> 4), a_hi),
+                                                               gdesc(b_lo0 + ((j * kFcRowBytes + s * 32) >> 4), b_hi), acc);
+          acc = 1;
         }
-        umma_commit(&bars->empty[slot]);
-        umma_commit(&bars->acc_full[acc_slot]);
       }
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(d);
       __syncwarp();
+      if (lane == 0) mbar_arrive(&bars->empty[slot]);
+      mbar_wait(&bars->acc_empty, (i & 1) ^ 1);
+      acc_store<kFcPix>(sacc, d, wg * 64, tid);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars->acc_full);
     }
   } else {
-    // ================= epilogue: TMEM lane = (row phase p, channel co), columns = pixels =================
-    // 16 epilogue warps (0-3, 6-17): four column groups x four TMEM lane quarters (a warp may only touch quarter
-    // warp % 4).  Each warp owns two 32-pixel chunks of an item; both TMEM loads are issued together and the
-    // accumulator is handed back to the MMA warp as soon as they have landed in registers -- the per-warp chain
-    // load -> arithmetic -> stores was what bounded the 8-warp version (90 us for 16 frames against 30 us of MMA).
-    const int quarter = warp & 3, group = warp < 4 ? 0 : 1 + ((warp - 6) >> 2);
+    // ================= epilogue: row = (row phase p, channel co), columns = pixels =================
+    // 8 epilogue warps: two column groups x four row quarters.  Each warp owns two 32-pixel chunks of an item; both are read
+    // before the accumulator tile is handed back to the MMA warpgroups.
+    const int quarter = warp & 3, group = warp >> 2;
     const int m = quarter * 32 + lane;
     const int p = m >> 6, co = m & 63;
     const float bias = a.bias ? a.bias[co] : 0.f;
-    uint8_t* stage = smemStage + (group * 4 + quarter) * 2048;
+    uint8_t* stage = smemStage + warp * 2048;
     float ssum = 0.f, ssq = 0.f;
     int n_cur = -1;
     auto flush = [&]() {
@@ -238,23 +230,18 @@ __global__ void __launch_bounds__(576, 1) first_conv_umma_kernel(const FcArgs a)
         flush();
         n_cur = n;
       }
-      const int slot = i & 1;
       const bool row_ok = (y + p) < a.Ho;
       // this warp's 32 channels of the output row: channel offset (quarter & 1) * 32
       T* orow32 = reinterpret_cast<T*>(a.out) + (((size_t)n * a.Ho + (row_ok ? y + p : 0)) * a.Wo) * 64 + (quarter & 1) * 32;
-      mbar_wait(&bars->acc_full[slot], (i >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + slot * 256 + ((uint32_t)(quarter * 32) << 16);
+      mbar_wait(&bars->acc_full, i & 1);
       uint32_t r[2][32];
-      tmem_ld_32x32(taddr + group * 32, r[0]);
-      tmem_ld_32x32(taddr + group * 32 + 128, r[1]);
-      tmem_ld_wait();
-      tc_fence_before();
+      acc_ld32(sacc, m, group * 32, r[0]);
+      acc_ld32(sacc, m, group * 32 + 64, r[1]);
       __syncwarp();
-      if (lane == 0) mbar_arrive(&bars->acc_empty[slot]);
+      if (lane == 0) mbar_arrive(&bars->acc_empty);
 #pragma unroll
       for (int k = 0; k < 2; ++k) {
-        const int xb = x0 + group * 32 + 128 * k;
+        const int xb = x0 + group * 32 + 64 * k;
         if (!row_ok || xb >= a.Wo) continue;  // warp-uniform
         const int nv = a.Wo - xb;
         float v[32];
@@ -272,9 +259,6 @@ __global__ void __launch_bounds__(576, 1) first_conv_umma_kernel(const FcArgs a)
     }
     flush();
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc<512>(tmem_base);
 }
 
 
@@ -283,7 +267,7 @@ __global__ void __launch_bounds__(576, 1) first_conv_umma_kernel(const FcArgs a)
 // iteration.  Same overlapping-window trick with stride 1: the fp32 flow is split into hi + lo halves of the storage
 // type (fx_hi, fy_hi, fx_lo, fy_lo, 0, 0, 0, 0 = one 16-byte pixel, so no precision is lost against the fp32 SIMT
 // kernel it replaces), output pixel x reads pixels x-4 .. x+3 = 128 contiguous bytes, 16 bytes after pixel x-1's.
-// M = 128 output channels, N = 256 pixel columns (one image row segment), K = 64 per filter row, 28 MMAs per row.
+// M = 128 output channels (two warpgroups of 64), N = 128 pixel columns (one image row segment), K = 64 per filter row.
 // Loader warps build the split rows in shared memory (generic stores + fence.proxy.async): no global staging buffer.
 struct FlowConvArgs {
   const float* flow;  // [B][H][W][2]
@@ -294,17 +278,16 @@ struct FlowConvArgs {
   int nseg, n_items, per_cta, ab_fmt;
 };
 constexpr int kFlRows = 7;
-constexpr int kFlSlotBytes = kFlRows * kFcRowBytes;
+constexpr int kFlSlotBytes = kFlRows * kFcRowBytes;  // (128 + 8) pixels x 16 B per row
 constexpr int kFlABytes = 7 * 16384;
 constexpr int kFlLoaders = 128;
 
 struct __align__(8) FlBars {
   uint64_t full[2];
   uint64_t empty[2];
-  uint64_t acc_full[2];
-  uint64_t acc_empty[2];
+  uint64_t acc_full;
+  uint64_t acc_empty;
   uint64_t a_full;
-  uint32_t tmem_base;
 };
 
 template <typename T>
@@ -319,33 +302,32 @@ __device__ __forceinline__ uint4 split_flow(float fx, float fy) {
   return u;
 }
 
+// 20 warps: 0-7 epilogue, 8-15 the two MMA warpgroups, 16-19 loaders
+constexpr int kFlThreads = 20 * 32;
 template <typename T>
-__global__ void __launch_bounds__(448, 1) flow_conv7x7_umma_kernel(const FlowConvArgs a) {
+__global__ void __launch_bounds__(kFlThreads, 1) flow_conv7x7_umma_kernel(const FlowConvArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smemA = smem;
   uint8_t* smemX = smem + kFlABytes;
-  uint8_t* smemStage = smemX + 2 * kFlSlotBytes;  // 8 epilogue warps x 2 KB
+  float* sacc = reinterpret_cast<float*>(smemX + 2 * kFlSlotBytes);  // fp32 accumulator tile, kFcPix columns
+  uint8_t* smemStage = reinterpret_cast<uint8_t*>(sacc) + acc_tile_bytes(kFcPix);  // 8 epilogue warps x 2 KB
   FlBars* bars = reinterpret_cast<FlBars*>(smemStage + 8 * 2048);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < 2; ++s) {
       mbar_init(&bars->full[s], kFlLoaders);
-      mbar_init(&bars->empty[s], 1);
-      mbar_init(&bars->acc_full[s], 1);
-      mbar_init(&bars->acc_empty[s], 8);
+      mbar_init(&bars->empty[s], 8);  // one arrival per MMA warp
     }
+    mbar_init(&bars->acc_full, 8);
+    mbar_init(&bars->acc_empty, 8);  // one arrival per epilogue warp
     mbar_init(&bars->a_full, 1);
     fence_barrier_init();
   }
-  if (warp == 5) tmem_alloc<512>(&bars->tmem_base);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = bars->tmem_base;
   // the weights do not depend on the previous kernel: request them before the PDL wait
-  if (warp == 4 && lane == 0) {
+  if (warp == 16 && lane == 0) {
     mbar_arrive_expect_tx(&bars->a_full, kFlABytes);
     for (int j = 0; j < 7; ++j) bulk_g2s(smemA + j * 16384, reinterpret_cast<const uint8_t*>(a.wpack) + j * 16384, 16384, &bars->a_full);
   }
@@ -356,14 +338,14 @@ __global__ void __launch_bounds__(448, 1) flow_conv7x7_umma_kernel(const FlowCon
   const int w1 = min(a.n_items, w0 + a.per_cta);
   auto decode = [&](int w, int& n, int& y, int& x0) {
     const int row = w / a.nseg;
-    x0 = (w - row * a.nseg) * 256;
+    x0 = (w - row * a.nseg) * kFcPix;
     n = row / a.H;
     y = row - n * a.H;
   };
 
-  if (warp >= 10) {
+  if (warp >= 16) {
     // ================= loaders: fp32 flow rows -> split 16-byte pixels with zero halo =================
-    const int t = threadIdx.x - 320;  // 0..127
+    const int t = threadIdx.x - 512;  // 0..127
     int i = 0;
     for (int w = w0; w < w1; ++w, ++i) {
       int n, y, x0;
@@ -371,9 +353,9 @@ __global__ void __launch_bounds__(448, 1) flow_conv7x7_umma_kernel(const FlowCon
       const int slot = i & 1;
       mbar_wait(&bars->empty[slot], ((i >> 1) & 1) ^ 1);
       uint8_t* base = smemX + slot * kFlSlotBytes;
-      // buffer pixel i <-> image pixel x0 - 4 + i, i in [0, 264)
-      for (int e = t; e < kFlRows * 264; e += kFlLoaders) {
-        const int j = e / 264, bi = e - j * 264;
+      // buffer pixel i <-> image pixel x0 - 4 + i, i in [0, kFcPix + 8)
+      for (int e = t; e < kFlRows * (kFcPix + 8); e += kFlLoaders) {
+        const int j = e / (kFcPix + 8), bi = e - j * (kFcPix + 8);
         const int r = y + j - 3, px = x0 - 4 + bi;
         uint4 u = make_uint4(0u, 0u, 0u, 0u);
         if (r >= 0 && r < a.H && px >= 0 && px < a.W) {
@@ -385,79 +367,66 @@ __global__ void __launch_bounds__(448, 1) flow_conv7x7_umma_kernel(const FlowCon
       fence_proxy_async();
       mbar_arrive(&bars->full[slot]);
     }
-  } else if (warp == 5) {
-    // ================= MMA issuer =================
-    const uint32_t idesc = make_idesc_f16(128, 256, a.ab_fmt);
-    const uint32_t a_hi = (1024u >> 4) | (1u << 14), b_hi = (128u >> 4) | (1u << 14);
-    const uint32_t a_lo0 = ((smem_u32(smemA) & 0x3FFFF) >> 4) | ((128u >> 4) << 16);
+  } else if (warp >= 8) {
+    // ================= MMA warpgroups: output channels 0-63 and 64-127 =================
+    const int wg = (threadIdx.x >> 7) - 2, tid = threadIdx.x & 127;
+    const uint32_t a_hi = gdesc_hi(1024, 0), b_hi = gdesc_hi(128, 0);
+    const uint32_t a_lo0 = gdesc_lo(smem_u32(smemA) + wg * 8192, 128);
     mbar_wait(&bars->a_full, 0);
+    float d[kFcPix / 2];
     int i = 0;
     for (int w = w0; w < w1; ++w, ++i) {
       int n, y, x0;
       decode(w, n, y, x0);
       const int slot = i & 1;
-      mbar_wait(&bars->acc_empty[slot], ((i >> 1) & 1) ^ 1);
       mbar_wait(&bars->full[slot], (i >> 1) & 1);
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t d = tmem_base + slot * 256;
-        const uint32_t b_lo0 = ((smem_u32(smemX + slot * kFlSlotBytes) & 0x3FFFF) >> 4) | ((16u >> 4) << 16);
-        uint32_t acc = 0;
-        for (int j = 0; j < kFlRows; ++j) {
-          if (y + j - 3 < 0 || y + j - 3 >= a.H) continue;  // rows outside the image are zero
+      const uint32_t b_lo0 = gdesc_lo(smem_u32(smemX + slot * kFlSlotBytes), 16);
+      uint32_t acc = 0;
+      wgmma_fence();
+      for (int j = 0; j < kFlRows; ++j) {
+        if (y + j - 3 < 0 || y + j - 3 >= a.H) continue;  // rows outside the image are zero
 #pragma unroll
-          for (int s = 0; s < 4; ++s) {
-            const uint32_t al = a_lo0 + ((j * 16384 + s * 256) >> 4);
-            const uint32_t bl = b_lo0 + ((j * kFcRowBytes + s * 32) >> 4);
-            asm volatile(
-                "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-                "mov.b64 da, {%1, %3};\n\t"
-                "mov.b64 db, {%2, %4};\n\t"
-                "setp.ne.b32 p, %6, 0;\n\t"
-                "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}" ::"r"(d),
-                "r"(al), "r"(bl), "r"(a_hi), "r"(b_hi), "r"(idesc), "r"(acc)
-                : "memory");
-            acc = 1;
-          }
+        for (int s = 0; s < 4; ++s) {
+          wgmma<kFcPix, std::is_same<T, __nv_bfloat16>::value>(d, gdesc(a_lo0 + ((j * 16384 + s * 256) >> 4), a_hi),
+                                                               gdesc(b_lo0 + ((j * kFcRowBytes + s * 32) >> 4), b_hi), acc);
+          acc = 1;
         }
-        umma_commit(&bars->empty[slot]);
-        umma_commit(&bars->acc_full[slot]);
       }
+      wgmma_commit();
+      wgmma_wait<0>();
+      reg_fence(d);
       __syncwarp();
+      if (lane == 0) mbar_arrive(&bars->empty[slot]);
+      mbar_wait(&bars->acc_empty, (i & 1) ^ 1);
+      acc_store<kFcPix>(sacc, d, wg * 64, tid);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&bars->acc_full);
     }
-  } else if (warp != 4) {
-    // ================= epilogue: TMEM lane = output channel, columns = pixels =================
-    const int quarter = warp & 3, group = warp < 4 ? 0 : 1;
+  } else {
+    // ================= epilogue: row = output channel, columns = pixels =================
+    const int quarter = warp & 3, group = warp >> 2;
     const int co = quarter * 32 + lane;
     const float bias = a.bias ? a.bias[co] : 0.f;
-    uint8_t* stage = smemStage + (group * 4 + quarter) * 2048;
+    uint8_t* stage = smemStage + warp * 2048;
     int i = 0;
     for (int w = w0; w < w1; ++w, ++i) {
       int n, y, x0;
       decode(w, n, y, x0);
-      const int slot = i & 1;
       T* orow32 = reinterpret_cast<T*>(a.out) + (((size_t)n * a.H + y) * a.W) * a.out_stride + a.out_offset + quarter * 32;
-      mbar_wait(&bars->acc_full[slot], (i >> 1) & 1);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + slot * 256 + ((uint32_t)(quarter * 32) << 16);
-      for (int c = group * 32; c < 256 && x0 + c < a.W; c += 64) {
+      mbar_wait(&bars->acc_full, i & 1);
+      for (int c = group * 32; c < kFcPix && x0 + c < a.W; c += 64) {
         uint32_t r[32];
-        tmem_ld_32x32(taddr + c, r);
-        tmem_ld_wait();
+        acc_ld32(sacc, co, c, r);
         const int xb = x0 + c;
         float v[32];
 #pragma unroll
         for (int e = 0; e < 32; ++e) v[e] = fmaxf(__uint_as_float(r[e]) + bias, 0.f);
         store_chunk_transposed<T>(stage, v, orow32 + (size_t)xb * a.out_stride, a.out_stride, a.W - xb, lane);
       }
-      tc_fence_before();
       __syncwarp();
-      if (lane == 0) mbar_arrive(&bars->acc_empty[slot]);
+      if (lane == 0) mbar_arrive(&bars->acc_empty);
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 5) tmem_dealloc<512>(tmem_base);
 }
 
 }  // namespace pfb
@@ -475,7 +444,7 @@ extern "C" PFB_API int pfb_first_conv7x7s2(const void* x, const void* wpack, con
   a.x = x; a.wpack = wpack; a.out = out; a.bias = bias; a.stats = stats;
   a.N = N; a.H = H; a.W = W; a.Ho = H / 2; a.Wo = W / 2;
   a.pairs = ceil_div(a.Ho, 2);
-  a.nseg = ceil_div(a.Wo, 256);
+  a.nseg = ceil_div(a.Wo, kFcPix);
   a.n_items = N * a.pairs * a.nseg;
   int grid = sm_count();
   if (grid > a.n_items) grid = a.n_items;
@@ -483,14 +452,14 @@ extern "C" PFB_API int pfb_first_conv7x7s2(const void* x, const void* wpack, con
   grid = ceil_div(a.n_items, a.per_cta);
   a.relu = relu;
   a.ab_fmt = dtype == PFB_F16 ? 0 : 1;
-  const size_t smem = kFcABytes + kFcSlots * kFcSlotBytes + 16 * 2048 + sizeof(FcBars) + 1024;
+  const size_t smem = kFcABytes + kFcSlots * kFcSlotBytes + acc_tile_bytes(kFcPix) + 8 * 2048 + sizeof(FcBars) + 1024;
   ProfScope prof(KC_ENC_CONV1, s);  // encoder side: not part of the update-block conv roofline
   if (dtype == PFB_F16) {
     PFB_CUDA(cudaFuncSetAttribute(first_conv_umma_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    PFB_CUDA(launch_pdl(first_conv_umma_kernel<__half>, dim3(grid), dim3(576), smem, s, a));
+    PFB_CUDA(launch_pdl(first_conv_umma_kernel<__half>, dim3(grid), dim3(kFcThreads), smem, s, a));
   } else {
     PFB_CUDA(cudaFuncSetAttribute(first_conv_umma_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    PFB_CUDA(launch_pdl(first_conv_umma_kernel<__nv_bfloat16>, dim3(grid), dim3(576), smem, s, a));
+    PFB_CUDA(launch_pdl(first_conv_umma_kernel<__nv_bfloat16>, dim3(grid), dim3(kFcThreads), smem, s, a));
   }
   return PFB_OK;
 }
@@ -507,21 +476,21 @@ extern "C" PFB_API int pfb_flow_conv7x7(const float* flow, const void* wpack, co
   FlowConvArgs a{};
   a.flow = flow; a.wpack = wpack; a.bias = bias; a.out = out;
   a.B = B; a.H = H; a.W = W; a.out_stride = out_stride; a.out_offset = out_offset;
-  a.nseg = ceil_div(W, 256);
+  a.nseg = ceil_div(W, kFcPix);
   a.n_items = B * H * a.nseg;
   int grid = sm_count();
   if (grid > a.n_items) grid = a.n_items;
   a.per_cta = ceil_div(a.n_items, grid);
   grid = ceil_div(a.n_items, a.per_cta);
   a.ab_fmt = dtype == PFB_F16 ? 0 : 1;
-  const size_t smem = kFlABytes + 2 * kFlSlotBytes + 8 * 2048 + sizeof(FlBars) + 1024;
+  const size_t smem = kFlABytes + 2 * kFlSlotBytes + acc_tile_bytes(kFcPix) + 8 * 2048 + sizeof(FlBars) + 1024;
   ProfScope prof(KC_FLOWCONV, s);
   if (dtype == PFB_F16) {
     PFB_CUDA(cudaFuncSetAttribute(flow_conv7x7_umma_kernel<__half>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    PFB_CUDA(launch_pdl(flow_conv7x7_umma_kernel<__half>, dim3(grid), dim3(448), smem, s, a));
+    PFB_CUDA(launch_pdl(flow_conv7x7_umma_kernel<__half>, dim3(grid), dim3(kFlThreads), smem, s, a));
   } else {
     PFB_CUDA(cudaFuncSetAttribute(flow_conv7x7_umma_kernel<__nv_bfloat16>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    PFB_CUDA(launch_pdl(flow_conv7x7_umma_kernel<__nv_bfloat16>, dim3(grid), dim3(448), smem, s, a));
+    PFB_CUDA(launch_pdl(flow_conv7x7_umma_kernel<__nv_bfloat16>, dim3(grid), dim3(kFlThreads), smem, s, a));
   }
   return PFB_OK;
 }

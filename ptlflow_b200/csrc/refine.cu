@@ -260,7 +260,7 @@ static int update_iter(const Ctx& x, const void* corr_ext, void* mask_out) {
     if (tensor_path && env_batched) {
       // ONE launch for all samples: pixels = queries, input channels = the N attention columns, per-sample weights = that
       // sample's v^T (K-major [128][n_pad], rows b * 128 ...).  B x 55 row tiles fill the machine; one launch per sample left
-      // 55 of 148 SMs busy.
+      // only 55 row tiles, a fraction of the machine.
       pfb_conv_params p{};
       p.src[0] = src_of(x.b->attention, N, N);
       p.nsrc = 1;

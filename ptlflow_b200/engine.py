@@ -35,7 +35,7 @@ class RaftEngine:
         planes = corr_levels * (2 * corr_radius + 1) ** 2
         hd, cd = hidden_dim, context_dim
 
-        def P(srcs, *convs):  # srcs: channel counts of the concatenated inputs, in order (tcgen05 K-major pack)
+        def P(srcs, *convs):  # srcs: channel counts of the concatenated inputs, in order (wgmma K-major pack)
             return ops.PackedConv(convs, dtype, device, src_channels=srcs)
 
         layers: Dict[int, ops.PackedConv] = {}

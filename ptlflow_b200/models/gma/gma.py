@@ -5,8 +5,8 @@ Surface kept from ptlflow/models/gma/gma.py:50-222: class name ``gma``, construc
 position_and_content, alternate_corr``), state_dict keys (``fnet.*, cnet.*, update_block.*`` incl.
 ``update_block.aggregator.{to_v.weight,gamma}``, ``att.{to_qk.weight,pos_emb.*}``), ``forward(dict) -> dict``.
 
-B200 mapping of the extras (SURVEY.md section 8(a) row a13):
-  * attention logits  scale * q . k   == level 0 of pfb_corr_volume_build(q, k) (same tcgen05 GEMM as the
+Kernel mapping of the extras (SURVEY.md section 8(a) row a13):
+  * attention logits  scale * q . k   == level 0 of pfb_corr_volume_build(q, k) (same wgmma GEMM as the
     correlation volume: 1/sqrt(dim_head) is its built-in scale), then an in-place row softmax;
   * per iteration  motion + gamma * attn @ to_v(motion)  == a 1x1 convolution over the N attention columns
     with the sample's v as weights and an AXPY epilogue, inside pfb_raft_refine (variant 2).

@@ -165,7 +165,7 @@ class _Encoder(nn.Module):
                 and self.norm_fn in ("instance", "batch", "none")):
             folded = _fold(self.conv1, self.norm1, torch.float32, device)
             prep["conv1_native"] = (ops.pack_first_conv(folded[0], dtype), folded[1])
-        # the output projection (1x1, w3 -> output_dim) on this library's tcgen05 implicit-GEMM kernel with the bias in its
+        # the output projection (1x1, w3 -> output_dim) on this library's wgmma implicit-GEMM kernel with the bias in its
         # epilogue: cuDNN picked an sm_80 kernel without shared-memory staging for it (50 us per encoder, ncu launch list r02f)
         # and the bias needed a pass of its own
         c2 = self.conv2
@@ -201,7 +201,7 @@ class _Encoder(nn.Module):
         native_c1 = ("conv1_native" in prep and x.shape[-1] == 4 and tuple(self.conv1.weight.shape) == (64, 3, 7, 7) and x.dtype in (torch.float16, torch.bfloat16)
                      and x.shape[1] % 2 == 0 and x.shape[2] % 2 == 0)
         if native_c1:
-            # tcgen05 first convolution (csrc/first_conv.cu): statistics of the instance norm come out of its epilogue,
+            # wgmma first convolution (csrc/first_conv.cu): statistics of the instance norm come out of its epilogue,
             # bias + ReLU of the folded batch norm are applied in it
             wpack, bias = prep["conv1_native"]
             if inst:

@@ -5,7 +5,7 @@ Kept from the reference (ptlflow/models/raft/raft.py:48-247): class names, const
 [B,1,2,H,W] and ``flow_small`` [B,2,H/8,W/8], the warm-start input ``prev_preds.flow_small``.
 Replaced: everything between the encoders and the returned flow -- correlation volume + pyramid,
 the ``iters`` x {lookup, motion encoder, (Sep)ConvGRU, flow head}, mask head and the convex
-upsample run as hand-written sm_100a kernels through one C call (ptlflow_b200/engine.py).
+upsample run as hand-written sm_90a kernels through one C call (ptlflow_b200/engine.py).
 """
 from __future__ import annotations
 
@@ -131,7 +131,7 @@ class RAFT(BaseModel):
         self.dropout, self.gamma, self.max_flow = dropout, gamma, max_flow
         self.iters, self.alternate_corr = iters, alternate_corr
         self.has_trained_on_ptlflow = True
-        # backend knobs (not hparams): 0 auto, 1 SIMT fp32-accumulate kernels, 2 force tcgen05
+        # backend knobs (not hparams): 0 auto, 1 SIMT fp32-accumulate kernels, 2 force the tensor-core (wgmma) kernels
         self.kernel_impl = 0
         self.strict_fp32 = True  # fp32 models: keep cuDNN off TF32 so the 1e-3 parity gate holds
         # images per encoder pass (0 = whole batch).  Smaller passes keep the 1/2-resolution intermediates of the
@@ -399,7 +399,7 @@ class RAFT(BaseModel):
         """Estimate optical flow between a pair of frames (eval semantics of raft.py:125-194)."""
         images = inputs["images"]
         if not images.is_cuda:
-            raise RuntimeError("ptlflow_b200 runs on CUDA (sm_100a) only: move the model and inputs to the GPU. There is no CPU path.")
+            raise RuntimeError("ptlflow_b200 runs on CUDA (sm_90a) only: move the model and inputs to the GPU. There is no CPU path.")
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.update_block.parameters()) and self.training:
             raise NotImplementedError("ptlflow_b200 implements the inference hot path; call under torch.no_grad() / model.eval()")
         with torch.no_grad(), torch.cuda.device(images.device):

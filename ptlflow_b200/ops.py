@@ -220,7 +220,7 @@ class PackedConv:
 
     def __init__(self, convs, dtype: torch.dtype, device, cout_align: int = 8, src_channels=None):
         """``src_channels`` (list of the concatenated sources' channel counts) additionally builds the K-major
-        packing [KH*KW][Cout_pad_k][Cin_pad] consumed by the tcgen05 kernels (f16 / bf16 only)."""
+        packing [KH*KW][Cout_pad_k][Cin_pad] consumed by the wgmma kernels (f16 / bf16 only)."""
         convs = list(convs)
         w0 = convs[0].weight
         self.Cin, self.KH, self.KW = w0.shape[1], w0.shape[2], w0.shape[3]
@@ -429,7 +429,7 @@ def instance_norm_act(x: torch.Tensor, relu: bool = True, residual: Optional[tor
 
 def pack_first_conv(weight: torch.Tensor, dtype: torch.dtype) -> torch.Tensor:
     """weight [64,3,7,7] (fp32, any device) -> the 9 x [128][32] operand tiles of pfb_first_conv7x7s2 (see the header):
-    row p*64+co, column 4*t+c of tile j = weight[co, c, j-2p, t-1]; non-swizzled UMMA core-matrix order."""
+    row p*64+co, column 4*t+c of tile j = weight[co, c, j-2p, t-1]; non-swizzled wgmma core-matrix order."""
     co, ci, kh, kw = weight.shape
     if (co, ci, kh, kw) != (64, 3, 7, 7):
         raise RuntimeError("pack_first_conv: expected a [64,3,7,7] filter")

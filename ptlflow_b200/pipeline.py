@@ -2,8 +2,7 @@
 
 One forward of a RAFT-family model is a chain of ~250 dependent kernels that alternate between tensor-bound
 (update-block convolutions), HBM-bound (encoder normalisation passes, lookup, volume) and latency-bound phases.
-Two independent batches on two CUDA streams fill each other's gaps: measured on B200, RAFT 1024x436 / 12 iterations
-/ f16 / 8 pairs per batch, 818 -> 894 pairs/s with two batches in flight (three bring nothing more).
+Two independent batches on two CUDA streams fill each other's gaps (``bench.py --inflight 2`` measures what that brings).
 
 Each slot owns a CUDA stream, a host thread (kernel launches of one forward take ~6 ms of host time; cuDNN's
 autotune cache in torch is thread-local, so the thread is long-lived and warms up once) and, through the

@@ -27,3 +27,9 @@ def e2e_inputs(recipe):
 
 
 E2E = ["e2e_raft_small_cfg1", "e2e_raft_small_b2", "e2e_raft_noise", "e2e_raft_smooth_b2", "e2e_raft_altcorr", "e2e_raft_r3_l3", "e2e_gma"]
+
+
+def load_golden_arrays(name):
+    """A golden file without a recipe: every array it holds."""
+    z = np.load(os.path.join(GOLDEN, name + ".npz"))
+    return {k: z[k] for k in z.files}

@@ -1,4 +1,4 @@
-"""CPU: the C-ABI library builds for sm_100a, loads without a GPU, exports every symbol the header
+"""CPU: the C-ABI library builds for sm_90a, loads without a GPU, exports every symbol the header
 declares, and rejects bad arguments with an error message before touching the device."""
 import ctypes as C
 import os

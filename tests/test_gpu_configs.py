@@ -57,7 +57,6 @@ def _model(variant, kwargs, sd, dtype):
 # (name, variant, kwargs, B, H, W, kind, dtype, max gate, mean gate)
 CASES = [
     # config 2: raft 1024x436, 12 iterations, f16 (the benchmarked configuration), noise frames like model_benchmark.py feeds
-    # measured (B200, round 2): noise 0.049 max / 0.011 mean, smooth 0.031 / 0.0077; with enable_fp32_context() 0.018 / 0.0046
     ("cfg2_raft_f16_noise", "raft", dict(iters=12), 2, 436, 1024, "noise", torch.float16, 8e-2, 2e-2),
     ("cfg2_raft_f16_smooth", "raft", dict(iters=12), 2, 436, 1024, "smooth", torch.float16, 8e-2, 2e-2),
     ("cfg2_raft_fp32", "raft", dict(iters=12), 1, 436, 1024, "smooth", torch.float32, 1e-3, 1e-4),

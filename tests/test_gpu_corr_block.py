@@ -192,7 +192,7 @@ OTF_CASES = [
     (1, 128, 16, 32, 3, 12.0, torch.float16, 2e-2),  # rough flow: most queries are flagged and recomputed
     (1, 256, 55, 128, 4, 2.0, torch.bfloat16, 1.5e-1),
     (1, 64, 9, 17, 2, 1.0, torch.float16, 2e-2),     # C = 64: a single K chunk
-    (1, 128, 135, 240, 4, 1.0, torch.float16, 2e-2), # 1020 work items on 148 CTAs: every ring / region slot wraps several times
+    (1, 128, 135, 240, 4, 1.0, torch.float16, 2e-2), # 1020 work items on 132 CTAs: every ring / region slot wraps several times
 ]
 
 

@@ -119,7 +119,7 @@ def test_warm_start_and_input_not_mutated():
 
 
 def test_simt_and_auto_paths_agree_in_half():
-    """kernel_impl=1 (SIMT, fp32 accumulate) vs auto (tcgen05 where available) on identical f16 inputs."""
+    """kernel_impl=1 (SIMT, fp32 accumulate) vs auto (wgmma where available) on identical f16 inputs."""
     recipe, g = load_golden("e2e_raft_noise")
     sd, img, kw = e2e_inputs(recipe)
     outs = []

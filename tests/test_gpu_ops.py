@@ -46,7 +46,7 @@ def test_library_loads_on_device():
 
     lib = _lib.load()
     assert lib.pfb_version() >= 100
-    assert lib.pfb_device_arch() >= 100, "expected an sm_100 class device"
+    assert lib.pfb_device_arch() == 90, "expected an sm_90 (Hopper) device"
 
 
 @pytest.mark.parametrize("dtype,tol", [(torch.float32, 2e-5), (torch.float16, 2e-2), (torch.bfloat16, 1.5e-1)])
@@ -360,7 +360,7 @@ def test_gma_attention_and_aggregate_vs_oracle(dtype, tol, h, w):
 @pytest.mark.parametrize("dtype", [torch.float16, torch.bfloat16])
 @pytest.mark.parametrize("mode", ["instance", "bias_relu"])
 def test_first_conv7x7s2_vs_torch(n, h, w, dtype, mode):
-    """tcgen05 first convolution (overlapping-window operand descriptors) against F.conv2d on the same rounded
+    """wgmma first convolution (overlapping-window operand descriptors) against F.conv2d on the same rounded
     inputs, fp32 accumulate; the instance-norm sums from its epilogue against torch sums of the fp32 result."""
     import torch.nn.functional as F
 

@@ -1,4 +1,4 @@
-"""GPU parity tests for the tcgen05 / TMA kernels (f16, bf16): the tensor-core correlation-volume GEMM
+"""GPU parity tests for the wgmma / TMA kernels (f16, bf16): the tensor-core correlation-volume GEMM
 with its fused pyramid epilogue, the implicit-GEMM convolution with every fused epilogue, and the two
 dedicated small convolutions.  Checkers: torch fp32 on storage-rounded inputs, and the SIMT kernels
 (impl=1) of the same library, which tests/test_gpu_ops.py pins to the reference vectors."""
@@ -168,7 +168,7 @@ def test_conv_umma_append_flow_and_special_kernels(dtype):
 
 
 def test_update_block_tcgen05_vs_simt():
-    """One full BasicUpdateBlock evaluation: auto (tcgen05 + dedicated kernels) against SIMT, f16."""
+    """One full BasicUpdateBlock evaluation: auto (wgmma + dedicated kernels) against SIMT, f16."""
     import ptlflow_b200 as pb
     from ptlflow_b200.engine import RaftEngine
 

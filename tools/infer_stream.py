@@ -3,7 +3,7 @@
 
 The caller-side loop of the reference (``infer.py``: ``cv.imread`` -> forward -> write, one pair at a time) rebuilt on
 ``ptlflow_b200.pipeline.FrameFeeder`` / ``FramePipeline`` and ``ptlflow_b200.utils.flow_utils.AsyncFlowWriter``
-(SURVEY.md section 8(f) rank 4).  Needs a B200; consecutive frames of the sorted directory listing form the pairs.
+(SURVEY.md section 8(f) rank 4).  Needs a CUDA GPU; consecutive frames of the sorted directory listing form the pairs.
 
     python tools/infer_stream.py --model raft --ckpt things --frames /data/clip --out /data/clip_flow --batch 8
 """

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Stress the multi-threaded CUDA-graph capture path (needs a B200): fresh models, two pipeline slots that see their shape for
+"""Stress the multi-threaded CUDA-graph capture path (needs a CUDA GPU): fresh models, two pipeline slots that see their shape for
 the first and second time while the other slot is mid-forward, many rounds.  Prints full tracebacks of any failure.
 
     python tools/stress_capture.py [--rounds 12]

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """BASELINE config 4 (raft, 1920x1080, 32 iterations, no 4D volume materialised) -- the lookup operator alone, timed three ways
 on the same tensors (SURVEY.md section 8(d)): this library's on-the-fly kernel, the reference's own ``alt_cuda_corr`` built for
-sm_100 (oracle/_ref, fp32 only like the reference uses it: corr.py:90-96), and this library's materialised-pyramid path
+sm_90 (oracle/_ref, fp32 only like the reference uses it: corr.py:90-96), and this library's materialised-pyramid path
 (volume build once + tiled lookup per iteration).  Prints one JSON line."""
 import json
 import os
