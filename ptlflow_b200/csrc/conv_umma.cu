@@ -34,6 +34,8 @@ using namespace sm90;
 constexpr int kATileBytes = 128 * 128;
 constexpr int kMaxBias = 1024;  // output channels per layer whose bias is kept in shared memory (Cout_pad_k <= 1024)
 constexpr int kMaxAStages = 8, kMaxBStages = 32;
+// warp roles (conv_umma_kernel): epilogue warpgroup, two MMA warpgroups, producer warpgroup
+constexpr int kEpilogueWarps = 4, kMmaWarp0 = 4, kProducerWarp = 12;
 
 struct __align__(8) ConvBars {
   uint64_t a_full[kMaxAStages];
@@ -132,11 +134,14 @@ __device__ __forceinline__ void load32(const T* src, float (&v)[32]) {
 }
 
 // The MMA role: two warpgroups, rows 0-63 and 64-127 of the M tile, each m64nNT per 16-channel K step with the
-// accumulator in registers.  A pipeline step (b_group taps x 4 K steps) is committed as one wgmma group; its ring slots are
-// released when the group has completed.  At the end of a tile the fragments go to the shared-memory accumulator tile
+// accumulator in registers.  A pipeline step (b_group taps x 4 K steps) is committed as one wgmma group and the next
+// step is issued before it has completed; its ring slots are released once it has (so the role holds one step more of
+// each ring than it computes on).  At the end of a tile the fragments go to the shared-memory accumulator tile
 // (once the epilogue has released it), so the epilogue of tile i overlaps the MMAs of tile i + 1.
 template <int NT, bool BF16, int G>
 __device__ __forceinline__ void issue_taps(float (&d)[NT / 2], uint32_t a_lo, uint32_t a_tap16, uint32_t b_lo, uint32_t b_tap16, uint32_t acc) {
+  // fence and commit in the MMAs' own basic block: ptxas injects warpgroup.arrive instructions of its own when they are outside it
+  wgmma_fence();
 #pragma unroll
   for (int g = 0; g < G; ++g) {
 #pragma unroll
@@ -145,12 +150,13 @@ __device__ __forceinline__ void issue_taps(float (&d)[NT / 2], uint32_t a_lo, ui
       wgmma<NT, BF16>(d, gdesc(a_lo + g * a_tap16 + 2 * kk, kDescHiSw128), gdesc(b_lo + g * b_tap16 + 2 * kk, kDescHiSw128), en);
     }
   }
+  wgmma_commit();
 }
 
 template <int NT, bool BF16>
 __device__ __forceinline__ void conv_mma_role(const ConvUmmaArgs& a, ConvBars* bars, uint8_t* smemA, uint8_t* smemB, float* sacc,
                                               int chunks, int group0, int group_stride) {
-  const int wg = (threadIdx.x >> 7) - 2, tid = threadIdx.x & 127, lane = threadIdx.x & 31;
+  const int wg = (threadIdx.x >> 7) - kMmaWarp0 / 4, tid = threadIdx.x & 127, lane = threadIdx.x & 31;
   const uint32_t a_slot16 = (uint32_t)a.a_slot_bytes >> 4, b_slot16 = (uint32_t)a.b_slot_bytes >> 4;
   const uint32_t a_lo0 = gdesc_lo(smem_u32(smemA) + wg * 64 * 128, 16);  // this warpgroup's 64 pixel rows
   const uint32_t b_lo0 = gdesc_lo(smem_u32(smemB), 16);
@@ -163,6 +169,15 @@ __device__ __forceinline__ void conv_mma_role(const ConvUmmaArgs& a, ConvBars* b
   int sa = 0, sb = 0, i = 0;
   uint32_t pha = 0, phb = 0;
   uint32_t a_lo = a_lo0, b_lo = b_lo0;
+  // slots of the step still in flight: weight stage (-1: none) and activation slot (-1: the step does not finish its patch)
+  int held_b = -1, held_a = -1;
+  auto release_held = [&]() {
+    __syncwarp();
+    if (lane == 0 && held_b >= 0) {
+      mbar_arrive(&bars->b_empty[held_b]);
+      if (held_a >= 0) mbar_arrive(&bars->a_empty[held_a]);
+    }
+  };
   float d[NT / 2];
   for (int w = group0; w < a.n_work; w += group_stride, ++i) {
     uint32_t acc = 0;  // first MMA of the tile overwrites the accumulator
@@ -171,20 +186,18 @@ __device__ __forceinline__ void conv_mma_role(const ConvUmmaArgs& a, ConvBars* b
       for (int kx = 0; kx < kw_halo; kx += a.b_group) {
         mbar_wait_uniform(bar_b_full + 8 * sb, phb);
         const uint32_t al = a_lo + tap_step16 * kx;  // x halo: +1 pixel row (128 B) per tap; y halo: +TW rows
-        wgmma_fence();
         switch (a.b_group) {
           case 5: issue_taps<NT, BF16, 5>(d, al, tap_step16, b_lo, b_tap16, acc); break;
           case 3: issue_taps<NT, BF16, 3>(d, al, tap_step16, b_lo, b_tap16, acc); break;
           default: issue_taps<NT, BF16, 1>(d, al, tap_step16, b_lo, b_tap16, acc); break;
         }
-        wgmma_commit();
-        wgmma_wait<0>();
+        // one group stays in flight: this step's MMAs queue behind the previous step's, whose slots are free once it has
+        // completed
+        wgmma_wait<1>();
         reg_fence(d);
-        __syncwarp();
-        if (lane == 0) {
-          mbar_arrive(&bars->b_empty[sb]);
-          if (kx + a.b_group >= kw_halo) mbar_arrive(&bars->a_empty[sa]);
-        }
+        release_held();
+        held_b = sb;
+        held_a = kx + a.b_group >= kw_halo ? sa : -1;
         acc = 1;
         b_lo += b_slot16;
         if (++sb == a.b_stages) { sb = 0; phb ^= 1; b_lo = b_lo0; }
@@ -192,6 +205,10 @@ __device__ __forceinline__ void conv_mma_role(const ConvUmmaArgs& a, ConvBars* b
       a_lo += a_slot16;
       if (++sa == a.a_stages) { sa = 0; pha ^= 1; a_lo = a_lo0; }
     }
+    wgmma_wait<0>();
+    reg_fence(d);
+    release_held();
+    held_b = -1;
     mbar_wait(&bars->acc_empty, (i & 1) ^ 1);
     acc_store<NT>(sacc, d, wg * 64, tid);
     __syncwarp();
@@ -199,10 +216,18 @@ __device__ __forceinline__ void conv_mma_role(const ConvUmmaArgs& a, ConvBars* b
   }
 }
 
-// 17 warps: 0-7 epilogue (two groups of four that split the accumulator columns), 8-15 the two MMA warpgroups, 16 TMA producer.
+// Four warpgroups: warps 0-3 the epilogue (thread = pixel row, all NT columns), 4-11 the two MMA warpgroups, 12-15 the
+// producer warpgroup (warp 12 issues the TMA loads; 13-15 only give their registers away).
 // EPI (the pfb_epilogue) is a template parameter: with a run-time switch the register allocation of every epilogue was the
 // union of all of them (h, z, addend and bias operands live together), and the staged-store version spilled.
-constexpr int kConvThreads = 17 * 32;
+constexpr int kConvThreads = 16 * 32;
+// Register budget per role (setmaxnreg).  512 threads at one CTA per SM launch with 128 registers each: 65536 for the CTA.
+// The producer warpgroup drops to 48 (at 40 its loop spills) and the epilogue takes what it frees; the MMA warpgroups keep
+// 128 (they need 96 for NT = 128 without spilling).  The gate epilogues (GRU z|r and q, which hold h / z / addend operands
+// one chunk ahead) need 168: with two epilogue warpgroups (640 threads, 96 registers each at launch) no split of the 61440
+// registers gives them that next to the MMA and producer warpgroups, hence one epilogue warpgroup.
+constexpr int kProducerRegs = 48, kEpilogueRegs = 208, kMmaRegs = 128;
+static_assert(128 * (kProducerRegs + kEpilogueRegs + 2 * kMmaRegs) <= 65536, "register budget exceeds the register file");
 template <typename T, int EPI>
 __global__ void __launch_bounds__(kConvThreads, 1)
 conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1,
@@ -243,13 +268,13 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
       mbar_init(&bars->b_empty[s], 8);
     }
     mbar_init(&bars->acc_full, 8);
-    mbar_init(&bars->acc_empty, 8);  // one arrival per epilogue warp
+    mbar_init(&bars->acc_empty, kEpilogueWarps);  // one arrival per epilogue warp
     fence_barrier_init();
   }
   // the bias vector is read by every epilogue thread for every 32-column chunk: one copy in shared memory instead of 8
   // dependent global loads per chunk
   for (int k = threadIdx.x; k < a.n_tiles * a.NT && k < kMaxBias; k += blockDim.x) sbias[k] = a.bias ? a.bias[k] : 0.f;
-  if (warp == 16 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     prefetch_tmap(&tm0);
     prefetch_tmap(&tmW);
     if (tma_out) prefetch_tmap(&tmO0);
@@ -274,56 +299,59 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
     x0 = px * a.TW;
   };
 
-  if (warp == 16) {
-    // ================= TMA producer (warp-uniform loop, one elected lane issues) =================
-    const int ph2 = a.KH >> 1, pw2 = a.KW >> 1;
-    const uint32_t btx = a.NT * 128;  // bytes of one weight tap
-    // ring positions advance incrementally (stage index + phase bit): no integer division on the issue path
-    int sta = 0, stb = 0, bg = 0;
-    uint32_t pha = 0, phb = 0;
-    PFB_TR(3);
-    for (int w = group0; w < a.n_work; w += group_stride) {
-      int n0, b, y0, x0;
-      decode(w, n0, b, y0, x0);
-      int kidx = 0;
-      const int wrow0 = b * a.w_rows_per_sample;  // per-sample weights (GMA aggregate: the sample's v^T)
-      for (int s = 0; s < a.nsrc; ++s) {
-        const CUtensorMap* tm = s == 0 ? &tm0 : (s == 1 ? &tm1 : &tm2);
-        for (int c = 0; c < a.src_chunks[s]; ++c, ++kidx) {
-          int wrow = wrow0;  // + (ky * KW + kx) * Cout_pad_k
-          for (int ky = 0; ky < a.KH; ++ky) {
-            for (int kx = 0; kx < a.KW; ++kx) {
-              // activation patch: once per (chunk, ky) with the x halo, once per chunk with the y halo, else per tap
-              if (a.halo == 0 || (a.halo == 1 && kx == 0) || (a.halo == 2 && ky == 0)) {
-                mbar_wait(&bars->a_empty[sta], pha ^ 1);
+  if (warp >= kProducerWarp) {
+    setmaxnreg_dec<kProducerRegs>();
+    if (warp == kProducerWarp) {
+      // ================= TMA producer (warp-uniform loop, one elected lane issues) =================
+      const int ph2 = a.KH >> 1, pw2 = a.KW >> 1;
+      const uint32_t btx = a.NT * 128;  // bytes of one weight tap
+      // ring positions advance incrementally (stage index + phase bit): no integer division on the issue path
+      int sta = 0, stb = 0, bg = 0;
+      uint32_t pha = 0, phb = 0;
+      PFB_TR(3);
+      for (int w = group0; w < a.n_work; w += group_stride) {
+        int n0, b, y0, x0;
+        decode(w, n0, b, y0, x0);
+        int kidx = 0;
+        const int wrow0 = b * a.w_rows_per_sample;  // per-sample weights (GMA aggregate: the sample's v^T)
+        for (int s = 0; s < a.nsrc; ++s) {
+          const CUtensorMap* tm = s == 0 ? &tm0 : (s == 1 ? &tm1 : &tm2);
+          for (int c = 0; c < a.src_chunks[s]; ++c, ++kidx) {
+            int wrow = wrow0;  // + (ky * KW + kx) * Cout_pad_k
+            for (int ky = 0; ky < a.KH; ++ky) {
+              for (int kx = 0; kx < a.KW; ++kx) {
+                // activation patch: once per (chunk, ky) with the x halo, once per chunk with the y halo, else per tap
+                if (a.halo == 0 || (a.halo == 1 && kx == 0) || (a.halo == 2 && ky == 0)) {
+                  mbar_wait(&bars->a_empty[sta], pha ^ 1);
+                  if (elect_one()) {
+                    mbar_arrive_expect_tx(&bars->a_full[sta], a.a_tx_bytes);
+                    tma_load_4d(smemA + sta * a.a_slot_bytes, tm, &bars->a_full[sta], a.src_coff[s] + c * 64,
+                                x0 - pw2 + (a.halo ? 0 : kx), y0 + ky - ph2, b);
+                  }
+                  __syncwarp();
+                  if (++sta == a.a_stages) { sta = 0; pha ^= 1; }
+                }
+                // weight stage: b_group consecutive taps of this patch share one barrier (fewer, larger pipeline steps)
+                if (bg == 0) mbar_wait(&bars->b_empty[stb], phb ^ 1);
                 if (elect_one()) {
-                  mbar_arrive_expect_tx(&bars->a_full[sta], a.a_tx_bytes);
-                  tma_load_4d(smemA + sta * a.a_slot_bytes, tm, &bars->a_full[sta], a.src_coff[s] + c * 64,
-                              x0 - pw2 + (a.halo ? 0 : kx), y0 + ky - ph2, b);
+                  if (bg == 0) mbar_arrive_expect_tx(&bars->b_full[stb], btx * a.b_group);
+                  tma_load_2d(smemB + stb * a.b_slot_bytes + bg * a.b_tap_bytes, &tmW, &bars->b_full[stb], kidx * 64, wrow + n0);
                 }
                 __syncwarp();
-                if (++sta == a.a_stages) { sta = 0; pha ^= 1; }
-              }
-              // weight stage: b_group consecutive taps of this patch share one barrier (fewer, larger pipeline steps)
-              if (bg == 0) mbar_wait(&bars->b_empty[stb], phb ^ 1);
-              if (elect_one()) {
-                if (bg == 0) mbar_arrive_expect_tx(&bars->b_full[stb], btx * a.b_group);
-                tma_load_2d(smemB + stb * a.b_slot_bytes + bg * a.b_tap_bytes, &tmW, &bars->b_full[stb], kidx * 64, wrow + n0);
-              }
-              __syncwarp();
-              wrow += a.Cout_pad_k;
-              if (++bg == a.b_group) {
-                bg = 0;
-                if (++stb == a.b_stages) { stb = 0; phb ^= 1; }
+                wrow += a.Cout_pad_k;
+                if (++bg == a.b_group) {
+                  bg = 0;
+                  if (++stb == a.b_stages) { stb = 0; phb ^= 1; }
+                }
               }
             }
           }
         }
       }
+      PFB_TR(4);
     }
-    PFB_TR(4);
-  } else if (warp >= 8) {
-    // ================= MMA warpgroups =================
+  } else if (warp >= kMmaWarp0) {
+    // ================= MMA warpgroups (kMmaRegs: the launch budget) =================
     switch (a.NT) {
       case 32: conv_mma_role<32, std::is_same<T, __nv_bfloat16>::value>(a, bars, smemA, smemB, sacc, chunks, group0, group_stride); break;
       case 64: conv_mma_role<64, std::is_same<T, __nv_bfloat16>::value>(a, bars, smemA, smemB, sacc, chunks, group0, group_stride); break;
@@ -331,10 +359,9 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
       default: conv_mma_role<128, std::is_same<T, __nv_bfloat16>::value>(a, bars, smemA, smemB, sacc, chunks, group0, group_stride); break;
     }
   } else {
+    setmaxnreg_inc<kEpilogueRegs>();
     // ================= epilogue: thread <-> pixel, 32 output channels at a time =================
-    // warps 0-3 take the even 32-column chunks, warps 4-7 the odd ones
-    const int quarter = warp & 3, group = warp >> 2;
-    const int row = quarter * 32 + lane;
+    const int row = warp * 32 + lane;
     const int hd = a.hidden;
     int i = 0;
     for (int w = group0; w < a.n_work; w += group_stride, ++i) {
@@ -378,32 +405,31 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
       // Operand prefetch.  Plain epilogues: the next chunk's accumulator / residual is requested as soon as the current chunk
       // has been moved out of r[] ("early").  Gate epilogues (z|r, q, axpy) also hold h / z / addend: they request the next
       // chunk's operands only AFTER the current chunk has been packed ("late"), when its registers are dead -- the loads then
-      // fly under the staging barriers and the TMA issue.  That keeps every instantiation inside the 168-register ceiling
+      // fly under the staging barriers and the TMA issue.  That keeps every instantiation inside its register budget
       // without spills and without exposing the L2 latency per chunk (in-place loads cost +2..6 us per gate launch, r02e).
       // Measured (launch lists r02c / r02e / r02f): the staged stores win on the plain epilogues (convc1 27.7 -> 20.8 us, flow
       // head 35.1 -> 29.4 us) but lose on the gate epilogues, whose warps are unevenly loaded (r half vs z half) and meet at two
       // barriers per 64-column block: z|r 41.7 -> 45.0 us, q 40.0 -> 49.2 us.  The host therefore stages only plain epilogues
       // (conv2d_umma: tma_out), and the gates keep direct stores with everything requested one chunk ahead.
       constexpr bool kLate = false;
-      if (aux_h_any) issue_h(group * 32, hnext);
-      issue_z(group * 32, znext);
-      issue_add(group * 32, anext);
+      if (aux_h_any) issue_h(0, hnext);
+      issue_z(0, znext);
+      issue_add(0, anext);
       mbar_wait(&bars->acc_full, i & 1);
       if (warp == 0 && i < 3) PFB_TR(12 + i);
-      // accumulator reads are software-pipelined too: chunk c + 64 is loaded as soon as chunk c has been moved to v[]
+      // accumulator reads are software-pipelined too: chunk c + 32 is loaded as soon as chunk c has been moved to v[]
       uint32_t r[32];
-      if (group * 32 < a.NT) acc_ld32(sacc, row, group * 32, r);
-      // 32 packed values -> this thread's half (group) of its pixel's 128-byte row in the staging buffer
-      auto stage32 = [&](const uint4 (&pk)[4]) {
+      acc_ld32(sacc, row, 0, r);
+      // 32 packed values -> half `half` of this thread's pixel's 128-byte row in the staging buffer
+      auto stage32 = [&](const uint4 (&pk)[4], int half) {
         uint8_t* sb = smemO + row * 128;
 #pragma unroll
-        for (int q = 0; q < 4; ++q) *reinterpret_cast<uint4*>(sb + (((group * 4 + q) ^ (row & 7)) << 4)) = pk[q];
+        for (int q = 0; q < 4; ++q) *reinterpret_cast<uint4*>(sb + (((half * 4 + q) ^ (row & 7)) << 4)) = pk[q];
       };
-      for (int cb = 0; cb < a.NT; cb += 64) {
-       const int c = cb + group * 32;
+      for (int c = 0; c < a.NT; c += 32) {
        uint4 pk[4];  // the chunk's 32 results, converted: what stays live across the staging barrier
-       if (c < a.NT) {
-        float v[32];  // (the last block of an NT % 64 == 32 tile has no chunk for group 1, which still joins the barriers below)
+       {
+        float v[32];
         const int n = n0 + c;  // first output channel of this chunk
         uint4 hraw[4], zraw[4];
 #pragma unroll
@@ -431,11 +457,11 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
             v[4 * q + 3] = __uint_as_float(r[4 * q + 3]) + bb[q].w;
           }
         }
-        if (!kLate && c + 64 < a.NT) {  // warp-uniform
-          acc_ld32(sacc, row, c + 64, r);
-          if (aux_h_any) issue_h(c + 64, hnext);
-          issue_z(c + 64, znext);
-          issue_add(c + 64, anext);
+        if (!kLate && c + 32 < a.NT) {  // warp-uniform
+          acc_ld32(sacc, row, c + 32, r);
+          if (aux_h_any) issue_h(c + 32, hnext);
+          issue_z(c + 32, znext);
+          issue_add(c + 32, anext);
         }
         if (ok || tma_out) {  // (staged rows of out-of-image pixels are clipped by the TMA unit)
         T* out = reinterpret_cast<T*>(a.out);
@@ -537,32 +563,36 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
             pk[q].w = pack2<T>(v[8 * q + 6], v[8 * q + 7]);
           }
         }
-        if (kLate && c + 64 < a.NT) {  // warp-uniform
-          acc_ld32(sacc, row, c + 64, r);
-          if (aux_h_any) issue_h(c + 64, hnext);
-          issue_z(c + 64, znext);
-          issue_add(c + 64, anext);
+        if (kLate && c + 32 < a.NT) {  // warp-uniform
+          acc_ld32(sacc, row, c + 32, r);
+          if (aux_h_any) issue_h(c + 32, hnext);
+          issue_z(c + 32, znext);
+          issue_add(c + 32, anext);
         }
        }
        if (tma_out) {
-         // One 64-column block, staged by both epilogue groups, leaves as one bulk store (single staging buffer: the previous
-         // block's store has had this block's arithmetic to drain; thread 0 confirms it before anybody overwrites the buffer).
-         if (threadIdx.x == 0) tma_store_wait_read();
-         named_barrier_sync(1, 256);
-         if (c < a.NT) stage32(pk);
-         fence_proxy_async();
-         named_barrier_sync(1, 256);
-         if (threadIdx.x == 0) {
-           const int nb = n0 + cb;
+         // One 64-column block (two chunks) leaves as one bulk store (single staging buffer: the previous block's store has
+         // had this chunk's arithmetic to drain; thread 0 confirms it before anybody overwrites the buffer).
+         if ((c & 32) == 0) {
+           if (threadIdx.x == 0) tma_store_wait_read();
+           named_barrier_sync(1, 32 * kEpilogueWarps);
+         }
+         stage32(pk, (c >> 5) & 1);
+         if ((c & 32) != 0 || c + 32 >= a.NT) {
+          fence_proxy_async();
+          named_barrier_sync(1, 32 * kEpilogueWarps);
+          if (threadIdx.x == 0) {
+           const int nb = n0 + (c & ~63);
            if (EPI == PFB_EPI_GRU_ZR && nb < hd) tma_store_4d(&tmO1, smemO, nb, x0, y0, b);
            else tma_store_4d(&tmO0, smemO, a.out_offset + (EPI == PFB_EPI_GRU_ZR ? nb - hd : nb), x0, y0, b);
            tma_store_commit();
+          }
          }
        }
       }
       __syncwarp();
       if (warp == 0 && i < 3) PFB_TR(15 + i);
-      if (warp == 4 && i < 3) PFB_TR(21 + i);
+      if (warp == kEpilogueWarps - 1 && i < 3) PFB_TR(21 + i);
       if (lane == 0) mbar_arrive(&bars->acc_empty);
     }
   }
@@ -767,7 +797,9 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
   {
     // Split the rest between the rings.  A slot is reused only once per round trip (release -> producer wake-up -> TMA ->
     // MMA), so the number of K steps in flight, not the bytes, sets the pace of the small-N layers: maximise min(steps
-    // covered by the activation ring, weight stages).
+    // covered by the activation ring, weight stages).  The MMA warpgroups hold the stage of the step in flight on top of
+    // the one they issue from, so one stage of each ring counts as consumed: 2 weight stages (the least that does not
+    // deadlock) leave the producer no lead and are chosen only where the activation patches leave room for no more.
     const int budget = ring_budget;
     const int taps_per_patch = a.halo == 1 ? p->KW : (a.halo == 2 ? p->KH : 1);
     int best = -1;
@@ -775,7 +807,8 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
       int bs = (budget - as * a.a_slot_bytes) / a.b_slot_bytes;
       if (bs > kMaxBStages) bs = kMaxBStages;
       if (bs < 2) continue;
-      const int cover = as * taps_per_patch < bs * a.b_group ? as * taps_per_patch : bs * a.b_group;
+      const int cover_a = (as - 1) * taps_per_patch, cover_b = (bs - 1) * a.b_group;
+      const int cover = cover_a < cover_b ? cover_a : cover_b;
       if (cover > best || (cover == best && bs > a.b_stages)) { best = cover; a.a_stages = as; a.b_stages = bs; }
     }
     if (best < 0) return PFB_ERR_UNSUPPORTED;

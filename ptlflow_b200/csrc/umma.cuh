@@ -122,6 +122,12 @@ __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.a
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 template <int N>
 __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// Per-warpgroup register budget (all four warps of a warpgroup execute it).  dec returns registers to the CTA's pool,
+// inc blocks until the pool can supply them, so the increases of a kernel must add up to no more than its decreases.
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+template <uint32_t N>
+__device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 // keeps the compiler from moving accumulator accesses across the asynchronous MMAs
 template <int R>
 __device__ __forceinline__ void reg_fence(float (&d)[R]) {
