@@ -248,6 +248,14 @@ PFB_API int pfb_upflow8(const float* coords, float* out, float* flow_small, int 
 /* GMA attention: in-place softmax over the last axis of sim [rows, cols] (sim = pfb_corr_volume_build(q, k)
  * level 0: <q, k> / sqrt(dim_head) is exactly the content attention logit).   gma_utils.py:58-76 */
 PFB_API int pfb_softmax_rows(void* x, size_t rows, int cols, pfb_dtype dtype, pfb_stream stream);
+/* GMA attention with the relative-position term (position_only / position_and_content, gma_utils.py:6-30, 62-74).
+ * Row r of attn [rows, H*W] (rows = heads * B * H*W, head-major) is the query i = r % (H*W) at grid row x = i / W, column y = i % W:
+ *   attn[r][u*W + v] = softmax over (u, v) of  logits[r][u*W + v] + th[r*table_stride + u - x + P - 1] + tw[r*table_stride + v - y + P - 1]
+ * logits [rows, H*W] dtype (content logits, may alias attn) or NULL (position only); th, tw fp32 per-query tables of 2P-1 entries
+ * (scale * q . rel_height / rel_width), row stride table_stride >= 2P-1.  H, W <= P.  Softmax in fp32; each row is read once
+ * and written once. */
+PFB_API int pfb_attention_softmax_relpos(const void* logits, const float* th, const float* tw, size_t table_stride, void* attn,
+                                         size_t rows, int H, int W, int P, pfb_dtype dtype, pfb_stream stream);
 /* [B, HW, C] pixel-major -> [B, C, HW_pad] (zero padded): K-major operand for the attn @ v GEMM */
 PFB_API int pfb_transpose_pm(const void* in, void* out, int B, int HW, int C, int HW_pad, pfb_dtype dtype, pfb_stream stream);
 
@@ -285,6 +293,7 @@ typedef enum {
   /* ... and convc2 (256 -> 192) | convf2 (128 -> 64) as ONE block-diagonal 3x3 layer 384 -> 256 (update.py:98-102): N = 256
    * runs the tensor core at its nominal rate, the two separate layers (N = 192, 64) do not */
   PFB_L_CONVC2F2,
+  PFB_L_AGG_PROJ, /* GMA Aggregate.project (1x1, heads*128 -> 128, no bias); present iff num_heads > 1 */
   PFB_L_COUNT
 } pfb_layer_id;
 
@@ -313,6 +322,7 @@ typedef struct {
   int fork_flow;      /* 1: the flow branch of the motion encoder (convf1, convf2) and the once-per-forward context terms run on a second
                          stream of the calling host thread, forked / joined with events (parallel branches when the caller captures a
                          CUDA graph); 0: everything on `stream`.  Half-precision tensor path only, ignored elsewhere. */
+  int num_heads;      /* gma: attention heads (0 is read as 1); > 1 needs layer PFB_L_AGG_PROJ */
 } pfb_raft_cfg;
 
 typedef struct {
@@ -329,7 +339,8 @@ typedef struct {
   float* flow_small;          /* [B,2,H,W] fp32 */
   void* workspace;            /* pfb_raft_workspace_bytes(cfg) */
   size_t workspace_bytes;
-  const void* attention;      /* gma: softmax attention [B, H*W, H*W] dtype (pfb_gma_attention_softmax) */
+  const void* attention;      /* gma: softmax attention [heads, B, H*W, H*W] dtype, head-major (pfb_softmax_rows or
+                                 pfb_attention_softmax_relpos) */
   float agg_gamma;            /* gma: Aggregate.gamma */
 } pfb_raft_buffers;
 

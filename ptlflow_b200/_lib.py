@@ -26,7 +26,7 @@ EPI_LINEAR, EPI_RELU, EPI_GRU_ZR, EPI_GRU_Q, EPI_FLOW, EPI_RELU_APPEND_FLOW, EPI
 
 (L_CONVC1, L_CONVC2, L_CONVF1, L_CONVF2, L_CONV, L_GRU_ZR1, L_GRU_Q1, L_GRU_ZR2, L_GRU_Q2,
  L_FLOW1, L_FLOW2, L_MASK1, L_MASK2, L_AGG_V, L_FLOW2T,
- L_CTX_ZR1, L_CTX_Q1, L_CTX_ZR2, L_CTX_Q2, L_GRUX_ZR1, L_GRUX_Q1, L_GRUX_ZR2, L_GRUX_Q2, L_CONVC2F2, L_COUNT) = range(25)
+ L_CTX_ZR1, L_CTX_Q1, L_CTX_ZR2, L_CTX_Q2, L_GRUX_ZR1, L_GRUX_Q1, L_GRUX_ZR2, L_GRUX_Q2, L_CONVC2F2, L_AGG_PROJ, L_COUNT) = range(26)
 
 
 class ConvSrc(C.Structure):
@@ -61,7 +61,7 @@ class RaftCfg(C.Structure):
         ("feat_dim", C.c_int), ("corr_levels", C.c_int), ("corr_radius", C.c_int),
         ("hidden_dim", C.c_int), ("context_dim", C.c_int), ("iters", C.c_int), ("alternate_corr", C.c_int),
         ("out_h", C.c_int), ("out_w", C.c_int), ("pad_top", C.c_int), ("pad_left", C.c_int), ("impl", C.c_int),
-        ("volume_layout", C.c_int), ("fork_flow", C.c_int),
+        ("volume_layout", C.c_int), ("fork_flow", C.c_int), ("num_heads", C.c_int),
     ]
 
 
@@ -109,6 +109,7 @@ SIGNATURES = {
     "pfb_convex_upsample": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
     "pfb_upflow8": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _S]),
     "pfb_softmax_rows": (_I, [_P, C.c_size_t, _I, _I, _S]),
+    "pfb_attention_softmax_relpos": (_I, [_P, _P, _P, C.c_size_t, _P, C.c_size_t, _I, _I, _I, _I, _S]),
     "pfb_transpose_pm": (_I, [_P, _P, _I, _I, _I, _I, _I, _S]),
     "pfb_flow_tap_gather": (_I, [_P, _I, _P, _P, _P, _I, _I, _I, _S]),
     "pfb_context_split": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _S]),

@@ -2,6 +2,7 @@
 #include <stdarg.h>
 
 #include <algorithm>
+#include <atomic>
 
 #include "common.cuh"
 
@@ -257,6 +258,107 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(T* __restrict__ x, in
   for (int c = threadIdx.x; c < cols; c += blockDim.x) row[c] = from_f32<T>(expf(to_f32(row[c]) - m) * inv);
 }
 
+constexpr int kRelposThreads = 256;
+
+template <bool MAX>
+__device__ __forceinline__ float relpos_block_reduce(float v, float* red) {
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  for (int o = 16; o > 0; o >>= 1) {
+    const float w = __shfl_xor_sync(0xffffffffu, v, o);
+    v = MAX ? fmaxf(v, w) : v + w;
+  }
+  if (lane == 0) red[warp] = v;
+  __syncthreads();
+  v = red[0];
+  for (int i = 1; i < kRelposThreads / 32; ++i) v = MAX ? fmaxf(v, red[i]) : v + red[i];
+  __syncthreads();
+  return v;
+}
+
+// GMA attention with the relative-position term (gma_utils.py:6-30, 62-74): one CTA per row r = (head, b, query i = x*W + y),
+// logit[u*W + v] = C[r][u*W + v] (or 0 without content) + Th[r][u - x + P - 1] + Tw[r][v - y + P - 1], softmax over the row in
+// fp32.  The row lives in shared memory between the passes, so HBM sees one read of C and one write of attn; the row's H + W
+// table entries are staged in shared memory too.  VEC: rows of a multiple of 16 bytes, moved with 16-byte loads / stores.
+template <typename T, bool VEC>
+__global__ void __launch_bounds__(kRelposThreads) attention_softmax_relpos_kernel(const T* __restrict__ logits, const float* __restrict__ th_tab,
+                                                                                  const float* __restrict__ tw_tab, size_t tstride,
+                                                                                  T* __restrict__ attn, int H, int W, int P) {
+  constexpr int EV = VEC ? 16 / (int)sizeof(T) : 1;
+  extern __shared__ __align__(16) float srow[];  // [N] row, then th [H], tw [W]
+  __shared__ float red[kRelposThreads / 32];
+  const int N = H * W;
+  float* th = srow + N;
+  float* tw = th + H;
+  const size_t r = blockIdx.x;
+  const int i = (int)(r % (size_t)N), x = i / W, y = i - x * W;
+  const float* thr = th_tab + r * tstride + (P - 1 - x);
+  const float* twr = tw_tab + r * tstride + (P - 1 - y);
+  for (int u = threadIdx.x; u < H; u += kRelposThreads) th[u] = thr[u];
+  for (int v = threadIdx.x; v < W; v += kRelposThreads) tw[v] = twr[v];
+  __syncthreads();
+  const T* lrow = logits ? logits + r * N : nullptr;
+  T* arow = attn + r * N;
+  const int nvec = N / EV;
+
+  float m = -INFINITY;
+  for (int c = threadIdx.x; c < nvec; c += kRelposThreads) {
+    const int j0 = c * EV;
+    float f[EV];
+    if (lrow) {
+      if constexpr (VEC) {
+        const uint4 raw = *reinterpret_cast<const uint4*>(lrow + j0);
+        const T* e = reinterpret_cast<const T*>(&raw);
+#pragma unroll
+        for (int k = 0; k < EV; ++k) f[k] = to_f32(e[k]);
+      } else {
+        f[0] = to_f32(lrow[j0]);
+      }
+    } else {
+#pragma unroll
+      for (int k = 0; k < EV; ++k) f[k] = 0.f;
+    }
+    int u = j0 / W, v = j0 - u * W;
+#pragma unroll
+    for (int k = 0; k < EV; ++k) {
+      f[k] += th[u] + tw[v];
+      m = fmaxf(m, f[k]);
+      if (++v == W) { v = 0; ++u; }
+    }
+#pragma unroll
+    for (int k = 0; k < EV; k += 4 > EV ? EV : 4) {
+      if constexpr (EV >= 4) *reinterpret_cast<float4*>(srow + j0 + k) = make_float4(f[k], f[k + 1], f[k + 2], f[k + 3]);
+      else srow[j0 + k] = f[k];
+    }
+  }
+  m = relpos_block_reduce<true>(m, red);
+
+  float sum = 0.f;  // every thread revisits the entries it wrote: no barrier needed before this pass
+  for (int c = threadIdx.x; c < nvec; c += kRelposThreads) {
+    const int j0 = c * EV;
+#pragma unroll
+    for (int k = 0; k < EV; ++k) {
+      const float e = __expf(srow[j0 + k] - m);
+      srow[j0 + k] = e;
+      sum += e;
+    }
+  }
+  sum = relpos_block_reduce<false>(sum, red);
+  const float inv = 1.f / sum;
+
+  for (int c = threadIdx.x; c < nvec; c += kRelposThreads) {
+    const int j0 = c * EV;
+    if constexpr (VEC) {
+      uint4 raw;
+      T* e = reinterpret_cast<T*>(&raw);
+#pragma unroll
+      for (int k = 0; k < EV; ++k) e[k] = from_f32<T>(srow[j0 + k] * inv);
+      *reinterpret_cast<uint4*>(arow + j0) = raw;
+    } else {
+      arow[j0] = from_f32<T>(srow[j0] * inv);
+    }
+  }
+}
+
 // [B][HW][C] -> [B][C][HW_pad], zero fill for hw >= HW (32x32 smem tile transpose)
 template <typename T>
 __global__ void transpose_pm_kernel(const T* __restrict__ in, T* __restrict__ out, int HW, int C, int HW_pad) {
@@ -420,6 +522,45 @@ extern "C" PFB_API int pfb_softmax_rows(void* x, size_t rows, int cols, pfb_dtyp
   cudaStream_t s = as_stream(stream);
   ProfScope prof(KC_MISC, s);
   PFB_DISPATCH_DTYPE(dtype, T, { softmax_rows_kernel<T><<<(unsigned)rows, 256, 0, s>>>((T*)x, cols); });
+  PFB_LAUNCH_CHECK();
+  return PFB_OK;
+}
+
+template <typename T, bool VEC>
+static int launch_relpos_softmax(const void* logits, const float* th, const float* tw, size_t tstride, void* attn, size_t rows, int H,
+                                 int W, int P, cudaStream_t s) {
+  const size_t smem = (size_t)(H * W + H + W) * sizeof(float);
+  // once per (instantiation, device): rows of more than 12 288 entries need more than the default 48 KB
+  static std::atomic<unsigned long long> attr_done{0};
+  int dev = 0;
+  PFB_CUDA(cudaGetDevice(&dev));
+  if (!(attr_done.load(std::memory_order_acquire) & (1ull << (dev & 63)))) {
+    PFB_CUDA(cudaFuncSetAttribute(attention_softmax_relpos_kernel<T, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+    attr_done.fetch_or(1ull << (dev & 63), std::memory_order_release);
+  }
+  attention_softmax_relpos_kernel<T, VEC><<<(unsigned)rows, kRelposThreads, smem, s>>>((const T*)logits, th, tw, tstride, (T*)attn, H, W, P);
+  return PFB_OK;
+}
+
+extern "C" PFB_API int pfb_attention_softmax_relpos(const void* logits, const float* th, const float* tw, size_t table_stride, void* attn,
+                                                    size_t rows, int H, int W, int P, pfb_dtype dtype, pfb_stream stream) {
+  PFB_CHECK_ARG(th && tw && attn && dtype_ok(dtype), "attention_softmax_relpos: null pointer or bad dtype");
+  PFB_CHECK_ARG(P > 0 && H > 0 && W > 0 && H <= P && W <= P, "attention_softmax_relpos: %dx%d grid outside the %dx%d position table", H, W, P, P);
+  PFB_CHECK_ARG(table_stride >= (size_t)(2 * P - 1), "attention_softmax_relpos: table_stride %zu < 2P-1 = %d", table_stride, 2 * P - 1);
+  const size_t N = (size_t)H * W;
+  PFB_CHECK_ARG(rows > 0 && rows < (1ull << 31) && rows % N == 0, "attention_softmax_relpos: rows=%zu is not a multiple of H*W=%zu", rows, N);
+  cudaStream_t s = as_stream(stream);
+  const size_t ev = 16 / dtype_size(dtype);
+  const bool vec = N % ev == 0 && ((reinterpret_cast<uintptr_t>(logits) | reinterpret_cast<uintptr_t>(attn)) & 15) == 0;
+  int rc = PFB_OK;
+  {
+    ProfScope prof(KC_MISC, s);
+    PFB_DISPATCH_DTYPE(dtype, T, {
+      rc = vec ? launch_relpos_softmax<T, true>(logits, th, tw, table_stride, attn, rows, H, W, P, s)
+               : launch_relpos_softmax<T, false>(logits, th, tw, table_stride, attn, rows, H, W, P, s);
+    });
+  }
+  if (rc != PFB_OK) return rc;
   PFB_LAUNCH_CHECK();
   return PFB_OK;
 }

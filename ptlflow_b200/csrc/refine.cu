@@ -25,7 +25,8 @@ struct Workspace {
   int planes, corr_stride;
   size_t off_corr, off_cor1, off_corflo, off_flo1, off_motion, off_z, off_rh, off_fh, off_mh, off_mask, off_flow;
   size_t off_taps;          // flow head conv2 per-tap products [P][32] fp32 (tensor-core path)
-  size_t off_vbuf, off_vT;  // gma: to_v(motion) [P][128] and its per-sample transpose [B][128][n_pad]
+  size_t off_vbuf, off_vT;  // gma: to_v(motion) [P][heads*128] and its per-sample transpose [B][heads*128][n_pad]
+  size_t off_agg;           // gma, heads > 1: the concatenated per-head attn @ v [P][heads*128] (input of Aggregate.project)
   size_t off_flags;         // on-the-fly tensor-core lookup: one flag per query (queries recomputed by the SIMT pass)
   size_t off_ctx[4];        // iteration-invariant context terms of the GRU gates: zr1 [P][2hd], q1 [P][hd], zr2, q2 (tensor path)
   int n_pad;
@@ -33,8 +34,11 @@ struct Workspace {
   int c_cor1, c_corflo, c_cor2, c_flo1, c_flo2, c_motion, c_fh;
 };
 
+static int heads_of(const pfb_raft_cfg* c) { return c->num_heads > 0 ? c->num_heads : 1; }
+
 static Workspace plan(const pfb_raft_cfg* c) {
   Workspace w{};
+  const size_t vdim = (size_t)heads_of(c) * 128;
   const size_t P = (size_t)c->B * c->H * c->W;
   const size_t es = dtype_size(c->dtype);
   const int K = 2 * c->corr_radius + 1;
@@ -64,8 +68,9 @@ static Workspace plan(const pfb_raft_cfg* c) {
   w.off_flow = take(P * 2 * sizeof(float));
   w.off_taps = take(c->variant != 1 ? P * 32 * sizeof(float) : 0);
   w.n_pad = (int)align_up((size_t)c->H * c->W, 64);
-  w.off_vbuf = take(c->variant == 2 ? P * 128 * es : 0);
-  w.off_vT = take(c->variant == 2 ? (size_t)c->B * 128 * w.n_pad * es : 0);
+  w.off_vbuf = take(c->variant == 2 ? P * vdim * es : 0);
+  w.off_vT = take(c->variant == 2 ? (size_t)c->B * vdim * w.n_pad * es : 0);
+  w.off_agg = take(c->variant == 2 && vdim > 128 ? P * vdim * es : 0);
   w.off_flags = take(c->alternate_corr ? P : 0);
   for (int i = 0; i < 4; ++i)
     w.off_ctx[i] = take((c->variant != 1 && c->dtype != PFB_F32) ? P * (size_t)((i & 1) ? c->hidden_dim : 2 * c->hidden_dim) * es : 0);
@@ -83,6 +88,7 @@ static int check_cfg(const pfb_raft_cfg* c) {
   PFB_CHECK_ARG((c->H >> (c->corr_levels - 1)) >= 1 && (c->W >> (c->corr_levels - 1)) >= 1,
                 "raft: %dx%d grid too small for %d levels", c->H, c->W, c->corr_levels);
   PFB_CHECK_ARG(c->hidden_dim > 0 && c->context_dim > 0 && c->iters >= 0, "raft: bad dims");
+  PFB_CHECK_ARG(c->num_heads >= 0 && c->num_heads <= 64 && (c->variant == 2 || heads_of(c) == 1), "raft: num_heads=%d", c->num_heads);
   PFB_CHECK_ARG(c->volume_layout == 0 || (c->volume_layout == 1 && c->dtype != PFB_F32 && !c->alternate_corr && c->corr_levels <= 4),
                 "raft: volume_layout=%d needs f16/bf16, a materialised pyramid and <= 4 levels", c->volume_layout);
   if (c->variant != 1) PFB_CHECK_ARG(c->hidden_dim == 128 && c->context_dim == 128, "raft/gma: the update block expects hidden=context=128");
@@ -249,49 +255,70 @@ static int update_iter(const Ctx& x, const void* corr_ext, void* mask_out) {
   // ---- gma: motion_global = motion + gamma * (attention @ to_v(motion))   gma_utils.py:101-113, gma/update.py:149 ----
   if (c->variant == 2) {
     PFB_CHECK_ARG(x.b->attention, "gma: null attention");
-    const int N = c->H * c->W;
+    const int N = c->H * c->W, heads = heads_of(c), vdim = heads * 128;
     const size_t es = dtype_size(c->dtype);
+    const char* attention = reinterpret_cast<const char*>(x.b->attention);
     char* vbuf = reinterpret_cast<char*>(x.at(ws.off_vbuf));
     char* vT = reinterpret_cast<char*>(x.at(ws.off_vT));
-    PFB_TRY(run_conv(x, PFB_L_AGG_V, {src_of(motion, 128, ws.c_motion)}, PFB_EPI_LINEAR, vbuf, 128, 0));
+    // one head: attn @ v goes straight into the AXPY epilogue.  Several heads (gma_utils.py:101-111): every head's attn @ v
+    // lands in its 128 columns of `agg`, then project (heads*128 -> 128) carries the AXPY epilogue.
+    char* agg = heads > 1 ? reinterpret_cast<char*>(x.at(ws.off_agg)) : nullptr;
+    PFB_CHECK_ARG(heads == 1 || (x.w->layers[PFB_L_AGG_PROJ].weight && x.w->layers[PFB_L_AGG_PROJ].Cin == vdim),
+                  "gma: num_heads=%d needs the Aggregate.project layer (%d -> 128)", heads, vdim);
+    PFB_TRY(run_conv(x, PFB_L_AGG_V, {src_of(motion, 128, ws.c_motion)}, PFB_EPI_LINEAR, vbuf, vdim, 0));
     const bool tensor_path = c->dtype != PFB_F32 && c->impl != 1 && (N % 8) == 0;
-    if (tensor_path) PFB_TRY(pfb_transpose_pm(vbuf, vT, c->B, N, 128, ws.n_pad, c->dtype, (pfb_stream)x.s));
+    if (tensor_path) PFB_TRY(pfb_transpose_pm(vbuf, vT, c->B, N, vdim, ws.n_pad, c->dtype, (pfb_stream)x.s));
     static const int env_batched = getenv("PFB_GMA_BATCHED") ? atoi(getenv("PFB_GMA_BATCHED")) : 1;
-    if (tensor_path && env_batched) {
-      // ONE launch for all samples: pixels = queries, input channels = the N attention columns, per-sample weights = that
-      // sample's v^T (K-major [128][n_pad], rows b * 128 ...).  B x 55 row tiles fill the machine; one launch per sample left
-      // only 55 row tiles, a fraction of the machine.
+    // "1x1 convolution" of head h over sample b (b < 0: all samples in one launch): pixels = queries, input channels = the N
+    // attention columns, weights = the sample's v (SIMT layout [N][vdim], columns h*128...) / v^T (K-major [vdim][n_pad], rows
+    // h*128...).  The attention is head-major, so every operand is affine in the pixel index.
+    auto attn_v = [&](int h, int b) -> int {
+      const int b0 = b < 0 ? 0 : b;
       pfb_conv_params p{};
-      p.src[0] = src_of(x.b->attention, N, N);
+      p.src[0] = src_of(attention + ((size_t)h * c->B + b0) * N * N * es, N, N);
+      p.nsrc = 1;
+      p.B = b < 0 ? c->B : 1; p.H = c->H; p.W = c->W; p.KH = 1; p.KW = 1;
+      p.Cout = 128; p.Cout_pad = vdim;
+      p.weight = vbuf + ((size_t)b0 * N * vdim + (size_t)h * 128) * es;
+      p.bias = nullptr;
+      if (heads == 1) {
+        char* mrow = reinterpret_cast<char*>(motion) + (size_t)b0 * N * ws.c_motion * es;
+        p.epilogue = PFB_EPI_AXPY; p.scale = x.b->agg_gamma;
+        p.out = mrow; p.out_stride = ws.c_motion; p.out_offset = 128;
+        p.aux_h = mrow; p.hidden = ws.c_motion;
+      } else {
+        p.epilogue = PFB_EPI_LINEAR; p.scale = 1.f;
+        p.out = agg + (size_t)b0 * N * vdim * es; p.out_stride = vdim; p.out_offset = h * 128;
+      }
+      p.dtype = c->dtype; p.impl = c->impl;
+      if (tensor_path) {
+        p.weight_k = vT + ((size_t)b0 * vdim + (size_t)h * 128) * ws.n_pad * es; p.Cin_pad = ws.n_pad; p.Cout_pad_k = 128;
+      }
+      if (b < 0) {
+        // ONE launch for all samples: per-sample weights = that sample's v^T (rows b * vdim + h * 128 ...).  B x 55 row tiles
+        // fill the machine; one launch per sample left only 55 row tiles, a fraction of the machine.
+        p.impl = 2;
+        p.w_rows_per_sample = vdim;
+      }
+      return pfb_conv2d(&p, (pfb_stream)x.s);
+    };
+    for (int h = 0; h < heads; ++h) {
+      if (tensor_path && env_batched) PFB_TRY(attn_v(h, -1));
+      else for (int b = 0; b < c->B; ++b) PFB_TRY(attn_v(h, b));
+    }
+    if (heads > 1) {  // motion_global = motion + gamma * project(out)   gma_utils.py:108-111
+      const pfb_layer& L = x.w->layers[PFB_L_AGG_PROJ];
+      pfb_conv_params p{};
+      p.src[0] = src_of(agg, vdim, vdim);
       p.nsrc = 1;
       p.B = c->B; p.H = c->H; p.W = c->W; p.KH = 1; p.KW = 1;
-      p.Cout = 128; p.Cout_pad = 128;
-      p.weight = vbuf;  // (SIMT layout, unused on this path)
-      p.bias = nullptr;
+      p.Cout = L.Cout; p.Cout_pad = L.Cout_pad;
+      p.weight = L.weight; p.bias = nullptr;
       p.epilogue = PFB_EPI_AXPY; p.scale = x.b->agg_gamma;
       p.out = motion; p.out_stride = ws.c_motion; p.out_offset = 128;
       p.aux_h = motion; p.hidden = ws.c_motion;
-      p.dtype = c->dtype; p.impl = 2;
-      p.weight_k = vT; p.Cin_pad = ws.n_pad; p.Cout_pad_k = 128;
-      p.w_rows_per_sample = 128;
-      PFB_TRY(pfb_conv2d(&p, (pfb_stream)x.s));
-    } else
-    for (int b = 0; b < c->B; ++b) {
-      // one "1x1 convolution" per sample: pixels = queries, input channels = the N attention columns,
-      // weights = this sample's v (SIMT layout [N][128]) / v^T (K-major [128][n_pad])
-      pfb_conv_params p{};
-      p.src[0] = src_of(reinterpret_cast<const char*>(x.b->attention) + (size_t)b * N * N * es, N, N);
-      p.nsrc = 1;
-      p.B = 1; p.H = c->H; p.W = c->W; p.KH = 1; p.KW = 1;
-      p.Cout = 128; p.Cout_pad = 128;
-      p.weight = vbuf + (size_t)b * N * 128 * es;
-      p.bias = nullptr;
-      p.epilogue = PFB_EPI_AXPY; p.scale = x.b->agg_gamma;
-      char* mrow = reinterpret_cast<char*>(motion) + (size_t)b * N * ws.c_motion * es;
-      p.out = mrow; p.out_stride = ws.c_motion; p.out_offset = 128;
-      p.aux_h = mrow; p.hidden = ws.c_motion;
       p.dtype = c->dtype; p.impl = c->impl;
-      if (tensor_path) { p.weight_k = vT + (size_t)b * 128 * ws.n_pad * es; p.Cin_pad = ws.n_pad; p.Cout_pad_k = 128; }
+      p.weight_k = L.weight_k; p.Cin_pad = L.Cin_pad; p.Cout_pad_k = L.Cout_pad_k;
       PFB_TRY(pfb_conv2d(&p, (pfb_stream)x.s));
     }
   }

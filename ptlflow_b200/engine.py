@@ -103,20 +103,35 @@ class RaftEngine:
             layers[_lib.L_FLOW1] = P(None, fh.conv1)
             layers[_lib.L_FLOW2] = P(None, fh.conv2)
         self.agg_gamma = 0.0
-        self.att_q = self.att_k = None
+        self.num_heads = 1
+        self.att_q = self.att_k = self.att_pos = None
         if variant == 2:
             agg = ub.aggregator
+            self.num_heads = agg.heads
             layers[_lib.L_AGG_V] = P([128], agg.to_v)
+            if agg.project is not None:
+                layers[_lib.L_AGG_PROJ] = P([agg.project.weight.shape[1]], agg.project)
             self.agg_gamma = float(agg.gamma.detach().float().cpu().item())
 
-            class _Half:  # q / k halves of Attention.to_qk as separate 1x1 layers (contiguous outputs for the GEMM)
+            class _Half:  # one head's q / k block of Attention.to_qk as a 1x1 layer (contiguous head-major outputs for the GEMM)
                 def __init__(self, w):
                     self.weight, self.bias = w, None
 
             wqk = attention_module.to_qk.weight
             c = wqk.shape[0] // 2
-            self.att_q = ops.PackedConv([_Half(wqk[:c])], dtype, device, src_channels=[wqk.shape[1]])
-            self.att_k = ops.PackedConv([_Half(wqk[c:])], dtype, device, src_channels=[wqk.shape[1]])
+            d = c // self.num_heads  # dim_head
+            cin = [wqk.shape[1]]
+            self.att_q = [ops.PackedConv([_Half(wqk[h * d:(h + 1) * d])], dtype, device, src_channels=cin) for h in range(self.num_heads)]
+            self.att_k = [ops.PackedConv([_Half(wqk[c + h * d:c + (h + 1) * d])], dtype, device, src_channels=cin)
+                          for h in range(self.num_heads)]
+            if attention_module.position_only or attention_module.position_and_content:
+                # per-query position tables of head h: scale * q_h . [rel_height; rel_width] (gma_utils.py:18-30) = a 1x1 layer on
+                # `inp` whose weight is [E_h; E_w] @ W_q,h ((2P-1) * 2 rows, folded in fp64), scale applied by the epilogue
+                pe = attention_module.pos_emb
+                emb = torch.cat([pe.rel_height.weight, pe.rel_width.weight], 0).detach().double()
+                self.att_pos = [ops.PackedConv([_Half((emb @ wqk[h * d:(h + 1) * d, :, 0, 0].detach().double()).float()[:, :, None, None])],
+                                               dtype, device, src_channels=cin) for h in range(self.num_heads)]
+                self.max_pos = pe.rel_height.weight.shape[0] // 2 + 1
         self.layers = layers
         self.weights = _lib.RaftWeights()
         for k, v in layers.items():
@@ -136,7 +151,7 @@ class RaftEngine:
     def make_cfg(self, B: int, H: int, W: int, iters: int, out_hw, pad, alternate_corr: bool, feat_dim: int, volume_layout: int = 0) -> _lib.RaftCfg:
         return _lib.RaftCfg(self.variant, dtype_code(self.dtype), B, H, W, feat_dim, self.corr_levels, self.corr_radius,
                             self.hidden_dim, self.context_dim, iters, int(alternate_corr), out_hw[0], out_hw[1], pad[0], pad[1],
-                            self.impl, 0 if alternate_corr else int(volume_layout), int(getattr(self, "fork_flow", False)))
+                            self.impl, 0 if alternate_corr else int(volume_layout), int(getattr(self, "fork_flow", False)), self.num_heads)
 
     def build_volume(self, fmap1: torch.Tensor, fmap2: torch.Tensor, impl: int = 0):
         """a1 + a2 for the refinement loop of this engine.  f16 / bf16 with tensor-core-shaped features get the tiled
@@ -197,15 +212,17 @@ class RaftEngine:
         return flow_up, flow_small
 
     def update_iter(self, net: torch.Tensor, inp: torch.Tensor, coords: torch.Tensor, corr: Optional[torch.Tensor] = None,
-                    pyramid: Optional[Sequence[torch.Tensor]] = None, want_mask: bool = False):
-        """One update-block evaluation (operator-level tests).  corr: pixel-major [B,H,W,planes]."""
+                    pyramid: Optional[Sequence[torch.Tensor]] = None, want_mask: bool = False, attention: Optional[torch.Tensor] = None):
+        """One update-block evaluation (operator-level tests).  corr: pixel-major [B,H,W,planes]; attention (gma): head-major
+        [heads*B*N, N]."""
         B, H, W, _ = net.shape
         cfg = self.make_cfg(B, H, W, 1, (8 * H, 8 * W), (0, 0), False, 0)
         ws = self.workspace(cfg)
         mask = torch.empty((B, H, W, 576), dtype=self.dtype, device=self.device) if (want_mask and self.variant == 0) else None
         pyr = ptr_array(pyramid) if pyramid is not None else None
         buf = _lib.RaftBuffers(C.cast(pyr, C.POINTER(C.c_void_p)) if pyr is not None else None, None, net.data_ptr(), inp.data_ptr(),
-                               coords.data_ptr(), None, None, ws.data_ptr(), ws.numel(), None, 0.0)
+                               coords.data_ptr(), None, None, ws.data_ptr(), ws.numel(),
+                               attention.data_ptr() if attention is not None else None, self.agg_gamma)
         with torch.cuda.device(self.device):
             check(load().pfb_raft_update_iter(C.byref(cfg), C.byref(self.weights), C.byref(buf),
                                               corr.data_ptr() if corr is not None else None,

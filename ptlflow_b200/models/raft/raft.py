@@ -194,6 +194,9 @@ class RAFT(BaseModel):
     def _attention(self, inp: torch.Tensor, eng):
         return None
 
+    def _check_grid(self, h8: int, w8: int) -> None:
+        """Raises ValueError, before anything is launched, for a 1/8-resolution grid (after padding) the model cannot run."""
+
     def _encode(self, frames: torch.Tensor, B: int):
         """frames: pixel-major [2B,Hp,Wp,3] (frame 1 of every pair first).  Both frames go through fnet as one
         batch (instance norm is per sample, extractor.py:173-176); cnet sees frame 1 only."""
@@ -402,6 +405,8 @@ class RAFT(BaseModel):
             raise RuntimeError("ptlflow_b200 runs on CUDA (sm_90a) only: move the model and inputs to the GPU. There is no CPU path.")
         if torch.is_grad_enabled() and any(p.requires_grad for p in self.update_block.parameters()) and self.training:
             raise NotImplementedError("ptlflow_b200 implements the inference hot path; call under torch.no_grad() / model.eval()")
+        stride = self.output_stride
+        self._check_grid(-(-images.shape[-2] // stride), -(-images.shape[-1] // stride))
         with torch.no_grad(), torch.cuda.device(images.device):
             images = images.contiguous()
             flow_init = None

@@ -325,6 +325,34 @@ def softmax_rows(x: torch.Tensor) -> torch.Tensor:
     return x
 
 
+def attention_softmax_relpos(logits: Optional[torch.Tensor], th: torch.Tensor, tw: torch.Tensor, H: int, W: int, P: int,
+                             out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """GMA attention with the relative-position term (gma_utils.py:6-30, 62-74): row r of the result ([rows, H*W], rows =
+    heads*B*H*W head-major) is softmax over (u, v) of ``logits[r, u*W+v] + th[r, u-x+P-1] + tw[r, v-y+P-1]`` for the query
+    (x, y) = divmod(r % (H*W), W).  ``logits``: content logits in the storage dtype or None (position only); may be ``out``.
+    ``th``, ``tw``: fp32 [rows, 2P-1] views with unit column stride and one shared row stride."""
+    if not (th.is_cuda and tw.is_cuda):
+        raise RuntimeError("attention_softmax_relpos: th / tw must be CUDA tensors")
+    rows = th.shape[0]
+    if th.dtype != torch.float32 or tw.dtype != torch.float32 or th.shape != (rows, 2 * P - 1) or tw.shape != th.shape \
+            or th.stride() != tw.stride() or th.stride(1) != 1:
+        raise RuntimeError("attention_softmax_relpos: th / tw must be fp32 [rows, 2P-1] views with equal strides")
+    if logits is not None:
+        require_cuda(logits, "logits")
+        if logits.shape != (rows, H * W):
+            raise RuntimeError(f"attention_softmax_relpos: logits {tuple(logits.shape)} != ({rows}, {H * W})")
+    if out is None:
+        out = torch.empty((rows, H * W), dtype=logits.dtype if logits is not None else torch.float32, device=th.device)
+    require_cuda(out, "out")
+    if logits is not None and out.dtype != logits.dtype:
+        raise RuntimeError("attention_softmax_relpos: logits and out must share the storage dtype")
+    with torch.cuda.device(th.device):
+        check(load().pfb_attention_softmax_relpos(logits.data_ptr() if logits is not None else None, th.data_ptr(), tw.data_ptr(),
+                                                  th.stride(0), out.data_ptr(), rows, H, W, P, dtype_code(out.dtype),
+                                                  stream_ptr(th.device)), "attention_softmax_relpos")
+    return out
+
+
 def init_coords(B: int, H: int, W: int, device, flow_init: Optional[torch.Tensor] = None) -> torch.Tensor:
     coords = torch.empty((B, H, W, 2), dtype=torch.float32, device=device)
     fi = None
