@@ -167,8 +167,14 @@ typedef enum {
                           next two columns                          update.py:111-112      */
   PFB_EPI_AXPY = 6,    /* out = residual + scale * (acc + bias); residual = aux_h[p * hidden + n]
                           (GMA Aggregate: fmap + gamma * attn@v)    gma_utils.py:101-113   */
-  PFB_EPI_LINEAR_F32 = 7 /* out(fp32) = scale * (acc + bias): per-tap partial products of the flow head's
+  PFB_EPI_LINEAR_F32 = 7, /* out(fp32) = scale * (acc + bias): per-tap partial products of the flow head's
                           last convolution, summed over the 3x3 neighbourhood by pfb_flow_tap_gather */
+  PFB_EPI_GELU = 8,    /* out = gelu(acc + bias), exact erf GELU (F.gelu default)   skflow/update.py:20-29 */
+  PFB_EPI_RESIDUAL_GELU = 9, /* y = gelu(res + acc + bias), res = residual[p * residual_stride + residual_offset + n];
+                          then, if post_w != NULL, out = gelu(y * (1 + post_w[n]) + post_b[n]) (a following depthwise
+                          1x1 step x = gelu(x + dw1(x)) of a PCBlock, skflow/update.py:32-34), else out = y */
+  PFB_EPI_LINEAR_APPEND_FLOW = 10 /* linear into cols [0,Cout) and flow (fp32 [.,2]) into the next two columns
+                          (SKFlow motion encoder: cat[conv(cor_flo), flow], skflow/update.py:53-61) */
 } pfb_epilogue;
 
 typedef struct {
@@ -212,6 +218,12 @@ typedef struct {
    * of weight_k [B * w_rows_per_sample][Cin_pad] -- one launch for all samples of "attention @ v" (gma_utils.py:101-113),
    * where the "weights" are the sample's transposed v.  0 = one weight matrix for all samples. */
   int w_rows_per_sample;
+  /* PFB_EPI_RESIDUAL_GELU: the residual operand [B,H,W,residual_stride] dtype (fp32 when dtype is fp32), channels from
+   * residual_offset, and the optional per-channel fp32 step post_w / post_b [Cout] (both NULL or both set) */
+  const void* residual;
+  int residual_stride, residual_offset;
+  const float* post_w;
+  const float* post_b;
 } pfb_conv_params;
 
 PFB_API int pfb_conv2d(const pfb_conv_params* p, pfb_stream stream);
@@ -229,6 +241,15 @@ PFB_API int pfb_pack_bias(const void* src, float* dst, int n, int offset, pfb_dt
 PFB_API int pfb_pack_conv_weight_kmajor(const void* src, void* dst, int Cout, int Cin, int KH, int KW, int Cout_pad_k,
                                         int row_offset, const int* src_channels, int nsrc, int Cin_pad,
                                         pfb_dtype src_dtype, pfb_dtype dst_dtype, pfb_stream stream);
+
+/* Depthwise k x k convolution with its PCBlock residual and activation (skflow/update.py:32-33):
+ *   out[p, c] = gelu(x[p, c] + bias[c] + sum_{ky, kx} weight[ky * k + kx][c] * x[p + (ky - k/2, kx - k/2), c])
+ * stride 1, zero "same" padding, any odd k <= 31 (grids smaller than the kernel included), C % 2 == 0.
+ * x: [B,H,W,in_stride] from channel in_offset; out: [B,H,W,out_stride] from out_offset (must not overlap x); offsets and
+ * strides even.  weight [k*k][C], bias [C]: fp32.  dtype is the storage type of x / out; accumulation is fp32. */
+PFB_API int pfb_depthwise_conv_gelu(const void* x, int in_stride, int in_offset, void* out, int out_stride, int out_offset,
+                                    const float* weight, const float* bias, int B, int H, int W, int C, int k, pfb_dtype dtype,
+                                    pfb_stream stream);
 
 /* ------------------------------------------------------------------------------------
  * a10: upsampling
@@ -356,6 +377,52 @@ PFB_API int pfb_raft_update_iter(const pfb_raft_cfg* cfg, const pfb_raft_weights
                          const void* corr, void* mask_out, pfb_stream stream);
 
 /* ------------------------------------------------------------------------------------
+ * a15: SKFlow's refinement loop (SKUpdateBlock6_Deep_nopoolres_AllDecoder + the GMA loop)
+ *   ptlflow/models/skflow/update.py:7-99, ptlflow/models/skflow/skflow.py:197-232
+ * pfb_raft_cfg with variant = 3 (accepted by the pfb_skflow_* entry points only), hidden = context = 128, any num_heads;
+ * pfb_raft_buffers as for gma (attention and agg_gamma are required).
+ * ---------------------------------------------------------------------------------- */
+#define PFB_SK_MAX_DW 8
+/* PCBlock4_Deep_nopool_res(C_in, C_out, k_conv), every activation padded to C = align(C_in, 32) channels whose padding stays
+ * exactly zero (zero weights and biases), the FFN hidden width to hid = align(int(1.5 * C_in), 32):
+ *   x = gelu(x + ffn1b(gelu(ffn1a(x))));  x = gelu(x + dw_k(x)) for k in k_conv;  x = gelu(x + pw(x));  out = ffn2b(gelu(ffn2a(x)))
+ * ffn1a: 1x1 C -> hid, ffn1b: hid -> C, pw: C -> C, ffn2a: C -> hid, ffn2b: hid -> C_out (pfb_layer packing as in the raft
+ * loop).  dw_weight[i] [k*k][C], dw_bias[i] [C] fp32.  When dw_k[0] == 1 that step rides ffn1b's epilogue. */
+typedef struct {
+  pfb_layer ffn1a, ffn1b, pw, ffn2a, ffn2b;
+  int C, hid;
+  int n_dw;
+  int dw_k[PFB_SK_MAX_DW];
+  const float* dw_weight[PFB_SK_MAX_DW];
+  const float* dw_bias[PFB_SK_MAX_DW];
+} pfb_pc_block;
+
+typedef enum {
+  PFB_SK_CONVC1 = 0, /* encoder.convc1: planes -> 256 (followed by a GELU) */
+  PFB_SK_CONVC2,     /* encoder.convc2: 256 -> 192 */
+  PFB_SK_CONVF2,     /* encoder.convf2: 128 -> 64 */
+  PFB_SK_CONV,       /* encoder.conv: 256 -> 126 (+ flow) */
+  PFB_SK_GRU,        /* gru: [net | inp | motion | motion_global] 512 -> 128, k_conv = PCUpdater_conv */
+  PFB_SK_FLOW_HEAD,  /* flow_head: 128 -> 2 */
+  PFB_SK_BLOCKS
+} pfb_skflow_block_id;
+
+typedef struct {
+  pfb_pc_block blocks[PFB_SK_BLOCKS];
+  pfb_layer convf1;           /* encoder.convf1: 1x1 2 -> 128 on the fp32 flow, no activation */
+  pfb_layer mask1, mask2;     /* mask.0 (3x3 128 -> 256, ReLU), mask.2 (1x1 256 -> 576, x0.25) */
+  pfb_layer agg_v, agg_proj;  /* aggregator.to_v, aggregator.project (num_heads > 1) */
+} pfb_skflow_weights;
+
+PFB_API size_t pfb_skflow_workspace_bytes(const pfb_raft_cfg* cfg);
+/* cfg->iters update iterations, then the convex upsample (mask head on the last iteration only). */
+PFB_API int pfb_skflow_refine(const pfb_raft_cfg* cfg, const pfb_skflow_weights* w, const pfb_raft_buffers* buf, pfb_stream stream);
+/* One update iteration without the upsample; corr (pixel-major [B,H,W,corr_stride], columns past the planes zero, where
+ * corr_stride = align(planes, 32)) replaces the lookup when non-NULL; mask_out [B,H,W,576] may be NULL. */
+PFB_API int pfb_skflow_update_iter(const pfb_raft_cfg* cfg, const pfb_skflow_weights* w, const pfb_raft_buffers* buf,
+                                   const void* corr, void* mask_out, pfb_stream stream);
+
+/* ------------------------------------------------------------------------------------
  * Encoder-side kernels (SURVEY.md section 8(f) rank 1: the callers either side of the path).
  * The 3x3 / 7x7 / 1x1 convolutions of BasicEncoder / SmallEncoder (extractor.py:122-267) still run in
  * cuDNN; pre-processing, instance norm + ReLU (+ residual) and the residual joins are fused here.
@@ -406,11 +473,11 @@ PFB_API int pfb_bias_act(const void* x, const float* bias, const void* residual,
  * Measurement hooks (bench.py): launch accounting and live per-kernel-class timing.
  * kernel_class: 0 volume, 1 pool, 2 lookup, 3 on-the-fly lookup, 4 update-block conv (wgmma / SIMT), 5 upsample,
  * 6 misc (packing, coords, softmax, transposes), 7 encoder normalise / bias / activation passes, 8 encoder instance-norm
- * statistics, 9 first encoder convolution (wgmma), 10 convf1 (7x7 on the flow, wgmma), 11 flow-head tap gather;
- * -1 = all.  pfb_profile_collect synchronises the device, writes summed milliseconds and span
+ * statistics, 9 first encoder convolution (wgmma), 10 convf1 (7x7 on the flow, wgmma), 11 flow-head tap gather,
+ * 12 depthwise convolution (SKFlow); -1 = all.  pfb_profile_collect synchronises the device, writes summed milliseconds and span
  * counts per class (arrays of >= PFB_KERNEL_CLASSES entries) and clears the recorded spans.
  * ---------------------------------------------------------------------------------- */
-#define PFB_KERNEL_CLASSES 12
+#define PFB_KERNEL_CLASSES 13
 PFB_API unsigned long long pfb_launch_count(int kernel_class);
 PFB_API int pfb_profile_enable(int on);
 PFB_API int pfb_profile_collect(double* ms, unsigned long long* n, int len);

@@ -23,6 +23,7 @@ F32, F16, BF16 = 0, 1, 2
 _DTYPES = {torch.float32: F32, torch.float16: F16, torch.bfloat16: BF16}
 
 EPI_LINEAR, EPI_RELU, EPI_GRU_ZR, EPI_GRU_Q, EPI_FLOW, EPI_RELU_APPEND_FLOW, EPI_AXPY, EPI_LINEAR_F32 = range(8)
+EPI_GELU, EPI_RESIDUAL_GELU, EPI_LINEAR_APPEND_FLOW = range(8, 11)
 
 (L_CONVC1, L_CONVC2, L_CONVF1, L_CONVF2, L_CONV, L_GRU_ZR1, L_GRU_Q1, L_GRU_ZR2, L_GRU_Q2,
  L_FLOW1, L_FLOW2, L_MASK1, L_MASK2, L_AGG_V, L_FLOW2T,
@@ -46,6 +47,8 @@ class ConvParams(C.Structure):
         ("dtype", C.c_int), ("impl", C.c_int),
         ("weight_k", C.c_void_p), ("Cin_pad", C.c_int), ("Cout_pad_k", C.c_int),
         ("addend", C.c_void_p), ("addend_stride", C.c_int), ("w_rows_per_sample", C.c_int),
+        ("residual", C.c_void_p), ("residual_stride", C.c_int), ("residual_offset", C.c_int),
+        ("post_w", C.c_void_p), ("post_b", C.c_void_p),
     ]
 
 
@@ -76,6 +79,23 @@ class RaftBuffers(C.Structure):
         ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
         ("attention", C.c_void_p), ("agg_gamma", C.c_float),
     ]
+
+
+# SKFlow (include/ptlflow_b200.h, a15)
+PFB_SK_MAX_DW = 8
+SK_CONVC1, SK_CONVC2, SK_CONVF2, SK_CONV, SK_GRU, SK_FLOW_HEAD, SK_BLOCKS = range(7)
+KERNEL_CLASSES = 13  # PFB_KERNEL_CLASSES (12 = depthwise convolution)
+
+
+class PcBlock(C.Structure):
+    _fields_ = [("ffn1a", Layer), ("ffn1b", Layer), ("pw", Layer), ("ffn2a", Layer), ("ffn2b", Layer),
+                ("C", C.c_int), ("hid", C.c_int), ("n_dw", C.c_int), ("dw_k", C.c_int * PFB_SK_MAX_DW),
+                ("dw_weight", C.c_void_p * PFB_SK_MAX_DW), ("dw_bias", C.c_void_p * PFB_SK_MAX_DW)]
+
+
+class SkflowWeights(C.Structure):
+    _fields_ = [("blocks", PcBlock * SK_BLOCKS), ("convf1", Layer), ("mask1", Layer), ("mask2", Layer),
+                ("agg_v", Layer), ("agg_proj", Layer)]
 
 
 _lib: Optional[C.CDLL] = None
@@ -128,6 +148,10 @@ SIGNATURES = {
     "pfb_profile_enable": (_I, [_I]),
     "pfb_profile_collect": (_I, [C.POINTER(C.c_double), C.POINTER(C.c_ulonglong), _I]),
     "pfb_raft_update_iter": (_I, [C.POINTER(RaftCfg), C.POINTER(RaftWeights), C.POINTER(RaftBuffers), _P, _P, _S]),
+    "pfb_depthwise_conv_gelu": (_I, [_P, _I, _I, _P, _I, _I, _P, _P, _I, _I, _I, _I, _I, _I, _S]),
+    "pfb_skflow_workspace_bytes": (C.c_size_t, [C.POINTER(RaftCfg)]),
+    "pfb_skflow_refine": (_I, [C.POINTER(RaftCfg), C.POINTER(SkflowWeights), C.POINTER(RaftBuffers), _S]),
+    "pfb_skflow_update_iter": (_I, [C.POINTER(RaftCfg), C.POINTER(SkflowWeights), C.POINTER(RaftBuffers), _P, _P, _S]),
 }
 
 

@@ -62,6 +62,8 @@ __device__ __forceinline__ void store_from_f32(void* p, size_t i, int dt, float 
 }
 
 __device__ __forceinline__ float sigmoid_f32(float x) { return 1.0f / (1.0f + expf(-x)); }
+// exact (erf) GELU, the default of F.gelu / nn.GELU
+__device__ __forceinline__ float gelu_f32(float x) { return 0.5f * x * (1.0f + erff(x * 0.70710678118654752f)); }
 
 // Dispatch a templated launcher on the storage dtype.
 #define PFB_DISPATCH_DTYPE(dt, T, ...)                        \
@@ -104,7 +106,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 }
 
 enum KernelClass { KC_VOLUME = 0, KC_POOL, KC_LOOKUP, KC_ONTHEFLY, KC_CONV, KC_UPSAMPLE, KC_MISC,
-                   KC_ENC_AFFINE, KC_ENC_STATS, KC_ENC_CONV1, KC_FLOWCONV, KC_GATHER, KC_COUNT };
+                   KC_ENC_AFFINE, KC_ENC_STATS, KC_ENC_CONV1, KC_FLOWCONV, KC_GATHER, KC_DEPTHWISE, KC_COUNT };
 class ProfScope {
  public:
   ProfScope(int kc, cudaStream_t s);

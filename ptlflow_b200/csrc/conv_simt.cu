@@ -28,6 +28,10 @@ struct ConvDev {
   int hidden;
   float* coords;
   const float* flow;
+  const void* residual;
+  int residual_stride, residual_offset;
+  const float* post_w;
+  const float* post_b;
 };
 
 template <typename T>
@@ -176,6 +180,19 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvDev a) {
         case PFB_EPI_RELU_APPEND_FLOW:
           reinterpret_cast<T*>(a.out)[(size_t)p * a.out_stride + a.out_offset + n] = from_f32<T>(fmaxf(v, 0.f));
           break;
+        case PFB_EPI_LINEAR_APPEND_FLOW:
+          reinterpret_cast<T*>(a.out)[(size_t)p * a.out_stride + a.out_offset + n] = from_f32<T>(v);
+          break;
+        case PFB_EPI_GELU:
+          reinterpret_cast<T*>(a.out)[(size_t)p * a.out_stride + a.out_offset + n] = from_f32<T>(gelu_f32(v));
+          break;
+        case PFB_EPI_RESIDUAL_GELU: {
+          const float res = to_f32(reinterpret_cast<const T*>(a.residual)[(size_t)p * a.residual_stride + a.residual_offset + n]);
+          float y = gelu_f32(res + v);
+          if (a.post_w) y = gelu_f32(fmaf(y, 1.f + a.post_w[n], a.post_b[n]));
+          reinterpret_cast<T*>(a.out)[(size_t)p * a.out_stride + a.out_offset + n] = from_f32<T>(y);
+          break;
+        }
         case PFB_EPI_GRU_ZR: {
           float g = sigmoid_f32(v);
           if (n < hd) {
@@ -213,7 +230,7 @@ __global__ void __launch_bounds__(256) conv_simt_kernel(const ConvDev a) {
           break;
       }
     }
-    if (a.epilogue == PFB_EPI_RELU_APPEND_FLOW && blockIdx.y == 0 && tx == 0) {
+    if ((a.epilogue == PFB_EPI_RELU_APPEND_FLOW || a.epilogue == PFB_EPI_LINEAR_APPEND_FLOW) && blockIdx.y == 0 && tx == 0) {
       T* o = reinterpret_cast<T*>(a.out) + (size_t)p * a.out_stride + a.out_offset + a.Cout;
       o[0] = from_f32<T>(a.flow[(size_t)p * 2]);
       o[1] = from_f32<T>(a.flow[(size_t)p * 2 + 1]);
@@ -238,6 +255,8 @@ int conv2d_simt(const pfb_conv_params* p, cudaStream_t s) {
   a.weight = p->weight; a.bias = p->bias; a.epilogue = p->epilogue; a.scale = p->scale;
   a.out = p->out; a.out_stride = p->out_stride; a.out_offset = p->out_offset;
   a.aux_h = p->aux_h; a.aux_z = p->aux_z; a.hidden = p->hidden; a.coords = p->coords; a.flow = p->flow;
+  a.residual = p->residual; a.residual_stride = p->residual_stride; a.residual_offset = p->residual_offset;
+  a.post_w = p->post_w; a.post_b = p->post_b;
   const int P = p->B * p->H * p->W;
   // small images: smaller pixel tiles until the grid covers the machine (each CTA's K loop is a latency chain)
   const int n_tiles = ceil_div(p->Cout, 64), sms = sm_count();
@@ -270,7 +289,12 @@ extern "C" PFB_API int pfb_conv2d(const pfb_conv_params* p, pfb_stream stream) {
                   "conv2d: bad source %d", i);
   }
   switch (p->epilogue) {
-    case PFB_EPI_LINEAR: case PFB_EPI_RELU: case PFB_EPI_LINEAR_F32: break;
+    case PFB_EPI_LINEAR: case PFB_EPI_RELU: case PFB_EPI_LINEAR_F32: case PFB_EPI_GELU: break;
+    case PFB_EPI_RESIDUAL_GELU:
+      PFB_CHECK_ARG(p->residual && p->residual_stride >= p->residual_offset + p->Cout && p->residual_offset >= 0,
+                    "conv2d: RESIDUAL_GELU needs a residual with stride >= offset + Cout");
+      PFB_CHECK_ARG((p->post_w == nullptr) == (p->post_b == nullptr), "conv2d: RESIDUAL_GELU needs both post_w and post_b, or neither");
+      break;
     case PFB_EPI_AXPY:
       PFB_CHECK_ARG(p->aux_h && p->hidden >= p->Cout, "conv2d: AXPY needs aux_h (residual) with stride hidden >= Cout");
       break;
@@ -284,6 +308,7 @@ extern "C" PFB_API int pfb_conv2d(const pfb_conv_params* p, pfb_stream stream) {
       PFB_CHECK_ARG(p->coords && p->Cout == 2, "conv2d: FLOW epilogue needs coords and Cout == 2");
       break;
     case PFB_EPI_RELU_APPEND_FLOW:
+    case PFB_EPI_LINEAR_APPEND_FLOW:
       PFB_CHECK_ARG(p->flow && p->out_stride >= p->out_offset + p->Cout + 2, "conv2d: APPEND_FLOW needs flow and room for 2 channels");
       break;
     default:

@@ -75,6 +75,10 @@ struct ConvUmmaArgs {
   int w_rows_per_sample;         // > 0: every sample b has its own weight matrix, rows [b * w_rows_per_sample, ...) of the weight map
   const void* addend;            // optional per-pixel pre-activation term [B*H*W][addend_stride] (storage type), added instead of the bias
   int addend_stride;
+  const void* residual;          // PFB_EPI_RESIDUAL_GELU: residual operand [B*H*W][residual_stride] (storage type) from residual_offset
+  int residual_stride, residual_offset;
+  const float* post_w;           // PFB_EPI_RESIDUAL_GELU: optional per-channel second step gelu(y * (1 + post_w) + post_b)
+  const float* post_b;
   int ab_fmt;
   int tma_out;                   // 1: outputs leave through shared-memory staging + TMA bulk stores (tmO0 = out, tmO1 = aux_z)
   unsigned long long* trace;     // debug timeline (PFB_CONV_TRACE): 32 clock64 slots per CTA, null in production
@@ -235,7 +239,8 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
                  const __grid_constant__ CUtensorMap tmO0, const __grid_constant__ CUtensorMap tmO1, const ConvUmmaArgs a) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // only the plain epilogues stage their outputs (compile-time: the gate instantiations carry none of the staging state)
-  constexpr bool kPlain = EPI == PFB_EPI_LINEAR || EPI == PFB_EPI_RELU || EPI == PFB_EPI_RELU_APPEND_FLOW;
+  constexpr bool kPlain = EPI == PFB_EPI_LINEAR || EPI == PFB_EPI_RELU || EPI == PFB_EPI_RELU_APPEND_FLOW || EPI == PFB_EPI_GELU ||
+                          EPI == PFB_EPI_LINEAR_APPEND_FLOW;
   const bool tma_out = kPlain && a.tma_out;
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* smemA = smem;
@@ -373,12 +378,14 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
       // Operands that do not depend on the accumulator (h, z, residual) are requested BEFORE waiting for the MMAs
       // of this tile, and the next chunk's while the current one is processed (exposed L2 latency otherwise makes the
       // GRU layers epilogue-bound).
-      const bool aux_h_any = EPI == PFB_EPI_GRU_ZR || EPI == PFB_EPI_GRU_Q || EPI == PFB_EPI_AXPY;
+      const bool aux_h_any = EPI == PFB_EPI_GRU_ZR || EPI == PFB_EPI_GRU_Q || EPI == PFB_EPI_AXPY || EPI == PFB_EPI_RESIDUAL_GELU;
       auto issue_h = [&](int c, uint4 (&hq)[4]) {
         const int n = n0 + c;
-        const bool need_h = ok && ((EPI == PFB_EPI_GRU_ZR && n >= hd) || EPI == PFB_EPI_GRU_Q || (EPI == PFB_EPI_AXPY && n + 32 <= a.Cout));
+        const bool need_h = ok && ((EPI == PFB_EPI_GRU_ZR && n >= hd) || EPI == PFB_EPI_GRU_Q || ((EPI == PFB_EPI_AXPY || EPI == PFB_EPI_RESIDUAL_GELU) && n + 32 <= a.Cout));
         if (need_h) {
-          const T* hp = reinterpret_cast<const T*>(a.aux_h) + p * hd + (EPI == PFB_EPI_GRU_ZR ? n - hd : n);
+          const T* hp = EPI == PFB_EPI_RESIDUAL_GELU
+                            ? reinterpret_cast<const T*>(a.residual) + p * a.residual_stride + a.residual_offset + n
+                            : reinterpret_cast<const T*>(a.aux_h) + p * hd + (EPI == PFB_EPI_GRU_ZR ? n - hd : n);
 #pragma unroll
           for (int q = 0; q < 4; ++q) hq[q] = reinterpret_cast<const uint4*>(hp)[q];
         }
@@ -501,9 +508,40 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
             if (!tma_out) store32<T>(out + p * a.out_stride + a.out_offset + n, v, a.Cout - n);
             break;
           }
-          case PFB_EPI_RELU_APPEND_FLOW: {
+          case PFB_EPI_GELU: {
 #pragma unroll
-            for (int e = 0; e < 32; ++e) v[e] = fmaxf(v[e], 0.f);
+            for (int e = 0; e < 32; ++e) v[e] = gelu_f32(v[e]);
+            if (!tma_out) store32<T>(out + p * a.out_stride + a.out_offset + n, v, a.Cout - n);
+            break;
+          }
+          case PFB_EPI_RESIDUAL_GELU: {  // gelu(residual + acc + bias) (+ the optional per-channel step)
+#pragma unroll
+            for (int q = 0; q < 4; ++q) {
+              float h[8];
+              unpack8<T>(hraw[q], h);
+#pragma unroll
+              for (int e = 0; e < 8; ++e) v[8 * q + e] = gelu_f32(h[e] + v[8 * q + e]);
+            }
+            if (a.post_w) {  // warp-uniform
+#pragma unroll
+              for (int q = 0; q < 8; ++q) {
+                const float4 w4 = __ldg(reinterpret_cast<const float4*>(a.post_w + n) + q);
+                const float4 b4 = __ldg(reinterpret_cast<const float4*>(a.post_b + n) + q);
+                v[4 * q + 0] = gelu_f32(fmaf(v[4 * q + 0], 1.f + w4.x, b4.x));
+                v[4 * q + 1] = gelu_f32(fmaf(v[4 * q + 1], 1.f + w4.y, b4.y));
+                v[4 * q + 2] = gelu_f32(fmaf(v[4 * q + 2], 1.f + w4.z, b4.z));
+                v[4 * q + 3] = gelu_f32(fmaf(v[4 * q + 3], 1.f + w4.w, b4.w));
+              }
+            }
+            if (!tma_out) store32<T>(out + p * a.out_stride + a.out_offset + n, v, a.Cout - n);
+            break;
+          }
+          case PFB_EPI_RELU_APPEND_FLOW:
+          case PFB_EPI_LINEAR_APPEND_FLOW: {
+            if (EPI == PFB_EPI_RELU_APPEND_FLOW) {
+#pragma unroll
+              for (int e = 0; e < 32; ++e) v[e] = fmaxf(v[e], 0.f);
+            }
             int valid = a.Cout - n;
             if (valid > 0 && valid <= 30) {  // the chunk that holds the last real channel also takes the 2 flow columns
               const float fx = a.flow[2 * p], fy = a.flow[2 * p + 1];
@@ -626,7 +664,13 @@ bool conv2d_umma_supported(const pfb_conv_params* p) {
   }
   if (cin_pad != p->Cin_pad) return false;
   switch (p->epilogue) {
-    case PFB_EPI_LINEAR: case PFB_EPI_RELU: case PFB_EPI_RELU_APPEND_FLOW: break;
+    case PFB_EPI_LINEAR: case PFB_EPI_RELU: case PFB_EPI_RELU_APPEND_FLOW: case PFB_EPI_GELU: case PFB_EPI_LINEAR_APPEND_FLOW: break;
+    case PFB_EPI_RESIDUAL_GELU:
+      if (!p->residual || p->residual_stride % 8 || p->residual_offset % 8 || p->Cout % 32 ||
+          (reinterpret_cast<uintptr_t>(p->residual) & 15))
+        return false;
+      if (p->post_w && ((reinterpret_cast<uintptr_t>(p->post_w) & 15) || (reinterpret_cast<uintptr_t>(p->post_b) & 15))) return false;
+      break;
     case PFB_EPI_LINEAR_F32:
       if (p->out_stride % 4 || p->out_offset % 4) return false;
       break;
@@ -683,6 +727,9 @@ static int launch_conv_umma(const CUtensorMap* tms, const CUtensorMap& tmW, cons
     case PFB_EPI_RELU_APPEND_FLOW: return launch_conv_umma_e<T, PFB_EPI_RELU_APPEND_FLOW>(tms, tmW, tmO, a, grid, smem, s);
     case PFB_EPI_AXPY: return launch_conv_umma_e<T, PFB_EPI_AXPY>(tms, tmW, tmO, a, grid, smem, s);
     case PFB_EPI_LINEAR_F32: return launch_conv_umma_e<T, PFB_EPI_LINEAR_F32>(tms, tmW, tmO, a, grid, smem, s);
+    case PFB_EPI_GELU: return launch_conv_umma_e<T, PFB_EPI_GELU>(tms, tmW, tmO, a, grid, smem, s);
+    case PFB_EPI_RESIDUAL_GELU: return launch_conv_umma_e<T, PFB_EPI_RESIDUAL_GELU>(tms, tmW, tmO, a, grid, smem, s);
+    case PFB_EPI_LINEAR_APPEND_FLOW: return launch_conv_umma_e<T, PFB_EPI_LINEAR_APPEND_FLOW>(tms, tmW, tmO, a, grid, smem, s);
     default: break;
   }
   set_error("conv_umma: epilogue %d has no tensor-core instantiation", a.epilogue);
@@ -757,7 +804,8 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
   a.b_tap_bytes = a.NT * 128;
   {
     static const int env_tma_out = getenv("PFB_CONV_TMA_STORE") ? atoi(getenv("PFB_CONV_TMA_STORE")) : 1;
-    const bool plain = p->epilogue == PFB_EPI_LINEAR || p->epilogue == PFB_EPI_RELU || p->epilogue == PFB_EPI_RELU_APPEND_FLOW;
+    const bool plain = p->epilogue == PFB_EPI_LINEAR || p->epilogue == PFB_EPI_RELU || p->epilogue == PFB_EPI_RELU_APPEND_FLOW ||
+                       p->epilogue == PFB_EPI_GELU || p->epilogue == PFB_EPI_LINEAR_APPEND_FLOW;
     // a staged store writes whole 64-channel blocks: with several N tiles of NT % 64 == 32 the last block of a tile would
     // overwrite the first 32 channels of the next one (a single tile is clipped at the layer's last channel by the tensor map)
     a.tma_out = env_tma_out && plain && (reinterpret_cast<uintptr_t>(p->out) & 15) == 0 && (a.NT % 64 == 0 || a.n_tiles == 1);
@@ -780,7 +828,8 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
   {
     const bool zr = p->epilogue == PFB_EPI_GRU_ZR;
     if (a.tma_out) {
-      const int ncols = zr ? p->hidden : (p->epilogue == PFB_EPI_RELU_APPEND_FLOW ? p->Cout + 2 : p->Cout);
+      const bool append = p->epilogue == PFB_EPI_RELU_APPEND_FLOW || p->epilogue == PFB_EPI_LINEAR_APPEND_FLOW;
+      const int ncols = zr ? p->hidden : (append ? p->Cout + 2 : p->Cout);
       uint64_t dims[4] = {(uint64_t)(p->out_offset + ncols), (uint64_t)p->W, (uint64_t)p->H, (uint64_t)p->B};
       uint64_t str[3] = {(uint64_t)p->out_stride * 2, (uint64_t)p->W * p->out_stride * 2, (uint64_t)p->H * p->W * p->out_stride * 2};
       uint32_t box[4] = {64, (uint32_t)a.TW, (uint32_t)a.TH, 1};
@@ -817,6 +866,8 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
   a.out = p->out; a.out_stride = p->out_stride; a.out_offset = p->out_offset;
   a.aux_h = p->aux_h; a.aux_z = p->aux_z; a.hidden = p->hidden; a.flow = p->flow;
   a.addend = p->addend; a.addend_stride = p->addend_stride;
+  a.residual = p->residual; a.residual_stride = p->residual_stride; a.residual_offset = p->residual_offset;
+  a.post_w = p->post_w; a.post_b = p->post_b;
   a.w_rows_per_sample = p->w_rows_per_sample;
   a.ab_fmt = p->dtype == PFB_F16 ? 0 : 1;
   const size_t smem = (size_t)a.a_stages * a.a_slot_bytes + (size_t)a.b_stages * a.b_slot_bytes + (a.tma_out ? kATileBytes : 0) +

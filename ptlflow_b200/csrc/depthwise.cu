@@ -1,0 +1,164 @@
+// Depthwise k x k convolution fused with the residual and the GELU of SKFlow's PCBlock (skflow/update.py:32-33):
+//   out[p, c] = gelu(x[p, c] + bias[c] + sum_{ky, kx} w[ky][kx][c] * x[p + (ky - k/2, kx - k/2), c])
+// CUDA-core work (one multiply-add per tap and channel, nothing for the tensor cores to share).  A CTA owns an 8 x 16 pixel
+// tile of CC channels: the tile plus its halo is staged once in shared memory as fp32 (zero outside the image, which is the
+// "same" padding), next to the fp32 weights of those channels.  A thread owns a channel pair and a strip of R = 8 consecutive
+// pixels of one row; per filter row it loads the R + k - 1 input pairs of that row once into registers and slides the k taps
+// over them, so every staged value is read from shared memory k times fewer than a per-output loop would.
+#include <atomic>
+
+#include "common.cuh"
+
+namespace pfb {
+
+template <typename T> struct Pair;
+template <> struct Pair<float> {
+  using V = float2;
+  static __device__ __forceinline__ float2 f2(V v) { return v; }
+  static __device__ __forceinline__ V from(float a, float b) { return make_float2(a, b); }
+};
+template <> struct Pair<__half> {
+  using V = __half2;
+  static __device__ __forceinline__ float2 f2(V v) { return __half22float2(v); }
+  static __device__ __forceinline__ V from(float a, float b) { return __floats2half2_rn(a, b); }
+};
+template <> struct Pair<__nv_bfloat16> {
+  using V = __nv_bfloat162;
+  static __device__ __forceinline__ float2 f2(V v) { return __bfloat1622float2(v); }
+  static __device__ __forceinline__ V from(float a, float b) { return __floats2bfloat162_rn(a, b); }
+};
+
+constexpr int kDwTH = 8, kDwR = 8, kDwSX = 2, kDwTW = kDwR * kDwSX;  // output tile: 8 rows x 16 columns
+// channels per CTA: 32 up to k = 15 (two CTAs of 110 KB per SM at k = 15); 8 above, where the halo tile grows quadratically
+__host__ __device__ constexpr int dw_cc(int K) { return K <= 15 ? 32 : 8; }
+__host__ __device__ constexpr int dw_threads(int K) { return dw_cc(K) / 2 * kDwSX * kDwTH; }
+__host__ __device__ constexpr size_t dw_smem(int K) {
+  return ((size_t)(kDwTH + K - 1) * (kDwTW + K - 1) + (size_t)K * K) * dw_cc(K) * sizeof(float);
+}
+
+template <typename T, int K>
+__global__ void __launch_bounds__(dw_threads(K)) depthwise_gelu_kernel(const T* __restrict__ x, int in_stride, T* __restrict__ out,
+                                                                      int out_stride, const float* __restrict__ wgt,
+                                                                      const float* __restrict__ bias, int H, int W, int C, int tiles_x) {
+  constexpr int CC = dw_cc(K), NP = CC / 2, THR = dw_threads(K);
+  constexpr int PH = kDwTH + K - 1, PW = kDwTW + K - 1;
+  using V = typename Pair<T>::V;
+  extern __shared__ __align__(16) float dw_sm[];
+  float* s_in = dw_sm;                 // [PH][PW][CC]
+  float* s_w = dw_sm + PH * PW * CC;   // [K*K][CC]
+  const int tile = blockIdx.x, c0 = blockIdx.y * CC, b = blockIdx.z;
+  const int y0 = (tile / tiles_x) * kDwTH, x0 = (tile % tiles_x) * kDwTW;
+  const int tid = threadIdx.x;
+
+  for (int i = tid; i < K * K * NP; i += THR) {
+    const int tap = i / NP, cp = i - tap * NP, c = c0 + 2 * cp;
+    float2 w = make_float2(0.f, 0.f);
+    if (c < C) w = make_float2(wgt[(size_t)tap * C + c], wgt[(size_t)tap * C + c + 1]);
+    reinterpret_cast<float2*>(s_w)[i] = w;
+  }
+  const size_t img = (size_t)b * H * W;
+  for (int i = tid; i < PH * PW * NP; i += THR) {
+    const int cp = i % NP, pix = i / NP;
+    const int iy = y0 - K / 2 + pix / PW, ix = x0 - K / 2 + pix % PW, c = c0 + 2 * cp;
+    float2 v = make_float2(0.f, 0.f);
+    if (iy >= 0 && iy < H && ix >= 0 && ix < W && c < C)
+      v = Pair<T>::f2(*reinterpret_cast<const V*>(x + (img + (size_t)iy * W + ix) * in_stride + c));
+    reinterpret_cast<float2*>(s_in)[i] = v;
+  }
+  __syncthreads();
+
+  const int cp = tid % NP, sx = (tid / NP) % kDwSX, ty = tid / (NP * kDwSX);
+  float2 acc[kDwR];
+#pragma unroll
+  for (int r = 0; r < kDwR; ++r) acc[r] = make_float2(0.f, 0.f);
+  const float2* in2 = reinterpret_cast<const float2*>(s_in);
+  const float2* w2 = reinterpret_cast<const float2*>(s_w);
+#pragma unroll 1
+  for (int ky = 0; ky < K; ++ky) {
+    const float2* row = in2 + ((ty + ky) * PW + sx * kDwR) * NP + cp;
+    float2 win[kDwR + K - 1];
+#pragma unroll
+    for (int j = 0; j < kDwR + K - 1; ++j) win[j] = row[j * NP];
+#pragma unroll
+    for (int kx = 0; kx < K; ++kx) {
+      const float2 w = w2[(ky * K + kx) * NP + cp];
+#pragma unroll
+      for (int r = 0; r < kDwR; ++r) {
+        acc[r].x = fmaf(win[r + kx].x, w.x, acc[r].x);
+        acc[r].y = fmaf(win[r + kx].y, w.y, acc[r].y);
+      }
+    }
+  }
+  const int c = c0 + 2 * cp, oy = y0 + ty;
+  if (c >= C || oy >= H) return;
+  const float b0 = bias[c], b1 = bias[c + 1];
+#pragma unroll
+  for (int r = 0; r < kDwR; ++r) {
+    const int ox = x0 + sx * kDwR + r;
+    if (ox < W) {
+      const float2 xc = in2[((ty + K / 2) * PW + sx * kDwR + r + K / 2) * NP + cp];  // the residual: the centre tap's input
+      *reinterpret_cast<V*>(out + (img + (size_t)oy * W + ox) * out_stride + c) =
+          Pair<T>::from(gelu_f32(xc.x + (acc[r].x + b0)), gelu_f32(xc.y + (acc[r].y + b1)));
+    }
+  }
+}
+
+template <typename T, int K>
+static int launch_dw(const T* x, int in_stride, T* out, int out_stride, const float* w, const float* bias, int B, int H, int W, int C,
+                     cudaStream_t s) {
+  static std::atomic<unsigned long long> attr_done{0};
+  const size_t smem = dw_smem(K);
+  int dev = 0;
+  PFB_CUDA(cudaGetDevice(&dev));
+  if (smem > 48 * 1024 && !(attr_done.load(std::memory_order_acquire) & (1ull << (dev & 63)))) {
+    PFB_CUDA(cudaFuncSetAttribute(depthwise_gelu_kernel<T, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    attr_done.fetch_or(1ull << (dev & 63), std::memory_order_release);
+  }
+  const int tiles_x = ceil_div(W, kDwTW), tiles_y = ceil_div(H, kDwTH);
+  dim3 grid(tiles_x * tiles_y, ceil_div(C, dw_cc(K)), B);
+  ProfScope prof(KC_DEPTHWISE, s);
+  depthwise_gelu_kernel<T, K><<<grid, dw_threads(K), smem, s>>>(x, in_stride, out, out_stride, w, bias, H, W, C, tiles_x);
+  PFB_LAUNCH_CHECK();
+  return PFB_OK;
+}
+
+template <typename T>
+static int dispatch_dw(const T* x, int in_stride, T* out, int out_stride, const float* w, const float* bias, int B, int H, int W, int C,
+                       int k, cudaStream_t s) {
+  switch (k) {
+#define PFB_DW_CASE(K) \
+  case K: return launch_dw<T, K>(x, in_stride, out, out_stride, w, bias, B, H, W, C, s);
+    PFB_DW_CASE(1) PFB_DW_CASE(3) PFB_DW_CASE(5) PFB_DW_CASE(7) PFB_DW_CASE(9) PFB_DW_CASE(11) PFB_DW_CASE(13) PFB_DW_CASE(15)
+    PFB_DW_CASE(17) PFB_DW_CASE(19) PFB_DW_CASE(21) PFB_DW_CASE(23) PFB_DW_CASE(25) PFB_DW_CASE(27) PFB_DW_CASE(29) PFB_DW_CASE(31)
+#undef PFB_DW_CASE
+    default: break;
+  }
+  set_error("depthwise_conv_gelu: kernel size %d (odd, 1..31)", k);
+  return PFB_ERR_ARG;
+}
+
+}  // namespace pfb
+
+using namespace pfb;
+
+extern "C" PFB_API int pfb_depthwise_conv_gelu(const void* x, int in_stride, int in_offset, void* out, int out_stride, int out_offset,
+                                               const float* weight, const float* bias, int B, int H, int W, int C, int k, pfb_dtype dtype,
+                                               pfb_stream stream) {
+  PFB_CHECK_ARG(x && out && weight && bias, "depthwise_conv_gelu: null pointer");
+  PFB_CHECK_ARG(dtype_ok(dtype), "depthwise_conv_gelu: bad dtype");
+  PFB_CHECK_ARG(B > 0 && H > 0 && W > 0 && C > 0 && C % 2 == 0, "depthwise_conv_gelu: bad shape %dx%dx%dx%d (C must be even)", B, H, W, C);
+  PFB_CHECK_ARG((k & 1) && k >= 1 && k <= 31, "depthwise_conv_gelu: kernel size %d (odd, 1..31)", k);
+  PFB_CHECK_ARG(in_offset >= 0 && out_offset >= 0 && in_stride >= in_offset + C && out_stride >= out_offset + C &&
+                    in_offset % 2 == 0 && out_offset % 2 == 0 && in_stride % 2 == 0 && out_stride % 2 == 0,
+                "depthwise_conv_gelu: strides / offsets must be even and hold C channels");
+  const size_t es = dtype_size(dtype);
+  const char* xb = reinterpret_cast<const char*>(x) + (size_t)in_offset * es;
+  char* ob = reinterpret_cast<char*>(out) + (size_t)out_offset * es;
+  PFB_CHECK_ARG((reinterpret_cast<uintptr_t>(xb) % (2 * es)) == 0 && (reinterpret_cast<uintptr_t>(ob) % (2 * es)) == 0,
+                "depthwise_conv_gelu: misaligned channel pairs");
+  cudaStream_t s = as_stream(stream);
+  PFB_DISPATCH_DTYPE(dtype, T, {
+    return dispatch_dw<T>(reinterpret_cast<const T*>(xb), in_stride, reinterpret_cast<T*>(ob), out_stride, weight, bias, B, H, W, C, k, s);
+  });
+  return PFB_ERR_ARG;
+}

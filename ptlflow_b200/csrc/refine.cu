@@ -8,7 +8,7 @@
 
 #include <stdlib.h>
 
-#include "common.cuh"
+#include "refine.cuh"
 
 #define PFB_TRY(expr)        \
   do {                       \
@@ -17,8 +17,6 @@
   } while (0)
 
 namespace pfb {
-
-int launch_flow_from_coords(const float* coords, float* flow, int B, int H, int W, cudaStream_t s);
 
 struct Workspace {
   // element strides (channels per pixel) and byte offsets inside the caller's workspace
@@ -189,23 +187,114 @@ static int run_context_terms(const Ctx& x) {
   return PFB_OK;
 }
 
-static int lookup(const Ctx& x) {
-  const pfb_raft_cfg* c = x.c;
+int raft_lookup(const pfb_raft_cfg* c, void* const* pyramid, const void* fmap1, const float* coords, void* out, int out_stride,
+                void* flags, cudaStream_t s) {
   if (c->alternate_corr) {
     static const int env_tc = getenv("PFB_ONTHEFLY_TC") ? atoi(getenv("PFB_ONTHEFLY_TC")) : 1;
-    if (env_tc && c->impl != 1 && corr_onthefly_umma_supported(c->B, c->H, c->W, c->feat_dim, c->corr_levels, c->corr_radius, c->dtype, x.ws.corr_stride))
-      return pfb_corr_lookup_onthefly_tc(x.b->fmap1, x.b->pyramid, x.b->coords, x.at(x.ws.off_corr), x.at(x.ws.off_flags), c->B, c->H, c->W,
-                                         c->feat_dim, c->corr_levels, c->corr_radius, c->dtype, x.ws.corr_stride, (pfb_stream)x.s);
+    if (env_tc && c->impl != 1 && corr_onthefly_umma_supported(c->B, c->H, c->W, c->feat_dim, c->corr_levels, c->corr_radius, c->dtype, out_stride))
+      return pfb_corr_lookup_onthefly_tc(fmap1, pyramid, coords, out, flags, c->B, c->H, c->W,
+                                         c->feat_dim, c->corr_levels, c->corr_radius, c->dtype, out_stride, (pfb_stream)s);
   }
   if (c->alternate_corr)
-    return pfb_corr_lookup_onthefly(x.b->fmap1, x.b->pyramid, x.b->coords, x.at(x.ws.off_corr), c->B, c->H, c->W,
+    return pfb_corr_lookup_onthefly(fmap1, pyramid, coords, out, c->B, c->H, c->W,
                                     c->feat_dim, c->corr_levels, c->corr_radius, c->dtype, c->dtype, 0,
-                                    x.ws.corr_stride, (pfb_stream)x.s);
+                                    out_stride, (pfb_stream)s);
   if (c->volume_layout == 1)
-    return pfb_corr_lookup_tiled(x.b->pyramid, x.b->coords, x.at(x.ws.off_corr), c->B, c->H, c->W, c->H, c->W, c->corr_levels,
-                                 c->corr_radius, c->dtype, x.ws.corr_stride, (pfb_stream)x.s);
-  return pfb_corr_lookup(x.b->pyramid, x.b->coords, x.at(x.ws.off_corr), c->B, c->H, c->W, c->corr_levels,
-                         c->corr_radius, c->dtype, c->dtype, 0, x.ws.corr_stride, (pfb_stream)x.s);
+    return pfb_corr_lookup_tiled(pyramid, coords, out, c->B, c->H, c->W, c->H, c->W, c->corr_levels,
+                                 c->corr_radius, c->dtype, out_stride, (pfb_stream)s);
+  return pfb_corr_lookup(pyramid, coords, out, c->B, c->H, c->W, c->corr_levels,
+                         c->corr_radius, c->dtype, c->dtype, 0, out_stride, (pfb_stream)s);
+}
+
+static int lookup(const Ctx& x) {
+  return raft_lookup(x.c, x.b->pyramid, x.b->fmap1, x.b->coords, x.at(x.ws.off_corr), x.ws.corr_stride, x.at(x.ws.off_flags), x.s);
+}
+
+int gma_aggregate(const pfb_raft_cfg* c, const pfb_layer& agg_v, const pfb_layer& agg_proj, const void* attention_ptr, float gamma,
+                  void* motion, int motion_stride, int motion_offset, int out_offset, void* vbuf_ptr, void* vT_ptr, void* agg_ptr, int n_pad,
+                  cudaStream_t s) {
+  PFB_CHECK_ARG(attention_ptr, "gma: null attention");
+  const int N = c->H * c->W, heads = heads_of(c), vdim = heads * 128;
+  const size_t es = dtype_size(c->dtype);
+  const char* attention = reinterpret_cast<const char*>(attention_ptr);
+  char* vbuf = reinterpret_cast<char*>(vbuf_ptr);
+  char* vT = reinterpret_cast<char*>(vT_ptr);
+  // one head: attn @ v goes straight into the AXPY epilogue.  Several heads (gma_utils.py:101-111): every head's attn @ v
+  // lands in its 128 columns of `agg`, then project (heads*128 -> 128) carries the AXPY epilogue.
+  char* agg = heads > 1 ? reinterpret_cast<char*>(agg_ptr) : nullptr;
+  PFB_CHECK_ARG(heads == 1 || (agg_proj.weight && agg_proj.Cin == vdim),
+                "gma: num_heads=%d needs the Aggregate.project layer (%d -> 128)", heads, vdim);
+  PFB_CHECK_ARG(agg_v.weight && agg_v.Cin == 128, "gma: Aggregate.to_v layer missing");
+  {  // v = to_v(motion)
+    pfb_conv_params p{};
+    p.src[0] = src_of(motion, 128, motion_stride, motion_offset);
+    p.nsrc = 1;
+    p.B = c->B; p.H = c->H; p.W = c->W; p.KH = agg_v.KH; p.KW = agg_v.KW;
+    p.Cout = agg_v.Cout; p.Cout_pad = agg_v.Cout_pad;
+    p.weight = agg_v.weight; p.bias = agg_v.bias;
+    p.epilogue = PFB_EPI_LINEAR; p.scale = 1.f;
+    p.out = vbuf; p.out_stride = vdim; p.out_offset = 0;
+    p.hidden = c->hidden_dim;
+    p.dtype = c->dtype; p.impl = c->impl;
+    p.weight_k = agg_v.weight_k; p.Cin_pad = agg_v.Cin_pad; p.Cout_pad_k = agg_v.Cout_pad_k;
+    PFB_TRY(pfb_conv2d(&p, (pfb_stream)s));
+  }
+  const bool tensor_path = c->dtype != PFB_F32 && c->impl != 1 && (N % 8) == 0;
+  if (tensor_path) PFB_TRY(pfb_transpose_pm(vbuf, vT, c->B, N, vdim, n_pad, c->dtype, (pfb_stream)s));
+  static const int env_batched = getenv("PFB_GMA_BATCHED") ? atoi(getenv("PFB_GMA_BATCHED")) : 1;
+  // "1x1 convolution" of head h over sample b (b < 0: all samples in one launch): pixels = queries, input channels = the N
+  // attention columns, weights = the sample's v (SIMT layout [N][vdim], columns h*128...) / v^T (K-major [vdim][n_pad], rows
+  // h*128...).  The attention is head-major, so every operand is affine in the pixel index.
+  auto attn_v = [&](int h, int b) -> int {
+    const int b0 = b < 0 ? 0 : b;
+    pfb_conv_params p{};
+    p.src[0] = src_of(attention + ((size_t)h * c->B + b0) * N * N * es, N, N);
+    p.nsrc = 1;
+    p.B = b < 0 ? c->B : 1; p.H = c->H; p.W = c->W; p.KH = 1; p.KW = 1;
+    p.Cout = 128; p.Cout_pad = vdim;
+    p.weight = vbuf + ((size_t)b0 * N * vdim + (size_t)h * 128) * es;
+    p.bias = nullptr;
+    if (heads == 1) {
+      char* mrow = reinterpret_cast<char*>(motion) + (size_t)b0 * N * motion_stride * es;
+      p.epilogue = PFB_EPI_AXPY; p.scale = gamma;
+      p.out = mrow; p.out_stride = motion_stride; p.out_offset = out_offset;
+      p.aux_h = mrow + (size_t)motion_offset * es; p.hidden = motion_stride;
+    } else {
+      p.epilogue = PFB_EPI_LINEAR; p.scale = 1.f;
+      p.out = agg + (size_t)b0 * N * vdim * es; p.out_stride = vdim; p.out_offset = h * 128;
+    }
+    p.dtype = c->dtype; p.impl = c->impl;
+    if (tensor_path) {
+      p.weight_k = vT + ((size_t)b0 * vdim + (size_t)h * 128) * n_pad * es; p.Cin_pad = n_pad; p.Cout_pad_k = 128;
+    }
+    if (b < 0) {
+      // ONE launch for all samples: per-sample weights = that sample's v^T (rows b * vdim + h * 128 ...).  B x 55 row tiles
+      // fill the machine; one launch per sample left only 55 row tiles, a fraction of the machine.
+      p.impl = 2;
+      p.w_rows_per_sample = vdim;
+    }
+    return pfb_conv2d(&p, (pfb_stream)s);
+  };
+  for (int h = 0; h < heads; ++h) {
+    if (tensor_path && env_batched) PFB_TRY(attn_v(h, -1));
+    else for (int b = 0; b < c->B; ++b) PFB_TRY(attn_v(h, b));
+  }
+  if (heads > 1) {  // motion_global = motion + gamma * project(out)   gma_utils.py:108-111
+    const pfb_layer& L = agg_proj;
+    pfb_conv_params p{};
+    p.src[0] = src_of(agg, vdim, vdim);
+    p.nsrc = 1;
+    p.B = c->B; p.H = c->H; p.W = c->W; p.KH = 1; p.KW = 1;
+    p.Cout = L.Cout; p.Cout_pad = L.Cout_pad;
+    p.weight = L.weight; p.bias = nullptr;
+    p.epilogue = PFB_EPI_AXPY; p.scale = gamma;
+    p.out = motion; p.out_stride = motion_stride; p.out_offset = out_offset;
+    p.aux_h = reinterpret_cast<char*>(motion) + (size_t)motion_offset * es; p.hidden = motion_stride;
+    p.dtype = c->dtype; p.impl = c->impl;
+    p.weight_k = L.weight_k; p.Cin_pad = L.Cin_pad; p.Cout_pad_k = L.Cout_pad_k;
+    PFB_TRY(pfb_conv2d(&p, (pfb_stream)s));
+  }
+  return PFB_OK;
 }
 
 // One BasicUpdateBlock / SmallUpdateBlock evaluation + coords update.  update.py:122-153
@@ -253,75 +342,9 @@ static int update_iter(const Ctx& x, const void* corr_ext, void* mask_out) {
   PFB_TRY(run_conv(x, PFB_L_CONV, {src_of(corflo, ws.c_corflo, ws.c_corflo)}, PFB_EPI_RELU_APPEND_FLOW, motion, ws.c_motion, 0));
 
   // ---- gma: motion_global = motion + gamma * (attention @ to_v(motion))   gma_utils.py:101-113, gma/update.py:149 ----
-  if (c->variant == 2) {
-    PFB_CHECK_ARG(x.b->attention, "gma: null attention");
-    const int N = c->H * c->W, heads = heads_of(c), vdim = heads * 128;
-    const size_t es = dtype_size(c->dtype);
-    const char* attention = reinterpret_cast<const char*>(x.b->attention);
-    char* vbuf = reinterpret_cast<char*>(x.at(ws.off_vbuf));
-    char* vT = reinterpret_cast<char*>(x.at(ws.off_vT));
-    // one head: attn @ v goes straight into the AXPY epilogue.  Several heads (gma_utils.py:101-111): every head's attn @ v
-    // lands in its 128 columns of `agg`, then project (heads*128 -> 128) carries the AXPY epilogue.
-    char* agg = heads > 1 ? reinterpret_cast<char*>(x.at(ws.off_agg)) : nullptr;
-    PFB_CHECK_ARG(heads == 1 || (x.w->layers[PFB_L_AGG_PROJ].weight && x.w->layers[PFB_L_AGG_PROJ].Cin == vdim),
-                  "gma: num_heads=%d needs the Aggregate.project layer (%d -> 128)", heads, vdim);
-    PFB_TRY(run_conv(x, PFB_L_AGG_V, {src_of(motion, 128, ws.c_motion)}, PFB_EPI_LINEAR, vbuf, vdim, 0));
-    const bool tensor_path = c->dtype != PFB_F32 && c->impl != 1 && (N % 8) == 0;
-    if (tensor_path) PFB_TRY(pfb_transpose_pm(vbuf, vT, c->B, N, vdim, ws.n_pad, c->dtype, (pfb_stream)x.s));
-    static const int env_batched = getenv("PFB_GMA_BATCHED") ? atoi(getenv("PFB_GMA_BATCHED")) : 1;
-    // "1x1 convolution" of head h over sample b (b < 0: all samples in one launch): pixels = queries, input channels = the N
-    // attention columns, weights = the sample's v (SIMT layout [N][vdim], columns h*128...) / v^T (K-major [vdim][n_pad], rows
-    // h*128...).  The attention is head-major, so every operand is affine in the pixel index.
-    auto attn_v = [&](int h, int b) -> int {
-      const int b0 = b < 0 ? 0 : b;
-      pfb_conv_params p{};
-      p.src[0] = src_of(attention + ((size_t)h * c->B + b0) * N * N * es, N, N);
-      p.nsrc = 1;
-      p.B = b < 0 ? c->B : 1; p.H = c->H; p.W = c->W; p.KH = 1; p.KW = 1;
-      p.Cout = 128; p.Cout_pad = vdim;
-      p.weight = vbuf + ((size_t)b0 * N * vdim + (size_t)h * 128) * es;
-      p.bias = nullptr;
-      if (heads == 1) {
-        char* mrow = reinterpret_cast<char*>(motion) + (size_t)b0 * N * ws.c_motion * es;
-        p.epilogue = PFB_EPI_AXPY; p.scale = x.b->agg_gamma;
-        p.out = mrow; p.out_stride = ws.c_motion; p.out_offset = 128;
-        p.aux_h = mrow; p.hidden = ws.c_motion;
-      } else {
-        p.epilogue = PFB_EPI_LINEAR; p.scale = 1.f;
-        p.out = agg + (size_t)b0 * N * vdim * es; p.out_stride = vdim; p.out_offset = h * 128;
-      }
-      p.dtype = c->dtype; p.impl = c->impl;
-      if (tensor_path) {
-        p.weight_k = vT + ((size_t)b0 * vdim + (size_t)h * 128) * ws.n_pad * es; p.Cin_pad = ws.n_pad; p.Cout_pad_k = 128;
-      }
-      if (b < 0) {
-        // ONE launch for all samples: per-sample weights = that sample's v^T (rows b * vdim + h * 128 ...).  B x 55 row tiles
-        // fill the machine; one launch per sample left only 55 row tiles, a fraction of the machine.
-        p.impl = 2;
-        p.w_rows_per_sample = vdim;
-      }
-      return pfb_conv2d(&p, (pfb_stream)x.s);
-    };
-    for (int h = 0; h < heads; ++h) {
-      if (tensor_path && env_batched) PFB_TRY(attn_v(h, -1));
-      else for (int b = 0; b < c->B; ++b) PFB_TRY(attn_v(h, b));
-    }
-    if (heads > 1) {  // motion_global = motion + gamma * project(out)   gma_utils.py:108-111
-      const pfb_layer& L = x.w->layers[PFB_L_AGG_PROJ];
-      pfb_conv_params p{};
-      p.src[0] = src_of(agg, vdim, vdim);
-      p.nsrc = 1;
-      p.B = c->B; p.H = c->H; p.W = c->W; p.KH = 1; p.KW = 1;
-      p.Cout = L.Cout; p.Cout_pad = L.Cout_pad;
-      p.weight = L.weight; p.bias = nullptr;
-      p.epilogue = PFB_EPI_AXPY; p.scale = x.b->agg_gamma;
-      p.out = motion; p.out_stride = ws.c_motion; p.out_offset = 128;
-      p.aux_h = motion; p.hidden = ws.c_motion;
-      p.dtype = c->dtype; p.impl = c->impl;
-      p.weight_k = L.weight_k; p.Cin_pad = L.Cin_pad; p.Cout_pad_k = L.Cout_pad_k;
-      PFB_TRY(pfb_conv2d(&p, (pfb_stream)x.s));
-    }
-  }
+  if (c->variant == 2)
+    PFB_TRY(gma_aggregate(c, x.w->layers[PFB_L_AGG_V], x.w->layers[PFB_L_AGG_PROJ], x.b->attention, x.b->agg_gamma, motion, ws.c_motion, 0,
+                          128, x.at(ws.off_vbuf), x.at(ws.off_vT), x.at(ws.off_agg), ws.n_pad, x.s));
 
   // ---- GRU (update.py:24-32 ConvGRU, :58-73 SepConvGRU); x = [inp, motion (, motion_global)] ----
   const int halves = (c->variant != 1) ? 2 : 1;

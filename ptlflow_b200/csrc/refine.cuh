@@ -1,0 +1,22 @@
+// Stages of the raft / gma refinement loop (refine.cu) that other loops built from the same operators reuse (skflow.cu).
+#pragma once
+#include "common.cuh"
+
+namespace pfb {
+
+// flow = coords - grid, fp32 [B,H,W,2] (misc.cu)
+int launch_flow_from_coords(const float* coords, float* flow, int B, int H, int W, cudaStream_t s);
+
+// The multi-scale lookup of the loop configured by `c` (dense, tiled or on-the-fly pyramid, as pfb_raft_refine picks it) into
+// out [B,H,W,out_stride] (storage type); flags: the on-the-fly tensor-core lookup's per-query workspace (alternate_corr only).
+int raft_lookup(const pfb_raft_cfg* c, void* const* pyramid, const void* fmap1, const float* coords, void* out, int out_stride,
+                void* flags, cudaStream_t s);
+
+// GMA Aggregate (gma_utils.py:79-113): motion_global = motion + gamma * project(attn_h @ to_v(motion)_h), written into the
+// motion buffer itself.  motion [B,H,W,motion_stride]: the motion features from channel motion_offset, motion_global to channels
+// out_offset .. +127.  vbuf [P][heads*128], vT [B][heads*128][n_pad], agg (heads > 1) [P][heads*128]: scratch of the storage type.
+int gma_aggregate(const pfb_raft_cfg* c, const pfb_layer& agg_v, const pfb_layer& agg_proj, const void* attention, float gamma,
+                  void* motion, int motion_stride, int motion_offset, int out_offset, void* vbuf, void* vT, void* agg, int n_pad,
+                  cudaStream_t s);
+
+}  // namespace pfb

@@ -106,32 +106,9 @@ class RaftEngine:
         self.num_heads = 1
         self.att_q = self.att_k = self.att_pos = None
         if variant == 2:
-            agg = ub.aggregator
-            self.num_heads = agg.heads
-            layers[_lib.L_AGG_V] = P([128], agg.to_v)
-            if agg.project is not None:
-                layers[_lib.L_AGG_PROJ] = P([agg.project.weight.shape[1]], agg.project)
-            self.agg_gamma = float(agg.gamma.detach().float().cpu().item())
-
-            class _Half:  # one head's q / k block of Attention.to_qk as a 1x1 layer (contiguous head-major outputs for the GEMM)
-                def __init__(self, w):
-                    self.weight, self.bias = w, None
-
-            wqk = attention_module.to_qk.weight
-            c = wqk.shape[0] // 2
-            d = c // self.num_heads  # dim_head
-            cin = [wqk.shape[1]]
-            self.att_q = [ops.PackedConv([_Half(wqk[h * d:(h + 1) * d])], dtype, device, src_channels=cin) for h in range(self.num_heads)]
-            self.att_k = [ops.PackedConv([_Half(wqk[c + h * d:c + (h + 1) * d])], dtype, device, src_channels=cin)
-                          for h in range(self.num_heads)]
-            if attention_module.position_only or attention_module.position_and_content:
-                # per-query position tables of head h: scale * q_h . [rel_height; rel_width] (gma_utils.py:18-30) = a 1x1 layer on
-                # `inp` whose weight is [E_h; E_w] @ W_q,h ((2P-1) * 2 rows, folded in fp64), scale applied by the epilogue
-                pe = attention_module.pos_emb
-                emb = torch.cat([pe.rel_height.weight, pe.rel_width.weight], 0).detach().double()
-                self.att_pos = [ops.PackedConv([_Half((emb @ wqk[h * d:(h + 1) * d, :, 0, 0].detach().double()).float()[:, :, None, None])],
-                                               dtype, device, src_channels=cin) for h in range(self.num_heads)]
-                self.max_pos = pe.rel_height.weight.shape[0] // 2 + 1
+            layers[_lib.L_AGG_V], proj = self._pack_attention(ub.aggregator, attention_module)
+            if proj is not None:
+                layers[_lib.L_AGG_PROJ] = proj
         self.layers = layers
         self.weights = _lib.RaftWeights()
         for k, v in layers.items():
@@ -141,6 +118,36 @@ class RaftEngine:
         # the pack kernels ran on the constructing thread's stream; other streams / host threads (pipeline slots) may use
         # the packed weights as soon as the engine is published, so finish them first (one-time cost)
         torch.cuda.current_stream(device).synchronize()
+
+    def _pack_attention(self, agg: torch.nn.Module, attention_module: torch.nn.Module):
+        """GMA's Aggregate and Attention (gma_utils.py:32-113): sets num_heads, agg_gamma and the per-head q / k / position layers
+        of the attention; returns the packed (to_v, project or None) of the per-iteration aggregate."""
+        dtype, device = self.dtype, self.device
+        self.num_heads = agg.heads
+        to_v = ops.PackedConv([agg.to_v], dtype, device, src_channels=[128])
+        proj = ops.PackedConv([agg.project], dtype, device, src_channels=[agg.project.weight.shape[1]]) if agg.project is not None else None
+        self.agg_gamma = float(agg.gamma.detach().float().cpu().item())
+
+        class _Half:  # one head's q / k block of Attention.to_qk as a 1x1 layer (contiguous head-major outputs for the GEMM)
+            def __init__(self, w):
+                self.weight, self.bias = w, None
+
+        wqk = attention_module.to_qk.weight
+        c = wqk.shape[0] // 2
+        d = c // self.num_heads  # dim_head
+        cin = [wqk.shape[1]]
+        self.att_q = [ops.PackedConv([_Half(wqk[h * d:(h + 1) * d])], dtype, device, src_channels=cin) for h in range(self.num_heads)]
+        self.att_k = [ops.PackedConv([_Half(wqk[c + h * d:c + (h + 1) * d])], dtype, device, src_channels=cin)
+                      for h in range(self.num_heads)]
+        if attention_module.position_only or attention_module.position_and_content:
+            # per-query position tables of head h: scale * q_h . [rel_height; rel_width] (gma_utils.py:18-30) = a 1x1 layer on
+            # `inp` whose weight is [E_h; E_w] @ W_q,h ((2P-1) * 2 rows, folded in fp64), scale applied by the epilogue
+            pe = attention_module.pos_emb
+            emb = torch.cat([pe.rel_height.weight, pe.rel_width.weight], 0).detach().double()
+            self.att_pos = [ops.PackedConv([_Half((emb @ wqk[h * d:(h + 1) * d, :, 0, 0].detach().double()).float()[:, :, None, None])],
+                                           dtype, device, src_channels=cin) for h in range(self.num_heads)]
+            self.max_pos = pe.rel_height.weight.shape[0] // 2 + 1
+        return to_v, proj
 
     # -- cache invalidation --------------------------------------------------------------------
     @staticmethod
@@ -164,13 +171,16 @@ class RaftEngine:
             return ops.corr_volume_build_tiled(fmap1, fmap2, self.corr_levels)
         return ops.corr_volume_build(fmap1, fmap2, self.corr_levels, impl=impl)
 
+    # C entry points of this engine's loop (SKFlowEngine runs its own with the same cfg / buffers)
+    _ws_symbol, _refine_symbol, _iter_symbol = "pfb_raft_workspace_bytes", "pfb_raft_refine", "pfb_raft_update_iter"
+
     def workspace(self, cfg: _lib.RaftCfg, scratch: Optional[dict] = None) -> torch.Tensor:
         if scratch is not None:
             # the caller owns the scratch memory (a CUDA graph keeps the workspace it was captured with alive)
             key = ("raft_ws", cfg.B, cfg.H, cfg.W)
             ws = scratch.get(key)
             if ws is None:
-                nbytes = load().pfb_raft_workspace_bytes(C.byref(cfg))
+                nbytes = getattr(load(), self._ws_symbol)(C.byref(cfg))
                 if nbytes == 0:
                     check(-1, "raft_workspace_bytes")
                 ws = scratch[key] = torch.empty(nbytes, dtype=torch.uint8, device=self.device)
@@ -181,7 +191,7 @@ class RaftEngine:
         key = (cfg.B, cfg.H, cfg.W)
         ent = self._workspaces.get(sid)
         if ent is None or ent[0] != key:
-            nbytes = load().pfb_raft_workspace_bytes(C.byref(cfg))
+            nbytes = getattr(load(), self._ws_symbol)(C.byref(cfg))
             if nbytes == 0:
                 check(-1, "raft_workspace_bytes")
             ent = (key, torch.empty(nbytes, dtype=torch.uint8, device=self.device))
@@ -208,7 +218,8 @@ class RaftEngine:
                                inp.data_ptr(), coords.data_ptr(), flow_up.data_ptr(), flow_small.data_ptr(),
                                ws.data_ptr(), ws.numel(), attention.data_ptr() if attention is not None else None, self.agg_gamma)
         with torch.cuda.device(self.device):
-            check(load().pfb_raft_refine(C.byref(cfg), C.byref(self.weights), C.byref(buf), stream_ptr(self.device)), "raft_refine")
+            check(getattr(load(), self._refine_symbol)(C.byref(cfg), C.byref(self.weights), C.byref(buf), stream_ptr(self.device)),
+                  self._refine_symbol[4:])
         return flow_up, flow_small
 
     def update_iter(self, net: torch.Tensor, inp: torch.Tensor, coords: torch.Tensor, corr: Optional[torch.Tensor] = None,
@@ -218,13 +229,107 @@ class RaftEngine:
         B, H, W, _ = net.shape
         cfg = self.make_cfg(B, H, W, 1, (8 * H, 8 * W), (0, 0), False, 0)
         ws = self.workspace(cfg)
-        mask = torch.empty((B, H, W, 576), dtype=self.dtype, device=self.device) if (want_mask and self.variant == 0) else None
+        mask = torch.empty((B, H, W, 576), dtype=self.dtype, device=self.device) if (want_mask and self.variant in (0, 3)) else None
         pyr = ptr_array(pyramid) if pyramid is not None else None
         buf = _lib.RaftBuffers(C.cast(pyr, C.POINTER(C.c_void_p)) if pyr is not None else None, None, net.data_ptr(), inp.data_ptr(),
                                coords.data_ptr(), None, None, ws.data_ptr(), ws.numel(),
                                attention.data_ptr() if attention is not None else None, self.agg_gamma)
         with torch.cuda.device(self.device):
-            check(load().pfb_raft_update_iter(C.byref(cfg), C.byref(self.weights), C.byref(buf),
-                                              corr.data_ptr() if corr is not None else None,
-                                              mask.data_ptr() if mask is not None else None, stream_ptr(self.device)), "raft_update_iter")
+            check(getattr(load(), self._iter_symbol)(C.byref(cfg), C.byref(self.weights), C.byref(buf),
+                                                     corr.data_ptr() if corr is not None else None,
+                                                     mask.data_ptr() if mask is not None else None, stream_ptr(self.device)),
+                  self._iter_symbol[4:])
         return mask
+
+
+def _align(n: int, a: int) -> int:
+    return (n + a - 1) // a * a
+
+
+class _View:
+    """weight / bias pair shaped like an nn.Conv2d, for PackedConv."""
+
+    def __init__(self, weight, bias):
+        self.weight, self.bias = weight, bias
+
+
+def _pad_conv(conv: torch.nn.Module, cout: int, cin: int) -> _View:
+    """conv's weight / bias zero-padded to [cout, cin, kh, kw] / [cout]."""
+    w = conv.weight.detach()
+    wp = torch.zeros((cout, cin) + tuple(w.shape[2:]), dtype=w.dtype, device=w.device)
+    wp[: w.shape[0], : w.shape[1]] = w
+    b = None
+    if conv.bias is not None:
+        b = torch.zeros(cout, dtype=conv.bias.dtype, device=conv.bias.device)
+        b[: conv.bias.shape[0]] = conv.bias.detach()
+    return _View(wp, b)
+
+
+class SKFlowEngine(RaftEngine):
+    """SKFlow's update block (skflow/update.py:7-99) packed for pfb_skflow_refine: every PCBlock's 1x1 layers through
+    ops.PackedConv, its depthwise filters as fp32 [k*k][C], all channel counts zero-padded to multiples of 32 (the padding stays
+    exactly zero through the block).  Same lifecycle and invalidation as RaftEngine; the attention is GMA's."""
+
+    _ws_symbol, _refine_symbol, _iter_symbol = "pfb_skflow_workspace_bytes", "pfb_skflow_refine", "pfb_skflow_update_iter"
+
+    def __init__(self, update_block: torch.nn.Module, variant: int, hidden_dim: int, context_dim: int,
+                 corr_levels: int, corr_radius: int, dtype: torch.dtype, device: torch.device, impl: int = 0,
+                 attention_module: Optional[torch.nn.Module] = None):
+        self.variant, self.hidden_dim, self.context_dim = variant, hidden_dim, context_dim
+        self.corr_levels, self.corr_radius = corr_levels, corr_radius
+        self.dtype, self.device, self.impl = dtype, device, impl
+        ub = update_block
+        enc = ub.encoder
+        planes = corr_levels * (2 * corr_radius + 1) ** 2
+        self._keep: List[object] = []  # everything the weight struct points into
+        w = _lib.SkflowWeights()
+        blocks = ((_lib.SK_CONVC1, enc.convc1, planes), (_lib.SK_CONVC2, enc.convc2, 256), (_lib.SK_CONVF2, enc.convf2, 128),
+                  (_lib.SK_CONV, enc.conv, 256), (_lib.SK_GRU, ub.gru, 512), (_lib.SK_FLOW_HEAD, ub.flow_head, 128))
+        for bid, blk, cin in blocks:
+            w.blocks[bid] = self._pack_block(blk, cin)
+        self.corr_stride = _align(planes, 32)  # the lookup buffer: planes channels, zero up to the padded width
+        for name, conv, srcs in (("convf1", enc.convf1, None), ("mask1", ub.mask[0], [128]), ("mask2", ub.mask[2], [256])):
+            setattr(w, name, self._layer(ops.PackedConv([conv], dtype, device, src_channels=srcs)))
+        to_v, proj = self._pack_attention(ub.aggregator, attention_module)
+        w.agg_v = self._layer(to_v)
+        if proj is not None:
+            w.agg_proj = self._layer(proj)
+        self.weights = w
+        self._workspaces: Dict[Tuple, torch.Tensor] = {}
+        self.signature = self.param_signature(update_block)
+        torch.cuda.current_stream(device).synchronize()
+
+    def _layer(self, pc: ops.PackedConv) -> _lib.Layer:
+        self._keep.append(pc)
+        return pc.layer_struct()
+
+    def _pack_block(self, blk: torch.nn.Module, cin: int) -> _lib.PcBlock:
+        """PCBlock4_Deep_nopool_res(cin, cout, k_conv) -> pfb_pc_block (C = align(cin, 32), hid = align(int(1.5 cin), 32))."""
+        dtype, device = self.dtype, self.device
+        C, hid = _align(cin, 32), _align(int(1.5 * cin), 32)
+        cout = blk.ffn2[2].weight.shape[0]
+
+        def P(view, srcs):
+            return self._layer(ops.PackedConv([view], dtype, device, src_channels=srcs))
+
+        k = _lib.PcBlock()
+        k.ffn1a = P(_pad_conv(blk.ffn1[0], hid, C), [C])
+        k.ffn1b = P(_pad_conv(blk.ffn1[2], C, hid), [hid])
+        k.pw = P(_pad_conv(blk.pw, C, C), [C])
+        k.ffn2a = P(_pad_conv(blk.ffn2[0], hid, C), [C])
+        k.ffn2b = P(_pad_conv(blk.ffn2[2], cout, hid), [hid])
+        k.C, k.hid = C, hid
+        convs = list(blk.conv_list)
+        if len(convs) > _lib.PFB_SK_MAX_DW:
+            raise ValueError(f"skflow: at most {_lib.PFB_SK_MAX_DW} depthwise convolutions per block, got {len(convs)}")
+        k.n_dw = len(convs)
+        for i, conv in enumerate(convs):
+            ks = conv.weight.shape[-1]
+            wt = torch.zeros((ks * ks, C), dtype=torch.float32, device=device)  # [tap][channel]
+            wt[:, :cin] = conv.weight.detach().to(device, torch.float32).reshape(cin, ks * ks).t()
+            bt = torch.zeros(C, dtype=torch.float32, device=device)
+            if conv.bias is not None:
+                bt[:cin] = conv.bias.detach().to(device, torch.float32)
+            self._keep += [wt, bt]
+            k.dw_k[i], k.dw_weight[i], k.dw_bias[i] = ks, wt.data_ptr(), bt.data_ptr()
+        return k

@@ -123,6 +123,7 @@ class RAFT(BaseModel):
         "kitti": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/raft-kitti-3a831a4b.ckpt",
     }
     _variant = 0  # pfb_raft_cfg.variant
+    _engine_cls = RaftEngine  # packs the update block and runs its loop (SKFlow brings its own)
 
     def __init__(self, corr_levels: int = 4, corr_radius: int = 4, dropout: float = 0.0, gamma: float = 0.8,
                  max_flow: float = 400, iters: int = 32, alternate_corr: bool = False, **kwargs) -> None:
@@ -173,11 +174,12 @@ class RAFT(BaseModel):
     # -- engine lifecycle ------------------------------------------------------------------
     def _get_engine(self, dtype: torch.dtype, device: torch.device) -> RaftEngine:
         eng = self._engine
+        cls = self._engine_cls
         if (eng is None or eng.dtype != dtype or eng.device != device or eng.impl != self.kernel_impl
                 or eng.corr_levels != self.corr_levels or eng.corr_radius != self.corr_radius
-                or eng.signature != RaftEngine.param_signature(self.update_block)
+                or eng.signature != cls.param_signature(self.update_block)
                 or getattr(eng, "extra_signature", None) != self._extra_signature()):
-            eng = RaftEngine(self.update_block, self._variant, self.hidden_dim, self.context_dim, self.corr_levels,
+            eng = cls(self.update_block, self._variant, self.hidden_dim, self.context_dim, self.corr_levels,
                              self.corr_radius, dtype, device, impl=self.kernel_impl, **self._extra_engine_args())
             eng.extra_signature = self._extra_signature()
             self._engine = eng

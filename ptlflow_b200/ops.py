@@ -260,8 +260,10 @@ class PackedConv:
 
 
 def conv2d(srcs, packed: PackedConv, out: torch.Tensor, epilogue: int = _lib.EPI_LINEAR, out_offset: int = 0,
-           scale: float = 1.0, aux_h=None, aux_z=None, hidden: int = 0, coords=None, flow=None, impl: int = 0) -> torch.Tensor:
-    """srcs: list of tensors [B,H,W,Ci] or (tensor, channels, offset) triples.  Mostly for tests."""
+           scale: float = 1.0, aux_h=None, aux_z=None, hidden: int = 0, coords=None, flow=None, impl: int = 0,
+           residual=None, post_w: Optional[torch.Tensor] = None, post_b: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """srcs: list of tensors [B,H,W,Ci] or (tensor, channels, offset) triples.  Mostly for tests.
+    ``residual`` (EPI_RESIDUAL_GELU): a tensor [B,H,W,Cr] or a (tensor, offset) pair; ``post_w`` / ``post_b``: fp32 [Cout]."""
     p = _lib.ConvParams()
     first = srcs[0][0] if isinstance(srcs[0], tuple) else srcs[0]
     B, H, W = first.shape[:3]
@@ -283,8 +285,34 @@ def conv2d(srcs, packed: PackedConv, out: torch.Tensor, epilogue: int = _lib.EPI
     p.dtype, p.impl = dtype_code(packed.dtype), impl
     p.weight_k = packed.weight_k.data_ptr() if packed.weight_k is not None else None
     p.Cin_pad, p.Cout_pad_k = packed.Cin_pad, packed.Cout_pad_k
+    if residual is not None:
+        rt, roff = residual if isinstance(residual, tuple) else (residual, 0)
+        require_cuda(rt, "residual")
+        p.residual, p.residual_stride, p.residual_offset = rt.data_ptr(), rt.shape[-1], roff
+    if post_w is not None:
+        p.post_w, p.post_b = post_w.data_ptr(), post_b.data_ptr()
     with torch.cuda.device(out.device):
         check(load().pfb_conv2d(C.byref(p), stream_ptr(out.device)), "conv2d")
+    return out
+
+
+def depthwise_conv_gelu(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, k: int, channels: Optional[int] = None,
+                        in_offset: int = 0, out: Optional[torch.Tensor] = None, out_offset: int = 0) -> torch.Tensor:
+    """gelu(x + depthwise_conv_kxk(x) + bias) of a PCBlock (skflow/update.py:32-33).  x [B,H,W,Cs] pixel-major, the ``channels``
+    channels from ``in_offset``; weight fp32 [k*k, C] (tap-major), bias fp32 [C].  Returns [B,H,W,C] (or writes ``out`` from
+    ``out_offset``)."""
+    require_cuda(x, "x")
+    B, H, W, Cs = x.shape
+    Cc = Cs - in_offset if channels is None else channels
+    if out is None:
+        out = torch.empty((B, H, W, Cc), dtype=x.dtype, device=x.device)
+    require_cuda(out, "out")
+    if weight.dtype != torch.float32 or bias.dtype != torch.float32 or tuple(weight.shape) != (k * k, Cc) or bias.numel() != Cc:
+        raise RuntimeError("depthwise_conv_gelu: weight must be fp32 [k*k, C] and bias fp32 [C]")
+    with torch.cuda.device(x.device):
+        check(load().pfb_depthwise_conv_gelu(x.data_ptr(), Cs, in_offset, out.data_ptr(), out.shape[-1], out_offset, weight.data_ptr(),
+                                             bias.data_ptr(), B, H, W, Cc, k, dtype_code(x.dtype), stream_ptr(x.device)),
+              "depthwise_conv_gelu")
     return out
 
 
