@@ -251,6 +251,18 @@ PFB_API int pfb_depthwise_conv_gelu(const void* x, int in_stride, int in_offset,
                                     const float* weight, const float* bias, int B, int H, int W, int C, int k, pfb_dtype dtype,
                                     pfb_stream stream);
 
+/* Depthwise k x k convolution followed by a LayerNorm over all C channels of each pixel, without the LayerNorm's affine part
+ * (SEA-RAFT's ConvNextBlock, sea_raft/layer.py:71-75; the affine folds into the next 1x1 layer):
+ *   y[p, c]   = bias[c] + sum_{ky, kx} weight[ky * k + kx][c] * x[p + (ky - k/2, kx - k/2), c]
+ *   out[p, c] = (y[p, c] - mean_c y[p, .]) * rsqrt(var_c y[p, .] + eps)          (biased variance)
+ * stride 1, zero "same" padding, any odd k <= 31, C even and <= 512.  Two passes: y is stored into `out` in the storage type, then
+ * normalised in place with fp32 statistics (mean, then the variance about it).  x: [B,H,W,in_stride] from channel in_offset; out:
+ * [B,H,W,out_stride] from out_offset (must not overlap x); offsets and strides even.  weight [k*k][C], bias [C]: fp32.  dtype is the
+ * storage type of x / out; accumulation is fp32. */
+PFB_API int pfb_depthwise_conv_layernorm(const void* x, int in_stride, int in_offset, void* out, int out_stride, int out_offset,
+                                         const float* weight, const float* bias, int B, int H, int W, int C, int k, float eps,
+                                         pfb_dtype dtype, pfb_stream stream);
+
 /* ------------------------------------------------------------------------------------
  * a10: upsampling
  *   convex 8x : RAFT.upsample_flow               ptlflow/models/raft/raft.py:112-123
@@ -423,6 +435,48 @@ PFB_API int pfb_skflow_update_iter(const pfb_raft_cfg* cfg, const pfb_skflow_wei
                                    const void* corr, void* mask_out, pfb_stream stream);
 
 /* ------------------------------------------------------------------------------------
+ * a16: SEA-RAFT's refinement loop (BasicUpdateBlock of ConvNeXt blocks + the SEARAFT.forward loop)
+ *   ptlflow/models/sea_raft/update.py:18-54, layer.py:41-83, sea_raft.py:189-236
+ * pfb_raft_cfg with variant = 4 (accepted by the pfb_searaft_* entry points only), hidden = context = 128.  The correlation pyramid
+ * is RAFT's (SEA-RAFT's per-level volumes against a bilinearly halved fmap2 are exactly the 2x2-pooled levels), so `pyramid`,
+ * `fmap1` and alternate_corr mean what they mean for pfb_raft_refine.
+ * ---------------------------------------------------------------------------------- */
+#define PFB_SR_MAX_BLOCKS 8
+/* One ConvNextBlock(384 -> 128) on x = [net | context | motion | flow]:
+ *   x^ = LayerNorm(dw_k(x)) without affine (pfb_depthwise_conv_layernorm);  h = gelu(pw1(x^));  net' = out([h | x])
+ * pw1: 1x1 384 -> 512 = pwconv1 with the LayerNorm affine folded in (W1 diag(ln_w), b1 + W1 ln_b);
+ * out: 1x1 [h (512) | x (384)] -> 128 = final(x + gamma * pwconv2(h)) as one layer ([Wf diag(gamma) W2 | Wf], Wf (gamma b2) + bf). */
+typedef struct {
+  int dw_k;
+  const float* dw_weight; /* [k*k][384] fp32 */
+  const float* dw_bias;   /* [384] fp32 */
+  pfb_layer pw1, out;
+} pfb_convnext_block;
+
+typedef struct {
+  pfb_layer init_conv;                      /* 3x3 256 -> 256, no activation (sea_raft.py:105) */
+  pfb_layer convc1, convc2, convf1, convf2, conv;  /* motion encoder, as RAFT's (update.py:18-36) */
+  int num_blocks;
+  pfb_convnext_block blocks[PFB_SR_MAX_BLOCKS];
+  float ln_eps;                             /* LayerNorm eps (1e-6) */
+  pfb_layer flow1;                          /* flow_head.0: 3x3 128 -> 256, ReLU */
+  pfb_layer flow2;                          /* flow_head.2 restricted to its flow outputs: 3x3 256 -> 2 */
+  pfb_layer flow2t;                         /* the same as a 1x1 layer to the 9 x 2 tap products (PFB_L_FLOW2T), or weight = NULL */
+  pfb_layer mask1, mask2;                   /* upsample_weight.0 (3x3 128 -> 256, ReLU), upsample_weight.2 (1x1 256 -> 576, x0.25) */
+} pfb_searaft_weights;
+
+PFB_API size_t pfb_searaft_workspace_bytes(const pfb_raft_cfg* cfg);
+/* The whole SEA-RAFT forward after the encoders: init_conv on buf->inp (the context network's output [B,H,W,256]), the initial
+ * flow head at coords = buf->coords (the grid on entry), cfg->iters update iterations (none when iters = 0: no pyramid is read),
+ * the mask head on the final net and the convex upsample.  buf->net [B,H,W,128] receives the final net; buf->coords the final
+ * coordinates. */
+PFB_API int pfb_searaft_refine(const pfb_raft_cfg* cfg, const pfb_searaft_weights* w, const pfb_raft_buffers* buf, pfb_stream stream);
+/* One update iteration without the upsample: buf->net [B,H,W,128] in/out, buf->inp the context [B,H,W,128], buf->coords in/out;
+ * corr (pixel-major [B,H,W,planes]) replaces the lookup when non-NULL; mask_out [B,H,W,576] may be NULL. */
+PFB_API int pfb_searaft_update_iter(const pfb_raft_cfg* cfg, const pfb_searaft_weights* w, const pfb_raft_buffers* buf,
+                                    const void* corr, void* mask_out, pfb_stream stream);
+
+/* ------------------------------------------------------------------------------------
  * Encoder-side kernels (SURVEY.md section 8(f) rank 1: the callers either side of the path).
  * The 3x3 / 7x7 / 1x1 convolutions of BasicEncoder / SmallEncoder (extractor.py:122-267) still run in
  * cuDNN; pre-processing, instance norm + ReLU (+ residual) and the residual joins are fused here.
@@ -474,10 +528,11 @@ PFB_API int pfb_bias_act(const void* x, const float* bias, const void* residual,
  * kernel_class: 0 volume, 1 pool, 2 lookup, 3 on-the-fly lookup, 4 update-block conv (wgmma / SIMT), 5 upsample,
  * 6 misc (packing, coords, softmax, transposes), 7 encoder normalise / bias / activation passes, 8 encoder instance-norm
  * statistics, 9 first encoder convolution (wgmma), 10 convf1 (7x7 on the flow, wgmma), 11 flow-head tap gather,
- * 12 depthwise convolution (SKFlow); -1 = all.  pfb_profile_collect synchronises the device, writes summed milliseconds and span
- * counts per class (arrays of >= PFB_KERNEL_CLASSES entries) and clears the recorded spans.
+ * 12 depthwise convolution (SKFlow), 13 depthwise convolution + LayerNorm (SEA-RAFT); -1 = all.  pfb_profile_collect synchronises
+ * the device, writes summed milliseconds and span counts per class (arrays of >= PFB_KERNEL_CLASSES entries) and clears the
+ * recorded spans.
  * ---------------------------------------------------------------------------------- */
-#define PFB_KERNEL_CLASSES 13
+#define PFB_KERNEL_CLASSES 14
 PFB_API unsigned long long pfb_launch_count(int kernel_class);
 PFB_API int pfb_profile_enable(int on);
 PFB_API int pfb_profile_collect(double* ms, unsigned long long* n, int len);

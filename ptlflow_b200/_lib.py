@@ -84,7 +84,7 @@ class RaftBuffers(C.Structure):
 # SKFlow (include/ptlflow_b200.h, a15)
 PFB_SK_MAX_DW = 8
 SK_CONVC1, SK_CONVC2, SK_CONVF2, SK_CONV, SK_GRU, SK_FLOW_HEAD, SK_BLOCKS = range(7)
-KERNEL_CLASSES = 13  # PFB_KERNEL_CLASSES (12 = depthwise convolution)
+KERNEL_CLASSES = 14  # PFB_KERNEL_CLASSES (12 = depthwise convolution, 13 = depthwise convolution + LayerNorm)
 
 
 class PcBlock(C.Structure):
@@ -96,6 +96,20 @@ class PcBlock(C.Structure):
 class SkflowWeights(C.Structure):
     _fields_ = [("blocks", PcBlock * SK_BLOCKS), ("convf1", Layer), ("mask1", Layer), ("mask2", Layer),
                 ("agg_v", Layer), ("agg_proj", Layer)]
+
+
+# SEA-RAFT (include/ptlflow_b200.h, a16)
+PFB_SR_MAX_BLOCKS = 8
+
+
+class ConvNextBlock(C.Structure):
+    _fields_ = [("dw_k", C.c_int), ("dw_weight", C.c_void_p), ("dw_bias", C.c_void_p), ("pw1", Layer), ("out", Layer)]
+
+
+class SearaftWeights(C.Structure):
+    _fields_ = [("init_conv", Layer), ("convc1", Layer), ("convc2", Layer), ("convf1", Layer), ("convf2", Layer), ("conv", Layer),
+                ("num_blocks", C.c_int), ("blocks", ConvNextBlock * PFB_SR_MAX_BLOCKS), ("ln_eps", C.c_float),
+                ("flow1", Layer), ("flow2", Layer), ("flow2t", Layer), ("mask1", Layer), ("mask2", Layer)]
 
 
 _lib: Optional[C.CDLL] = None
@@ -152,6 +166,10 @@ SIGNATURES = {
     "pfb_skflow_workspace_bytes": (C.c_size_t, [C.POINTER(RaftCfg)]),
     "pfb_skflow_refine": (_I, [C.POINTER(RaftCfg), C.POINTER(SkflowWeights), C.POINTER(RaftBuffers), _S]),
     "pfb_skflow_update_iter": (_I, [C.POINTER(RaftCfg), C.POINTER(SkflowWeights), C.POINTER(RaftBuffers), _P, _P, _S]),
+    "pfb_depthwise_conv_layernorm": (_I, [_P, _I, _I, _P, _I, _I, _P, _P, _I, _I, _I, _I, _I, C.c_float, _I, _S]),
+    "pfb_searaft_workspace_bytes": (C.c_size_t, [C.POINTER(RaftCfg)]),
+    "pfb_searaft_refine": (_I, [C.POINTER(RaftCfg), C.POINTER(SearaftWeights), C.POINTER(RaftBuffers), _S]),
+    "pfb_searaft_update_iter": (_I, [C.POINTER(RaftCfg), C.POINTER(SearaftWeights), C.POINTER(RaftBuffers), _P, _P, _S]),
 }
 
 

@@ -4,7 +4,8 @@
 // tile of CC channels: the tile plus its halo is staged once in shared memory as fp32 (zero outside the image, which is the
 // "same" padding), next to the fp32 weights of those channels.  A thread owns a channel pair and a strip of R = 8 consecutive
 // pixels of one row; per filter row it loads the R + k - 1 input pairs of that row once into registers and slides the k taps
-// over them, so every staged value is read from shared memory k times fewer than a per-output loop would.
+// over them, so every staged value is read from shared memory k times fewer than a per-output loop would.  Without the residual
+// and the GELU (kResidualGelu = false) the same kernel is the first pass of pfb_depthwise_conv_layernorm below.
 #include <atomic>
 
 #include "common.cuh"
@@ -36,7 +37,7 @@ __host__ __device__ constexpr size_t dw_smem(int K) {
   return ((size_t)(kDwTH + K - 1) * (kDwTW + K - 1) + (size_t)K * K) * dw_cc(K) * sizeof(float);
 }
 
-template <typename T, int K>
+template <typename T, int K, bool kResidualGelu>
 __global__ void __launch_bounds__(dw_threads(K)) depthwise_gelu_kernel(const T* __restrict__ x, int in_stride, T* __restrict__ out,
                                                                       int out_stride, const float* __restrict__ wgt,
                                                                       const float* __restrict__ bias, int H, int W, int C, int tiles_x) {
@@ -96,14 +97,18 @@ __global__ void __launch_bounds__(dw_threads(K)) depthwise_gelu_kernel(const T* 
   for (int r = 0; r < kDwR; ++r) {
     const int ox = x0 + sx * kDwR + r;
     if (ox < W) {
-      const float2 xc = in2[((ty + K / 2) * PW + sx * kDwR + r + K / 2) * NP + cp];  // the residual: the centre tap's input
-      *reinterpret_cast<V*>(out + (img + (size_t)oy * W + ox) * out_stride + c) =
-          Pair<T>::from(gelu_f32(xc.x + (acc[r].x + b0)), gelu_f32(xc.y + (acc[r].y + b1)));
+      V* o = reinterpret_cast<V*>(out + (img + (size_t)oy * W + ox) * out_stride + c);
+      if (kResidualGelu) {
+        const float2 xc = in2[((ty + K / 2) * PW + sx * kDwR + r + K / 2) * NP + cp];  // the residual: the centre tap's input
+        *o = Pair<T>::from(gelu_f32(xc.x + (acc[r].x + b0)), gelu_f32(xc.y + (acc[r].y + b1)));
+      } else {
+        *o = Pair<T>::from(acc[r].x + b0, acc[r].y + b1);
+      }
     }
   }
 }
 
-template <typename T, int K>
+template <typename T, int K, bool kResidualGelu = true>
 static int launch_dw(const T* x, int in_stride, T* out, int out_stride, const float* w, const float* bias, int B, int H, int W, int C,
                      cudaStream_t s) {
   static std::atomic<unsigned long long> attr_done{0};
@@ -111,13 +116,13 @@ static int launch_dw(const T* x, int in_stride, T* out, int out_stride, const fl
   int dev = 0;
   PFB_CUDA(cudaGetDevice(&dev));
   if (smem > 48 * 1024 && !(attr_done.load(std::memory_order_acquire) & (1ull << (dev & 63)))) {
-    PFB_CUDA(cudaFuncSetAttribute(depthwise_gelu_kernel<T, K>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    PFB_CUDA(cudaFuncSetAttribute(depthwise_gelu_kernel<T, K, kResidualGelu>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_done.fetch_or(1ull << (dev & 63), std::memory_order_release);
   }
   const int tiles_x = ceil_div(W, kDwTW), tiles_y = ceil_div(H, kDwTH);
   dim3 grid(tiles_x * tiles_y, ceil_div(C, dw_cc(K)), B);
-  ProfScope prof(KC_DEPTHWISE, s);
-  depthwise_gelu_kernel<T, K><<<grid, dw_threads(K), smem, s>>>(x, in_stride, out, out_stride, w, bias, H, W, C, tiles_x);
+  ProfScope prof(kResidualGelu ? KC_DEPTHWISE : KC_DW_LAYERNORM, s);
+  depthwise_gelu_kernel<T, K, kResidualGelu><<<grid, dw_threads(K), smem, s>>>(x, in_stride, out, out_stride, w, bias, H, W, C, tiles_x);
   PFB_LAUNCH_CHECK();
   return PFB_OK;
 }
@@ -137,9 +142,98 @@ static int dispatch_dw(const T* x, int in_stride, T* out, int out_stride, const 
   return PFB_ERR_ARG;
 }
 
+// ------------------------------------------------------------------------------------------------
+// Depthwise k x k convolution + LayerNorm over the channels (SEA-RAFT's ConvNextBlock, sea_raft/layer.py:71-75) as two passes:
+// the halo-tiled depthwise kernel above without its residual and GELU, y = dw_k(x) + bias, stored in the storage type, then a row
+// LayerNorm over each pixel's C channels, in place.  Measured against a fused kernel that kept all channels of an 8-pixel strip in
+// registers and read its window straight from global memory (DESIGN.md section 5): the fused kernel saved the round trip of y
+// but took 1.4-1.5x as long at the config-3 grid, because it staged nothing in shared memory.
+constexpr int kLnMaxC = 512;
+
+// Row LayerNorm without affine, in place allowed: one warp per pixel, lane l holds the channel pairs 2l + 64j in registers, mean
+// then the variance about it by warp shuffles.
+template <typename T>
+__global__ void __launch_bounds__(256) layernorm_rows_kernel(const T* y, T* out, int out_stride, size_t P, int C, float eps) {
+  using V = typename Pair<T>::V;
+  constexpr int NJ = kLnMaxC / 64;
+  const size_t p = (size_t)blockIdx.x * 8 + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (p >= P) return;
+  float2 v[NJ];
+  float s = 0.f;
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int c = 2 * lane + 64 * j;
+    v[j] = c < C ? Pair<T>::f2(*reinterpret_cast<const V*>(y + p * out_stride + c)) : make_float2(0.f, 0.f);
+    s += v[j].x + v[j].y;
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  const float mu = s / (float)C;
+  float q = 0.f;
+#pragma unroll
+  for (int j = 0; j < NJ; ++j)
+    if (2 * lane + 64 * j < C) q += (v[j].x - mu) * (v[j].x - mu) + (v[j].y - mu) * (v[j].y - mu);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) q += __shfl_xor_sync(0xffffffffu, q, o);
+  const float rs = rsqrtf(q / (float)C + eps);
+#pragma unroll
+  for (int j = 0; j < NJ; ++j) {
+    const int c = 2 * lane + 64 * j;
+    if (c < C) *reinterpret_cast<V*>(out + p * out_stride + c) = Pair<T>::from((v[j].x - mu) * rs, (v[j].y - mu) * rs);
+  }
+}
+
+template <typename T>
+static int launch_dwln(const T* x, int in_stride, T* out, int out_stride, const float* w, const float* bias, int B, int H, int W, int C,
+                       int k, float eps, cudaStream_t s) {
+  int rc = PFB_ERR_ARG;
+  switch (k) {
+#define PFB_DWS_CASE(K) \
+  case K: rc = launch_dw<T, K, false>(x, in_stride, out, out_stride, w, bias, B, H, W, C, s); break;
+    PFB_DWS_CASE(1) PFB_DWS_CASE(3) PFB_DWS_CASE(5) PFB_DWS_CASE(7) PFB_DWS_CASE(9) PFB_DWS_CASE(11) PFB_DWS_CASE(13)
+    PFB_DWS_CASE(15) PFB_DWS_CASE(17) PFB_DWS_CASE(19) PFB_DWS_CASE(21) PFB_DWS_CASE(23) PFB_DWS_CASE(25) PFB_DWS_CASE(27)
+    PFB_DWS_CASE(29) PFB_DWS_CASE(31)
+#undef PFB_DWS_CASE
+    default: set_error("depthwise_conv_layernorm: kernel size %d (odd, 1..31)", k); break;
+  }
+  if (rc != PFB_OK) return rc;
+  const size_t P = (size_t)B * H * W;
+  ProfScope prof(KC_DW_LAYERNORM, s);
+  layernorm_rows_kernel<T><<<(unsigned)ceil_div_sz(P, 8), 256, 0, s>>>(out, out, out_stride, P, C, eps);
+  PFB_LAUNCH_CHECK();
+  return PFB_OK;
+}
+
 }  // namespace pfb
 
 using namespace pfb;
+
+extern "C" PFB_API int pfb_depthwise_conv_layernorm(const void* x, int in_stride, int in_offset, void* out, int out_stride, int out_offset,
+                                                    const float* weight, const float* bias, int B, int H, int W, int C, int k, float eps,
+                                                    pfb_dtype dtype, pfb_stream stream) {
+  PFB_CHECK_ARG(x && out && weight && bias, "depthwise_conv_layernorm: null pointer");
+  PFB_CHECK_ARG(dtype_ok(dtype), "depthwise_conv_layernorm: bad dtype");
+  PFB_CHECK_ARG(B > 0 && H > 0 && W > 0 && C > 0 && C % 2 == 0 && C <= kLnMaxC,
+                "depthwise_conv_layernorm: bad shape %dx%dx%dx%d (C even, <= %d)", B, H, W, C, kLnMaxC);
+  PFB_CHECK_ARG(B <= 65535, "depthwise_conv_layernorm: batch %d too large", B);
+  PFB_CHECK_ARG((k & 1) && k >= 1 && k <= 31, "depthwise_conv_layernorm: kernel size %d (odd, 1..31)", k);
+  PFB_CHECK_ARG(eps > 0.f, "depthwise_conv_layernorm: eps must be positive");
+  PFB_CHECK_ARG(in_offset >= 0 && out_offset >= 0 && in_stride >= in_offset + C && out_stride >= out_offset + C &&
+                    in_offset % 2 == 0 && out_offset % 2 == 0 && in_stride % 2 == 0 && out_stride % 2 == 0,
+                "depthwise_conv_layernorm: strides / offsets must be even and hold C channels");
+  const size_t es = dtype_size(dtype);
+  const char* xb = reinterpret_cast<const char*>(x) + (size_t)in_offset * es;
+  char* ob = reinterpret_cast<char*>(out) + (size_t)out_offset * es;
+  PFB_CHECK_ARG((reinterpret_cast<uintptr_t>(xb) % (2 * es)) == 0 && (reinterpret_cast<uintptr_t>(ob) % (2 * es)) == 0,
+                "depthwise_conv_layernorm: misaligned channel pairs");
+  cudaStream_t s = as_stream(stream);
+  PFB_DISPATCH_DTYPE(dtype, T, {
+    return launch_dwln<T>(reinterpret_cast<const T*>(xb), in_stride, reinterpret_cast<T*>(ob), out_stride, weight, bias, B, H, W, C, k,
+                          eps, s);
+  });
+  return PFB_ERR_ARG;
+}
 
 extern "C" PFB_API int pfb_depthwise_conv_gelu(const void* x, int in_stride, int in_offset, void* out, int out_stride, int out_offset,
                                                const float* weight, const float* bias, int B, int H, int W, int C, int k, pfb_dtype dtype,

@@ -229,7 +229,7 @@ class RaftEngine:
         B, H, W, _ = net.shape
         cfg = self.make_cfg(B, H, W, 1, (8 * H, 8 * W), (0, 0), False, 0)
         ws = self.workspace(cfg)
-        mask = torch.empty((B, H, W, 576), dtype=self.dtype, device=self.device) if (want_mask and self.variant in (0, 3)) else None
+        mask = torch.empty((B, H, W, 576), dtype=self.dtype, device=self.device) if (want_mask and self.variant in (0, 3, 4)) else None
         pyr = ptr_array(pyramid) if pyramid is not None else None
         buf = _lib.RaftBuffers(C.cast(pyr, C.POINTER(C.c_void_p)) if pyr is not None else None, None, net.data_ptr(), inp.data_ptr(),
                                coords.data_ptr(), None, None, ws.data_ptr(), ws.numel(),
@@ -333,3 +333,90 @@ class SKFlowEngine(RaftEngine):
             self._keep += [wt, bt]
             k.dw_k[i], k.dw_weight[i], k.dw_bias[i] = ks, wt.data_ptr(), bt.data_ptr()
         return k
+
+
+def _searaft_params(model: torch.nn.Module):
+    """The parameters SEARaftEngine packs: init_conv, the heads and (iters > 0) the update block."""
+    mods = [model.init_conv, model.flow_head, model.upsample_weight] + ([model.update_block] if hasattr(model, "update_block") else [])
+    return [p for m in mods for p in m.parameters()]
+
+
+class SEARaftEngine(RaftEngine):
+    """SEA-RAFT's heads and update block (sea_raft.py:104-133, update.py:18-54, layer.py:41-83) packed for pfb_searaft_refine.  Each
+    ConvNextBlock becomes its depthwise filter (fp32 [k*k][384]) and two 1x1 layers, folded in fp64 from the parameters:
+    pw1 = pwconv1 with the LayerNorm affine (W1 diag(ln_w), b1 + W1 ln_b), and out = final(x + gamma * pwconv2(h)) over the two
+    sources [h | x] ([Wf diag(gamma) W2 | Wf], Wf (gamma b2) + bf).  Same lifecycle and invalidation as RaftEngine, keyed on
+    every parameter it packs."""
+
+    _ws_symbol, _refine_symbol, _iter_symbol = "pfb_searaft_workspace_bytes", "pfb_searaft_refine", "pfb_searaft_update_iter"
+
+    @staticmethod
+    def param_signature(model: torch.nn.Module):
+        return tuple((p.data_ptr(), p._version, p.dtype, str(p.device)) for p in _searaft_params(model))
+
+    def __init__(self, model: torch.nn.Module, variant: int, hidden_dim: int, context_dim: int, corr_levels: int, corr_radius: int,
+                 dtype: torch.dtype, device: torch.device, impl: int = 0):
+        self.variant, self.hidden_dim, self.context_dim = variant, hidden_dim, context_dim
+        self.corr_levels, self.corr_radius = corr_levels, corr_radius
+        self.dtype, self.device, self.impl = dtype, device, impl
+        self.agg_gamma, self.num_heads = 0.0, 1
+        self._keep: List[object] = []  # everything the weight struct points into
+        w = _lib.SearaftWeights()
+
+        def P(conv, srcs):
+            return self._layer(ops.PackedConv([conv], dtype, device, src_channels=srcs))
+
+        w.init_conv = P(model.init_conv, [256])
+        fh = model.flow_head
+        w.flow1 = P(fh[0], [128])
+        w2, b2 = fh[2].weight.detach()[:2], fh[2].bias.detach()[:2]  # the flow outputs; info (2:6) feeds training only
+        w.flow2 = P(_View(w2.contiguous(), b2.contiguous()), [256])
+        if dtype != torch.float32:  # 3x3 -> 2 as a 1x1 layer to the 9 x 2 per-tap products (row = tap*2 + o); the gather adds the bias
+            w.flow2t = P(_View(w2.permute(2, 3, 0, 1).reshape(18, w2.shape[1], 1, 1).contiguous(), None), [256])
+        w.mask1 = P(model.upsample_weight[0], [128])
+        w.mask2 = P(model.upsample_weight[2], [256])
+        w.ln_eps = 1e-6
+        ub = getattr(model, "update_block", None)
+        if ub is not None:
+            enc = ub.encoder
+            planes = corr_levels * (2 * corr_radius + 1) ** 2
+            w.convc1, w.convc2 = P(enc.convc1, [planes]), P(enc.convc2, [256])
+            w.convf1 = P(enc.convf1, None)
+            if dtype != torch.float32 and tuple(enc.convf1.weight.shape) == (128, 2, 7, 7):
+                pc = self._keep[-1]  # tensor-core form (csrc/first_conv.cu): the K-major slot carries the overlapping-window tiles
+                pc.weight_k = ops.pack_flow_conv(enc.convf1.weight, dtype).to(device)
+                pc.Cin_pad, pc.Cout_pad_k = 64, 128
+                w.convf1 = pc.layer_struct()
+            w.convf2, w.conv = P(enc.convf2, [128]), P(enc.conv, [256])
+            if len(ub.refine) > _lib.PFB_SR_MAX_BLOCKS:
+                raise ValueError(f"sea_raft: at most {_lib.PFB_SR_MAX_BLOCKS} ConvNeXt blocks, got {len(ub.refine)}")
+            w.num_blocks = len(ub.refine)
+            for i, blk in enumerate(ub.refine):
+                w.blocks[i] = self._pack_block(blk)
+                w.ln_eps = blk.norm.eps
+        self.weights = w
+        self._workspaces: Dict[Tuple, torch.Tensor] = {}
+        self.signature = self.param_signature(model)
+        torch.cuda.current_stream(device).synchronize()
+
+    def _layer(self, pc: ops.PackedConv) -> _lib.Layer:
+        self._keep.append(pc)
+        return pc.layer_struct()
+
+    def _pack_block(self, blk: torch.nn.Module) -> _lib.ConvNextBlock:
+        dtype, device = self.dtype, self.device
+        f64 = lambda t: t.detach().to(device, torch.float64)  # noqa: E731
+        W1, b1, lw, lb = f64(blk.pwconv1.weight), f64(blk.pwconv1.bias), f64(blk.norm.weight), f64(blk.norm.bias)
+        W2, b2, g = f64(blk.pwconv2.weight), f64(blk.pwconv2.bias), f64(blk.gamma)
+        Wf, bf = f64(blk.final.weight)[:, :, 0, 0], f64(blk.final.bias)
+        pw1 = _View((W1 * lw[None, :]).float()[:, :, None, None].contiguous(), (b1 + W1 @ lb).float())
+        out = _View(torch.cat([Wf @ (g[:, None] * W2), Wf], 1).float()[:, :, None, None].contiguous(), (Wf @ (g * b2) + bf).float())
+        C, k = blk.dwconv.weight.shape[0], blk.dwconv.weight.shape[-1]
+        dw_w = blk.dwconv.weight.detach().to(device, torch.float32).reshape(C, k * k).t().contiguous()  # [tap][channel]
+        dw_b = blk.dwconv.bias.detach().to(device, torch.float32).contiguous()
+        self._keep += [dw_w, dw_b]
+        b = _lib.ConvNextBlock()
+        b.dw_k, b.dw_weight, b.dw_bias = k, dw_w.data_ptr(), dw_b.data_ptr()
+        b.pw1 = self._layer(ops.PackedConv([pw1], dtype, device, src_channels=[C]))
+        b.out = self._layer(ops.PackedConv([out], dtype, device, src_channels=[4 * Wf.shape[0], C]))
+        return b

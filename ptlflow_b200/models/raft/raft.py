@@ -186,6 +186,10 @@ class RAFT(BaseModel):
         eng.fork_flow = self.fork_flow  # pfb_raft_cfg.fork_flow of the next refine() calls
         return eng
 
+    def _loop_parameters(self):
+        """The parameters the refinement engine runs on (the training guard of forward() looks at them)."""
+        return self.update_block.parameters()
+
     def _extra_engine_args(self) -> Dict:
         return {}
 
@@ -199,9 +203,12 @@ class RAFT(BaseModel):
     def _check_grid(self, h8: int, w8: int) -> None:
         """Raises ValueError, before anything is launched, for a 1/8-resolution grid (after padding) the model cannot run."""
 
-    def _encode(self, frames: torch.Tensor, B: int):
+    def _encode(self, frames: torch.Tensor, B: int, cnet_in: Optional[torch.Tensor] = None, with_fnet: bool = True):
         """frames: pixel-major [2B,Hp,Wp,3] (frame 1 of every pair first).  Both frames go through fnet as one
-        batch (instance norm is per sample, extractor.py:173-176); cnet sees frame 1 only."""
+        batch (instance norm is per sample, extractor.py:173-176); cnet sees frame 1 only, or ``cnet_in`` when given.
+        ``with_fnet = False`` runs cnet alone and returns None for both feature maps."""
+        if cnet_in is None:
+            cnet_in = frames[:B]
         def run(net, x):
             n = self.encoder_chunk
             if n <= 0 or x.shape[0] <= n:
@@ -218,7 +225,7 @@ class RAFT(BaseModel):
             tuned = tuned_key in self._enc_tuned  # first sight of a shape runs serially: cuDNN's autotuner times kernels then
             self._enc_tuned.add(tuned_key)
             half = frames.dtype != torch.float32
-            lanes = self.encoder_lanes if (self.fork_encoders and half) else 1
+            lanes = self.encoder_lanes if (self.fork_encoders and half and with_fnet) else 1
             split_fnet = lanes >= 3  # instance norm is per sample, so fnet on the two frames of the pairs separately is exact
             fmap1 = fmap2 = None
             if lanes >= 2 and tuned and own_cnet:
@@ -231,7 +238,7 @@ class RAFT(BaseModel):
                 aux = _lib.thread_stream(frames.device, "aux")
                 aux.wait_stream(cur)
                 with torch.cuda.stream(aux):
-                    cnet = run(self.cnet, frames[:B])
+                    cnet = run(self.cnet, cnet_in)
                 if split_fnet:
                     aux2 = _lib.thread_stream(frames.device, "aux2")
                     aux2.wait_stream(cur)
@@ -245,16 +252,16 @@ class RAFT(BaseModel):
             else:
                 if split_fnet:
                     fmap1, fmap2 = run(self.fnet, frames[:B]), run(self.fnet, frames[B:])
-                else:
+                elif with_fnet:
                     fmaps = run(self.fnet, frames)
                 if own_cnet:
-                    cnet = run(self.cnet, frames[:B])
-            if fmap1 is None:
+                    cnet = run(self.cnet, cnet_in)
+            if fmap1 is None and with_fnet:
                 fmap1, fmap2 = fmaps[:B], fmaps[B:]
         if cnet32 is not None and frames.dtype != torch.float32:
             # accuracy mode (enable_fp32_context): the context encoder in true fp32, its output rounded once to the storage type
             with _cudnn_flags(self.cudnn_benchmark, False):
-                cnet = run(cnet32, frames[:B].float()).to(frames.dtype)
+                cnet = run(cnet32, cnet_in.float()).to(frames.dtype)
         return fmap1, fmap2, cnet
 
     def enable_fp32_context(self, on: bool = True) -> "RAFT":
@@ -405,7 +412,7 @@ class RAFT(BaseModel):
         images = inputs["images"]
         if not images.is_cuda:
             raise RuntimeError("ptlflow_b200 runs on CUDA (sm_90a) only: move the model and inputs to the GPU. There is no CPU path.")
-        if torch.is_grad_enabled() and any(p.requires_grad for p in self.update_block.parameters()) and self.training:
+        if torch.is_grad_enabled() and any(p.requires_grad for p in self._loop_parameters()) and self.training:
             raise NotImplementedError("ptlflow_b200 implements the inference hot path; call under torch.no_grad() / model.eval()")
         stride = self.output_stride
         self._check_grid(-(-images.shape[-2] // stride), -(-images.shape[-1] // stride))

@@ -316,6 +316,27 @@ def depthwise_conv_gelu(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tenso
     return out
 
 
+def depthwise_conv_layernorm(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, k: int, channels: Optional[int] = None,
+                             in_offset: int = 0, eps: float = 1e-6, out: Optional[torch.Tensor] = None, out_offset: int = 0) -> torch.Tensor:
+    """LayerNorm over the channels (no affine) of depthwise_conv_kxk(x) + bias: SEA-RAFT's ConvNextBlock before pwconv1
+    (sea_raft/layer.py:71-75).  x [B,H,W,Cs] pixel-major, the ``channels`` channels from ``in_offset``; weight fp32 [k*k, C]
+    (tap-major), bias fp32 [C].  Returns [B,H,W,C] (or writes ``out`` from ``out_offset``)."""
+    require_cuda(x, "x")
+    B, H, W, Cs = x.shape
+    Cc = Cs - in_offset if channels is None else channels
+    if out is None:
+        out = torch.empty((B, H, W, Cc), dtype=x.dtype, device=x.device)
+    require_cuda(out, "out")
+    if weight.dtype != torch.float32 or bias.dtype != torch.float32 or tuple(weight.shape) != (k * k, Cc) or bias.numel() != Cc:
+        raise RuntimeError("depthwise_conv_layernorm: weight must be fp32 [k*k, C] and bias fp32 [C]")
+    require_cuda(weight, "weight"); require_cuda(bias, "bias")
+    with torch.cuda.device(x.device):
+        check(load().pfb_depthwise_conv_layernorm(x.data_ptr(), Cs, in_offset, out.data_ptr(), out.shape[-1], out_offset, weight.data_ptr(),
+                                                  bias.data_ptr(), B, H, W, Cc, k, eps, dtype_code(x.dtype), stream_ptr(x.device)),
+              "depthwise_conv_layernorm")
+    return out
+
+
 # ------------------------------------------------------------------------------------------
 # a10 and small helpers
 # ------------------------------------------------------------------------------------------
