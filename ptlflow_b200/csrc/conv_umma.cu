@@ -650,9 +650,16 @@ static int conv_n_tiles(int cout_pad) {
   return 0;
 }
 
+static bool aligned16(const void* ptr) { return (reinterpret_cast<uintptr_t>(ptr) & 15) == 0; }
+
+static bool plan_conv_umma(const pfb_conv_params* p, ConvUmmaArgs& a);
+
 bool conv2d_umma_supported(const pfb_conv_params* p) {
   if (p->dtype != PFB_F16 && p->dtype != PFB_BF16) return false;
   if (!p->weight_k || p->Cout_pad_k < 16 || p->Cout_pad_k % 16 || p->Cout_pad_k > kMaxBias) return false;
+  // the epilogue writes out (and reads / writes aux_h, aux_z below) 16 bytes at a time; the weight tensor map needs an
+  // aligned base
+  if (!aligned16(p->out) || !aligned16(p->weight_k)) return false;
   if (p->nsrc > 3) return false;
   int cin_pad = 0;
   for (int i = 0; i < p->nsrc; ++i) {
@@ -664,7 +671,11 @@ bool conv2d_umma_supported(const pfb_conv_params* p) {
   }
   if (cin_pad != p->Cin_pad) return false;
   switch (p->epilogue) {
-    case PFB_EPI_LINEAR: case PFB_EPI_RELU: case PFB_EPI_RELU_APPEND_FLOW: case PFB_EPI_GELU: case PFB_EPI_LINEAR_APPEND_FLOW: break;
+    case PFB_EPI_LINEAR: case PFB_EPI_RELU: case PFB_EPI_GELU: break;
+    case PFB_EPI_RELU_APPEND_FLOW: case PFB_EPI_LINEAR_APPEND_FLOW:
+      // the two flow columns go into the 32-column chunk that holds the last real channel, after it
+      if (p->Cout % 32 == 0 || p->Cout % 32 == 31) return false;
+      break;
     case PFB_EPI_RESIDUAL_GELU:
       if (!p->residual || p->residual_stride % 8 || p->residual_offset % 8 || p->Cout % 32 ||
           (reinterpret_cast<uintptr_t>(p->residual) & 15))
@@ -675,20 +686,23 @@ bool conv2d_umma_supported(const pfb_conv_params* p) {
       if (p->out_stride % 4 || p->out_offset % 4) return false;
       break;
     case PFB_EPI_AXPY:
-      if (!p->aux_h || p->hidden % 8 || p->Cout % 32) return false;
+      if (!p->aux_h || !aligned16(p->aux_h) || p->hidden % 8 || p->Cout % 32) return false;
       break;
     case PFB_EPI_GRU_ZR:
       if (p->hidden % 32 || p->Cout_pad_k != 2 * p->hidden || p->Cout_pad_k > 256) return false;
+      if (!aligned16(p->aux_h) || !aligned16(p->aux_z)) return false;
       break;
     case PFB_EPI_GRU_Q:
       if (p->hidden % 32 || p->Cout_pad_k != p->hidden) return false;
+      if (!aligned16(p->aux_h) || !aligned16(p->aux_z)) return false;
       break;
     default: return false;
   }
   if (p->out_stride % 8 || p->out_offset % 8) return false;
   if (p->w_rows_per_sample && (p->KH != 1 || p->KW != 1 || p->w_rows_per_sample < p->Cout_pad_k)) return false;
   if (p->addend && (p->addend_stride % 8 || (reinterpret_cast<uintptr_t>(p->addend) & 15) || p->addend_stride < p->Cout_pad_k)) return false;
-  return conv_n_tiles(p->Cout_pad_k) > 0;
+  ConvUmmaArgs a{};
+  return plan_conv_umma(p, a);
 }
 
 template <typename T, int EPI>
@@ -746,30 +760,106 @@ static void pick_tile(int H, int W, int& TW, int& TH) {
   }
 }
 
-int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
-  ConvUmmaArgs a{};
-  CUtensorMap tms[3];
-  pick_tile(p->H, p->W, a.TW, a.TH);
+// The activation patch of the M tile in `a` (TW, TH, halo) and the rings around it: b_group, a_stages, b_stages.  False when
+// not even two stages of each ring fit next to each other.
+static bool plan_rings(const pfb_conv_params* p, ConvUmmaArgs& a, int ring_budget) {
+  const int patch_w = a.TW + (a.halo == 1 ? p->KW - 1 : 0);
+  const int patch_h = a.TH + (a.halo == 2 ? p->KH - 1 : 0);
+  a.a_tx_bytes = patch_w * patch_h * 128;
+  a.a_slot_bytes = (int)align_up((size_t)a.a_tx_bytes, 1024);
+  const int taps_per_patch = a.halo == 1 ? p->KW : (a.halo == 2 ? p->KH : 1);
+  {
+    static const int env_group = getenv("PFB_CONV_TAP_GROUP") ? atoi(getenv("PFB_CONV_TAP_GROUP")) : 1;
+    a.b_group = 1;
+    // all taps of a patch in one weight stage when at least 3 such stages fit next to 3 activation patches
+    if (env_group && (taps_per_patch == 3 || taps_per_patch == 5) && 3 * taps_per_patch * a.b_tap_bytes + 3 * a.a_slot_bytes <= ring_budget)
+      a.b_group = taps_per_patch;
+  }
+  a.b_slot_bytes = a.b_group * a.b_tap_bytes;
+  // Split the rest between the rings.  A slot is reused only once per round trip (release -> producer wake-up -> TMA ->
+  // MMA), so the number of K steps in flight, not the bytes, sets the pace of the small-N layers: maximise min(steps
+  // covered by the activation ring, weight stages).  The MMA warpgroups hold the stage of the step in flight on top of
+  // the one they issue from, so one stage of each ring counts as consumed: 2 weight stages (the least that does not
+  // deadlock) leave the producer no lead and are chosen only where the activation patches leave room for no more.
+  int best = -1;
+  for (int as = 2; as <= kMaxAStages; ++as) {
+    int bs = (ring_budget - as * a.a_slot_bytes) / a.b_slot_bytes;
+    if (bs > kMaxBStages) bs = kMaxBStages;
+    if (bs < 2) continue;
+    const int cover_a = (as - 1) * taps_per_patch, cover_b = (bs - 1) * a.b_group;
+    const int cover = cover_a < cover_b ? cover_a : cover_b;
+    if (cover > best || (cover == best && bs > a.b_stages)) { best = cover; a.a_stages = as; a.b_stages = bs; }
+  }
+  return best >= 0;
+}
+
+// Everything about a launch but its operands: N tiling, output staging, M tile, halo mode, rings and work items.
+// conv2d_umma_supported and conv2d_umma both call it, so every shape the predicate accepts can be launched.  The M tiles are
+// tried in order of preference until the rings fit: for vertical kernels the vertical-halo tiles (fewest tiles first, then
+// the smallest patch), whose patches of TH + KH - 1 rows can leave no room for two weight stages on short or wide grids;
+// then the generic tile, with the horizontal halo where it applies and without any halo (one 16 KB patch per tap, which
+// always fits).
+static bool plan_conv_umma(const pfb_conv_params* p, ConvUmmaArgs& a) {
+  a.n_tiles = conv_n_tiles(p->Cout_pad_k);
+  if (a.n_tiles == 0) return false;
+  a.NT = p->Cout_pad_k / a.n_tiles;
+  a.b_tap_bytes = a.NT * 128;
+  {
+    static const int env_tma_out = getenv("PFB_CONV_TMA_STORE") ? atoi(getenv("PFB_CONV_TMA_STORE")) : 1;
+    const bool plain = p->epilogue == PFB_EPI_LINEAR || p->epilogue == PFB_EPI_RELU || p->epilogue == PFB_EPI_RELU_APPEND_FLOW ||
+                       p->epilogue == PFB_EPI_GELU || p->epilogue == PFB_EPI_LINEAR_APPEND_FLOW;
+    // a staged store writes whole 64-channel blocks: with several N tiles of NT % 64 == 32 the last block of a tile would
+    // overwrite the first 32 channels of the next one (a single tile is clipped at the layer's last channel by the tensor map)
+    a.tma_out = env_tma_out && plain && aligned16(p->out) && (a.NT % 64 == 0 || a.n_tiles == 1);
+  }
+  // 227 KB less the accumulator tile, the output staging, the bias, the barriers and the alignment slack
+  const int ring_budget = 227 * 1024 - acc_tile_bytes(a.NT) - (a.tma_out ? kATileBytes : 0) - kMaxBias * (int)sizeof(float) -
+                          (int)sizeof(ConvBars) - 1024;
   static const int env_halo = getenv("PFB_CONV_HALO") ? atoi(getenv("PFB_CONV_HALO")) : 1;
   static const int env_vhalo = getenv("PFB_CONV_VHALO") ? atoi(getenv("PFB_CONV_VHALO")) : 1;
-  a.halo = (env_halo && a.TH == 1 && p->KW > 1) ? 1 : 0;
+  int cand_tw[6], cand_th[6], cand_halo[6], nc = 0;
   if (env_vhalo && p->KW == 1 && p->KH > 1) {
     // vertical taps: a (TH + KH - 1) x TW patch serves all KH taps of a chunk when the per-tap offset TW * 128 B keeps
-    // the 1024-byte swizzle phase (TW % 8 == 0).  Fewest tiles first, then the smallest patch.
-    long best_tiles = -1, best_patch = 0;
+    // the 1024-byte swizzle phase (TW % 8 == 0).  Insertion by (tiles, patch); equal keys keep the wider tile first.
+    long tiles[4], patch[4];
     for (int tw = 64; tw >= 8; tw >>= 1) {
       const int th = 128 / tw;
-      const long tiles = (long)ceil_div(p->W, tw) * ceil_div(p->H, th), patch = (long)(th + p->KH - 1) * tw;
-      if (best_tiles < 0 || tiles < best_tiles || (tiles == best_tiles && patch < best_patch)) {
-        best_tiles = tiles; best_patch = patch; a.TW = tw; a.TH = th;
+      const long t = (long)ceil_div(p->W, tw) * ceil_div(p->H, th), pt = (long)(th + p->KH - 1) * tw;
+      int i = nc++;
+      for (; i > 0 && (t < tiles[i - 1] || (t == tiles[i - 1] && pt < patch[i - 1])); --i) {
+        tiles[i] = tiles[i - 1]; patch[i] = patch[i - 1]; cand_tw[i] = cand_tw[i - 1]; cand_th[i] = cand_th[i - 1];
       }
+      tiles[i] = t; patch[i] = pt; cand_tw[i] = tw; cand_th[i] = th;
     }
-    a.halo = 2;
+    for (int i = 0; i < nc; ++i) cand_halo[i] = 2;
+  }
+  int TW = 128, TH = 1;
+  pick_tile(p->H, p->W, TW, TH);
+  const int hx = (env_halo && TH == 1 && p->KW > 1) ? 1 : 0;
+  cand_tw[nc] = TW; cand_th[nc] = TH; cand_halo[nc++] = hx;
+  if (hx) { cand_tw[nc] = TW; cand_th[nc] = TH; cand_halo[nc++] = 0; }
+  for (int i = 0; i < nc; ++i) {
+    a.TW = cand_tw[i]; a.TH = cand_th[i]; a.halo = cand_halo[i];
+    if (!plan_rings(p, a, ring_budget)) continue;
+    a.tw_shift = 0;
+    while ((1 << a.tw_shift) < a.TW) ++a.tw_shift;
+    a.tiles_x = ceil_div(p->W, a.TW);
+    a.tiles_y = ceil_div(p->H, a.TH);
+    a.n_work = a.tiles_x * a.tiles_y * p->B * a.n_tiles;
+    return true;
+  }
+  return false;
+}
+
+int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
+  ConvUmmaArgs a{};
+  if (!plan_conv_umma(p, a)) {
+    set_error("conv_umma: no tile and ring plan fits in shared memory");
+    return PFB_ERR_UNSUPPORTED;
   }
   const int patch_w = a.TW + (a.halo == 1 ? p->KW - 1 : 0);
   const int patch_h = a.TH + (a.halo == 2 ? p->KH - 1 : 0);
-  a.tw_shift = 0;
-  while ((1 << a.tw_shift) < a.TW) ++a.tw_shift;
+  CUtensorMap tms[3];
   a.nsrc = p->nsrc;
   for (int i = 0; i < p->nsrc; ++i) {
     const pfb_conv_src& src = p->src[i];
@@ -783,9 +873,6 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
     if (rc) return rc;
   }
   for (int i = p->nsrc; i < 3; ++i) tms[i] = tms[0];
-  a.n_tiles = conv_n_tiles(p->Cout_pad_k);
-  if (a.n_tiles == 0) return PFB_ERR_UNSUPPORTED;
-  a.NT = p->Cout_pad_k / a.n_tiles;
   CUtensorMap tmW;
   {
     uint64_t dims[2] = {(uint64_t)p->Cin_pad, p->w_rows_per_sample > 0 ? (uint64_t)p->B * p->w_rows_per_sample : (uint64_t)p->KH * p->KW * p->Cout_pad_k};
@@ -795,32 +882,7 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
     if (rc) return rc;
   }
   a.B = p->B; a.H = p->H; a.W = p->W; a.KH = p->KH; a.KW = p->KW;
-  a.tiles_x = ceil_div(p->W, a.TW);
-  a.tiles_y = ceil_div(p->H, a.TH);
-  a.n_work = a.tiles_x * a.tiles_y * p->B * a.n_tiles;
   a.Cout = p->Cout; a.Cout_pad_k = p->Cout_pad_k;
-  a.a_tx_bytes = patch_w * patch_h * 128;
-  a.a_slot_bytes = (int)align_up((size_t)a.a_tx_bytes, 1024);
-  a.b_tap_bytes = a.NT * 128;
-  {
-    static const int env_tma_out = getenv("PFB_CONV_TMA_STORE") ? atoi(getenv("PFB_CONV_TMA_STORE")) : 1;
-    const bool plain = p->epilogue == PFB_EPI_LINEAR || p->epilogue == PFB_EPI_RELU || p->epilogue == PFB_EPI_RELU_APPEND_FLOW ||
-                       p->epilogue == PFB_EPI_GELU || p->epilogue == PFB_EPI_LINEAR_APPEND_FLOW;
-    // a staged store writes whole 64-channel blocks: with several N tiles of NT % 64 == 32 the last block of a tile would
-    // overwrite the first 32 channels of the next one (a single tile is clipped at the layer's last channel by the tensor map)
-    a.tma_out = env_tma_out && plain && (reinterpret_cast<uintptr_t>(p->out) & 15) == 0 && (a.NT % 64 == 0 || a.n_tiles == 1);
-  }
-  // 227 KB less the accumulator tile, the output staging, the bias, the barriers and the alignment slack
-  const int ring_budget = 227 * 1024 - acc_tile_bytes(a.NT) - (a.tma_out ? kATileBytes : 0) - kMaxBias * (int)sizeof(float) -
-                          (int)sizeof(ConvBars) - 1024;
-  {
-    static const int env_group = getenv("PFB_CONV_TAP_GROUP") ? atoi(getenv("PFB_CONV_TAP_GROUP")) : 1;
-    const int taps = a.halo == 1 ? p->KW : (a.halo == 2 ? p->KH : 1);
-    a.b_group = 1;
-    // all taps of a patch in one weight stage when at least 3 such stages fit next to 3 activation patches
-    if (env_group && (taps == 3 || taps == 5) && 3 * taps * a.b_tap_bytes + 3 * a.a_slot_bytes <= ring_budget) a.b_group = taps;
-  }
-  a.b_slot_bytes = a.b_group * a.b_tap_bytes;
   // ---- outputs through staging + TMA bulk stores (everything but the fp32 tap products) ----
   CUtensorMap tmO[2];
   tmO[0] = tms[0];
@@ -842,25 +904,6 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
         if (rc) return rc;
       }
     }
-  }
-  {
-    // Split the rest between the rings.  A slot is reused only once per round trip (release -> producer wake-up -> TMA ->
-    // MMA), so the number of K steps in flight, not the bytes, sets the pace of the small-N layers: maximise min(steps
-    // covered by the activation ring, weight stages).  The MMA warpgroups hold the stage of the step in flight on top of
-    // the one they issue from, so one stage of each ring counts as consumed: 2 weight stages (the least that does not
-    // deadlock) leave the producer no lead and are chosen only where the activation patches leave room for no more.
-    const int budget = ring_budget;
-    const int taps_per_patch = a.halo == 1 ? p->KW : (a.halo == 2 ? p->KH : 1);
-    int best = -1;
-    for (int as = 2; as <= kMaxAStages; ++as) {
-      int bs = (budget - as * a.a_slot_bytes) / a.b_slot_bytes;
-      if (bs > kMaxBStages) bs = kMaxBStages;
-      if (bs < 2) continue;
-      const int cover_a = (as - 1) * taps_per_patch, cover_b = (bs - 1) * a.b_group;
-      const int cover = cover_a < cover_b ? cover_a : cover_b;
-      if (cover > best || (cover == best && bs > a.b_stages)) { best = cover; a.a_stages = as; a.b_stages = bs; }
-    }
-    if (best < 0) return PFB_ERR_UNSUPPORTED;
   }
   a.bias = p->bias; a.epilogue = p->epilogue; a.scale = p->scale;
   a.out = p->out; a.out_stride = p->out_stride; a.out_offset = p->out_offset;

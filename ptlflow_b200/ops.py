@@ -261,9 +261,13 @@ class PackedConv:
 
 def conv2d(srcs, packed: PackedConv, out: torch.Tensor, epilogue: int = _lib.EPI_LINEAR, out_offset: int = 0,
            scale: float = 1.0, aux_h=None, aux_z=None, hidden: int = 0, coords=None, flow=None, impl: int = 0,
-           residual=None, post_w: Optional[torch.Tensor] = None, post_b: Optional[torch.Tensor] = None) -> torch.Tensor:
+           residual=None, post_w: Optional[torch.Tensor] = None, post_b: Optional[torch.Tensor] = None,
+           addend: Optional[torch.Tensor] = None, w_rows_per_sample: int = 0) -> torch.Tensor:
     """srcs: list of tensors [B,H,W,Ci] or (tensor, channels, offset) triples.  Mostly for tests.
-    ``residual`` (EPI_RESIDUAL_GELU): a tensor [B,H,W,Cr] or a (tensor, offset) pair; ``post_w`` / ``post_b``: fp32 [Cout]."""
+    ``residual`` (EPI_RESIDUAL_GELU): a tensor [B,H,W,Cr] or a (tensor, offset) pair; ``post_w`` / ``post_b``: fp32 [Cout].
+    ``addend``: a per-pixel term [B,H,W,S] (S >= Cout_pad_k) added instead of the bias.  ``w_rows_per_sample`` > 0 (1x1 layers):
+    sample b multiplies with rows [b * w_rows_per_sample, + Cout_pad_k) of ``packed.weight_k`` viewed as [B * w_rows_per_sample,
+    Cin_pad].  Both are served by the wgmma path only."""
     p = _lib.ConvParams()
     first = srcs[0][0] if isinstance(srcs[0], tuple) else srcs[0]
     B, H, W = first.shape[:3]
@@ -291,6 +295,10 @@ def conv2d(srcs, packed: PackedConv, out: torch.Tensor, epilogue: int = _lib.EPI
         p.residual, p.residual_stride, p.residual_offset = rt.data_ptr(), rt.shape[-1], roff
     if post_w is not None:
         p.post_w, p.post_b = post_w.data_ptr(), post_b.data_ptr()
+    if addend is not None:
+        require_cuda(addend, "addend")
+        p.addend, p.addend_stride = addend.data_ptr(), addend.shape[-1]
+    p.w_rows_per_sample = w_rows_per_sample
     with torch.cuda.device(out.device):
         check(load().pfb_conv2d(C.byref(p), stream_ptr(out.device)), "conv2d")
     return out
