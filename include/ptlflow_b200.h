@@ -125,6 +125,11 @@ PFB_API int pfb_corr_lookup_tiled(void* const* pyramid, const float* coords, voi
 PFB_API int pfb_corr_lookup_onthefly(const void* fmap1, void* const* fmap2_pyramid, const float* coords, void* out,
                              int B, int H, int W, int C, int levels, int radius, pfb_dtype dtype,
                              pfb_dtype out_dtype, int out_nchw, int out_stride, pfb_stream stream);
+/* Same with an explicit scale of the dot products (0 = 1/sqrt(C)): features stored in rows wider than their real width (zero
+ * channels up to a multiple of 64, MS-RAFT+'s 96-channel 1/4-scale features) keep the scale of the real width. */
+PFB_API int pfb_corr_lookup_onthefly_ex(const void* fmap1, void* const* fmap2_pyramid, const float* coords, void* out, int B, int H, int W,
+                                        int C, int levels, int radius, float scale, pfb_dtype dtype, pfb_dtype out_dtype, int out_nchw,
+                                        int out_stride, pfb_stream stream);
 
 /* a4 on the tensor cores (f16 / bf16, radius 4, C % 64 == 0, C <= 256, pixel-major output): every 8 x 16 tile of neighbouring queries
  * multiplies its query vectors with the region of fmap2_pyramid[l] that holds all its windows (wgmma GEMM, TMA-fed, out-of-map
@@ -136,6 +141,10 @@ PFB_API size_t pfb_corr_lookup_onthefly_tc_workspace_bytes(int B, int H, int W);
 PFB_API int pfb_corr_lookup_onthefly_tc(const void* fmap1, void* const* fmap2_pyramid, const float* coords, void* out, void* workspace,
                                         int B, int H, int W, int C, int levels, int radius, pfb_dtype dtype, int out_stride,
                                         pfb_stream stream);
+/* Same with an explicit scale (0 = 1/sqrt(C)); the SIMT pass for the flagged queries uses the same scale. */
+PFB_API int pfb_corr_lookup_onthefly_tc_ex(const void* fmap1, void* const* fmap2_pyramid, const float* coords, void* out, void* workspace,
+                                           int B, int H, int W, int C, int levels, int radius, float scale, pfb_dtype dtype, int out_stride,
+                                           pfb_stream stream);
 
 /* The reference plugin's own entry point, same tensor contract:
  *   alt_cuda_corr.forward(fmap1, fmap2, coords, radius) -> [corr]     correlation.cpp:23-33
@@ -477,6 +486,39 @@ PFB_API int pfb_searaft_update_iter(const pfb_raft_cfg* cfg, const pfb_searaft_w
                                     const void* corr, void* mask_out, pfb_stream stream);
 
 /* ------------------------------------------------------------------------------------
+ * a17: MS-RAFT+'s four-scale refinement (ptlflow/models/ms_raft_plus/ms_raft_plus.py:146-226)
+ * The scale loop runs RAFT's update block (pfb_raft_weights with CONVC1.Cin = levels*(2r+1)^2 and MASK2.Cout = 36) once per scale
+ * (1/16, 1/8, 1/4, 1/2), with pfb_raft_cfg variant = 5 (accepted by the pfb_msraft_* entry points only) describing that scale's
+ * grid.  pyramid / fmap1 / alternate_corr / volume_layout mean what they mean for pfb_raft_refine.
+ * ---------------------------------------------------------------------------------- */
+/* out [B,2H,2W,Cs+Ck] = cat[bilinear 2x (align_corners = False, edge clamped) of src [B,H,W,Cs], skip [B,2H,2W,Ck]] along the
+ * channels: TF.resize + torch.cat of the encoders' up path (extractor.py:193-210).  Cs, Ck multiples of 8 (Ck may be 0, skip
+ * NULL); 16-byte aligned pointers. */
+PFB_API int pfb_upsample2x_concat(const void* src, int src_channels, const void* skip, int skip_channels, void* out, int B, int H, int W,
+                                  pfb_dtype dtype, pfb_stream stream);
+/* Convex 2x upsample (upsample_flow with scale = 2, ms_raft_plus.py:138-149): mask [B,H,W,36] dtype, channel = tap*4 + sy*2 + sx,
+ * already scaled by 0.25; softmax over the 9 taps; the 3x3 neighbourhood of 2 * value is unfolded with ZERO padding.
+ *   mode 0: value = coords - grid; out [B,2,out_h,out_w] fp32, the window of the 2H x 2W result at (pad_top, pad_left)
+ *   mode 1: value = coords (absolute, the handover between scales); out [B,2H,2W,2] fp32 pixel-major; window arguments unused */
+PFB_API int pfb_convex_upsample2x(const float* coords, const void* mask, float* out, int mode, int B, int H, int W, int out_h, int out_w,
+                                  int pad_top, int pad_left, pfb_dtype dtype, pfb_stream stream);
+/* downflow (ms_raft_plus.py:22-35): flow [B,2,H,W] fp32 -> out [B,2,out_h,out_w], bilinear with align_corners = True, u scaled by
+ * out_w / W and v by out_h / H. */
+PFB_API int pfb_downflow(const float* flow, float* out, int B, int H, int W, int out_h, int out_w, pfb_stream stream);
+PFB_API size_t pfb_msraft_workspace_bytes(const pfb_raft_cfg* cfg);
+/* One scale: cfg->iters >= 1 update iterations from buf->coords (absolute, this scale's grid), the GRU context terms once, the mask
+ * head on the last iteration only.  corr_scale: the on-the-fly lookup's scale, 0 = 1/sqrt(feat_dim).  Then either
+ *   next_coords != NULL: pfb_convex_upsample2x mode 1 into next_coords [B,2H,2W,2] (the next scale's starting coordinates), or
+ *   next_coords == NULL: mode 0 into buf->flow_up (cfg out_h / out_w / pad window) and, if buf->flow_small != NULL, pfb_downflow
+ *                        of it into buf->flow_small [B,2,out_h/16,out_w/16]. */
+PFB_API int pfb_msraft_refine(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf, float corr_scale,
+                              float* next_coords, pfb_stream stream);
+/* One update iteration without the upsample; corr (pixel-major [B,H,W,planes]) replaces the lookup when non-NULL; mask_out
+ * [B,H,W,36] may be NULL. */
+PFB_API int pfb_msraft_update_iter(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf, const void* corr,
+                                   void* mask_out, float corr_scale, pfb_stream stream);
+
+/* ------------------------------------------------------------------------------------
  * Encoder-side kernels (SURVEY.md section 8(f) rank 1: the callers either side of the path).
  * The 3x3 / 7x7 / 1x1 convolutions of BasicEncoder / SmallEncoder (extractor.py:122-267) still run in
  * cuDNN; pre-processing, instance norm + ReLU (+ residual) and the residual joins are fused here.
@@ -496,6 +538,17 @@ PFB_API int pfb_instance_norm_act(const void* x, void* y, const void* residual, 
  * workspace = B*C*2 doubles (sum, sum of squares; zeroed by the caller before the producer ran) + B*C float2. */
 PFB_API int pfb_instance_norm_apply(const void* x, void* y, const void* residual, void* workspace, int B, int H, int W, int C,
                                     float eps, int relu, pfb_dtype dtype, pfb_stream stream);
+/* Group norm (nn.GroupNorm) of x + bias: statistics per (image, group of group_size consecutive channels), biased variance, then
+ * gamma / beta per channel; y = act(GN(x + bias)) or, with residual, relu(residual + act(GN(x + bias))).  bias (the producing
+ * convolution's, fp32 [C]), gamma, beta (fp32 [C]) may each be NULL.  group_size = 1 without bias and affine is instance norm.
+ * workspace: pfb_instance_norm_workspace_bytes(B, C).  C % 8 == 0, C <= 512, group_size divides C. */
+PFB_API int pfb_group_norm_act(const void* x, void* y, const void* residual, void* workspace, const float* bias, const float* gamma,
+                               const float* beta, int B, int H, int W, int C, int group_size, float eps, int relu, pfb_dtype dtype,
+                               pfb_stream stream);
+/* The same from per-(image, channel) sums of x already in the workspace (pfb_first_conv7x7s2's stats output). */
+PFB_API int pfb_group_norm_apply(const void* x, void* y, const void* residual, void* workspace, const float* bias, const float* gamma,
+                                 const float* beta, int B, int H, int W, int C, int group_size, float eps, int relu, pfb_dtype dtype,
+                                 pfb_stream stream);
 /* First encoder convolution: nn.Conv2d(3, 64, 7, stride=2, padding=3) of BasicEncoder (extractor.py:136,171-178)
  * on wgmma without an im2col buffer (overlapping-window operand descriptors, see csrc/first_conv.cu).
  *   x      [N,H,W,4]  f16/bf16 pixel-major frames from pfb_preprocess_frames(out_channels = 4); H, W even

@@ -170,6 +170,17 @@ SIGNATURES = {
     "pfb_searaft_workspace_bytes": (C.c_size_t, [C.POINTER(RaftCfg)]),
     "pfb_searaft_refine": (_I, [C.POINTER(RaftCfg), C.POINTER(SearaftWeights), C.POINTER(RaftBuffers), _S]),
     "pfb_searaft_update_iter": (_I, [C.POINTER(RaftCfg), C.POINTER(SearaftWeights), C.POINTER(RaftBuffers), _P, _P, _S]),
+    # MS-RAFT+ (a17)
+    "pfb_corr_lookup_onthefly_ex": (_I, [_P, _PP, _P, _P, _I, _I, _I, _I, _I, _I, C.c_float, _I, _I, _I, _I, _S]),
+    "pfb_corr_lookup_onthefly_tc_ex": (_I, [_P, _PP, _P, _P, _P, _I, _I, _I, _I, _I, _I, C.c_float, _I, _I, _S]),
+    "pfb_group_norm_act": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, C.c_float, _I, _I, _S]),
+    "pfb_group_norm_apply": (_I, [_P, _P, _P, _P, _P, _P, _P, _I, _I, _I, _I, _I, C.c_float, _I, _I, _S]),
+    "pfb_upsample2x_concat": (_I, [_P, _I, _P, _I, _P, _I, _I, _I, _I, _S]),
+    "pfb_convex_upsample2x": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
+    "pfb_downflow": (_I, [_P, _P, _I, _I, _I, _I, _I, _S]),
+    "pfb_msraft_workspace_bytes": (C.c_size_t, [C.POINTER(RaftCfg)]),
+    "pfb_msraft_refine": (_I, [C.POINTER(RaftCfg), C.POINTER(RaftWeights), C.POINTER(RaftBuffers), C.c_float, _P, _S]),
+    "pfb_msraft_update_iter": (_I, [C.POINTER(RaftCfg), C.POINTER(RaftWeights), C.POINTER(RaftBuffers), _P, _P, C.c_float, _S]),
 }
 
 

@@ -373,7 +373,7 @@ int corr_volume_simt(const void* f1, const void* f2, void* const* pyr, int B, in
 }
 
 int corr_onthefly_simt_flagged(const void* fmap1, void* const* pyr, const float* coords, void* out, const unsigned char* flags, int B, int H,
-                               int W, int C, int levels, int radius, pfb_dtype dtype, int out_stride, cudaStream_t s);
+                               int W, int C, int levels, int radius, pfb_dtype dtype, int out_stride, cudaStream_t s, float scale);
 
 }  // namespace pfb
 
@@ -509,6 +509,13 @@ extern "C" PFB_API int pfb_corr_lookup_onthefly(const void* fmap1, void* const* 
                                         void* out, int B, int H, int W, int C, int levels, int radius,
                                         pfb_dtype dtype, pfb_dtype out_dtype, int out_nchw, int out_stride,
                                         pfb_stream stream) {
+  return pfb_corr_lookup_onthefly_ex(fmap1, fmap2_pyramid, coords, out, B, H, W, C, levels, radius, 0.f, dtype, out_dtype, out_nchw,
+                                     out_stride, stream);
+}
+
+extern "C" PFB_API int pfb_corr_lookup_onthefly_ex(const void* fmap1, void* const* fmap2_pyramid, const float* coords, void* out, int B,
+                                                   int H, int W, int C, int levels, int radius, float scale, pfb_dtype dtype,
+                                                   pfb_dtype out_dtype, int out_nchw, int out_stride, pfb_stream stream) {
   PFB_CHECK_ARG(fmap1 && fmap2_pyramid && coords && out, "corr_lookup_onthefly: null pointer");
   PFB_CHECK_ARG(dtype_ok(dtype) && dtype_ok(out_dtype), "corr_lookup_onthefly: bad dtype");
   PFB_CHECK_ARG(B > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0, "corr_lookup_onthefly: C=%d must be a positive multiple of 8", C);
@@ -519,7 +526,8 @@ extern "C" PFB_API int pfb_corr_lookup_onthefly(const void* fmap1, void* const* 
   LevelTable lv;
   int rc = fill_levels(lv, fmap2_pyramid, H, W, levels);
   PFB_CHECK_ARG(rc == 0, "corr_lookup_onthefly: fmap2 level missing or empty (rc=%d)", rc);
-  const float scale = 1.0f / sqrtf((float)C);
+  PFB_CHECK_ARG(scale >= 0.f, "corr_lookup_onthefly: scale=%g", (double)scale);
+  if (scale == 0.f) scale = 1.0f / sqrtf((float)C);
   PFB_DISPATCH_DTYPE(dtype, T, {
     return launch_onthefly_t<T>(fmap1, lv, coords, out, B * H * W, H * W, C, levels, radius, scale, out_dtype,
                                 out_nchw, out_stride, as_stream(stream));
@@ -548,13 +556,13 @@ extern "C" PFB_API int pfb_alt_corr_forward(const void* fmap1, const void* fmap2
 
 namespace pfb {
 int corr_onthefly_simt_flagged(const void* fmap1, void* const* pyr, const float* coords, void* out, const unsigned char* flags, int B, int H,
-                               int W, int C, int levels, int radius, pfb_dtype dtype, int out_stride, cudaStream_t s) {
+                               int W, int C, int levels, int radius, pfb_dtype dtype, int out_stride, cudaStream_t s, float scale) {
   LevelTable lv;
   if (fill_levels(lv, pyr, H, W, levels) != 0) {
     set_error("corr_onthefly (flagged pass): fmap2 level missing or empty");
     return PFB_ERR_ARG;
   }
-  const float scale = 1.0f / sqrtf((float)C);
+  if (scale == 0.f) scale = 1.0f / sqrtf((float)C);
   PFB_DISPATCH_DTYPE(dtype, T, {
     return launch_onthefly_t<T>(fmap1, lv, coords, out, B * H * W, H * W, C, levels, radius, scale, dtype, 0, out_stride, s, flags);
   });

@@ -398,7 +398,7 @@ corr_onthefly_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
 
 // ------------------------------------------------------------------------------------------------
 int corr_onthefly_simt_flagged(const void* fmap1, void* const* pyr, const float* coords, void* out, const unsigned char* flags, int B, int H,
-                               int W, int C, int levels, int radius, pfb_dtype dtype, int out_stride, cudaStream_t s);  // corr.cu
+                               int W, int C, int levels, int radius, pfb_dtype dtype, int out_stride, cudaStream_t s, float scale);  // corr.cu
 
 bool corr_onthefly_umma_supported(int B, int H, int W, int C, int levels, int radius, pfb_dtype dt, int out_stride) {
   if (dt != PFB_F16 && dt != PFB_BF16) return false;
@@ -409,11 +409,11 @@ bool corr_onthefly_umma_supported(int B, int H, int W, int C, int levels, int ra
 }
 
 int corr_onthefly_umma(const void* fmap1, void* const* pyr, const float* coords, void* out, unsigned char* flags, int B, int H, int W, int C,
-                       int levels, pfb_dtype dt, int out_stride, cudaStream_t s) {
+                       int levels, pfb_dtype dt, int out_stride, cudaStream_t s, float scale) {
   OtfArgs a{};
   a.coords = coords; a.out = out; a.flags = flags;
   a.B = B; a.H = H; a.W = W; a.kchunks = C / 64; a.levels = levels; a.out_stride = out_stride;
-  a.scale = 1.0f / sqrtf((float)C);
+  a.scale = scale != 0.f ? scale : 1.0f / sqrtf((float)C);  // fmap rows wider than the features (zero channels) pass the real C's
   a.tiles_x = ceil_div(W, 16); a.tiles_y = ceil_div(H, 8); a.n_tiles = a.tiles_x * a.tiles_y * B;
   CUtensorMap tmA, tmB[4];
   {
@@ -475,7 +475,7 @@ int corr_onthefly_umma(const void* fmap1, void* const* pyr, const float* coords,
     }
   }
   // queries whose windows did not fit their tile's region: the SIMT kernel, one warp per flagged query
-  return corr_onthefly_simt_flagged(fmap1, pyr, coords, out, flags, B, H, W, C, levels, 4, dt, out_stride, s);
+  return corr_onthefly_simt_flagged(fmap1, pyr, coords, out, flags, B, H, W, C, levels, 4, dt, out_stride, s, a.scale);
 }
 
 }  // namespace pfb
@@ -487,8 +487,16 @@ extern "C" PFB_API size_t pfb_corr_lookup_onthefly_tc_workspace_bytes(int B, int
 extern "C" PFB_API int pfb_corr_lookup_onthefly_tc(const void* fmap1, void* const* fmap2_pyramid, const float* coords, void* out,
                                                    void* workspace, int B, int H, int W, int C, int levels, int radius, pfb_dtype dtype,
                                                    int out_stride, pfb_stream stream) {
+  return pfb_corr_lookup_onthefly_tc_ex(fmap1, fmap2_pyramid, coords, out, workspace, B, H, W, C, levels, radius, 0.f, dtype, out_stride,
+                                        stream);
+}
+
+extern "C" PFB_API int pfb_corr_lookup_onthefly_tc_ex(const void* fmap1, void* const* fmap2_pyramid, const float* coords, void* out,
+                                                      void* workspace, int B, int H, int W, int C, int levels, int radius, float scale,
+                                                      pfb_dtype dtype, int out_stride, pfb_stream stream) {
   using namespace pfb;
   PFB_CHECK_ARG(fmap1 && fmap2_pyramid && coords && out && workspace, "corr_lookup_onthefly_tc: null pointer");
+  PFB_CHECK_ARG(scale >= 0.f, "corr_lookup_onthefly_tc: scale=%g", (double)scale);
   for (int l = 0; l < levels && l < 4; ++l) PFB_CHECK_ARG(fmap2_pyramid[l], "corr_lookup_onthefly_tc: fmap2 level %d is null", l);
   PFB_CHECK_ARG((H >> (levels - 1)) >= 1 && (W >> (levels - 1)) >= 1, "corr_lookup_onthefly_tc: grid too small for %d levels", levels);
   if (!corr_onthefly_umma_supported(B, H, W, C, levels, radius, dtype, out_stride)) {
@@ -496,5 +504,5 @@ extern "C" PFB_API int pfb_corr_lookup_onthefly_tc(const void* fmap1, void* cons
     return PFB_ERR_UNSUPPORTED;
   }
   return corr_onthefly_umma(fmap1, fmap2_pyramid, coords, out, reinterpret_cast<unsigned char*>(workspace), B, H, W, C, levels, dtype, out_stride,
-                            as_stream(stream));
+                            as_stream(stream), scale);
 }

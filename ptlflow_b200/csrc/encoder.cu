@@ -168,18 +168,40 @@ __device__ __forceinline__ void store8<float>(float* p, const float (&f)[8]) {
 
 // scale/shift source: the accumulated instance-norm sums (stats != null: mean / rstd recomputed per thread for its 8
 // channels -- two fp64 loads each, cheaper than a separate finalize launch), or a per-channel bias (scale 1).
+// Group norm (stats != null and group > 1 or an affine / bias given): the per-channel sums of x are combined over the `group`
+// channels of each group, with the producer's per-channel bias folded in analytically (x + bias is what is normalised: a bias
+// differs between the channels of a group, so unlike instance norm it is not removed by the mean), then gamma / beta.
 template <typename T>
 __global__ void __launch_bounds__(256) affine_act_kernel(const T* __restrict__ x, const double* __restrict__ stats,
                                                          const float* __restrict__ bias, const T* __restrict__ residual,
-                                                         T* __restrict__ y, int HW, int C, float eps, int relu, int pix_per_block) {
+                                                         T* __restrict__ y, int HW, int C, float eps, int relu, int pix_per_block,
+                                                         const float* __restrict__ gamma, const float* __restrict__ beta, int group) {
   const int b = blockIdx.y;
   const int c8n = C / 8;
   const int lanes = blockDim.x / c8n;
   const int co = threadIdx.x % c8n, pl = threadIdx.x / c8n;
   __shared__ float2 ss_sm[512];
+  const bool gn = stats && (group > 1 || gamma || bias);
   for (int c = threadIdx.x; c < C; c += blockDim.x) {  // one fp64 mean / variance per channel and block, not per thread
     float2 v = make_float2(1.f, bias ? __ldg(bias + c) : 0.f);
-    if (stats) {
+    if (gn) {
+      const int c0 = c - c % group;
+      double s = 0.0, q = 0.0;
+      for (int k = c0; k < c0 + group; ++k) {
+        const double2 sq = *reinterpret_cast<const double2*>(stats + ((size_t)b * C + k) * 2);
+        const double bk = bias ? (double)__ldg(bias + k) : 0.0;
+        s += sq.x + bk * HW;
+        q += sq.y + 2.0 * bk * sq.x + bk * bk * HW;
+      }
+      const double n = (double)HW * group;
+      const double mean = s / n;
+      double var = q / n - mean * mean;
+      var = var < 0 ? 0 : var;
+      const double rstd = (double)rsqrtf((float)var + eps);
+      const double g = gamma ? (double)__ldg(gamma + c) : 1.0, be = beta ? (double)__ldg(beta + c) : 0.0;
+      const double bc = bias ? (double)__ldg(bias + c) : 0.0;
+      v = make_float2((float)(rstd * g), (float)((bc - mean) * rstd * g + be));
+    } else if (stats) {
       const double2 sq = *reinterpret_cast<const double2*>(stats + ((size_t)b * C + c) * 2);
       const double mean = sq.x / HW;
       double var = sq.y / HW - mean * mean;
@@ -363,10 +385,23 @@ extern "C" PFB_API size_t pfb_instance_norm_workspace_bytes(int B, int C) {
 
 template <typename T>
 static int launch_affine(const void* x, const double* stats, const float* bias, const void* residual, void* y, int B, int HW, int C,
-                         float eps, int relu, cudaStream_t s) {
+                         float eps, int relu, cudaStream_t s, const float* gamma = nullptr, const float* beta = nullptr, int group = 1) {
   const int ppb = HW >= 8192 ? 512 : (HW >= 1024 ? 128 : 32);
   dim3 grid(ceil_div(HW, ppb), B);
-  affine_act_kernel<T><<<grid, 256, 0, s>>>((const T*)x, stats, bias, (const T*)residual, (T*)y, HW, C, eps, relu, ppb);
+  affine_act_kernel<T><<<grid, 256, 0, s>>>((const T*)x, stats, bias, (const T*)residual, (T*)y, HW, C, eps, relu, ppb, gamma, beta, group);
+  PFB_LAUNCH_CHECK();
+  return PFB_OK;
+}
+
+// per-(image, channel) sums of x into the zeroed workspace (instance norm and group norm share them)
+static int launch_stats(const void* x, double* stats, int B, int HW, int C, pfb_dtype dtype, cudaStream_t s) {
+  // plenty of blocks, few global atomics (fewer, fatter blocks were measured slower: r01 launch list v19)
+  const int threads = 256;
+  static const int env_ppb = getenv("PFB_STATS_PPB") ? atoi(getenv("PFB_STATS_PPB")) : 0;  // tuning knob
+  const int ppb = env_ppb > 0 && HW >= 8192 ? env_ppb : (HW >= 65536 ? 1536 : (HW >= 8192 ? 768 : (HW >= 1024 ? 256 : 64)));
+  dim3 grid(ceil_div(HW, ppb), B);
+  ProfScope prof(KC_ENC_STATS, s);
+  PFB_DISPATCH_DTYPE(dtype, T, { inorm_stats_kernel<T><<<grid, threads, 2 * C * sizeof(float), s>>>((const T*)x, stats, HW, C, ppb); });
   PFB_LAUNCH_CHECK();
   return PFB_OK;
 }
@@ -404,16 +439,8 @@ extern "C" PFB_API int pfb_instance_norm_act(const void* x, void* y, const void*
       return PFB_OK;
     }
   }
-  // plenty of blocks, few global atomics (fewer, fatter blocks were measured slower: r01 launch list v19)
-  const int threads = 256;
-  static const int env_ppb = getenv("PFB_STATS_PPB") ? atoi(getenv("PFB_STATS_PPB")) : 0;  // tuning knob
-  const int ppb = env_ppb > 0 && HW >= 8192 ? env_ppb : (HW >= 65536 ? 1536 : (HW >= 8192 ? 768 : (HW >= 1024 ? 256 : 64)));
-  dim3 grid(ceil_div(HW, ppb), B);
-  {
-    ProfScope prof(KC_ENC_STATS, s);
-    PFB_DISPATCH_DTYPE(dtype, T, { inorm_stats_kernel<T><<<grid, threads, 2 * C * sizeof(float), s>>>((const T*)x, stats, HW, C, ppb); });
-  }
-  PFB_LAUNCH_CHECK();
+  int rc = launch_stats(x, stats, B, HW, C, dtype, s);
+  if (rc != PFB_OK) return rc;
   ProfScope prof(KC_ENC_AFFINE, s);
   PFB_DISPATCH_DTYPE(dtype, T, { return launch_affine<T>(x, stats, nullptr, residual, y, B, HW, C, eps, relu, s); });
   return PFB_OK;
@@ -431,6 +458,45 @@ extern "C" PFB_API int pfb_instance_norm_apply(const void* x, void* y, const voi
   double* stats = reinterpret_cast<double*>(workspace);
   ProfScope prof(KC_ENC_AFFINE, s);
   PFB_DISPATCH_DTYPE(dtype, T, { return launch_affine<T>(x, stats, nullptr, residual, y, B, HW, C, eps, relu, s); });
+  return PFB_OK;
+}
+
+static int check_group_norm(const void* x, const void* y, const void* workspace, int B, int H, int W, int C, int group_size,
+                            pfb_dtype dtype, const char* what) {
+  PFB_CHECK_ARG(x && y && workspace, "%s: null pointer", what);
+  PFB_CHECK_ARG(dtype_ok(dtype) && B > 0 && H > 0 && W > 0 && C > 0 && C % 8 == 0 && C <= 512 && B <= 65535,
+                "%s: bad shape (C=%d must be a multiple of 8, <= 512)", what, C);
+  PFB_CHECK_ARG(group_size >= 1 && C % group_size == 0, "%s: group_size=%d must divide C=%d", what, group_size, C);
+  return PFB_OK;
+}
+
+// Group norm: statistics per (image, group of group_size channels) of x + bias, then gamma / beta, then act / residual join.
+extern "C" PFB_API int pfb_group_norm_act(const void* x, void* y, const void* residual, void* workspace, const float* bias,
+                                          const float* gamma, const float* beta, int B, int H, int W, int C, int group_size, float eps,
+                                          int relu, pfb_dtype dtype, pfb_stream stream) {
+  int rc = check_group_norm(x, y, workspace, B, H, W, C, group_size, dtype, "group_norm_act");
+  if (rc != PFB_OK) return rc;
+  cudaStream_t s = as_stream(stream);
+  double* stats = reinterpret_cast<double*>(workspace);
+  PFB_CUDA(cudaMemsetAsync(stats, 0, (size_t)B * C * 2 * sizeof(double), s));
+  rc = launch_stats(x, stats, B, H * W, C, dtype, s);
+  if (rc != PFB_OK) return rc;
+  ProfScope prof(KC_ENC_AFFINE, s);
+  PFB_DISPATCH_DTYPE(dtype, T, { return launch_affine<T>(x, stats, bias, residual, y, B, H * W, C, eps, relu, s, gamma, beta, group_size); });
+  return PFB_OK;
+}
+
+extern "C" PFB_API int pfb_group_norm_apply(const void* x, void* y, const void* residual, void* workspace, const float* bias,
+                                            const float* gamma, const float* beta, int B, int H, int W, int C, int group_size, float eps,
+                                            int relu, pfb_dtype dtype, pfb_stream stream) {
+  int rc = check_group_norm(x, y, workspace, B, H, W, C, group_size, dtype, "group_norm_apply");
+  if (rc != PFB_OK) return rc;
+  cudaStream_t s = as_stream(stream);
+  ProfScope prof(KC_ENC_AFFINE, s);
+  PFB_DISPATCH_DTYPE(dtype, T, {
+    return launch_affine<T>(x, reinterpret_cast<const double*>(workspace), bias, residual, y, B, H * W, C, eps, relu, s, gamma, beta,
+                            group_size);
+  });
   return PFB_OK;
 }
 

@@ -33,6 +33,8 @@ struct Workspace {
 };
 
 static int heads_of(const pfb_raft_cfg* c) { return c->num_heads > 0 ? c->num_heads : 1; }
+// channels of the convex-upsample mask: 9 taps x 8 x 8 (raft, gma), 9 taps x 2 x 2 (ms_raft_plus, variant 5)
+static int mask_channels(const pfb_raft_cfg* c) { return c->variant == 5 ? 36 : 576; }
 
 static Workspace plan(const pfb_raft_cfg* c) {
   Workspace w{};
@@ -43,7 +45,7 @@ static Workspace plan(const pfb_raft_cfg* c) {
   w.planes = c->corr_levels * K * K;
   // 16-byte aligned rows for the tensor-core path (the TMA unit zero-fills a partial last 64-channel K chunk itself)
   w.corr_stride = (c->dtype == PFB_F32) ? w.planes : (int)align_up(w.planes, 8);
-  if (c->variant == 0 || c->variant == 2) {
+  if (c->variant == 0 || c->variant == 2 || c->variant == 5) {
     w.c_cor1 = 256; w.c_cor2 = 192; w.c_flo1 = 128; w.c_flo2 = 64; w.c_fh = 256;
     // gma keeps [motion | motion_global] side by side so the GRU still sees three sources (update.py:150-151)
     w.c_motion = c->variant == 2 ? 256 : 128;
@@ -62,7 +64,7 @@ static Workspace plan(const pfb_raft_cfg* c) {
   w.off_rh = take(P * (size_t)c->hidden_dim * es);
   w.off_fh = take(P * (size_t)w.c_fh * es);
   w.off_mh = take(c->variant != 1 ? P * 256 * es : 0);
-  w.off_mask = take(c->variant != 1 ? P * 576 * es : 0);
+  w.off_mask = take(c->variant != 1 ? P * (size_t)mask_channels(c) * es : 0);
   w.off_flow = take(P * 2 * sizeof(float));
   w.off_taps = take(c->variant != 1 ? P * 32 * sizeof(float) : 0);
   w.n_pad = (int)align_up((size_t)c->H * c->W, 64);
@@ -76,9 +78,11 @@ static Workspace plan(const pfb_raft_cfg* c) {
   return w;
 }
 
-static int check_cfg(const pfb_raft_cfg* c) {
+// variant 5 (ms_raft_plus) only through the pfb_msraft_* entry points, 0..2 only through the pfb_raft_* ones
+static int check_cfg(const pfb_raft_cfg* c, bool msraft = false) {
   PFB_CHECK_ARG(c, "raft: null cfg");
-  PFB_CHECK_ARG(c->variant >= 0 && c->variant <= 2, "raft: variant=%d", c->variant);
+  if (msraft) PFB_CHECK_ARG(c->variant == 5, "msraft: variant=%d (the ms_raft_plus loop is variant 5)", c->variant);
+  else PFB_CHECK_ARG(c->variant >= 0 && c->variant <= 2, "raft: variant=%d", c->variant);
   PFB_CHECK_ARG(dtype_ok(c->dtype), "raft: bad dtype");
   PFB_CHECK_ARG(c->B > 0 && c->H > 0 && c->W > 0, "raft: bad grid %dx%dx%d", c->B, c->H, c->W);
   PFB_CHECK_ARG(c->corr_levels >= 1 && c->corr_levels <= PFB_MAX_LEVELS && c->corr_radius >= 0 && c->corr_radius <= 15,
@@ -101,6 +105,7 @@ struct Ctx {
   Workspace ws;
   char* base;
   cudaStream_t s;
+  float corr_scale = 0.f;  // on-the-fly lookup scale (0: 1/sqrt(feat_dim))
   // flow branch of the motion encoder on a second stream (fork_flow_branch): null when not forked
   cudaStream_t side = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -188,17 +193,17 @@ static int run_context_terms(const Ctx& x) {
 }
 
 int raft_lookup(const pfb_raft_cfg* c, void* const* pyramid, const void* fmap1, const float* coords, void* out, int out_stride,
-                void* flags, cudaStream_t s) {
+                void* flags, cudaStream_t s, float scale) {
   if (c->alternate_corr) {
     static const int env_tc = getenv("PFB_ONTHEFLY_TC") ? atoi(getenv("PFB_ONTHEFLY_TC")) : 1;
     if (env_tc && c->impl != 1 && corr_onthefly_umma_supported(c->B, c->H, c->W, c->feat_dim, c->corr_levels, c->corr_radius, c->dtype, out_stride))
-      return pfb_corr_lookup_onthefly_tc(fmap1, pyramid, coords, out, flags, c->B, c->H, c->W,
-                                         c->feat_dim, c->corr_levels, c->corr_radius, c->dtype, out_stride, (pfb_stream)s);
+      return pfb_corr_lookup_onthefly_tc_ex(fmap1, pyramid, coords, out, flags, c->B, c->H, c->W,
+                                            c->feat_dim, c->corr_levels, c->corr_radius, scale, c->dtype, out_stride, (pfb_stream)s);
   }
   if (c->alternate_corr)
-    return pfb_corr_lookup_onthefly(fmap1, pyramid, coords, out, c->B, c->H, c->W,
-                                    c->feat_dim, c->corr_levels, c->corr_radius, c->dtype, c->dtype, 0,
-                                    out_stride, (pfb_stream)s);
+    return pfb_corr_lookup_onthefly_ex(fmap1, pyramid, coords, out, c->B, c->H, c->W,
+                                       c->feat_dim, c->corr_levels, c->corr_radius, scale, c->dtype, c->dtype, 0,
+                                       out_stride, (pfb_stream)s);
   if (c->volume_layout == 1)
     return pfb_corr_lookup_tiled(pyramid, coords, out, c->B, c->H, c->W, c->H, c->W, c->corr_levels,
                                  c->corr_radius, c->dtype, out_stride, (pfb_stream)s);
@@ -207,7 +212,8 @@ int raft_lookup(const pfb_raft_cfg* c, void* const* pyramid, const void* fmap1, 
 }
 
 static int lookup(const Ctx& x) {
-  return raft_lookup(x.c, x.b->pyramid, x.b->fmap1, x.b->coords, x.at(x.ws.off_corr), x.ws.corr_stride, x.at(x.ws.off_flags), x.s);
+  return raft_lookup(x.c, x.b->pyramid, x.b->fmap1, x.b->coords, x.at(x.ws.off_corr), x.ws.corr_stride, x.at(x.ws.off_flags), x.s,
+                     x.corr_scale);
 }
 
 int gma_aggregate(const pfb_raft_cfg* c, const pfb_layer& agg_v, const pfb_layer& agg_proj, const void* attention_ptr, float gamma,
@@ -373,7 +379,7 @@ static int update_iter(const Ctx& x, const void* corr_ext, void* mask_out) {
     PFB_CUDA(cudaStreamWaitEvent(x.side, x.ev_fork, 0));
     void* mh = x.at(ws.off_mh);
     PFB_TRY(run_conv(xf, PFB_L_MASK1, {src_of(x.b->net, hd, hd)}, PFB_EPI_RELU, mh, 256, 0));
-    PFB_TRY(run_conv(xf, PFB_L_MASK2, {src_of(mh, 256, 256)}, PFB_EPI_LINEAR, mask_out, 576, 0, 0.25f));
+    PFB_TRY(run_conv(xf, PFB_L_MASK2, {src_of(mh, 256, 256)}, PFB_EPI_LINEAR, mask_out, mask_channels(c), 0, 0.25f));
     PFB_CUDA(cudaEventRecord(x.ev_join, x.side));
   }
   PFB_TRY(run_conv(x, PFB_L_FLOW1, {src_of(x.b->net, hd, hd)}, PFB_EPI_RELU, fh, ws.c_fh, 0));
@@ -391,14 +397,14 @@ static int update_iter(const Ctx& x, const void* corr_ext, void* mask_out) {
   } else if (mask_out && c->variant != 1) {
     void* mh = x.at(ws.off_mh);
     PFB_TRY(run_conv(x, PFB_L_MASK1, {src_of(x.b->net, hd, hd)}, PFB_EPI_RELU, mh, 256, 0));
-    PFB_TRY(run_conv(x, PFB_L_MASK2, {src_of(mh, 256, 256)}, PFB_EPI_LINEAR, mask_out, 576, 0, 0.25f));
+    PFB_TRY(run_conv(x, PFB_L_MASK2, {src_of(mh, 256, 256)}, PFB_EPI_LINEAR, mask_out, mask_channels(c), 0, 0.25f));
   }
   return PFB_OK;
 }
 
 static int make_ctx(Ctx& x, const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf,
-                    cudaStream_t s, bool need_pyramid) {
-  PFB_TRY(check_cfg(cfg));
+                    cudaStream_t s, bool need_pyramid, bool msraft = false) {
+  PFB_TRY(check_cfg(cfg, msraft));
   PFB_CHECK_ARG(w && buf, "raft: null weights/buffers");
   PFB_CHECK_ARG(buf->net && buf->inp && buf->coords && buf->workspace, "raft: null state buffer");
   if (need_pyramid) {
@@ -431,14 +437,10 @@ extern "C" PFB_API int pfb_raft_update_iter(const pfb_raft_cfg* cfg, const pfb_r
   return update_iter(x, corr, mask_out);
 }
 
-extern "C" PFB_API int pfb_raft_refine(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf,
-                               pfb_stream stream) {
-  Ctx x;
-  PFB_TRY(make_ctx(x, cfg, w, buf, as_stream(stream), true));
-  PFB_CHECK_ARG(buf->flow_up, "raft_refine: null flow_up");
-  PFB_CHECK_ARG(cfg->variant == 1 || cfg->iters >= 1, "raft_refine: the convex upsample needs at least one iteration (mask)");
-  PFB_TRY(launch_flow_from_coords(buf->coords, reinterpret_cast<float*>(x.at(x.ws.off_flow)), cfg->B, cfg->H, cfg->W, x.s));
-  void* mask = cfg->variant != 1 ? x.at(x.ws.off_mask) : nullptr;
+// flow from the entry coordinates, the once-per-call context terms, then cfg->iters iterations (the mask head on the last one only)
+static int run_iterations(Ctx& x, void* mask) {
+  const pfb_raft_cfg* cfg = x.c;
+  PFB_TRY(launch_flow_from_coords(x.b->coords, reinterpret_cast<float*>(x.at(x.ws.off_flow)), cfg->B, cfg->H, cfg->W, x.s));
   PFB_TRY(fork_flow_setup(x));
   if (x.side) {
     // the once-per-forward context terms ride the side stream too: they are first read by the GRU of iteration 0, after that
@@ -459,9 +461,60 @@ extern "C" PFB_API int pfb_raft_refine(const pfb_raft_cfg* cfg, const pfb_raft_w
     PFB_TRY(lookup(x));
     PFB_TRY(update_iter(x, nullptr, it == cfg->iters - 1 ? mask : nullptr));
   }
+  return PFB_OK;
+}
+
+extern "C" PFB_API int pfb_raft_refine(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf,
+                               pfb_stream stream) {
+  Ctx x;
+  PFB_TRY(make_ctx(x, cfg, w, buf, as_stream(stream), true));
+  PFB_CHECK_ARG(buf->flow_up, "raft_refine: null flow_up");
+  PFB_CHECK_ARG(cfg->variant == 1 || cfg->iters >= 1, "raft_refine: the convex upsample needs at least one iteration (mask)");
+  void* mask = cfg->variant != 1 ? x.at(x.ws.off_mask) : nullptr;
+  PFB_TRY(run_iterations(x, mask));
   if (cfg->variant != 1)
     return pfb_convex_upsample(buf->coords, mask, buf->flow_up, buf->flow_small, cfg->B, cfg->H, cfg->W, cfg->out_h,
                                cfg->out_w, cfg->pad_top, cfg->pad_left, cfg->dtype, stream);
   return pfb_upflow8(buf->coords, buf->flow_up, buf->flow_small, cfg->B, cfg->H, cfg->W, cfg->out_h, cfg->out_w,
                      cfg->pad_top, cfg->pad_left, stream);
+}
+
+// ---- a17: MS-RAFT+ (one call per scale of ms_raft_plus.py:177-214) ----
+extern "C" PFB_API size_t pfb_msraft_workspace_bytes(const pfb_raft_cfg* cfg) {
+  if (check_cfg(cfg, true) != PFB_OK) return 0;
+  return plan(cfg).total;
+}
+
+extern "C" PFB_API int pfb_msraft_update_iter(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf,
+                                              const void* corr, void* mask_out, float corr_scale, pfb_stream stream) {
+  Ctx x;
+  PFB_TRY(make_ctx(x, cfg, w, buf, as_stream(stream), corr == nullptr, true));
+  PFB_CHECK_ARG(corr_scale >= 0.f, "msraft_update_iter: corr_scale=%g", (double)corr_scale);
+  x.corr_scale = corr_scale;
+  PFB_TRY(launch_flow_from_coords(buf->coords, reinterpret_cast<float*>(x.at(x.ws.off_flow)), cfg->B, cfg->H, cfg->W, x.s));
+  PFB_TRY(run_context_terms(x));
+  if (!corr) PFB_TRY(lookup(x));
+  return update_iter(x, corr, mask_out);
+}
+
+extern "C" PFB_API int pfb_msraft_refine(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf, float corr_scale,
+                                         float* next_coords, pfb_stream stream) {
+  Ctx x;
+  PFB_TRY(make_ctx(x, cfg, w, buf, as_stream(stream), true, true));
+  PFB_CHECK_ARG(cfg->iters >= 1, "msraft_refine: every scale needs at least one iteration (iters=%d)", cfg->iters);
+  PFB_CHECK_ARG(corr_scale >= 0.f, "msraft_refine: corr_scale=%g", (double)corr_scale);
+  PFB_CHECK_ARG(next_coords || buf->flow_up, "msraft_refine: needs next_coords (coarser scales) or flow_up (the finest)");
+  if (!next_coords && buf->flow_small)
+    PFB_CHECK_ARG(cfg->out_h >= 16 && cfg->out_w >= 16, "msraft_refine: output %dx%d smaller than 16 px per side", cfg->out_h, cfg->out_w);
+  x.corr_scale = corr_scale;
+  void* mask = x.at(x.ws.off_mask);
+  PFB_TRY(run_iterations(x, mask));
+  if (next_coords)  // handover: the absolute coordinates, doubled and convex-upsampled with zero-padded taps (ms_raft_plus.py:198-200)
+    return pfb_convex_upsample2x(buf->coords, mask, next_coords, 1, cfg->B, cfg->H, cfg->W, 0, 0, 0, 0, cfg->dtype, stream);
+  PFB_TRY(pfb_convex_upsample2x(buf->coords, mask, buf->flow_up, 0, cfg->B, cfg->H, cfg->W, cfg->out_h, cfg->out_w, cfg->pad_top,
+                                cfg->pad_left, cfg->dtype, stream));
+  if (!buf->flow_small) return PFB_OK;
+  // flow_small = downflow(flow_up, 1/16) at int(h / 16) x int(w / 16) of the un-padded size (ms_raft_plus.py:22-35, 221-224)
+  const int sh = cfg->out_h / 16, sw = cfg->out_w / 16;
+  return pfb_downflow(buf->flow_up, buf->flow_small, cfg->B, cfg->out_h, cfg->out_w, sh, sw, stream);
 }

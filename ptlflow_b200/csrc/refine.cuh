@@ -9,8 +9,9 @@ int launch_flow_from_coords(const float* coords, float* flow, int B, int H, int 
 
 // The multi-scale lookup of the loop configured by `c` (dense, tiled or on-the-fly pyramid, as pfb_raft_refine picks it) into
 // out [B,H,W,out_stride] (storage type); flags: the on-the-fly tensor-core lookup's per-query workspace (alternate_corr only).
+// scale: the on-the-fly lookup's scale, 0 = 1/sqrt(feat_dim) (ms_raft_plus passes the real C when its rows carry zero channels).
 int raft_lookup(const pfb_raft_cfg* c, void* const* pyramid, const void* fmap1, const float* coords, void* out, int out_stride,
-                void* flags, cudaStream_t s);
+                void* flags, cudaStream_t s, float scale = 0.f);
 
 // GMA Aggregate (gma_utils.py:79-113): motion_global = motion + gamma * project(attn_h @ to_v(motion)_h), written into the
 // motion buffer itself.  motion [B,H,W,motion_stride]: the motion features from channel motion_offset, motion_global to channels

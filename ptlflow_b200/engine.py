@@ -420,3 +420,58 @@ class SEARaftEngine(RaftEngine):
         b.pw1 = self._layer(ops.PackedConv([pw1], dtype, device, src_channels=[C]))
         b.out = self._layer(ops.PackedConv([out], dtype, device, src_channels=[4 * Wf.shape[0], C]))
         return b
+
+
+class MSRaftEngine(RaftEngine):
+    """MS-RAFT+'s update block (ms_raft_plus/update.py:119-153: RAFT's BasicUpdateBlock with convc1 over levels * (2r+1)^2 planes and
+    a 36-channel mask head) packed exactly as RaftEngine packs raft's, driven one scale at a time through pfb_msraft_refine
+    (pfb_raft_cfg variant 5)."""
+
+    _ws_symbol, _refine_symbol, _iter_symbol = "pfb_msraft_workspace_bytes", "pfb_msraft_refine", "pfb_msraft_update_iter"
+
+    def __init__(self, update_block: torch.nn.Module, variant: int, hidden_dim: int, context_dim: int, corr_levels: int, corr_radius: int,
+                 dtype: torch.dtype, device: torch.device, impl: int = 0, attention_module: Optional[torch.nn.Module] = None):
+        super().__init__(update_block, 0, hidden_dim, context_dim, corr_levels, corr_radius, dtype, device, impl=impl)  # raft's packing
+        self.variant = variant
+
+    def refine_scale(self, pyramid: Sequence[torch.Tensor], net: torch.Tensor, inp: torch.Tensor, coords: torch.Tensor, iters: int,
+                     out_hw, pad, ws: torch.Tensor, fmap1: Optional[torch.Tensor] = None, corr_scale: float = 0.0,
+                     volume_layout: int = 0, last: bool = False):
+        """One scale in place on (net, coords).  Not last: returns the next scale's coordinates fp32 [B,2H,2W,2].  Last: returns
+        (flow_up fp32 [B,2,oh,ow], flow_small fp32 [B,2,oh//16,ow//16])."""
+        B, H, W, _ = net.shape
+        alt = fmap1 is not None
+        cfg = self.make_cfg(B, H, W, iters, out_hw, pad, alt, fmap1.shape[-1] if alt else 0, volume_layout)
+        flow_up = flow_small = nxt = None
+        if last:
+            flow_up = torch.empty((B, 2, out_hw[0], out_hw[1]), dtype=torch.float32, device=self.device)
+            flow_small = torch.empty((B, 2, out_hw[0] // 16, out_hw[1] // 16), dtype=torch.float32, device=self.device)
+        else:
+            nxt = torch.empty((B, 2 * H, 2 * W, 2), dtype=torch.float32, device=self.device)
+        pyr = ptr_array(pyramid)
+        buf = _lib.RaftBuffers(C.cast(pyr, C.POINTER(C.c_void_p)), fmap1.data_ptr() if alt else None, net.data_ptr(), inp.data_ptr(),
+                               coords.data_ptr(), flow_up.data_ptr() if last else None, flow_small.data_ptr() if last else None,
+                               ws.data_ptr(), ws.numel(), None, 0.0)
+        with torch.cuda.device(self.device):
+            check(load().pfb_msraft_refine(C.byref(cfg), C.byref(self.weights), C.byref(buf), corr_scale,
+                                           nxt.data_ptr() if nxt is not None else None, stream_ptr(self.device)), "msraft_refine")
+        return (flow_up, flow_small) if last else nxt
+
+    def update_iter(self, net: torch.Tensor, inp: torch.Tensor, coords: torch.Tensor, corr: Optional[torch.Tensor] = None,
+                    pyramid: Optional[Sequence[torch.Tensor]] = None, want_mask: bool = False, attention: Optional[torch.Tensor] = None,
+                    fmap1: Optional[torch.Tensor] = None, corr_scale: float = 0.0):
+        """One update-block evaluation (operator-level tests); returns the [B,H,W,36] mask when asked."""
+        B, H, W, _ = net.shape
+        alt = fmap1 is not None
+        cfg = self.make_cfg(B, H, W, 1, (2 * H, 2 * W), (0, 0), alt, fmap1.shape[-1] if alt else 0)
+        ws = self.workspace(cfg)
+        mask = torch.empty((B, H, W, 36), dtype=self.dtype, device=self.device) if want_mask else None
+        pyr = ptr_array(pyramid) if pyramid is not None else None
+        buf = _lib.RaftBuffers(C.cast(pyr, C.POINTER(C.c_void_p)) if pyr is not None else None, fmap1.data_ptr() if alt else None,
+                               net.data_ptr(), inp.data_ptr(), coords.data_ptr(), None, None, ws.data_ptr(), ws.numel(), None, 0.0)
+        with torch.cuda.device(self.device):
+            check(load().pfb_msraft_update_iter(C.byref(cfg), C.byref(self.weights), C.byref(buf),
+                                                corr.data_ptr() if corr is not None else None,
+                                                mask.data_ptr() if mask is not None else None, corr_scale, stream_ptr(self.device)),
+                  "msraft_update_iter")
+        return mask

@@ -604,3 +604,106 @@ def bias_act(x: torch.Tensor, bias: Optional[torch.Tensor], relu: bool = True, r
                                   residual.data_ptr() if residual is not None else None, y.data_ptr(), ws.data_ptr(), B, H, W, Cc,
                                   int(relu), dtype_code(x.dtype), stream_ptr(x.device)), "bias_act")
     return y
+
+
+# ------------------------------------------------------------------------------------------
+# MS-RAFT+ (a17): group norm, the encoders' up-path resize, convex 2x, downflow, scaled on-the-fly lookups
+# ------------------------------------------------------------------------------------------
+def _opt_f32(t: Optional[torch.Tensor], n: int, name: str):
+    if t is None:
+        return None
+    if t.dtype != torch.float32 or t.numel() != n or not t.is_cuda or not t.is_contiguous():
+        raise RuntimeError(f"{name} must be a contiguous fp32 CUDA tensor of {n} elements")
+    return t.data_ptr()
+
+
+def group_norm_act(x: torch.Tensor, gamma: Optional[torch.Tensor], beta: Optional[torch.Tensor], group_size: int,
+                   bias: Optional[torch.Tensor] = None, relu: bool = True, residual: Optional[torch.Tensor] = None, eps: float = 1e-5,
+                   out: Optional[torch.Tensor] = None, stats_ws: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """x [B,H,W,C] -> act(GroupNorm(x + bias)) with ``group_size`` channels per group and the affine gamma / beta (fp32 [C] or
+    None), or relu(residual + act(...)).  ``stats_ws``: a workspace whose per-(image, channel) sums of x a producer already
+    accumulated (first_conv7x7s2); None computes them here."""
+    require_cuda(x, "x")
+    B, H, W, Cc = x.shape
+    y = out if out is not None else torch.empty_like(x)
+    if residual is not None:
+        require_cuda(residual, "residual")
+        assert residual.shape == x.shape
+    args = [_opt_f32(bias, Cc, "bias"), _opt_f32(gamma, Cc, "gamma"), _opt_f32(beta, Cc, "beta"), B, H, W, Cc, group_size, eps, int(relu),
+            dtype_code(x.dtype), stream_ptr(x.device)]
+    res = residual.data_ptr() if residual is not None else None
+    with torch.cuda.device(x.device):
+        if stats_ws is None:
+            ws = _scratch(("inorm", str(x.device), B * Cc), B * Cc * 3, x.device)
+            check(load().pfb_group_norm_act(x.data_ptr(), y.data_ptr(), res, ws.data_ptr(), *args), "group_norm_act")
+        else:
+            check(load().pfb_group_norm_apply(x.data_ptr(), y.data_ptr(), res, stats_ws.data_ptr(), *args), "group_norm_apply")
+    return y
+
+
+def upsample2x_concat(src: torch.Tensor, skip: Optional[torch.Tensor], out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """src [B,H,W,Cs], skip [B,2H,2W,Ck] -> cat[bilinear 2x (align_corners=False) of src, skip] along the channels."""
+    require_cuda(src, "src")
+    B, H, W, Cs = src.shape
+    Ck = 0 if skip is None else skip.shape[-1]
+    if skip is not None:
+        require_cuda(skip, "skip")
+        if tuple(skip.shape[:3]) != (B, 2 * H, 2 * W) or skip.dtype != src.dtype:
+            raise RuntimeError(f"upsample2x_concat: skip {tuple(skip.shape)} does not sit on the 2x grid of src {tuple(src.shape)}")
+    if out is None:
+        out = torch.empty((B, 2 * H, 2 * W, Cs + Ck), dtype=src.dtype, device=src.device)
+    require_cuda(out, "out")
+    with torch.cuda.device(src.device):
+        check(load().pfb_upsample2x_concat(src.data_ptr(), Cs, skip.data_ptr() if skip is not None else None, Ck, out.data_ptr(), B, H, W,
+                                           dtype_code(src.dtype), stream_ptr(src.device)), "upsample2x_concat")
+    return out
+
+
+def convex_upsample2x(coords: torch.Tensor, mask: torch.Tensor, mode: int = 0, out_hw=None, pad=(0, 0)) -> torch.Tensor:
+    """coords fp32 [B,H,W,2], mask [B,H,W,36] (x0.25 applied).  mode 0: flow window fp32 [B,2,oh,ow]; mode 1: the upsampled
+    absolute coordinates fp32 [B,2H,2W,2] (zero-padded taps)."""
+    require_cuda(coords, "coords"); require_cuda(mask, "mask")
+    B, H, W, _ = coords.shape
+    oh, ow = out_hw or (2 * H, 2 * W)
+    shape = (B, 2, oh, ow) if mode == 0 else (B, 2 * H, 2 * W, 2)
+    out = torch.empty(shape, dtype=torch.float32, device=coords.device)
+    with torch.cuda.device(coords.device):
+        check(load().pfb_convex_upsample2x(coords.data_ptr(), mask.data_ptr(), out.data_ptr(), mode, B, H, W, oh, ow, pad[0], pad[1],
+                                           dtype_code(mask.dtype), stream_ptr(coords.device)), "convex_upsample2x")
+    return out
+
+
+def downflow(flow: torch.Tensor, out_hw) -> torch.Tensor:
+    """flow fp32 [B,2,H,W] -> bilinear (align_corners=True) [B,2,oh,ow] with u x ow/W, v x oh/H (ms_raft_plus.py:22-35)."""
+    require_cuda(flow, "flow")
+    B, _, H, W = flow.shape
+    out = torch.empty((B, 2) + tuple(out_hw), dtype=torch.float32, device=flow.device)
+    with torch.cuda.device(flow.device):
+        check(load().pfb_downflow(flow.data_ptr(), out.data_ptr(), B, H, W, out_hw[0], out_hw[1], stream_ptr(flow.device)), "downflow")
+    return out
+
+
+def corr_lookup_onthefly_scaled(fmap1: torch.Tensor, fmap2_pyramid: Sequence[torch.Tensor], coords: torch.Tensor, radius: int, scale: float,
+                                tensor_cores: bool, out_stride: Optional[int] = None) -> torch.Tensor:
+    """The on-the-fly lookup (pixel-major [B,H,W,out_stride] output) with an explicit scale of the dot products: features stored in
+    rows with zero channels beyond their real width C pass 1/sqrt(C).  ``tensor_cores``: the wgmma kernel (+ its SIMT pass for
+    flagged queries), else the SIMT kernel."""
+    require_cuda(fmap1, "fmap1"); require_cuda(coords, "coords")
+    B, H, W, Cc = fmap1.shape
+    L = len(fmap2_pyramid)
+    planes = L * (2 * radius + 1) ** 2
+    stride = (planes + 7) // 8 * 8 if out_stride is None else out_stride
+    out = torch.empty((B, H, W, stride), dtype=fmap1.dtype, device=fmap1.device)
+    lib = load()
+    with torch.cuda.device(fmap1.device):
+        if tensor_cores:
+            ws = torch.empty(max(1, lib.pfb_corr_lookup_onthefly_tc_workspace_bytes(B, H, W)), dtype=torch.uint8, device=fmap1.device)
+            check(lib.pfb_corr_lookup_onthefly_tc_ex(fmap1.data_ptr(), ptr_array(fmap2_pyramid), coords.data_ptr(), out.data_ptr(),
+                                                     ws.data_ptr(), B, H, W, Cc, L, radius, scale, dtype_code(fmap1.dtype), stride,
+                                                     stream_ptr(fmap1.device)), "corr_lookup_onthefly_tc_ex")
+            out._pfb_flags = ws
+        else:
+            check(lib.pfb_corr_lookup_onthefly_ex(fmap1.data_ptr(), ptr_array(fmap2_pyramid), coords.data_ptr(), out.data_ptr(), B, H, W, Cc,
+                                                  L, radius, scale, dtype_code(fmap1.dtype), dtype_code(fmap1.dtype), 0, stride,
+                                                  stream_ptr(fmap1.device)), "corr_lookup_onthefly_ex")
+    return out
