@@ -350,7 +350,8 @@ typedef struct {
 typedef struct {
   int variant;        /* 0 = raft (BasicUpdateBlock, SepConvGRU, convex upsample)
                          1 = raft_small (SmallUpdateBlock, ConvGRU, bilinear upflow8)
-                         2 = gma (GMAUpdateBlock: raft + per-iteration attention aggregate, gma/update.py:127-160) */
+                         2 = gma (GMAUpdateBlock: raft + per-iteration attention aggregate, gma/update.py:127-160)
+                         (3 skflow, 4 sea_raft, 5 ms_raft_plus, 6 ccmr: their own entry points only) */
   pfb_dtype dtype;
   int B, H, W;        /* 1/8-resolution grid */
   int feat_dim;       /* C of fmap1/fmap2 (on-the-fly mode) */
@@ -517,6 +518,90 @@ PFB_API int pfb_msraft_refine(const pfb_raft_cfg* cfg, const pfb_raft_weights* w
  * [B,H,W,36] may be NULL. */
 PFB_API int pfb_msraft_update_iter(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf, const void* corr,
                                    void* mask_out, float corr_scale, pfb_stream stream);
+
+/* ------------------------------------------------------------------------------------
+ * a18: CCMR / CCMR+ (ptlflow/models/ccmr/ccmr.py:141-230): MS-RAFT+'s scale loop with XCiT global context (xcit.py:58-427).
+ * ---------------------------------------------------------------------------------- */
+/* The handover between scales (ccmr.py:195-202): pfb_convex_upsample2x of value = coords - grid, with zero-padded taps, plus the fine
+ * grid: out [B,2H,2W,2] fp32 pixel-major = the next scale's starting coordinates. */
+PFB_API int pfb_convex_handover2x(const float* coords, const void* mask, float* out, int B, int H, int W, pfb_dtype dtype, pfb_stream stream);
+/* Row LayerNorm over C channels (C even, <= 512) of P pixels, biased variance, fp32 statistics; x [P,in_stride] from in_offset, out
+ * [P,out_stride] from out_offset (may alias x exactly); gamma / beta fp32 [C] (both NULL: no affine). */
+PFB_API int pfb_layernorm(const void* x, int in_stride, int in_offset, void* out, int out_stride, int out_offset, const float* gamma,
+                          const float* beta, size_t P, int C, float eps, pfb_dtype dtype, pfb_stream stream);
+/* Depthwise 3x3 convolution, zero "same" padding, y = dw(x) + bias (weight fp32 [9][C] tap-major, bias fp32 [C]), then
+ *   mode 0: out = gelu(y);   mode 1: out = y + addend[p, addend_offset + c]  (addend [B,H,W,addend_stride], storage type)
+ * The two convolutions of LPI (xcit.py:98-139).  Strides / offsets even, C even; out must not overlap x. */
+PFB_API int pfb_depthwise_conv3x3_ex(const void* x, int in_stride, int in_offset, void* out, int out_stride, int out_offset,
+                                     const float* weight, const float* bias, const void* addend, int addend_stride, int addend_offset,
+                                     int B, int H, int W, int C, int mode, pfb_dtype dtype, pfb_stream stream);
+/* PositionalEncodingFourier's features (xcit.py:58-95) before token_projection, computed in fp32 and rounded once:
+ * out [H,W,64] storage type, channels 0..31 from the row index, 32..63 from the column index. */
+PFB_API int pfb_fourier_features(void* out, int H, int W, pfb_dtype dtype, pfb_stream stream);
+/* XCA statistics (xcit.py:167-186) of q = qk[., q_offset + h*16 + i], k = qk[., k_offset + h*16 + j] over the N = H*W pixels of each
+ * sample: per (sample, head) the 16 x 16 gram sum_n q_i k_j and the column sums of squares of q and k.  qk [B,N,qk_stride] storage
+ * type.  stats [B][2304] fp32: gram at h*256 + i*16 + j, sum q^2 at 2048 + c, sum k^2 at 2176 + c.  Each CTA sums 512 pixels in fp32,
+ * the partials are combined in a fixed order in fp64: the result does not depend on scheduling.
+ * workspace: pfb_xca_stats_workspace_bytes(B, N). */
+PFB_API size_t pfb_xca_stats_workspace_bytes(int B, int N);
+PFB_API int pfb_xca_stats(const void* qk, int qk_stride, int q_offset, int k_offset, int B, int N, float* stats, void* workspace,
+                          pfb_dtype dtype, pfb_stream stream);
+/* Folds the 8-head XCA into one linear layer per sample: A_h = softmax_j(temperature[h] * gram_ij / (max(|q_i|, 1e-12) max(|k_j|,
+ * 1e-12))) in fp32, then  W_b = proj_w blockdiag(A_1..A_8) v_w,  bias_b = proj_w blockdiag(A) v_b + proj_b  (v_w, proj_w fp32
+ * [128][128] row-major [out][in], v_b, proj_b fp32 [128]).  w_out [B][128 in][128 out] (the pfb_pack_conv_weight layout of a 1x1
+ * layer), w_out_k [B*128 out][128 in] (K-major, may be NULL): storage type; bias_out [B][128] fp32. */
+PFB_API int pfb_xca_fold(const float* stats, const float* temperature, const float* v_w, const float* v_b, const float* proj_w,
+                         const float* proj_b, void* w_out, void* w_out_k, float* bias_out, int B, pfb_dtype dtype, pfb_stream stream);
+/* upflow2 (ccmr/utils.py:97-99): 2 * bilinear 2x (align_corners = True) of flow [B,2,H,W] fp32 into out [B,2,out_h,out_w] fp32, the
+ * window of the 2H x 2W result at (pad_top, pad_left). */
+PFB_API int pfb_upflow2(const float* flow, float* out, int B, int H, int W, int out_h, int out_w, int pad_top, int pad_left,
+                        pfb_stream stream);
+
+/* One XCABlock of embed_dim 128, 8 heads, mlp_ratio 1 (xcit.py:242-300), folded for inference.  The LayerNorms' eps is ln_eps. */
+typedef struct {
+  pfb_layer pos_proj;          /* pos_embeder.token_projection: 1x1 64 -> 128 with bias */
+  pfb_layer qk;                /* q | k (1x1 128 -> 256) on norm1's output, norm1's affine folded in */
+  const float* v_weight;       /* [128][128] fp32: W_v diag(norm1.weight) */
+  const float* v_bias;         /* [128]: W_v norm1.bias + b_v */
+  const float* proj_weight;    /* [128][128]: diag(gamma1) W_proj */
+  const float* proj_bias;      /* [128]: gamma1 * b_proj */
+  const float* temperature;    /* [8] */
+  const float* ln3_weight;     /* norm3 affine [128] (applied: LPI's convolutions are zero padded) */
+  const float* ln3_bias;
+  const float* dw1_weight;     /* local_mp.conv1 [9][128] tap-major, bias [128] */
+  const float* dw1_bias;
+  const float* gn_weight;      /* local_mp.bn: GroupNorm(8, 128) */
+  const float* gn_bias;
+  const float* dw2_weight;     /* local_mp.conv2 times gamma3 [9][128], bias times gamma3 [128] */
+  const float* dw2_bias;
+  pfb_layer fc1;               /* mlp.fc1 (128 -> 128, GELU) with norm2's affine folded in */
+  pfb_layer fc2;               /* diag(gamma2) mlp.fc2 */
+  float ln_eps, gn_eps;
+} pfb_xcit_block;
+
+typedef struct {
+  pfb_raft_weights raft;        /* the update block: MS-RAFT+'s layers with the GRU over [h | inp | motion | motion_global] */
+  pfb_xcit_block context;       /* xcit[i]: self-attention on inp -> global_context */
+  pfb_xcit_block aggregator;    /* update_block.aggregator[i]: q, k from global_context, v from the motion features */
+} pfb_ccmr_weights;
+
+/* The whole XCiT (xcit.py:406-427) of one scale's context: x = inp + pos; x = block(x) -> out [B,H,W,128].  cfg describes the scale
+ * (variant 6); workspace: pfb_ccmr_workspace_bytes(cfg). */
+PFB_API int pfb_xcit_context(const pfb_raft_cfg* cfg, const pfb_ccmr_weights* w, const void* inp, void* out, void* workspace,
+                             size_t workspace_bytes, pfb_stream stream);
+PFB_API size_t pfb_ccmr_workspace_bytes(const pfb_raft_cfg* cfg);
+/* One scale (pfb_raft_cfg variant 6, accepted by the pfb_ccmr_* entry points only): the global context of buf->inp and the aggregator's
+ * folded attention once, the GRU context terms once, cfg->iters >= 1 iterations (lookup, motion encoder, aggregator written into the
+ * motion_global columns of the GRU input, GRU, flow head), the mask head on the last one.  Then either
+ *   next_coords != NULL: pfb_convex_handover2x into next_coords [B,2H,2W,2], or
+ *   next_coords == NULL: the convex 2x of the flow, followed by `upflow2` (0 or 1) pfb_upflow2 steps, into buf->flow_up (cfg's window
+ *                        of the result) and, if buf->flow_small != NULL, pfb_downflow of it into [B,2,out_h/16,out_w/16]. */
+PFB_API int pfb_ccmr_refine(const pfb_raft_cfg* cfg, const pfb_ccmr_weights* w, const pfb_raft_buffers* buf, float corr_scale, int upflow2,
+                            float* next_coords, pfb_stream stream);
+/* One update iteration after the scale's global context (no upsample); corr (pixel-major [B,H,W,planes]) replaces the lookup when
+ * non-NULL; mask_out [B,H,W,36] may be NULL. */
+PFB_API int pfb_ccmr_update_iter(const pfb_raft_cfg* cfg, const pfb_ccmr_weights* w, const pfb_raft_buffers* buf, const void* corr,
+                                 void* mask_out, float corr_scale, pfb_stream stream);
 
 /* ------------------------------------------------------------------------------------
  * Encoder-side kernels (SURVEY.md section 8(f) rank 1: the callers either side of the path).

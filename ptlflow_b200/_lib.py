@@ -112,6 +112,19 @@ class SearaftWeights(C.Structure):
                 ("flow1", Layer), ("flow2", Layer), ("flow2t", Layer), ("mask1", Layer), ("mask2", Layer)]
 
 
+# CCMR (include/ptlflow_b200.h, a18)
+class XcitBlock(C.Structure):
+    _fields_ = [("pos_proj", Layer), ("qk", Layer), ("v_weight", C.c_void_p), ("v_bias", C.c_void_p), ("proj_weight", C.c_void_p),
+                ("proj_bias", C.c_void_p), ("temperature", C.c_void_p), ("ln3_weight", C.c_void_p), ("ln3_bias", C.c_void_p),
+                ("dw1_weight", C.c_void_p), ("dw1_bias", C.c_void_p), ("gn_weight", C.c_void_p), ("gn_bias", C.c_void_p),
+                ("dw2_weight", C.c_void_p), ("dw2_bias", C.c_void_p), ("fc1", Layer), ("fc2", Layer), ("ln_eps", C.c_float),
+                ("gn_eps", C.c_float)]
+
+
+class CcmrWeights(C.Structure):
+    _fields_ = [("raft", RaftWeights), ("context", XcitBlock), ("aggregator", XcitBlock)]
+
+
 _lib: Optional[C.CDLL] = None
 
 # name -> (restype, argtypes); every symbol include/ptlflow_b200.h declares
@@ -181,6 +194,19 @@ SIGNATURES = {
     "pfb_msraft_workspace_bytes": (C.c_size_t, [C.POINTER(RaftCfg)]),
     "pfb_msraft_refine": (_I, [C.POINTER(RaftCfg), C.POINTER(RaftWeights), C.POINTER(RaftBuffers), C.c_float, _P, _S]),
     "pfb_msraft_update_iter": (_I, [C.POINTER(RaftCfg), C.POINTER(RaftWeights), C.POINTER(RaftBuffers), _P, _P, C.c_float, _S]),
+    # CCMR (a18)
+    "pfb_layernorm": (_I, [_P, _I, _I, _P, _I, _I, _P, _P, C.c_size_t, _I, C.c_float, _I, _S]),
+    "pfb_depthwise_conv3x3_ex": (_I, [_P, _I, _I, _P, _I, _I, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
+    "pfb_fourier_features": (_I, [_P, _I, _I, _I, _S]),
+    "pfb_xca_stats_workspace_bytes": (C.c_size_t, [_I, _I]),
+    "pfb_xca_stats": (_I, [_P, _I, _I, _I, _I, _I, _P, _P, _I, _S]),
+    "pfb_xca_fold": (_I, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _I, _I, _S]),
+    "pfb_convex_handover2x": (_I, [_P, _P, _P, _I, _I, _I, _I, _S]),
+    "pfb_upflow2": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _S]),
+    "pfb_xcit_context": (_I, [C.POINTER(RaftCfg), C.POINTER(CcmrWeights), _P, _P, _P, C.c_size_t, _S]),
+    "pfb_ccmr_workspace_bytes": (C.c_size_t, [C.POINTER(RaftCfg)]),
+    "pfb_ccmr_refine": (_I, [C.POINTER(RaftCfg), C.POINTER(CcmrWeights), C.POINTER(RaftBuffers), C.c_float, _I, _P, _S]),
+    "pfb_ccmr_update_iter": (_I, [C.POINTER(RaftCfg), C.POINTER(CcmrWeights), C.POINTER(RaftBuffers), _P, _P, C.c_float, _S]),
 }
 
 

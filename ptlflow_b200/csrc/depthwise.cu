@@ -4,8 +4,9 @@
 // tile of CC channels: the tile plus its halo is staged once in shared memory as fp32 (zero outside the image, which is the
 // "same" padding), next to the fp32 weights of those channels.  A thread owns a channel pair and a strip of R = 8 consecutive
 // pixels of one row; per filter row it loads the R + k - 1 input pairs of that row once into registers and slides the k taps
-// over them, so every staged value is read from shared memory k times fewer than a per-output loop would.  Without the residual
-// and the GELU (kResidualGelu = false) the same kernel is the first pass of pfb_depthwise_conv_layernorm below.
+// over them, so every staged value is read from shared memory k times fewer than a per-output loop would.  The epilogue is one of
+// the kDw* modes: without the residual and the GELU (kDwBias) the same kernel is the first pass of pfb_depthwise_conv_layernorm
+// below; kDwBiasGelu and kDwBiasAddend are the two depthwise convolutions of CCMR's LPI (pfb_depthwise_conv3x3_ex).
 #include <atomic>
 
 #include "common.cuh"
@@ -37,10 +38,14 @@ __host__ __device__ constexpr size_t dw_smem(int K) {
   return ((size_t)(kDwTH + K - 1) * (kDwTW + K - 1) + (size_t)K * K) * dw_cc(K) * sizeof(float);
 }
 
-template <typename T, int K, bool kResidualGelu>
+// epilogues: y = dw(x) + bias, then  kDwBias: y;  kDwResidualGelu: gelu(x + y);  kDwBiasGelu: gelu(y);  kDwBiasAddend: y + addend
+enum { kDwBias = 0, kDwResidualGelu = 1, kDwBiasGelu = 2, kDwBiasAddend = 3 };
+
+template <typename T, int K, int kMode>
 __global__ void __launch_bounds__(dw_threads(K)) depthwise_gelu_kernel(const T* __restrict__ x, int in_stride, T* __restrict__ out,
                                                                       int out_stride, const float* __restrict__ wgt,
-                                                                      const float* __restrict__ bias, int H, int W, int C, int tiles_x) {
+                                                                      const float* __restrict__ bias, int H, int W, int C, int tiles_x,
+                                                                      const T* __restrict__ addend, int addend_stride) {
   constexpr int CC = dw_cc(K), NP = CC / 2, THR = dw_threads(K);
   constexpr int PH = kDwTH + K - 1, PW = kDwTW + K - 1;
   using V = typename Pair<T>::V;
@@ -98,9 +103,14 @@ __global__ void __launch_bounds__(dw_threads(K)) depthwise_gelu_kernel(const T* 
     const int ox = x0 + sx * kDwR + r;
     if (ox < W) {
       V* o = reinterpret_cast<V*>(out + (img + (size_t)oy * W + ox) * out_stride + c);
-      if (kResidualGelu) {
+      if (kMode == kDwResidualGelu) {
         const float2 xc = in2[((ty + K / 2) * PW + sx * kDwR + r + K / 2) * NP + cp];  // the residual: the centre tap's input
         *o = Pair<T>::from(gelu_f32(xc.x + (acc[r].x + b0)), gelu_f32(xc.y + (acc[r].y + b1)));
+      } else if (kMode == kDwBiasGelu) {
+        *o = Pair<T>::from(gelu_f32(acc[r].x + b0), gelu_f32(acc[r].y + b1));
+      } else if (kMode == kDwBiasAddend) {
+        const float2 a = Pair<T>::f2(*reinterpret_cast<const V*>(addend + (img + (size_t)oy * W + ox) * addend_stride + c));
+        *o = Pair<T>::from((acc[r].x + b0) + a.x, (acc[r].y + b1) + a.y);
       } else {
         *o = Pair<T>::from(acc[r].x + b0, acc[r].y + b1);
       }
@@ -108,21 +118,22 @@ __global__ void __launch_bounds__(dw_threads(K)) depthwise_gelu_kernel(const T* 
   }
 }
 
-template <typename T, int K, bool kResidualGelu = true>
+template <typename T, int K, int kMode = kDwResidualGelu>
 static int launch_dw(const T* x, int in_stride, T* out, int out_stride, const float* w, const float* bias, int B, int H, int W, int C,
-                     cudaStream_t s) {
+                     cudaStream_t s, const T* addend = nullptr, int addend_stride = 0) {
   static std::atomic<unsigned long long> attr_done{0};
   const size_t smem = dw_smem(K);
   int dev = 0;
   PFB_CUDA(cudaGetDevice(&dev));
   if (smem > 48 * 1024 && !(attr_done.load(std::memory_order_acquire) & (1ull << (dev & 63)))) {
-    PFB_CUDA(cudaFuncSetAttribute(depthwise_gelu_kernel<T, K, kResidualGelu>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    PFB_CUDA(cudaFuncSetAttribute(depthwise_gelu_kernel<T, K, kMode>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     attr_done.fetch_or(1ull << (dev & 63), std::memory_order_release);
   }
   const int tiles_x = ceil_div(W, kDwTW), tiles_y = ceil_div(H, kDwTH);
   dim3 grid(tiles_x * tiles_y, ceil_div(C, dw_cc(K)), B);
-  ProfScope prof(kResidualGelu ? KC_DEPTHWISE : KC_DW_LAYERNORM, s);
-  depthwise_gelu_kernel<T, K, kResidualGelu><<<grid, dw_threads(K), smem, s>>>(x, in_stride, out, out_stride, w, bias, H, W, C, tiles_x);
+  ProfScope prof(kMode == kDwBias ? KC_DW_LAYERNORM : KC_DEPTHWISE, s);
+  depthwise_gelu_kernel<T, K, kMode><<<grid, dw_threads(K), smem, s>>>(x, in_stride, out, out_stride, w, bias, H, W, C, tiles_x, addend,
+                                                                       addend_stride);
   PFB_LAUNCH_CHECK();
   return PFB_OK;
 }
@@ -150,10 +161,11 @@ static int dispatch_dw(const T* x, int in_stride, T* out, int out_stride, const 
 // but took 1.4-1.5x as long at the config-3 grid, because it staged nothing in shared memory.
 constexpr int kLnMaxC = 512;
 
-// Row LayerNorm without affine, in place allowed: one warp per pixel, lane l holds the channel pairs 2l + 64j in registers, mean
-// then the variance about it by warp shuffles.
+// Row LayerNorm, in place allowed: one warp per pixel, lane l holds the channel pairs 2l + 64j in registers, mean then the variance
+// about it by warp shuffles; the affine gamma / beta (fp32 [C]) when gamma is not NULL.
 template <typename T>
-__global__ void __launch_bounds__(256) layernorm_rows_kernel(const T* y, T* out, int out_stride, size_t P, int C, float eps) {
+__global__ void __launch_bounds__(256) layernorm_rows_kernel(const T* y, int in_stride, T* out, int out_stride, size_t P, int C, float eps,
+                                                             const float* __restrict__ gamma, const float* __restrict__ beta) {
   using V = typename Pair<T>::V;
   constexpr int NJ = kLnMaxC / 64;
   const size_t p = (size_t)blockIdx.x * 8 + (threadIdx.x >> 5);
@@ -164,7 +176,7 @@ __global__ void __launch_bounds__(256) layernorm_rows_kernel(const T* y, T* out,
 #pragma unroll
   for (int j = 0; j < NJ; ++j) {
     const int c = 2 * lane + 64 * j;
-    v[j] = c < C ? Pair<T>::f2(*reinterpret_cast<const V*>(y + p * out_stride + c)) : make_float2(0.f, 0.f);
+    v[j] = c < C ? Pair<T>::f2(*reinterpret_cast<const V*>(y + p * in_stride + c)) : make_float2(0.f, 0.f);
     s += v[j].x + v[j].y;
   }
 #pragma unroll
@@ -180,7 +192,10 @@ __global__ void __launch_bounds__(256) layernorm_rows_kernel(const T* y, T* out,
 #pragma unroll
   for (int j = 0; j < NJ; ++j) {
     const int c = 2 * lane + 64 * j;
-    if (c < C) *reinterpret_cast<V*>(out + p * out_stride + c) = Pair<T>::from((v[j].x - mu) * rs, (v[j].y - mu) * rs);
+    if (c >= C) continue;
+    float2 n = make_float2((v[j].x - mu) * rs, (v[j].y - mu) * rs);
+    if (gamma) n = make_float2(fmaf(n.x, gamma[c], beta[c]), fmaf(n.y, gamma[c + 1], beta[c + 1]));
+    *reinterpret_cast<V*>(out + p * out_stride + c) = Pair<T>::from(n.x, n.y);
   }
 }
 
@@ -190,7 +205,7 @@ static int launch_dwln(const T* x, int in_stride, T* out, int out_stride, const 
   int rc = PFB_ERR_ARG;
   switch (k) {
 #define PFB_DWS_CASE(K) \
-  case K: rc = launch_dw<T, K, false>(x, in_stride, out, out_stride, w, bias, B, H, W, C, s); break;
+  case K: rc = launch_dw<T, K, kDwBias>(x, in_stride, out, out_stride, w, bias, B, H, W, C, s); break;
     PFB_DWS_CASE(1) PFB_DWS_CASE(3) PFB_DWS_CASE(5) PFB_DWS_CASE(7) PFB_DWS_CASE(9) PFB_DWS_CASE(11) PFB_DWS_CASE(13)
     PFB_DWS_CASE(15) PFB_DWS_CASE(17) PFB_DWS_CASE(19) PFB_DWS_CASE(21) PFB_DWS_CASE(23) PFB_DWS_CASE(25) PFB_DWS_CASE(27)
     PFB_DWS_CASE(29) PFB_DWS_CASE(31)
@@ -200,7 +215,7 @@ static int launch_dwln(const T* x, int in_stride, T* out, int out_stride, const 
   if (rc != PFB_OK) return rc;
   const size_t P = (size_t)B * H * W;
   ProfScope prof(KC_DW_LAYERNORM, s);
-  layernorm_rows_kernel<T><<<(unsigned)ceil_div_sz(P, 8), 256, 0, s>>>(out, out, out_stride, P, C, eps);
+  layernorm_rows_kernel<T><<<(unsigned)ceil_div_sz(P, 8), 256, 0, s>>>(out, out_stride, out, out_stride, P, C, eps, nullptr, nullptr);
   PFB_LAUNCH_CHECK();
   return PFB_OK;
 }
@@ -253,6 +268,62 @@ extern "C" PFB_API int pfb_depthwise_conv_gelu(const void* x, int in_stride, int
   cudaStream_t s = as_stream(stream);
   PFB_DISPATCH_DTYPE(dtype, T, {
     return dispatch_dw<T>(reinterpret_cast<const T*>(xb), in_stride, reinterpret_cast<T*>(ob), out_stride, weight, bias, B, H, W, C, k, s);
+  });
+  return PFB_ERR_ARG;
+}
+
+// ---- a18: CCMR's XCiT block (ccmr/xcit.py:98-139, 242-300) ----
+extern "C" PFB_API int pfb_layernorm(const void* x, int in_stride, int in_offset, void* out, int out_stride, int out_offset, const float* gamma,
+                                     const float* beta, size_t P, int C, float eps, pfb_dtype dtype, pfb_stream stream) {
+  PFB_CHECK_ARG(x && out, "layernorm: null pointer");
+  PFB_CHECK_ARG(dtype_ok(dtype), "layernorm: bad dtype");
+  PFB_CHECK_ARG(P > 0 && C > 0 && C % 2 == 0 && C <= kLnMaxC, "layernorm: bad shape P=%zu C=%d (C even, <= %d)", P, C, kLnMaxC);
+  PFB_CHECK_ARG((gamma == nullptr) == (beta == nullptr), "layernorm: gamma and beta must both be set or both be NULL");
+  PFB_CHECK_ARG(eps > 0.f, "layernorm: eps must be positive");
+  PFB_CHECK_ARG(in_offset >= 0 && out_offset >= 0 && in_stride >= in_offset + C && out_stride >= out_offset + C && in_offset % 2 == 0 &&
+                    out_offset % 2 == 0 && in_stride % 2 == 0 && out_stride % 2 == 0,
+                "layernorm: strides / offsets must be even and hold C channels");
+  const size_t es = dtype_size(dtype);
+  const char* xb = reinterpret_cast<const char*>(x) + (size_t)in_offset * es;
+  char* ob = reinterpret_cast<char*>(out) + (size_t)out_offset * es;
+  PFB_CHECK_ARG((reinterpret_cast<uintptr_t>(xb) % (2 * es)) == 0 && (reinterpret_cast<uintptr_t>(ob) % (2 * es)) == 0,
+                "layernorm: misaligned channel pairs");
+  cudaStream_t s = as_stream(stream);
+  ProfScope prof(KC_DW_LAYERNORM, s);
+  PFB_DISPATCH_DTYPE(dtype, T, {
+    layernorm_rows_kernel<T><<<(unsigned)ceil_div_sz(P, 8), 256, 0, s>>>(reinterpret_cast<const T*>(xb), in_stride, reinterpret_cast<T*>(ob),
+                                                                        out_stride, P, C, eps, gamma, beta);
+  });
+  PFB_LAUNCH_CHECK();
+  return PFB_OK;
+}
+
+extern "C" PFB_API int pfb_depthwise_conv3x3_ex(const void* x, int in_stride, int in_offset, void* out, int out_stride, int out_offset,
+                                                const float* weight, const float* bias, const void* addend, int addend_stride,
+                                                int addend_offset, int B, int H, int W, int C, int mode, pfb_dtype dtype, pfb_stream stream) {
+  PFB_CHECK_ARG(x && out && weight && bias, "depthwise_conv3x3_ex: null pointer");
+  PFB_CHECK_ARG(dtype_ok(dtype) && (mode == 0 || mode == 1), "depthwise_conv3x3_ex: bad dtype or mode %d", mode);
+  PFB_CHECK_ARG(B > 0 && B <= 65535 && H > 0 && W > 0 && C > 0 && C % 2 == 0, "depthwise_conv3x3_ex: bad shape %dx%dx%dx%d (C even)", B, H,
+                W, C);
+  PFB_CHECK_ARG(in_offset >= 0 && out_offset >= 0 && in_stride >= in_offset + C && out_stride >= out_offset + C && in_offset % 2 == 0 &&
+                    out_offset % 2 == 0 && in_stride % 2 == 0 && out_stride % 2 == 0,
+                "depthwise_conv3x3_ex: strides / offsets must be even and hold C channels");
+  if (mode == 1)
+    PFB_CHECK_ARG(addend && addend_offset >= 0 && addend_offset % 2 == 0 && addend_stride % 2 == 0 && addend_stride >= addend_offset + C,
+                  "depthwise_conv3x3_ex: mode 1 needs an addend with an even stride / offset holding C channels");
+  const size_t es = dtype_size(dtype);
+  const char* xb = reinterpret_cast<const char*>(x) + (size_t)in_offset * es;
+  char* ob = reinterpret_cast<char*>(out) + (size_t)out_offset * es;
+  const char* ab = mode == 1 ? reinterpret_cast<const char*>(addend) + (size_t)addend_offset * es : nullptr;
+  PFB_CHECK_ARG(((reinterpret_cast<uintptr_t>(xb) | reinterpret_cast<uintptr_t>(ob) | reinterpret_cast<uintptr_t>(ab)) % (2 * es)) == 0,
+                "depthwise_conv3x3_ex: misaligned channel pairs");
+  cudaStream_t s = as_stream(stream);
+  PFB_DISPATCH_DTYPE(dtype, T, {
+    const T* xt = reinterpret_cast<const T*>(xb);
+    T* ot = reinterpret_cast<T*>(ob);
+    if (mode == 0) return launch_dw<T, 3, kDwBiasGelu>(xt, in_stride, ot, out_stride, weight, bias, B, H, W, C, s);
+    return launch_dw<T, 3, kDwBiasAddend>(xt, in_stride, ot, out_stride, weight, bias, B, H, W, C, s, reinterpret_cast<const T*>(ab),
+                                          addend_stride);
   });
   return PFB_ERR_ARG;
 }

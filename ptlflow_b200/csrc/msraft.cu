@@ -81,7 +81,8 @@ __global__ void upsample2x_concat_kernel(const T* __restrict__ src, int Cs, cons
 
 // Convex 2x (ms_raft_plus.py:138-149 with scale = 2): one thread per (coarse pixel, sy, sx); mask channel = tap*4 + sy*2 + sx.
 // The 3x3 neighbourhood is unfolded with zero padding.  mode 0: the flow coords - grid, into the window of the un-padded NCHW
-// output; mode 1: the absolute coordinates, into the next scale's pixel-major [B,2H,2W,2] coordinates.
+// output; mode 1: the absolute coordinates, into the next scale's pixel-major [B,2H,2W,2] coordinates; mode 2 (pfb_convex_handover2x): the flow, plus the
+// fine grid, into the next scale's pixel-major coordinates (CCMR's handover, ccmr.py:195-202).
 template <typename T>
 __global__ void __launch_bounds__(256) convex_upsample2x_kernel(const float* __restrict__ coords, const T* __restrict__ mask,
                                                                 float* __restrict__ out, int mode, int B, int H, int W, int OH, int OW,
@@ -107,7 +108,7 @@ __global__ void __launch_bounds__(256) convex_upsample2x_kernel(const float* __r
     sum += e;
     if (ny >= 0 && ny < H && nx >= 0 && nx < W) {
       const float* c = coords + 2 * ((size_t)(b * H + ny) * W + nx);
-      const float gx = mode ? 0.f : (float)nx, gy = mode ? 0.f : (float)ny;
+      const float gx = mode == 1 ? 0.f : (float)nx, gy = mode == 1 ? 0.f : (float)ny;
       ax = fmaf(e, 2.f * (c[0] - gx), ax);
       ay = fmaf(e, 2.f * (c[1] - gy), ay);
     }
@@ -118,6 +119,10 @@ __global__ void __launch_bounds__(256) convex_upsample2x_kernel(const float* __r
     float* o = out + 2 * ((size_t)(b * 2 * H + oy) * (2 * W) + ox);
     o[0] = ax * inv;
     o[1] = ay * inv;
+    if (mode == 2) {
+      o[0] += (float)ox;
+      o[1] += (float)oy;
+    }
     return;
   }
   const int wy = oy - pad_top, wx = ox - pad_left;
@@ -187,6 +192,20 @@ extern "C" PFB_API int pfb_convex_upsample2x(const float* coords, const void* ma
   PFB_DISPATCH_DTYPE(dtype, T, {
     convex_upsample2x_kernel<T><<<(unsigned)ceil_div_sz(threads, 256), 256, 0, s>>>(coords, (const T*)mask, out, mode, B, H, W, out_h, out_w,
                                                                                     pad_top, pad_left);
+  });
+  PFB_LAUNCH_CHECK();
+  return PFB_OK;
+}
+
+extern "C" PFB_API int pfb_convex_handover2x(const float* coords, const void* mask, float* out, int B, int H, int W, pfb_dtype dtype,
+                                             pfb_stream stream) {
+  PFB_CHECK_ARG(coords && mask && out, "convex_handover2x: null pointer");
+  PFB_CHECK_ARG(dtype_ok(dtype) && B > 0 && H > 0 && W > 0, "convex_handover2x: bad arguments");
+  cudaStream_t s = as_stream(stream);
+  const size_t threads = (size_t)B * H * W * 4;
+  ProfScope prof(KC_UPSAMPLE, s);
+  PFB_DISPATCH_DTYPE(dtype, T, {
+    convex_upsample2x_kernel<T><<<(unsigned)ceil_div_sz(threads, 256), 256, 0, s>>>(coords, (const T*)mask, out, 2, B, H, W, 0, 0, 0, 0);
   });
   PFB_LAUNCH_CHECK();
   return PFB_OK;

@@ -33,8 +33,8 @@ struct Workspace {
 };
 
 static int heads_of(const pfb_raft_cfg* c) { return c->num_heads > 0 ? c->num_heads : 1; }
-// channels of the convex-upsample mask: 9 taps x 8 x 8 (raft, gma), 9 taps x 2 x 2 (ms_raft_plus, variant 5)
-static int mask_channels(const pfb_raft_cfg* c) { return c->variant == 5 ? 36 : 576; }
+// channels of the convex-upsample mask: 9 taps x 8 x 8 (raft, gma), 9 taps x 2 x 2 (ms_raft_plus, variant 5; ccmr, variant 6)
+static int mask_channels(const pfb_raft_cfg* c) { return c->variant == 5 || c->variant == 6 ? 36 : 576; }
 
 static Workspace plan(const pfb_raft_cfg* c) {
   Workspace w{};
@@ -45,10 +45,10 @@ static Workspace plan(const pfb_raft_cfg* c) {
   w.planes = c->corr_levels * K * K;
   // 16-byte aligned rows for the tensor-core path (the TMA unit zero-fills a partial last 64-channel K chunk itself)
   w.corr_stride = (c->dtype == PFB_F32) ? w.planes : (int)align_up(w.planes, 8);
-  if (c->variant == 0 || c->variant == 2 || c->variant == 5) {
+  if (c->variant == 0 || c->variant == 2 || c->variant == 5 || c->variant == 6) {
     w.c_cor1 = 256; w.c_cor2 = 192; w.c_flo1 = 128; w.c_flo2 = 64; w.c_fh = 256;
-    // gma keeps [motion | motion_global] side by side so the GRU still sees three sources (update.py:150-151)
-    w.c_motion = c->variant == 2 ? 256 : 128;
+    // gma and ccmr keep [motion | motion_global] side by side so the GRU still sees three sources (update.py:150-151)
+    w.c_motion = c->variant == 2 || c->variant == 6 ? 256 : 128;
   } else {
     w.c_cor1 = 0; w.c_cor2 = 96; w.c_flo1 = 64; w.c_flo2 = 32; w.c_motion = 82; w.c_fh = 128;
   }
@@ -78,10 +78,12 @@ static Workspace plan(const pfb_raft_cfg* c) {
   return w;
 }
 
-// variant 5 (ms_raft_plus) only through the pfb_msraft_* entry points, 0..2 only through the pfb_raft_* ones
-static int check_cfg(const pfb_raft_cfg* c, bool msraft = false) {
+// variant 5 (ms_raft_plus) only through the pfb_msraft_* entry points, 6 (ccmr) only through the pfb_ccmr_* ones, 0..2 only through
+// the pfb_raft_* ones
+static int check_cfg(const pfb_raft_cfg* c, bool msraft = false, bool ccmr = false) {
   PFB_CHECK_ARG(c, "raft: null cfg");
-  if (msraft) PFB_CHECK_ARG(c->variant == 5, "msraft: variant=%d (the ms_raft_plus loop is variant 5)", c->variant);
+  if (ccmr) PFB_CHECK_ARG(c->variant == 6, "ccmr: variant=%d (the ccmr loop is variant 6)", c->variant);
+  else if (msraft) PFB_CHECK_ARG(c->variant == 5, "msraft: variant=%d (the ms_raft_plus loop is variant 5)", c->variant);
   else PFB_CHECK_ARG(c->variant >= 0 && c->variant <= 2, "raft: variant=%d", c->variant);
   PFB_CHECK_ARG(dtype_ok(c->dtype), "raft: bad dtype");
   PFB_CHECK_ARG(c->B > 0 && c->H > 0 && c->W > 0, "raft: bad grid %dx%dx%d", c->B, c->H, c->W);
@@ -106,6 +108,8 @@ struct Ctx {
   char* base;
   cudaStream_t s;
   float corr_scale = 0.f;  // on-the-fly lookup scale (0: 1/sqrt(feat_dim))
+  const pfb_ccmr_weights* ccmr = nullptr;  // variant 6: the XCiT blocks of the scale, and their part of the workspace
+  char* ccmr_base = nullptr;
   // flow branch of the motion encoder on a second stream (fork_flow_branch): null when not forked
   cudaStream_t side = nullptr;
   cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
@@ -351,6 +355,8 @@ static int update_iter(const Ctx& x, const void* corr_ext, void* mask_out) {
   if (c->variant == 2)
     PFB_TRY(gma_aggregate(c, x.w->layers[PFB_L_AGG_V], x.w->layers[PFB_L_AGG_PROJ], x.b->attention, x.b->agg_gamma, motion, ws.c_motion, 0,
                           128, x.at(ws.off_vbuf), x.at(ws.off_vT), x.at(ws.off_agg), ws.n_pad, x.s));
+  // ---- ccmr: motion_global = aggregator(global_context, motion)   ccmr/update.py:156-161 ----
+  if (c->variant == 6) PFB_TRY(ccmr_aggregate(c, x.ccmr, motion, ws.c_motion, x.ccmr_base, x.s));
 
   // ---- GRU (update.py:24-32 ConvGRU, :58-73 SepConvGRU); x = [inp, motion (, motion_global)] ----
   const int halves = (c->variant != 1) ? 2 : 1;
@@ -403,8 +409,8 @@ static int update_iter(const Ctx& x, const void* corr_ext, void* mask_out) {
 }
 
 static int make_ctx(Ctx& x, const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf,
-                    cudaStream_t s, bool need_pyramid, bool msraft = false) {
-  PFB_TRY(check_cfg(cfg, msraft));
+                    cudaStream_t s, bool need_pyramid, bool msraft = false, bool ccmr = false) {
+  PFB_TRY(check_cfg(cfg, msraft, ccmr));
   PFB_CHECK_ARG(w && buf, "raft: null weights/buffers");
   PFB_CHECK_ARG(buf->net && buf->inp && buf->coords && buf->workspace, "raft: null state buffer");
   if (need_pyramid) {
@@ -413,7 +419,8 @@ static int make_ctx(Ctx& x, const pfb_raft_cfg* cfg, const pfb_raft_weights* w, 
   }
   x.c = cfg; x.w = w; x.b = buf; x.s = s;
   x.ws = plan(cfg);
-  PFB_CHECK_ARG(buf->workspace_bytes >= x.ws.total, "raft: workspace %zu bytes < required %zu", buf->workspace_bytes, x.ws.total);
+  const size_t need = x.ws.total + (ccmr ? ccmr_plan(cfg).total : 0);
+  PFB_CHECK_ARG(buf->workspace_bytes >= need, "raft: workspace %zu bytes < required %zu", buf->workspace_bytes, need);
   x.base = reinterpret_cast<char*>(buf->workspace);
   return PFB_OK;
 }
@@ -517,4 +524,66 @@ extern "C" PFB_API int pfb_msraft_refine(const pfb_raft_cfg* cfg, const pfb_raft
   // flow_small = downflow(flow_up, 1/16) at int(h / 16) x int(w / 16) of the un-padded size (ms_raft_plus.py:22-35, 221-224)
   const int sh = cfg->out_h / 16, sw = cfg->out_w / 16;
   return pfb_downflow(buf->flow_up, buf->flow_small, cfg->B, cfg->out_h, cfg->out_w, sh, sw, stream);
+}
+
+// ---- a18: CCMR / CCMR+ (one call per scale of ccmr.py:179-220) ----
+extern "C" PFB_API size_t pfb_ccmr_workspace_bytes(const pfb_raft_cfg* cfg) {
+  if (check_cfg(cfg, false, true) != PFB_OK) return 0;
+  return plan(cfg).total + ccmr_plan(cfg).total;
+}
+
+static int make_ccmr_ctx(Ctx& x, const pfb_raft_cfg* cfg, const pfb_ccmr_weights* w, const pfb_raft_buffers* buf, cudaStream_t s,
+                         bool need_pyramid, float corr_scale) {
+  PFB_CHECK_ARG(w, "ccmr: null weights");
+  PFB_TRY(make_ctx(x, cfg, &w->raft, buf, s, need_pyramid, false, true));
+  PFB_CHECK_ARG(corr_scale >= 0.f, "ccmr: corr_scale=%g", (double)corr_scale);
+  PFB_CHECK_ARG(cfg->context_dim == 128, "ccmr: the XCiT blocks expect 128 context channels");
+  x.corr_scale = corr_scale;
+  x.ccmr = w;
+  x.ccmr_base = x.base + x.ws.total;
+  return PFB_OK;
+}
+
+extern "C" PFB_API int pfb_xcit_context(const pfb_raft_cfg* cfg, const pfb_ccmr_weights* w, const void* inp, void* out, void* workspace,
+                                        size_t workspace_bytes, pfb_stream stream) {
+  PFB_CHECK_ARG(cfg && w && inp && out && workspace, "xcit_context: null pointer");
+  PFB_TRY(check_cfg(cfg, false, true));
+  const size_t off = plan(cfg).total, need = off + ccmr_plan(cfg).total;
+  PFB_CHECK_ARG(workspace_bytes >= need, "xcit_context: workspace %zu bytes < required %zu", workspace_bytes, need);
+  return ccmr_scale_setup(cfg, w, inp, out, false, reinterpret_cast<char*>(workspace) + off, as_stream(stream));
+}
+
+extern "C" PFB_API int pfb_ccmr_update_iter(const pfb_raft_cfg* cfg, const pfb_ccmr_weights* w, const pfb_raft_buffers* buf,
+                                            const void* corr, void* mask_out, float corr_scale, pfb_stream stream) {
+  Ctx x;
+  PFB_TRY(make_ccmr_ctx(x, cfg, w, buf, as_stream(stream), corr == nullptr, corr_scale));
+  PFB_TRY(ccmr_scale_setup(cfg, w, buf->inp, nullptr, true, x.ccmr_base, x.s));
+  PFB_TRY(launch_flow_from_coords(buf->coords, reinterpret_cast<float*>(x.at(x.ws.off_flow)), cfg->B, cfg->H, cfg->W, x.s));
+  PFB_TRY(run_context_terms(x));
+  if (!corr) PFB_TRY(lookup(x));
+  return update_iter(x, corr, mask_out);
+}
+
+extern "C" PFB_API int pfb_ccmr_refine(const pfb_raft_cfg* cfg, const pfb_ccmr_weights* w, const pfb_raft_buffers* buf, float corr_scale,
+                                       int upflow2, float* next_coords, pfb_stream stream) {
+  Ctx x;
+  PFB_TRY(make_ccmr_ctx(x, cfg, w, buf, as_stream(stream), true, corr_scale));
+  PFB_CHECK_ARG(cfg->iters >= 1, "ccmr_refine: every scale needs at least one iteration (iters=%d)", cfg->iters);
+  PFB_CHECK_ARG(upflow2 == 0 || upflow2 == 1, "ccmr_refine: upflow2=%d (0 or 1)", upflow2);
+  PFB_CHECK_ARG(next_coords || buf->flow_up, "ccmr_refine: needs next_coords (coarser scales) or flow_up (the finest)");
+  if (!next_coords) {
+    const int f = 2 << upflow2;  // the output grid is f times this scale's
+    PFB_CHECK_ARG(cfg->out_h > 0 && cfg->out_w > 0 && cfg->pad_top >= 0 && cfg->pad_left >= 0 && cfg->out_h + cfg->pad_top <= f * cfg->H &&
+                      cfg->out_w + cfg->pad_left <= f * cfg->W,
+                  "ccmr_refine: output window %dx%d+(%d,%d) outside %dx%d", cfg->out_h, cfg->out_w, cfg->pad_top, cfg->pad_left, f * cfg->H,
+                  f * cfg->W);
+    if (buf->flow_small)
+      PFB_CHECK_ARG(cfg->out_h >= 16 && cfg->out_w >= 16, "ccmr_refine: output %dx%d smaller than 16 px per side", cfg->out_h, cfg->out_w);
+  }
+  PFB_TRY(ccmr_scale_setup(cfg, w, buf->inp, nullptr, true, x.ccmr_base, x.s));
+  void* mask = x.at(x.ws.off_mask);
+  PFB_TRY(run_iterations(x, mask));
+  if (next_coords)  // handover: the convex 2x of the FLOW on the next scale's grid (ccmr.py:195-202)
+    return pfb_convex_handover2x(buf->coords, mask, next_coords, cfg->B, cfg->H, cfg->W, cfg->dtype, stream);
+  return ccmr_output(cfg, buf->coords, mask, buf->flow_up, buf->flow_small, upflow2, x.ccmr_base, x.s);
 }

@@ -40,19 +40,19 @@ class RaftEngine:
 
         layers: Dict[int, ops.PackedConv] = {}
         layers[_lib.L_CONVF1] = P(None, enc.convf1)  # 7x7 on the 2-channel fp32 flow: dedicated kernel
-        if variant in (0, 2) and dtype != torch.float32 and tuple(enc.convf1.weight.shape) == (128, 2, 7, 7):
+        if variant in (0, 2, 6) and dtype != torch.float32 and tuple(enc.convf1.weight.shape) == (128, 2, 7, 7):
             # tensor-core form (csrc/first_conv.cu): the K-major slot of the layer carries the overlapping-window tiles
             pc = layers[_lib.L_CONVF1]
             pc.weight_k = ops.pack_flow_conv(enc.convf1.weight, dtype).to(device)
             pc.Cin_pad, pc.Cout_pad_k = 64, 128
-        if variant in (0, 2):
+        if variant in (0, 2, 6):
             layers[_lib.L_CONVC1] = P([planes], enc.convc1)
             layers[_lib.L_CONVC2] = P([256], enc.convc2)
             layers[_lib.L_CONVF2] = P([128], enc.convf2)
             layers[_lib.L_CONV] = P([256], enc.conv)  # cat[cor(192), flo(64)] lives in one 256-channel buffer
             # cat[h or r*h, inp, motion (, motion_global)] -- three tensor maps, no concat copy (gma keeps
-            # motion | motion_global in one 256-channel buffer)
-            gsrc = [hd, cd, 256 if variant == 2 else 128]
+            # motion | motion_global in one 256-channel buffer, and so does ccmr)
+            gsrc = [hd, cd, 256 if variant in (2, 6) else 128]
             layers[_lib.L_GRU_ZR1] = P(gsrc, gru.convz1, gru.convr1)  # z | r share the input: one GEMM, N = 2*hidden
             layers[_lib.L_GRU_Q1] = P(gsrc, gru.convq1)
             layers[_lib.L_GRU_ZR2] = P(gsrc, gru.convz2, gru.convr2)
@@ -474,4 +474,131 @@ class MSRaftEngine(RaftEngine):
                                                 corr.data_ptr() if corr is not None else None,
                                                 mask.data_ptr() if mask is not None else None, corr_scale, stream_ptr(self.device)),
                   "msraft_update_iter")
+        return mask
+
+
+class CCMREngine(RaftEngine):
+    """CCMR's update block (ccmr/update.py:110-168: MS-RAFT+'s layers with a GMA-width GRU over [inp | motion | motion_global]) packed
+    as RaftEngine packs gma's, plus per scale the XCiT of the context (``xcit[i]``) and the aggregator (``update_block.aggregator[i]``)
+    as pfb_xcit_block descriptors, folded in fp64 (xcit.py:242-300): norm1's affine into q | k and v, gamma1 into proj, gamma3 into
+    LPI's second convolution, norm2's affine into fc1 and gamma2 into fc2.  Driven one scale at a time through pfb_ccmr_refine
+    (pfb_raft_cfg variant 6)."""
+
+    def __init__(self, update_block: torch.nn.Module, variant: int, hidden_dim: int, context_dim: int, corr_levels: int, corr_radius: int,
+                 dtype: torch.dtype, device: torch.device, impl: int = 0, xcit: Optional[torch.nn.Module] = None):
+        super().__init__(update_block, variant, hidden_dim, context_dim, corr_levels, corr_radius, dtype, device, impl=impl)
+        self._keep: List[object] = []
+        self.scale_weights = []
+        for i in range(len(update_block.aggregator)):
+            w = _lib.CcmrWeights()
+            w.raft = self.weights
+            w.context = self._pack_xcit(xcit[i], separate=False)
+            w.aggregator = self._pack_xcit(update_block.aggregator[i], separate=True)
+            self.scale_weights.append(w)
+        torch.cuda.current_stream(device).synchronize()
+
+    def _pack_xcit(self, xc: torch.nn.Module, separate: bool) -> _lib.XcitBlock:
+        dtype, device = self.dtype, self.device
+        blk = xc.blocks[0]
+        f64 = lambda t: t.detach().to(device, torch.float64)  # noqa: E731
+        f32 = lambda t: self._hold(t.float().contiguous())  # noqa: E731
+        C = blk.norm1.weight.shape[0]
+        ln1w, ln1b = f64(blk.norm1.weight), f64(blk.norm1.bias)
+        a = blk.attn
+        if separate:
+            wqk, wv = f64(a.to_qk.weight), f64(a.to_v.weight)
+            bqk = f64(a.to_qk.bias) if a.to_qk.bias is not None else torch.zeros(2 * C, dtype=torch.float64, device=device)
+            bv = f64(a.to_v.bias) if a.to_v.bias is not None else torch.zeros(C, dtype=torch.float64, device=device)
+        else:
+            wqkv = f64(a.qkv.weight)
+            bqkv = f64(a.qkv.bias) if a.qkv.bias is not None else torch.zeros(3 * C, dtype=torch.float64, device=device)
+            wqk, wv, bqk, bv = wqkv[: 2 * C], wqkv[2 * C:], bqkv[: 2 * C], bqkv[2 * C:]
+        g1, g2, g3 = f64(blk.gamma1), f64(blk.gamma2), f64(blk.gamma3)
+
+        def P(weight, bias, cin):
+            pc = ops.PackedConv([_View(weight.float()[:, :, None, None].contiguous(), bias.float().contiguous())], dtype, device,
+                                src_channels=[cin])
+            self._keep.append(pc)
+            return pc.layer_struct()
+
+        def dw(conv, scale):  # [C,1,3,3] -> fp32 [9][C] tap-major, times a per-channel scale
+            w = f64(conv.weight).reshape(C, 9) * scale[:, None]
+            return f32(w.t()), f32(f64(conv.bias) * scale)
+
+        x = _lib.XcitBlock()
+        tp = xc.pos_embeder.token_projection
+        x.pos_proj = P(f64(tp.weight)[:, :, 0, 0], f64(tp.bias), tp.weight.shape[1])
+        x.qk = P(wqk * ln1w[None, :], bqk + wqk @ ln1b, C)
+        x.v_weight, x.v_bias = f32(wv * ln1w[None, :]), f32(bv + wv @ ln1b)
+        wp, bp = f64(a.proj.weight), f64(a.proj.bias)
+        x.proj_weight, x.proj_bias = f32(g1[:, None] * wp), f32(g1 * bp)
+        x.temperature = f32(f64(a.temperature).reshape(-1))
+        x.ln3_weight, x.ln3_bias = f32(f64(blk.norm3.weight)), f32(f64(blk.norm3.bias))
+        lp = blk.local_mp
+        one = torch.ones(C, dtype=torch.float64, device=device)
+        x.dw1_weight, x.dw1_bias = dw(lp.conv1, one)
+        x.gn_weight, x.gn_bias = f32(f64(lp.bn.weight)), f32(f64(lp.bn.bias))
+        x.dw2_weight, x.dw2_bias = dw(lp.conv2, g3)
+        w1, b1, ln2w, ln2b = f64(blk.mlp.fc1.weight), f64(blk.mlp.fc1.bias), f64(blk.norm2.weight), f64(blk.norm2.bias)
+        x.fc1 = P(w1 * ln2w[None, :], b1 + w1 @ ln2b, C)
+        x.fc2 = P(g2[:, None] * f64(blk.mlp.fc2.weight), g2 * f64(blk.mlp.fc2.bias), w1.shape[0])
+        x.ln_eps, x.gn_eps = float(blk.norm1.eps), float(lp.bn.eps)
+        return x
+
+    def _hold(self, t: torch.Tensor) -> int:
+        self._keep.append(t)
+        return t.data_ptr()
+
+    _ws_symbol = "pfb_ccmr_workspace_bytes"
+
+    def refine_scale(self, scale: int, pyramid: Sequence[torch.Tensor], net: torch.Tensor, inp: torch.Tensor, coords: torch.Tensor, iters: int,
+                     out_hw, pad, ws: torch.Tensor, fmap1: Optional[torch.Tensor] = None, corr_scale: float = 0.0, volume_layout: int = 0,
+                     last: bool = False, upflow2: int = 0):
+        """One scale in place on (net, coords).  Not last: returns the next scale's coordinates fp32 [B,2H,2W,2].  Last: returns
+        (flow_up fp32 [B,2,oh,ow], flow_small fp32 [B,2,oh//16,ow//16])."""
+        B, H, W, _ = net.shape
+        alt = fmap1 is not None
+        cfg = self.make_cfg(B, H, W, iters, out_hw, pad, alt, fmap1.shape[-1] if alt else 0, volume_layout)
+        flow_up = flow_small = nxt = None
+        if last:
+            flow_up = torch.empty((B, 2, out_hw[0], out_hw[1]), dtype=torch.float32, device=self.device)
+            flow_small = torch.empty((B, 2, out_hw[0] // 16, out_hw[1] // 16), dtype=torch.float32, device=self.device)
+        else:
+            nxt = torch.empty((B, 2 * H, 2 * W, 2), dtype=torch.float32, device=self.device)
+        pyr = ptr_array(pyramid)
+        buf = _lib.RaftBuffers(C.cast(pyr, C.POINTER(C.c_void_p)), fmap1.data_ptr() if alt else None, net.data_ptr(), inp.data_ptr(),
+                               coords.data_ptr(), flow_up.data_ptr() if last else None, flow_small.data_ptr() if last else None,
+                               ws.data_ptr(), ws.numel(), None, 0.0)
+        with torch.cuda.device(self.device):
+            check(load().pfb_ccmr_refine(C.byref(cfg), C.byref(self.scale_weights[scale]), C.byref(buf), corr_scale, int(upflow2),
+                                         nxt.data_ptr() if nxt is not None else None, stream_ptr(self.device)), "ccmr_refine")
+        return (flow_up, flow_small) if last else nxt
+
+    def xcit_context(self, scale: int, inp: torch.Tensor) -> torch.Tensor:
+        """global_context = xcit[scale](inp) (operator-level tests): inp, result pixel-major [B,H,W,128]."""
+        B, H, W, _ = inp.shape
+        cfg = self.make_cfg(B, H, W, 1, (2 * H, 2 * W), (0, 0), False, 0)
+        ws = self.workspace(cfg)
+        out = torch.empty_like(inp)
+        with torch.cuda.device(self.device):
+            check(load().pfb_xcit_context(C.byref(cfg), C.byref(self.scale_weights[scale]), inp.data_ptr(), out.data_ptr(), ws.data_ptr(),
+                                          ws.numel(), stream_ptr(self.device)), "xcit_context")
+        return out
+
+    def update_iter(self, net: torch.Tensor, inp: torch.Tensor, coords: torch.Tensor, corr: Optional[torch.Tensor] = None,
+                    pyramid: Optional[Sequence[torch.Tensor]] = None, want_mask: bool = False, attention: Optional[torch.Tensor] = None,
+                    fmap1: Optional[torch.Tensor] = None, corr_scale: float = 0.0, scale: int = 0):
+        """One update-block evaluation of scale ``scale`` (operator-level tests); returns the [B,H,W,36] mask when asked."""
+        B, H, W, _ = net.shape
+        alt = fmap1 is not None
+        cfg = self.make_cfg(B, H, W, 1, (2 * H, 2 * W), (0, 0), alt, fmap1.shape[-1] if alt else 0)
+        ws = self.workspace(cfg)
+        mask = torch.empty((B, H, W, 36), dtype=self.dtype, device=self.device) if want_mask else None
+        pyr = ptr_array(pyramid) if pyramid is not None else None
+        buf = _lib.RaftBuffers(C.cast(pyr, C.POINTER(C.c_void_p)) if pyr is not None else None, fmap1.data_ptr() if alt else None,
+                               net.data_ptr(), inp.data_ptr(), coords.data_ptr(), None, None, ws.data_ptr(), ws.numel(), None, 0.0)
+        with torch.cuda.device(self.device):
+            check(load().pfb_ccmr_update_iter(C.byref(cfg), C.byref(self.scale_weights[scale]), C.byref(buf),
+                                              corr.data_ptr() if corr is not None else None, mask.data_ptr() if mask is not None else None,
+                                              corr_scale, stream_ptr(self.device)), "ccmr_update_iter")
         return mask

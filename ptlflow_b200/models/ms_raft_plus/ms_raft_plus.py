@@ -53,11 +53,16 @@ class ResidualBlock(nn.Module):
 class _PyramidEncoder(_Encoder):
     """BasicEncoder / Basic_Context_Encoder of ms_raft_plus/extractor.py:123-323: conv1 7x7 / 2 -> GroupNorm(8, 64) -> ReLU, layer1..4
     (64, 96, 128, 160 channels at 1/2 .. 1/16), conv2 1x1 -> ``output_dim``, then up_layer2 / 1 / 0 on cat[2x resize(coarser), skip].
-    forward_pm returns the four pixel-major outputs at 1/16, 1/8, 1/4 and 1/2."""
+    forward_pm returns the four pixel-major outputs at 1/16, 1/8, 1/4 and 1/2.
+
+    CCMR's encoders (ccmr/extractor.py:62-274) are the same with ``conv2_dim`` (conv2's width, default ``output_dim``), a 1x1
+    ``after_up_layer{k}_conv`` with bias after each up layer (``after_up_dims``, its output widths) and ``num_up`` = 2 (no up_layer0,
+    three outputs) or 3."""
 
     up_dims: Sequence[int] = (128, 96, 64)
 
-    def __init__(self, output_dim: int = 256) -> None:
+    def __init__(self, output_dim: int = 256, conv2_dim: Optional[int] = None, after_up_dims: Optional[Sequence[int]] = None,
+                 num_up: int = 3) -> None:
         nn.Module.__init__(self)
         self.norm_fn = "group"
         self.norm1 = nn.GroupNorm(8, 64)
@@ -68,14 +73,18 @@ class _PyramidEncoder(_Encoder):
         self.layer2 = self._make_layer(96, 2)
         self.layer3 = self._make_layer(128, 2)
         self.layer4 = self._make_layer(160, 2)
-        self.conv2 = nn.Conv2d(160, output_dim, 1)
+        c2 = output_dim if conv2_dim is None else conv2_dim
+        self.conv2 = nn.Conv2d(160, c2, 1)
         up = self._up_dims(output_dim)
-        self.in_planes = output_dim + 128
-        self.up_layer2 = self._make_layer(up[0], 1)
-        self.in_planes = up[0] + 96
-        self.up_layer1 = self._make_layer(up[1], 1)
-        self.in_planes = up[1] + 64
-        self.up_layer0 = self._make_layer(up[2], 1)
+        self.num_up = num_up
+        prev = c2
+        for k, skip in zip(range(2, 2 - num_up, -1), (128, 96, 64)):  # up_layer2, 1 (, 0)
+            self.in_planes = prev + skip
+            setattr(self, f"up_layer{k}", self._make_layer(up[2 - k], 1))
+            prev = up[2 - k]
+            if after_up_dims is not None:
+                setattr(self, f"after_up_layer{k}_conv", nn.Conv2d(up[2 - k], after_up_dims[2 - k], 1))
+                prev = after_up_dims[2 - k]
         for m in self.modules():
             if isinstance(m, nn.Conv2d):
                 nn.init.kaiming_normal_(m.weight, mode="fan_out", nonlinearity="relu")
@@ -103,8 +112,13 @@ class _PyramidEncoder(_Encoder):
                 e["group"] = c.out_channels // norm.num_groups
             return e
 
-        prep = {"conv1": conv(self.conv1, self.norm1), "conv2": conv(self.conv2, None), "layers": {}}
-        for name in ("layer1", "layer2", "layer3", "layer4", "up_layer2", "up_layer1", "up_layer0"):
+        prep = {"conv1": conv(self.conv1, self.norm1), "conv2": conv(self.conv2, None), "layers": {}, "after": {}}
+        ups = [f"up_layer{k}" for k in range(2, 2 - self.num_up, -1)]
+        for name in ups:
+            after = getattr(self, f"after_{name}_conv", None)
+            if after is not None:
+                prep["after"][name] = conv(after, None)
+        for name in ["layer1", "layer2", "layer3", "layer4"] + ups:
             blocks = []
             for blk in getattr(self, name):
                 e = {"conv1": conv(blk.conv1, blk.norm1), "conv2": conv(blk.conv2, blk.norm2),
@@ -160,10 +174,16 @@ class _PyramidEncoder(_Encoder):
         x = self._layer(e3, L["layer4"])
         y = _conv_pm(x, (prep["conv2"]["w"],), 1, 0)
         e4 = ops.bias_act(y, prep["conv2"]["b"], relu=False, out=y)
-        u2 = self._layer(ops.upsample2x_concat(e4, e3), L["up_layer2"])
-        u1 = self._layer(ops.upsample2x_concat(u2, e2), L["up_layer1"])
-        u0 = self._layer(ops.upsample2x_concat(u1, e1), L["up_layer0"])
-        return [e4, u2, u1, u0]
+        outs = [e4]
+        for k, skip in zip(range(2, 2 - self.num_up, -1), (e3, e2, e1)):
+            name = f"up_layer{k}"
+            u = self._layer(ops.upsample2x_concat(outs[-1], skip), L[name])
+            a = prep["after"].get(name)
+            if a is not None:  # CCMR's 1x1 after_up_layer conv with its bias
+                y = _conv_pm(u, (a["w"],), 1, 0)
+                u = ops.bias_act(y, a["b"], relu=False, out=y)
+            outs.append(u)
+        return outs
 
     forward = _no_forward
 

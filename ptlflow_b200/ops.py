@@ -707,3 +707,99 @@ def corr_lookup_onthefly_scaled(fmap1: torch.Tensor, fmap2_pyramid: Sequence[tor
                                                   L, radius, scale, dtype_code(fmap1.dtype), dtype_code(fmap1.dtype), 0, stride,
                                                   stream_ptr(fmap1.device)), "corr_lookup_onthefly_ex")
     return out
+
+
+# ------------------------------------------------------------------------------------------
+# CCMR (a18): the XCiT block's LayerNorm, LPI convolutions, Fourier features, XCA statistics and fold, upflow2
+# ------------------------------------------------------------------------------------------
+def layernorm(x: torch.Tensor, gamma: Optional[torch.Tensor] = None, beta: Optional[torch.Tensor] = None, eps: float = 1e-6,
+              channels: Optional[int] = None, in_offset: int = 0, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """LayerNorm over the ``channels`` channels from ``in_offset`` of each pixel of x [..., Cs]; the affine gamma / beta (fp32 [C])
+    when given.  Returns [..., C] (or writes ``out``)."""
+    require_cuda(x, "x")
+    Cs = x.shape[-1]
+    Cc = Cs - in_offset if channels is None else channels
+    P = x.numel() // Cs
+    if out is None:
+        out = torch.empty(tuple(x.shape[:-1]) + (Cc,), dtype=x.dtype, device=x.device)
+    require_cuda(out, "out")
+    with torch.cuda.device(x.device):
+        check(load().pfb_layernorm(x.data_ptr(), Cs, in_offset, out.data_ptr(), out.shape[-1], 0, _opt_f32(gamma, Cc, "gamma"),
+                                   _opt_f32(beta, Cc, "beta"), P, Cc, eps, dtype_code(x.dtype), stream_ptr(x.device)), "layernorm")
+    return out
+
+
+def depthwise_conv3x3_ex(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, mode: int, addend: Optional[torch.Tensor] = None) -> torch.Tensor:
+    """LPI's depthwise 3x3 convolutions (zero padded) of x [B,H,W,C]: mode 0 gelu(dw(x) + bias), mode 1 dw(x) + bias + addend.
+    weight fp32 [9, C] tap-major, bias fp32 [C]."""
+    require_cuda(x, "x")
+    B, H, W, Cc = x.shape
+    out = torch.empty_like(x)
+    if addend is not None:
+        require_cuda(addend, "addend")
+    with torch.cuda.device(x.device):
+        check(load().pfb_depthwise_conv3x3_ex(x.data_ptr(), Cc, 0, out.data_ptr(), Cc, 0, _opt_f32(weight, 9 * Cc, "weight"),
+                                              _opt_f32(bias, Cc, "bias"), addend.data_ptr() if addend is not None else None,
+                                              addend.shape[-1] if addend is not None else 0, 0, B, H, W, Cc, mode, dtype_code(x.dtype),
+                                              stream_ptr(x.device)), "depthwise_conv3x3_ex")
+    return out
+
+
+def fourier_features(H: int, W: int, dtype: torch.dtype, device) -> torch.Tensor:
+    """PositionalEncodingFourier's 64 features before token_projection (xcit.py:73-93): [H, W, 64]."""
+    out = torch.empty((H, W, 64), dtype=dtype, device=device)
+    with torch.cuda.device(out.device):
+        check(load().pfb_fourier_features(out.data_ptr(), H, W, dtype_code(dtype), stream_ptr(out.device)), "fourier_features")
+    return out
+
+
+def xca_stats(qk: torch.Tensor, q_offset: int = 0, k_offset: int = 128) -> torch.Tensor:
+    """qk [B,H,W,S] -> fp32 [B, 2304]: per head the 16x16 gram of q, k over the pixels, then the sums of squares of q and of k."""
+    require_cuda(qk, "qk")
+    B, S = qk.shape[0], qk.shape[-1]
+    N = qk.numel() // (B * S)
+    lib = load()
+    stats = torch.empty((B, 2304), dtype=torch.float32, device=qk.device)
+    ws = torch.empty(max(1, lib.pfb_xca_stats_workspace_bytes(B, N)), dtype=torch.uint8, device=qk.device)
+    with torch.cuda.device(qk.device):
+        check(lib.pfb_xca_stats(qk.data_ptr(), S, q_offset, k_offset, B, N, stats.data_ptr(), ws.data_ptr(), dtype_code(qk.dtype),
+                                stream_ptr(qk.device)), "xca_stats")
+    return stats
+
+
+def xca_fold(stats: torch.Tensor, temperature: torch.Tensor, v_w: torch.Tensor, v_b: torch.Tensor, proj_w: torch.Tensor, proj_b: torch.Tensor,
+             dtype: torch.dtype):
+    """-> (w [B,128 in,128 out], w_k [B*128 out,128 in] or None for fp32, bias fp32 [B,128]) of the folded XCA (pfb_xca_fold)."""
+    B = stats.shape[0]
+    dev = stats.device
+    w = torch.empty((B, 128, 128), dtype=dtype, device=dev)
+    wk = torch.empty((B * 128, 128), dtype=dtype, device=dev) if dtype != torch.float32 else None
+    bias = torch.empty((B, 128), dtype=torch.float32, device=dev)
+    with torch.cuda.device(dev):
+        check(load().pfb_xca_fold(stats.data_ptr(), _opt_f32(temperature, 8, "temperature"), _opt_f32(v_w, 128 * 128, "v_w"),
+                                  _opt_f32(v_b, 128, "v_b"), _opt_f32(proj_w, 128 * 128, "proj_w"), _opt_f32(proj_b, 128, "proj_b"),
+                                  w.data_ptr(), wk.data_ptr() if wk is not None else None, bias.data_ptr(), B, dtype_code(dtype),
+                                  stream_ptr(dev)), "xca_fold")
+    return w, wk, bias
+
+
+def upflow2(flow: torch.Tensor, out_hw=None, pad=(0, 0)) -> torch.Tensor:
+    """2 * bilinear 2x (align_corners=True) of flow fp32 [B,2,H,W], the (out_hw, pad) window of the result (ccmr/utils.py:97-99)."""
+    require_cuda(flow, "flow")
+    B, _, H, W = flow.shape
+    oh, ow = out_hw or (2 * H, 2 * W)
+    out = torch.empty((B, 2, oh, ow), dtype=torch.float32, device=flow.device)
+    with torch.cuda.device(flow.device):
+        check(load().pfb_upflow2(flow.data_ptr(), out.data_ptr(), B, H, W, oh, ow, pad[0], pad[1], stream_ptr(flow.device)), "upflow2")
+    return out
+
+
+def convex_handover2x(coords: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
+    """CCMR's handover: fine grid + convex 2x of (coords - grid), coords fp32 [B,H,W,2], mask [B,H,W,36] -> fp32 [B,2H,2W,2]."""
+    require_cuda(coords, "coords"); require_cuda(mask, "mask")
+    B, H, W, _ = coords.shape
+    out = torch.empty((B, 2 * H, 2 * W, 2), dtype=torch.float32, device=coords.device)
+    with torch.cuda.device(coords.device):
+        check(load().pfb_convex_handover2x(coords.data_ptr(), mask.data_ptr(), out.data_ptr(), B, H, W, dtype_code(mask.dtype),
+                                           stream_ptr(coords.device)), "convex_handover2x")
+    return out
