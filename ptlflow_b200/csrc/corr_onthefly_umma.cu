@@ -10,8 +10,8 @@
 // bands of 8 rows (band stride 7, so that every vertical tap pair lies inside one band):
 //     D[128 queries][256 targets] = F1_tile[128][C] . F2_band[256][C]^T        (wgmma: two warpgroups of m64n128 per band half)
 // Both operands are TMA boxes of the pixel-major feature maps (out-of-map targets are zero-filled by the TMA unit: the
-// zero padding of raft/utils.py:71-75 for free).  The MMA warpgroups dump the accumulator rows to shared memory (storage
-// type -- the same rounding the materialised volume has); each epilogue thread owns one query and blends the window rows that
+// zero padding of raft/utils.py:71-75 for free).  The MMA warpgroups dump the accumulator rows, scaled, to shared memory
+// (storage type -- the same rounding the materialised volume has); each epilogue thread owns one query and blends the window rows that
 // fall into this band (x-major order of corr.py:43-47) and stages the level's 81 outputs for a coalesced store.
 // Queries whose window does not fit the region (rough flow inside a tile) are flagged and recomputed by the SIMT kernel
 // (exact same values, one warp per flagged query), so the result never depends on the smoothness of the flow.
@@ -193,15 +193,17 @@ corr_onthefly_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
           if (++sb == a.b_stages) { sb = 0; phb ^= 1; }
         }
         if (threadIdx.x == 256) OTF_TR(8 + kb * 6 + 1);
-        // ---- accumulator -> dump rows (storage-type rounding, the rounding the materialised volume has) ----
+        // ---- accumulator -> dump rows: scaled, then rounded to the storage type (the materialised volume's rounding).
+        // Scaling first keeps f16 finite where |a.b| exceeds 65504 but the scaled correlation does not ----
         if (nh == 0) mbar_wait(&bars->dump_empty, (g & 1) ^ 1);  // the epilogue is done with band g - 1
         {
           const int r0 = mh * 64 + 16 * (tid >> 5) + ((tid & 31) >> 2), c0 = nh * 128 + 2 * (tid & 3);
           uint8_t* d0 = sD + r0 * kOtfDumpPitch + c0 * 2;
+          const float s = a.scale;
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
-            *reinterpret_cast<uint32_t*>(d0 + 16 * j) = otf_pack2<T>(d[4 * j + 0], d[4 * j + 1]);
-            *reinterpret_cast<uint32_t*>(d0 + 8 * kOtfDumpPitch + 16 * j) = otf_pack2<T>(d[4 * j + 2], d[4 * j + 3]);
+            *reinterpret_cast<uint32_t*>(d0 + 16 * j) = otf_pack2<T>(d[4 * j + 0] * s, d[4 * j + 1] * s);
+            *reinterpret_cast<uint32_t*>(d0 + 8 * kOtfDumpPitch + 16 * j) = otf_pack2<T>(d[4 * j + 2] * s, d[4 * j + 3] * s);
           }
         }
        }
@@ -241,10 +243,10 @@ corr_onthefly_umma_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_
         const bool finite = (fabsf(x) < 1e7f) && (fabsf(y) < 1e7f);
         const float xf = finite ? floorf(x) : -1e6f, yf = finite ? floorf(y) : -1e6f;
         const float fx = finite ? x - xf : 0.f, fy = finite ? y - yf : 0.f;
-        g.w00 = (1.f - fx) * (1.f - fy) * a.scale;
-        g.w10 = fx * (1.f - fy) * a.scale;
-        g.w01 = (1.f - fx) * fy * a.scale;
-        g.w11 = fx * fy * a.scale;
+        g.w00 = (1.f - fx) * (1.f - fy);  // (the dump rows already carry the scale)
+        g.w10 = fx * (1.f - fy);
+        g.w01 = (1.f - fx) * fy;
+        g.w11 = fx * fy;
         g.x0 = (int)xf - R;
         g.y0 = (int)yf - R;
         // (selects, not a.lw[g.l]: a dynamic index into the kernel parameters makes ptxas copy them to a stack frame)

@@ -178,19 +178,19 @@ __global__ void __launch_bounds__(kTlWarps * 32) corr_lookup_tiled_kernel(const 
 template <typename T>
 static int launch_lookup_tiled(const TiledLevels& lv, const float* coords, void* out, int nq, int levels, int radius, int out_stride,
                                cudaStream_t s) {
+  if (!(radius == 4 || (radius == 3 && levels >= 3))) {  // refused before the launch is counted
+    set_error("corr_lookup_tiled: radius=%d levels=%d not instantiated (radius 4 with 1-4 levels, radius 3 with 3-4)", radius, levels);
+    return PFB_ERR_UNSUPPORTED;
+  }
   dim3 grid(ceil_div(nq, kTlWarps));
   ProfScope prof(KC_LOOKUP, s);
 #define PFB_TL(R, L) PFB_CUDA(launch_pdl(corr_lookup_tiled_kernel<T, R, L>, grid, dim3(kTlWarps * 32), 0, s, lv, coords, (T*)out, nq, out_stride))
   if (radius == 4 && levels == 4) PFB_TL(4, 4);
   else if (radius == 4 && levels == 3) PFB_TL(4, 3);
   else if (radius == 4 && levels == 2) PFB_TL(4, 2);
-  else if (radius == 4 && levels == 1) PFB_TL(4, 1);
-  else if (radius == 3 && levels == 4) PFB_TL(3, 4);
-  else if (radius == 3 && levels == 3) PFB_TL(3, 3);
-  else {
-    set_error("corr_lookup_tiled: radius=%d levels=%d not instantiated (radius 4 with 1-4 levels, radius 3 with 3-4)", radius, levels);
-    return PFB_ERR_UNSUPPORTED;
-  }
+  else if (radius == 4) PFB_TL(4, 1);
+  else if (levels == 4) PFB_TL(3, 4);
+  else PFB_TL(3, 3);
 #undef PFB_TL
   PFB_LAUNCH_CHECK();
   return PFB_OK;
