@@ -605,8 +605,9 @@ PFB_API int pfb_ccmr_update_iter(const pfb_raft_cfg* cfg, const pfb_ccmr_weights
 
 /* ------------------------------------------------------------------------------------
  * Encoder-side kernels (SURVEY.md section 8(f) rank 1: the callers either side of the path).
- * The 3x3 / 7x7 / 1x1 convolutions of BasicEncoder / SmallEncoder (extractor.py:122-267) still run in
- * cuDNN; pre-processing, instance norm + ReLU (+ residual) and the residual joins are fused here.
+ * The first 7x7 convolution and the residual blocks' stride-1 3x3 convolutions of BasicEncoder (extractor.py:122-267)
+ * run here, the strided, 1x1 and bottleneck convolutions in cuDNN; pre-processing, instance norm + ReLU (+ residual)
+ * and the residual joins are fused here.
  * ---------------------------------------------------------------------------------- */
 /* images [B,2,3,H,W] BGR in [0,1] (NCHW) -> out [2B,Hp,Wp,out_channels] pixel-major RGB in [-1,1], replicate
  * padded; channels 3..out_channels-1 are zero (out_channels = 4 gives the first convolution 8-byte pixels, which
@@ -656,6 +657,23 @@ PFB_API int pfb_flow_conv7x7(const float* flow, const void* wpack, const float* 
                              int B, int H, int W, pfb_dtype dtype, pfb_stream stream);
 PFB_API int pfb_first_conv7x7s2(const void* x, const void* wpack, const float* bias, void* out, double* stats, int N, int H, int W,
                                 int relu, pfb_dtype dtype, pfb_stream stream);
+/* 3x3 stride-1 "same" convolution of the encoders' residual blocks on wgmma, output channels on the MMA's M dimension
+ * (csrc/enc_conv_umma.cu).
+ *   x         [B,H,W,Cin] f16/bf16 pixel-major, contiguous; Cin a multiple of 32
+ *   weight_k  the K-major packing of ptlflow_b200.ops.PackedConv: [9][Cout_pad_k][Cin_pad], Cout_pad_k = Cout rounded up to
+ *             32, Cin_pad = Cin rounded up to 64 (zero columns beyond Cin)
+ *   Cout      64, 96 or 128
+ *   epilogue  PFB_ENC_CONV_LINEAR: acc (bias ignored; instance norm follows);  PFB_ENC_CONV_BIAS_RELU: relu(acc + bias);
+ *             PFB_ENC_CONV_BIAS_RELU_RESIDUAL: relu(residual + relu(acc + bias)), residual [B,H,W,Cout] contiguous
+ *   bias      fp32 [Cout]
+ *   out       [B,H,W,out_stride], channels out_offset .. out_offset + Cout - 1 written (both multiples of 8)
+ * Accumulation in fp32, one rounding to the storage type. */
+enum pfb_enc_conv_epilogue { PFB_ENC_CONV_LINEAR = 0, PFB_ENC_CONV_BIAS_RELU = 1, PFB_ENC_CONV_BIAS_RELU_RESIDUAL = 2 };
+/* 1 when pfb_enc_conv3x3 runs these channel counts in this storage type (host only, no device needed). */
+PFB_API int pfb_enc_conv3x3_supported(int Cin, int Cout, pfb_dtype dtype);
+PFB_API int pfb_enc_conv3x3(const void* x, const void* weight_k, const float* bias, const void* residual, void* out, int B, int H,
+                            int W, int Cin, int Cout, int out_stride, int out_offset, int epilogue, pfb_dtype dtype,
+                            pfb_stream stream);
 /* y = act(x + bias[c]) or, with residual, y = relu(residual + act(x + bias[c]));  bias fp32 [C] (may be NULL);
  * workspace >= 8*C bytes.  Used for the batch-norm-folded context encoder (conv bias + BN shift) and conv2. */
 PFB_API int pfb_bias_act(const void* x, const float* bias, const void* residual, void* y, void* workspace, int B, int H, int W,

@@ -24,6 +24,8 @@ _DTYPES = {torch.float32: F32, torch.float16: F16, torch.bfloat16: BF16}
 
 EPI_LINEAR, EPI_RELU, EPI_GRU_ZR, EPI_GRU_Q, EPI_FLOW, EPI_RELU_APPEND_FLOW, EPI_AXPY, EPI_LINEAR_F32 = range(8)
 EPI_GELU, EPI_RESIDUAL_GELU, EPI_LINEAR_APPEND_FLOW = range(8, 11)
+# pfb_enc_conv_epilogue
+ENC_CONV_LINEAR, ENC_CONV_BIAS_RELU, ENC_CONV_BIAS_RELU_RESIDUAL = range(3)
 
 (L_CONVC1, L_CONVC2, L_CONVF1, L_CONVF2, L_CONV, L_GRU_ZR1, L_GRU_Q1, L_GRU_ZR2, L_GRU_Q2,
  L_FLOW1, L_FLOW2, L_MASK1, L_MASK2, L_AGG_V, L_FLOW2T,
@@ -171,6 +173,8 @@ SIGNATURES = {
     "pfb_flow_conv7x7": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _S]),
     "pfb_first_conv7x7s2": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _S]),
     "pfb_bias_act": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _S]),
+    "pfb_enc_conv3x3_supported": (_I, [_I, _I, _I]),
+    "pfb_enc_conv3x3": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
     "pfb_launch_count": (C.c_ulonglong, [_I]),
     "pfb_profile_enable": (_I, [_I]),
     "pfb_profile_collect": (_I, [C.POINTER(C.c_double), C.POINTER(C.c_ulonglong), _I]),

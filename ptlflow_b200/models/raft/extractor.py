@@ -5,6 +5,7 @@ from __future__ import annotations
 
 import os
 import threading
+from types import SimpleNamespace
 
 import torch
 import torch.nn as nn
@@ -94,6 +95,12 @@ def _fold(conv: nn.Conv2d, norm: nn.Module, dtype, device):
 
 _NATIVE_CONV1 = bool(int(os.environ.get("PFB_NATIVE_CONV1", "1")))
 _NATIVE_CONV2 = bool(int(os.environ.get("PFB_NATIVE_CONV2", "1")))
+# the residual blocks' 3x3 stride-1 convolutions on pfb_enc_conv3x3 (read at every forward: tools/time_encoder_convs.py
+# switches it to compare both paths in one process)
+_NATIVE_ENC_CONV = bool(int(os.environ.get("PFB_NATIVE_ENC_CONV", "1")))
+# (Cin, Cout) of eligible layers that stay on cuDNN unless the kernel also takes their residual join: at 96 output channels
+# the kernel computes 128 MMA rows, and cuDNN measured faster on the plain convolution (DESIGN.md section 5)
+_ENC_CONV_CUDNN_UNFUSED = frozenset({(96, 96)})
 # batch-norm-folded convolutions without a residual join: cuDNN's own conv + bias + ReLU epilogue instead of a separate pass
 _CUDNN_FUSED_RELU = bool(int(os.environ.get("PFB_CUDNN_FUSED_RELU", "1")))
 _prep_lock = threading.Lock()
@@ -106,6 +113,16 @@ def _conv_pm(x: torch.Tensor, wb, stride: int, padding: int) -> torch.Tensor:
     y = F.conv2d(x.permute(0, 3, 1, 2), wb[0], None, stride=stride, padding=padding)
     y = y.permute(0, 2, 3, 1)
     return y if y.is_contiguous() else y.contiguous()
+
+
+def enc_conv_eligible(conv: nn.Conv2d, dtype: torch.dtype, fused_residual: bool = False) -> bool:
+    """A 3x3 stride-1 "same" convolution that pfb_enc_conv3x3 runs in this storage type (f16 / bf16; Cin a multiple of 32,
+    Cout 64, 96 or 128), and that cuDNN did not measure faster on.  ``fused_residual``: the layer's bias, ReLU and residual
+    join would go into the kernel's epilogue (a batch-norm-folded block's second convolution)."""
+    return (tuple(conv.kernel_size) == (3, 3) and tuple(conv.stride) == (1, 1) and tuple(conv.padding) == (1, 1)
+            and tuple(conv.dilation) == (1, 1) and conv.groups == 1 and conv.padding_mode == "zeros"
+            and (fused_residual or (conv.in_channels, conv.out_channels) not in _ENC_CONV_CUDNN_UNFUSED)
+            and ops.enc_conv3x3_supported(conv.in_channels, conv.out_channels, dtype))
 
 
 class _Encoder(nn.Module):
@@ -172,6 +189,20 @@ class _Encoder(nn.Module):
         if (_NATIVE_CONV2 and dtype in (torch.float16, torch.bfloat16) and tuple(c2.kernel_size) == (1, 1) and c2.in_channels % 64 == 0
                 and c2.out_channels % 32 == 0 and c2.out_channels <= 1024):
             prep["conv2_native"] = ops.PackedConv([c2], dtype, device, src_channels=[c2.in_channels])
+        # the residual blocks' 3x3 stride-1 convolutions on pfb_enc_conv3x3 (output channels on the MMA's M dimension): packed
+        # from the folded fp32 weights (rounded to the storage type once, as _fold does for cuDNN), with the fp32 bias.  Packed
+        # whatever PFB_NATIVE_ENC_CONV says: forward_pm reads the switch at every call
+        if dtype in (torch.float16, torch.bfloat16):
+            blocks = [blk for layer in (self.layer1, self.layer2, self.layer3) for blk in layer]
+            for e, blk in zip(prep["blocks"], blocks):
+                if not isinstance(blk, ResidualBlock):
+                    continue
+                for nme, norm in (("conv1", blk.norm1), ("conv2", blk.norm2)):
+                    conv = getattr(blk, nme)
+                    if enc_conv_eligible(conv, dtype, fused_residual=nme == "conv2" and self.norm_fn != "instance"):
+                        w, b = _fold(conv, norm, torch.float32, device)
+                        folded = SimpleNamespace(weight=w, bias=None)
+                        e[nme + "_enc"] = (ops.PackedConv([folded], dtype, device, src_channels=[conv.in_channels]), b)
         # the fold / pack kernels ran on this thread's stream: finish them before other streams can see the cache
         torch.cuda.current_stream(device).synchronize()
         self._prep_cache = (sig, prep)
@@ -186,7 +217,15 @@ class _Encoder(nn.Module):
         inst = self.norm_fn == "instance"
         prep = self._prepared(x.dtype, x.device)
 
-        def conv_act(x, wb, stride, padding, relu=True, residual=None):
+        def conv_act(x, wb, stride, padding, relu=True, residual=None, native=None):
+            if (native is not None and _NATIVE_ENC_CONV and relu and x.is_contiguous()
+                    and (residual is None or residual.is_contiguous())):
+                packed, bias = native
+                if inst:  # the instance norm removes the bias
+                    y = ops.enc_conv3x3(x, packed)
+                    return ops.instance_norm_act(y, relu=True, residual=residual, out=y)
+                epi = _lib.ENC_CONV_BIAS_RELU if residual is None else _lib.ENC_CONV_BIAS_RELU_RESIDUAL
+                return ops.enc_conv3x3(x, packed, epi, bias=bias, residual=residual)
             if _CUDNN_FUSED_RELU and not inst and relu and residual is None and x.dtype != torch.float32:
                 bh = wb[2] if len(wb) > 2 else wb[1].to(x.dtype)
                 y = torch.cudnn_convolution_relu(x.permute(0, 3, 1, 2), wb[0], bh, (stride, stride), (padding, padding), (1, 1), 1)
@@ -227,8 +266,8 @@ class _Encoder(nn.Module):
                 y = conv_act(y, e["conv2"], s, 1)
                 x = conv_act(y, e["conv3"], 1, 0, relu=True, residual=xs)
             else:  # residual: 3x3 (stride) -> 3x3
-                y = conv_act(x, e["conv1"], s, 1)
-                x = conv_act(y, e["conv2"], 1, 1, relu=True, residual=xs)
+                y = conv_act(x, e["conv1"], s, 1, native=e.get("conv1_enc"))
+                x = conv_act(y, e["conv2"], 1, 1, relu=True, residual=xs, native=e.get("conv2_enc"))
         if "conv2_native" in prep and x.is_contiguous():
             packed = prep["conv2_native"]
             out = torch.empty(x.shape[:3] + (packed.Cout,), dtype=x.dtype, device=x.device)

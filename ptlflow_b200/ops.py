@@ -304,6 +304,38 @@ def conv2d(srcs, packed: PackedConv, out: torch.Tensor, epilogue: int = _lib.EPI
     return out
 
 
+def enc_conv3x3_supported(cin: int, cout: int, dtype: torch.dtype) -> bool:
+    """Whether enc_conv3x3 runs a 3x3 stride-1 convolution with these channel counts in this storage type (host only)."""
+    if dtype not in (torch.float16, torch.bfloat16):
+        return False
+    return bool(load().pfb_enc_conv3x3_supported(int(cin), int(cout), dtype_code(dtype)))
+
+
+def enc_conv3x3(x: torch.Tensor, packed: PackedConv, epilogue: int = _lib.ENC_CONV_LINEAR, bias: Optional[torch.Tensor] = None,
+                residual: Optional[torch.Tensor] = None, out: Optional[torch.Tensor] = None, out_offset: int = 0) -> torch.Tensor:
+    """3x3 stride-1 "same" convolution x [B,H,W,Cin] -> [B,H,W,Cout] on pfb_enc_conv3x3 (see the header).  ``packed``: a
+    PackedConv with the K-major packing (src_channels given); ``bias`` fp32 [Cout] (the epilogues with bias); ``residual``
+    [B,H,W,Cout] (ENC_CONV_BIAS_RELU_RESIDUAL).  ``out`` [B,H,W,S] receives channels out_offset .. out_offset + Cout - 1."""
+    require_cuda(x, "x")
+    B, H, W, Cin = x.shape
+    if packed.weight_k is None or (packed.KH, packed.KW) != (3, 3) or packed.Cin != Cin or not x.is_contiguous() or x.dtype != packed.dtype:
+        raise RuntimeError("enc_conv3x3: x must be contiguous [B,H,W,Cin] in the dtype of a 3x3 PackedConv with the K-major packing")
+    if out is None:
+        out = torch.empty((B, H, W, packed.Cout), dtype=x.dtype, device=x.device)
+    require_cuda(out, "out")
+    if out.shape[:3] != x.shape[:3] or not out.is_contiguous() or out.dtype != x.dtype:
+        raise RuntimeError("enc_conv3x3: out must be contiguous [B,H,W,S] in the input's dtype")
+    if bias is not None and (bias.dtype != torch.float32 or bias.numel() < packed.Cout or not bias.is_cuda):
+        raise RuntimeError("enc_conv3x3: bias must be fp32 [Cout] on the device")
+    if residual is not None and (tuple(residual.shape) != (B, H, W, packed.Cout) or not residual.is_contiguous() or residual.dtype != x.dtype):
+        raise RuntimeError("enc_conv3x3: residual must be contiguous [B,H,W,Cout] in the input's dtype")
+    with torch.cuda.device(x.device):
+        check(load().pfb_enc_conv3x3(x.data_ptr(), packed.weight_k.data_ptr(), bias.data_ptr() if bias is not None else None,
+                                     residual.data_ptr() if residual is not None else None, out.data_ptr(), B, H, W, Cin, packed.Cout,
+                                     out.shape[-1], out_offset, epilogue, dtype_code(x.dtype), stream_ptr(x.device)), "enc_conv3x3")
+    return out
+
+
 def depthwise_conv_gelu(x: torch.Tensor, weight: torch.Tensor, bias: torch.Tensor, k: int, channels: Optional[int] = None,
                         in_offset: int = 0, out: Optional[torch.Tensor] = None, out_offset: int = 0) -> torch.Tensor:
     """gelu(x + depthwise_conv_kxk(x) + bias) of a PCBlock (skflow/update.py:32-33).  x [B,H,W,Cs] pixel-major, the ``channels``
