@@ -429,19 +429,28 @@ static int make_ctx(Ctx& x, const pfb_raft_cfg* cfg, const pfb_raft_weights* w, 
 
 using namespace pfb;
 
-extern "C" PFB_API size_t pfb_raft_workspace_bytes(const pfb_raft_cfg* cfg) {
-  if (check_cfg(cfg) != PFB_OK) return 0;
-  return plan(cfg).total;
+// the workspace of the msraft / ccmr / raft entry points (ccmr's holds its XCiT plan after the loop's); 0 for a cfg they refuse
+static size_t workspace_bytes(const pfb_raft_cfg* cfg, bool msraft, bool ccmr) {
+  if (check_cfg(cfg, msraft, ccmr) != PFB_OK) return 0;
+  return plan(cfg).total + (ccmr ? ccmr_plan(cfg).total : 0);
 }
+
+// one update-block evaluation from the entry coordinates, on a built context: the flow, the context terms, the lookup unless the
+// caller hands in the correlation
+static int update_iter_once(Ctx& x, const void* corr, void* mask_out) {
+  PFB_TRY(launch_flow_from_coords(x.b->coords, reinterpret_cast<float*>(x.at(x.ws.off_flow)), x.c->B, x.c->H, x.c->W, x.s));
+  PFB_TRY(run_context_terms(x));
+  if (!corr) PFB_TRY(lookup(x));
+  return update_iter(x, corr, mask_out);
+}
+
+extern "C" PFB_API size_t pfb_raft_workspace_bytes(const pfb_raft_cfg* cfg) { return workspace_bytes(cfg, false, false); }
 
 extern "C" PFB_API int pfb_raft_update_iter(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf,
                                     const void* corr, void* mask_out, pfb_stream stream) {
   Ctx x;
   PFB_TRY(make_ctx(x, cfg, w, buf, as_stream(stream), corr == nullptr));
-  PFB_TRY(launch_flow_from_coords(buf->coords, reinterpret_cast<float*>(x.at(x.ws.off_flow)), cfg->B, cfg->H, cfg->W, x.s));
-  PFB_TRY(run_context_terms(x));
-  if (!corr) PFB_TRY(lookup(x));
-  return update_iter(x, corr, mask_out);
+  return update_iter_once(x, corr, mask_out);
 }
 
 // flow from the entry coordinates, the once-per-call context terms, then cfg->iters iterations (the mask head on the last one only)
@@ -487,10 +496,7 @@ extern "C" PFB_API int pfb_raft_refine(const pfb_raft_cfg* cfg, const pfb_raft_w
 }
 
 // ---- a17: MS-RAFT+ (one call per scale of ms_raft_plus.py:177-214) ----
-extern "C" PFB_API size_t pfb_msraft_workspace_bytes(const pfb_raft_cfg* cfg) {
-  if (check_cfg(cfg, true) != PFB_OK) return 0;
-  return plan(cfg).total;
-}
+extern "C" PFB_API size_t pfb_msraft_workspace_bytes(const pfb_raft_cfg* cfg) { return workspace_bytes(cfg, true, false); }
 
 extern "C" PFB_API int pfb_msraft_update_iter(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf,
                                               const void* corr, void* mask_out, float corr_scale, pfb_stream stream) {
@@ -498,10 +504,7 @@ extern "C" PFB_API int pfb_msraft_update_iter(const pfb_raft_cfg* cfg, const pfb
   PFB_TRY(make_ctx(x, cfg, w, buf, as_stream(stream), corr == nullptr, true));
   PFB_CHECK_ARG(corr_scale >= 0.f, "msraft_update_iter: corr_scale=%g", (double)corr_scale);
   x.corr_scale = corr_scale;
-  PFB_TRY(launch_flow_from_coords(buf->coords, reinterpret_cast<float*>(x.at(x.ws.off_flow)), cfg->B, cfg->H, cfg->W, x.s));
-  PFB_TRY(run_context_terms(x));
-  if (!corr) PFB_TRY(lookup(x));
-  return update_iter(x, corr, mask_out);
+  return update_iter_once(x, corr, mask_out);
 }
 
 extern "C" PFB_API int pfb_msraft_refine(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf, float corr_scale,
@@ -527,10 +530,7 @@ extern "C" PFB_API int pfb_msraft_refine(const pfb_raft_cfg* cfg, const pfb_raft
 }
 
 // ---- a18: CCMR / CCMR+ (one call per scale of ccmr.py:179-220) ----
-extern "C" PFB_API size_t pfb_ccmr_workspace_bytes(const pfb_raft_cfg* cfg) {
-  if (check_cfg(cfg, false, true) != PFB_OK) return 0;
-  return plan(cfg).total + ccmr_plan(cfg).total;
-}
+extern "C" PFB_API size_t pfb_ccmr_workspace_bytes(const pfb_raft_cfg* cfg) { return workspace_bytes(cfg, false, true); }
 
 static int make_ccmr_ctx(Ctx& x, const pfb_raft_cfg* cfg, const pfb_ccmr_weights* w, const pfb_raft_buffers* buf, cudaStream_t s,
                          bool need_pyramid, float corr_scale) {
@@ -558,10 +558,7 @@ extern "C" PFB_API int pfb_ccmr_update_iter(const pfb_raft_cfg* cfg, const pfb_c
   Ctx x;
   PFB_TRY(make_ccmr_ctx(x, cfg, w, buf, as_stream(stream), corr == nullptr, corr_scale));
   PFB_TRY(ccmr_scale_setup(cfg, w, buf->inp, nullptr, true, x.ccmr_base, x.s));
-  PFB_TRY(launch_flow_from_coords(buf->coords, reinterpret_cast<float*>(x.at(x.ws.off_flow)), cfg->B, cfg->H, cfg->W, x.s));
-  PFB_TRY(run_context_terms(x));
-  if (!corr) PFB_TRY(lookup(x));
-  return update_iter(x, corr, mask_out);
+  return update_iter_once(x, corr, mask_out);
 }
 
 extern "C" PFB_API int pfb_ccmr_refine(const pfb_raft_cfg* cfg, const pfb_ccmr_weights* w, const pfb_raft_buffers* buf, float corr_scale,

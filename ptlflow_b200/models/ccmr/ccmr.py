@@ -14,18 +14,14 @@ align_corners=True).  Images are padded to multiples of 32 (output_stride = 32).
 """
 from __future__ import annotations
 
-import math
-from typing import Optional, Sequence
+from typing import Sequence
 
 import torch
 import torch.nn as nn
-import torch.nn.functional as F
 
-from ... import ops
 from ...engine import CCMREngine
 from ...utils.registry import register_model, trainable
-from ..ms_raft_plus.ms_raft_plus import MSRAFTPlus, _PyramidEncoder, _VOLUME_MAX
-from ..raft.raft import RAFT, _cudnn_flags
+from ..ms_raft_plus.ms_raft_plus import MSRAFTPlus, _PyramidEncoder
 from ..raft.update import BasicMotionEncoder, FlowHead, SepConvGRU, _no_forward
 
 _SCALES = {"CCMR": 3, "CCMR+": 4}
@@ -150,14 +146,11 @@ class CCMR(MSRAFTPlus):
             raise ValueError(f"{self._name}: model_type={model_type!r} with num_scales={num_scales} cannot run: the reference's 'CCMR' "
                              f"encoders give 3 scales and 'CCMR+' 4")
         self.num_scales, self.model_type, self.cnet_norm, self.fnet_norm = num_scales, model_type, cnet_norm, fnet_norm
-        _check_iters(iters, num_scales, self._name)
         # the reference stores corr_levels / corr_radius as hyperparameters only; the lookups use lookup_pyramid_levels / radius
         self.ref_corr_levels, self.ref_corr_radius = corr_levels, corr_radius
-        RAFT.__init__(self, corr_levels=lookup_pyramid_levels, corr_radius=lookup_radius, iters=iters, alternate_corr=alternate_corr,
-                      **kwargs)
+        super().__init__(iters=iters, lookup_pyramid_levels=lookup_pyramid_levels, lookup_radius=lookup_radius, alternate_corr=alternate_corr,
+                         **kwargs)
         self.output_stride = 32
-        self.has_trained_on_ptlflow = False
-        self.correlation_depth = lookup_pyramid_levels * (2 * lookup_radius + 1) ** 2
 
     def _build_networks(self) -> None:
         self.hidden_dim = self.context_dim = 128
@@ -169,96 +162,8 @@ class CCMR(MSRAFTPlus):
     def _extra_engine_args(self):
         return {"xcit": self.xcit}
 
-    def _extra_signature(self):
-        return tuple((p.data_ptr(), p._version, p.dtype) for p in self.xcit.parameters())
-
     def _loop_parameters(self):
         return list(self.update_block.parameters()) + list(self.xcit.parameters())
-
-    def _check_grid(self, h32: int, w32: int) -> None:
-        _check_iters(self.iters, self.num_scales, self._name)
-        n = 2 ** (self.corr_levels - 1)
-        h16, w16 = 2 * h32, 2 * w32
-        if h16 < n or w16 < n:
-            raise ValueError(f"{self._name}: the 1/16-resolution grid {h16}x{w16} is smaller than 2**(lookup_pyramid_levels - 1) = {n} "
-                             f"on a side; pad the images to at least {16 * n} px per side")
-
-    def forward(self, inputs):
-        images = inputs["images"]
-        prev = inputs.get("prev_preds")
-        if prev is not None and prev.get("flow_small") is not None:
-            h, w = images.shape[-2:]
-            grid = (-(-h // 32) * 2, -(-w // 32) * 2)
-            fs = tuple(prev["flow_small"].shape[-2:])
-            if fs != grid:
-                # the reference adds the warm start on the padded 1/16 grid (padded to multiples of 32), so it fails unless H and W
-                # are multiples of 32
-                raise ValueError(f"{self._name}: the warm start flow_small is {fs[0]}x{fs[1]} but the padded 1/16 grid of {h}x{w} images "
-                                 f"is {grid[0]}x{grid[1]}; warm starts need H and W that are multiples of 32")
-        return super().forward(inputs)
-
-    def _check_volume(self, images: torch.Tensor) -> None:
-        if self.alternate_corr:
-            return
-        s = 2 ** (self.num_scales - 1)  # the finest scale's grid is s times the 1/16 one
-        h, w = -(-images.shape[-2] // 32) * 2 * s, -(-images.shape[-1] // 32) * 2 * s
-        n = h * w
-        if images.shape[0] * n * n >= _VOLUME_MAX:
-            raise ValueError(f"{self._name}: alternate_corr=False needs a {images.shape[0]} x {n} x {n} correlation volume at the finest "
-                             f"scale, more than the volume kernels address ({_VOLUME_MAX} elements); use alternate_corr=True")
-
-    def _forward_device_impl(self, images: torch.Tensor, flow_init: Optional[torch.Tensor], scratch: Optional[dict]):
-        """images [B,2,3,H,W] on the device -> (flow_up fp32 [B,2,H,W], flow_small fp32 [B,2,H//16,W//16]); enqueued without host
-        synchronisation, so the whole forward is one CUDA graph (ccmr.py:141-230 in eval)."""
-        from ...utils.utils import InputPadder
-
-        resizer = InputPadder(images.shape, stride=self.output_stride, pad_mode="replicate", two_side_pad=True)
-        B = images.shape[0]
-        frames = ops.preprocess_frames(images, resizer.tgt_size, resizer.pad_top_left, out_channels=self.frame_channels)
-        strict = frames.dtype == torch.float32 and self.strict_fp32
-        with _cudnn_flags(self.cudnn_benchmark, not strict):
-            fpyr = self.fnet.forward_pm(frames)  # both frames as one batch: GroupNorm is per sample
-            cpyr = self.cnet.forward_pm(frames[:B])
-        eng = self._get_engine(frames.dtype, frames.device)
-        orig_h, orig_w = images.shape[-2:]
-        h16, w16 = fpyr[0].shape[1:3]
-        coords = ops.init_coords(B, h16, w16, frames.device, flow_init)
-        S = self.num_scales
-        fine = 2 ** (S - 1)
-        ws = eng.workspace(eng.make_cfg(B, fine * h16, fine * w16, 1, (orig_h, orig_w), resizer.pad_top_left, self.alternate_corr, 128), scratch)
-        out = None
-        for i in range(S):
-            f = fpyr[i]
-            C = f.shape[-1]
-            fmap1, fmap2 = f[:B], f[B:]
-            net, inp = ops.context_split(cpyr[i], self.hidden_dim, self.context_dim)
-            scale, layout = 1.0 / math.sqrt(C), 0
-            if self.alternate_corr:
-                if C % 64 and frames.dtype != torch.float32:
-                    # 160 channels at 1/16, 96 at 1/4: rows of a multiple of 64 with zero channels, so the tensor-core lookup serves
-                    # the scale; the dot products are unchanged and the scale stays 1/sqrt(C)
-                    fmap1, fmap2 = F.pad(fmap1, (0, 64 - C % 64)), F.pad(fmap2, (0, 64 - C % 64))
-                pyramid, f1 = ops.feature_pyramid(fmap2.contiguous(), self.corr_levels), fmap1.contiguous()
-            else:
-                pyramid, f1 = eng.build_volume(fmap1.contiguous(), fmap2.contiguous(), impl=self.kernel_impl), None
-                layout = eng.volume_layout
-            last = i == S - 1
-            res = eng.refine_scale(i, pyramid, net, inp, coords, int(self.iters[i]), (orig_h, orig_w), resizer.pad_top_left, ws, fmap1=f1,
-                                   corr_scale=scale, volume_layout=layout, last=last, upflow2=(S - 1 if S == 4 else S) - i if last else 0)
-            if last:
-                out = res
-            else:
-                coords = res
-        return out
-
-
-def _check_iters(iters, num_scales: int, name: str) -> None:
-    try:
-        vals = [int(i) for i in iters]
-    except TypeError:
-        raise ValueError(f"{name}: iters must be a sequence of {num_scales} iteration counts, got {iters!r}") from None
-    if len(vals) != num_scales or min(vals) < 1:
-        raise ValueError(f"{name}: iters must hold num_scales = {num_scales} counts >= 1 (one per scale, coarsest first), got {tuple(iters)!r}")
 
 
 class CCMRPlus(CCMR):

@@ -141,6 +141,9 @@ class GMA(RAFT):
     def _extra_engine_args(self) -> Dict:
         return {"attention_module": self.att}
 
+    def _loop_parameters(self):
+        return list(self.update_block.parameters()) + list(self.att.parameters())
+
 
 @register_model
 @trainable

@@ -205,10 +205,12 @@ class MSRAFTPlus(RAFT):
     }
     _variant = 5
     _engine_cls = MSRaftEngine
+    _name = "ms_raft_p"
+    num_scales = 4  # 1/16, 1/8, 1/4, 1/2
 
     def __init__(self, gamma: float = 0.8, max_flow: float = 400, iters: Sequence[int] = (4, 6, 5, 10), lookup_pyramid_levels: int = 2,
                  lookup_radius: int = 4, alternate_corr: bool = True, **kwargs) -> None:
-        _check_iters(iters)
+        _check_iters(iters, self.num_scales, self._name)
         super().__init__(corr_levels=lookup_pyramid_levels, corr_radius=lookup_radius, gamma=gamma, max_flow=max_flow, iters=iters,
                          alternate_corr=alternate_corr, **kwargs)
         self.output_stride = 16
@@ -248,29 +250,37 @@ class MSRAFTPlus(RAFT):
         self.update_block = BasicUpdateBlock(self.corr_levels, self.corr_radius, hidden_dim=128)
         self.update_block.mask[2] = nn.Conv2d(256, 2 * 2 * 9, 1)  # scale = 2 (ms_raft_plus/update.py:144-148)
 
-    def _check_grid(self, h16: int, w16: int) -> None:
-        _check_iters(self.iters)
+    def _grid16(self, h: int, w: int):
+        """The padded 1/16-resolution grid of h x w images (images are padded to multiples of output_stride)."""
+        s = self.output_stride
+        return -(-h // s) * (s // 16), -(-w // s) * (s // 16)
+
+    def _check_grid(self, h: int, w: int) -> None:
+        """h, w: the grid at output_stride, after padding."""
+        _check_iters(self.iters, self.num_scales, self._name)
         n = 2 ** (self.corr_levels - 1)
+        f = self.output_stride // 16
+        h16, w16 = f * h, f * w
         if h16 < n or w16 < n:
-            raise ValueError(f"ms_raft_p: the 1/16-resolution grid {h16}x{w16} is smaller than 2**(lookup_pyramid_levels - 1) = {n} on "
-                             f"a side; pad the images to at least {16 * n} px per side")
+            raise ValueError(f"{self._name}: the 1/16-resolution grid {h16}x{w16} is smaller than 2**(lookup_pyramid_levels - 1) = {n} "
+                             f"on a side; pad the images to at least {16 * n} px per side")
 
     def forward(self, inputs):
         images = inputs["images"]
         prev = inputs.get("prev_preds")
         if prev is not None and prev.get("flow_small") is not None:
             h, w = images.shape[-2:]
-            grid = (-(-h // 16), -(-w // 16))
+            grid = self._grid16(h, w)
             fs = tuple(prev["flow_small"].shape[-2:])
             if fs != grid:
-                # the reference adds the warm start on the padded 1/16 grid, so it fails unless H and W are multiples of 16
-                raise ValueError(f"ms_raft_p: the warm start flow_small is {fs[0]}x{fs[1]} but the padded 1/16 grid of {h}x{w} images is "
-                                 f"{grid[0]}x{grid[1]}; warm starts need H and W that are multiples of 16")
+                # the reference adds the warm start on the padded 1/16 grid, so it fails unless H and W are multiples of the padding
+                raise ValueError(f"{self._name}: the warm start flow_small is {fs[0]}x{fs[1]} but the padded 1/16 grid of {h}x{w} images "
+                                 f"is {grid[0]}x{grid[1]}; warm starts need H and W that are multiples of {self.output_stride}")
         return super().forward(inputs)
 
     def _forward_device_impl(self, images: torch.Tensor, flow_init: Optional[torch.Tensor], scratch: Optional[dict]):
         """images [B,2,3,H,W] on the device -> (flow_up fp32 [B,2,H,W], flow_small fp32 [B,2,H//16,W//16]); enqueued without host
-        synchronisation, so the whole forward is one CUDA graph (ms_raft_plus.py:146-226 in eval)."""
+        synchronisation, so the whole forward is one CUDA graph (ms_raft_plus.py:146-226, ccmr.py:141-230 in eval)."""
         from ...utils.utils import InputPadder
 
         resizer = InputPadder(images.shape, stride=self.output_stride, pad_mode="replicate", two_side_pad=True)
@@ -281,56 +291,56 @@ class MSRAFTPlus(RAFT):
             fpyr = self.fnet.forward_pm(frames)  # both frames as one batch: GroupNorm is per sample
             cpyr = self.cnet.forward_pm(frames[:B])
         eng = self._get_engine(frames.dtype, frames.device)
-        orig_h, orig_w = images.shape[-2:]
+        out_hw = tuple(images.shape[-2:])
         h16, w16 = fpyr[0].shape[1:3]
         coords = ops.init_coords(B, h16, w16, frames.device, flow_init)
-        # one workspace, planned for the finest (largest) scale, serves the four calls in turn
-        ws = eng.workspace(eng.make_cfg(B, 8 * h16, 8 * w16, 1, (orig_h, orig_w), resizer.pad_top_left, self.alternate_corr, 128), scratch)
-        out = None
-        for i in range(4):
+        S = self.num_scales
+        fine = 2 ** (S - 1)
+        # one workspace, planned for the finest (largest) scale, serves the calls of every scale in turn
+        ws = eng.workspace(eng.make_cfg(B, fine * h16, fine * w16, 1, out_hw, resizer.pad_top_left, self.alternate_corr, 128), scratch)
+        for i in range(S):
             f = fpyr[i]
             C = f.shape[-1]
             fmap1, fmap2 = f[:B], f[B:]
             net, inp = ops.context_split(cpyr[i], self.hidden_dim, self.context_dim)
-            scale, layout = 1.0 / math.sqrt(C), 0
             if self.alternate_corr:
                 if C % 64 and frames.dtype != torch.float32:
-                    # 96 channels at 1/4: rows of 128 with zero channels, so the tensor-core lookup serves the scale; the dot
-                    # products are unchanged and the scale stays 1/sqrt(96)
+                    # 96 channels at 1/4 (and ccmr's 160 at 1/16): rows of a multiple of 64 with zero channels, so the tensor-core
+                    # lookup serves the scale; the dot products are unchanged and the scale stays 1/sqrt(C)
                     fmap1, fmap2 = F.pad(fmap1, (0, 64 - C % 64)), F.pad(fmap2, (0, 64 - C % 64))
-                pyramid, f1 = ops.feature_pyramid(fmap2.contiguous(), self.corr_levels), fmap1.contiguous()
+                pyramid, layout, f1 = ops.feature_pyramid(fmap2.contiguous(), self.corr_levels), 0, fmap1.contiguous()
             else:
-                pyramid, f1 = eng.build_volume(fmap1, fmap2, impl=self.kernel_impl), None
-                layout = eng.volume_layout
-            res = eng.refine_scale(pyramid, net, inp, coords, int(self.iters[i]), (orig_h, orig_w), resizer.pad_top_left, ws, fmap1=f1,
-                                   corr_scale=scale, volume_layout=layout, last=i == 3)
-            if i < 3:
+                (pyramid, layout), f1 = eng.build_volume(fmap1.contiguous(), fmap2.contiguous(), impl=self.kernel_impl), None
+            last = i == S - 1
+            # the last scale's convex 2x upsample reaches 1/2**(4 - S): bilinear 2x steps take it to full resolution
+            res = eng.refine_scale(i, pyramid, layout, net, inp, coords, int(self.iters[i]), out_hw, resizer.pad_top_left, ws, fmap1=f1,
+                                   corr_scale=1.0 / math.sqrt(C), last=last, upflow2=4 - S if last else 0, fork_flow=self.fork_flow)
+            if not last:
                 coords = res
-            else:
-                out = res
-        return out
+        return res
 
     def _check_volume(self, images: torch.Tensor) -> None:
         if self.alternate_corr:
             return
-        h, w = -(-images.shape[-2] // 16) * 8, -(-images.shape[-1] // 16) * 8  # the 1/2-scale grid after padding
-        n = h * w
+        h16, w16 = self._grid16(*images.shape[-2:])
+        fine = 2 ** (self.num_scales - 1)  # the finest scale's grid over the 1/16 one
+        n = h16 * fine * w16 * fine
         if images.shape[0] * n * n >= _VOLUME_MAX:
-            raise ValueError(f"ms_raft_p: alternate_corr=False needs a {images.shape[0]} x {n} x {n} correlation volume at 1/2 scale, more "
-                             f"than the volume kernels address ({_VOLUME_MAX} elements); use alternate_corr=True")
+            raise ValueError(f"{self._name}: alternate_corr=False needs a {images.shape[0]} x {n} x {n} correlation volume at the finest "
+                             f"scale, more than the volume kernels address ({_VOLUME_MAX} elements); use alternate_corr=True")
 
     def _forward_device(self, images: torch.Tensor, flow_init: Optional[torch.Tensor], scratch: Optional[dict] = None):
         self._check_volume(images)
         return super()._forward_device(images, flow_init, scratch)
 
 
-def _check_iters(iters) -> None:
+def _check_iters(iters, num_scales: int, name: str) -> None:
     try:
         vals = [int(i) for i in iters]
     except TypeError:
-        raise ValueError(f"ms_raft_p: iters must be a sequence of four iteration counts, got {iters!r}") from None
-    if len(vals) != 4 or min(vals) < 1:
-        raise ValueError(f"ms_raft_p: iters must hold four counts >= 1 (1/16, 1/8, 1/4, 1/2 scale), got {tuple(iters)!r}")
+        raise ValueError(f"{name}: iters must be a sequence of {num_scales} iteration counts, got {iters!r}") from None
+    if len(vals) != num_scales or min(vals) < 1:
+        raise ValueError(f"{name}: iters must hold num_scales = {num_scales} counts >= 1 (one per scale, coarsest first), got {tuple(iters)!r}")
 
 
 @register_model

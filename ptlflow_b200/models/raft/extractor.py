@@ -5,7 +5,6 @@ from __future__ import annotations
 
 import os
 import threading
-from types import SimpleNamespace
 
 import torch
 import torch.nn as nn
@@ -201,8 +200,7 @@ class _Encoder(nn.Module):
                     conv = getattr(blk, nme)
                     if enc_conv_eligible(conv, dtype, fused_residual=nme == "conv2" and self.norm_fn != "instance"):
                         w, b = _fold(conv, norm, torch.float32, device)
-                        folded = SimpleNamespace(weight=w, bias=None)
-                        e[nme + "_enc"] = (ops.PackedConv([folded], dtype, device, src_channels=[conv.in_channels]), b)
+                        e[nme + "_enc"] = (ops.PackedConv([ops.ConvWeights(w)], dtype, device, src_channels=[conv.in_channels]), b)
         # the fold / pack kernels ran on this thread's stream: finish them before other streams can see the cache
         torch.cuda.current_stream(device).synchronize()
         self._prep_cache = (sig, prep)

@@ -173,29 +173,26 @@ class RAFT(BaseModel):
 
     # -- engine lifecycle ------------------------------------------------------------------
     def _get_engine(self, dtype: torch.dtype, device: torch.device) -> RaftEngine:
+        """The engine, rebuilt when what it packed (the parameters of _loop_parameters()) or what it was built for changed."""
+        key = (dtype, device, self.kernel_impl, self.corr_levels, self.corr_radius,
+               tuple((p.data_ptr(), p._version, p.dtype, str(p.device)) for p in self._loop_parameters()))
         eng = self._engine
-        cls = self._engine_cls
-        if (eng is None or eng.dtype != dtype or eng.device != device or eng.impl != self.kernel_impl
-                or eng.corr_levels != self.corr_levels or eng.corr_radius != self.corr_radius
-                or eng.signature != cls.param_signature(self.update_block)
-                or getattr(eng, "extra_signature", None) != self._extra_signature()):
-            eng = cls(self.update_block, self._variant, self.hidden_dim, self.context_dim, self.corr_levels,
-                             self.corr_radius, dtype, device, impl=self.kernel_impl, **self._extra_engine_args())
-            eng.extra_signature = self._extra_signature()
+        if eng is None or eng.signature != key:
+            eng = self._engine_cls(self._engine_module(), self._variant, self.hidden_dim, self.context_dim, self.corr_levels,
+                                   self.corr_radius, dtype, device, impl=self.kernel_impl, **self._extra_engine_args())
+            eng.signature = key
             self._engine = eng
-        eng.fork_flow = self.fork_flow  # pfb_raft_cfg.fork_flow of the next refine() calls
         return eng
 
     def _loop_parameters(self):
-        """The parameters the refinement engine runs on (the training guard of forward() looks at them)."""
-        return self.update_block.parameters()
+        """The parameters the refinement engine packs (its cache key, and the training guard of forward())."""
+        return list(self.update_block.parameters())
+
+    def _engine_module(self) -> nn.Module:
+        return self.update_block
 
     def _extra_engine_args(self) -> Dict:
         return {}
-
-    def _extra_signature(self):
-        mod = self._extra_engine_args().get("attention_module")
-        return None if mod is None else tuple((p.data_ptr(), p._version) for p in mod.parameters())
 
     def _attention(self, inp: torch.Tensor, eng):
         return None
@@ -318,15 +315,15 @@ class RAFT(BaseModel):
         coords = ops.init_coords(B, H8, W8, fmap1.device, flow_init)
 
         if self.alternate_corr:
-            pyramid, f1 = ops.feature_pyramid(fmap2, self.corr_levels), fmap1
+            pyramid, layout, f1 = ops.feature_pyramid(fmap2, self.corr_levels), 0, fmap1
         else:
-            pyramid, f1 = eng.build_volume(fmap1, fmap2, impl=self.kernel_impl), None
+            (pyramid, layout), f1 = eng.build_volume(fmap1, fmap2, impl=self.kernel_impl), None
 
         orig_h, orig_w = images.shape[-2:]
         pad_top, pad_left = resizer.pad_top_left
         attention = self._attention(inp, eng)  # gma only (gma.py:181)
-        flow_up, flow_small = eng.refine(pyramid, net, inp, coords, self.iters, (orig_h, orig_w), (pad_top, pad_left), fmap1=f1,
-                                         attention=attention, scratch=scratch)
+        flow_up, flow_small = eng.refine(pyramid, layout, net, inp, coords, self.iters, (orig_h, orig_w), (pad_top, pad_left), fmap1=f1,
+                                         attention=attention, scratch=scratch, fork_flow=self.fork_flow)
         return self.postprocess_predictions(flow_up, resizer, is_flow=True), flow_small  # un-pad is a no-op: written un-padded
 
     # -- CUDA graph of the whole forward (SURVEY.md section 7 step 9, appendix B.9) ------------------------------

@@ -20,7 +20,7 @@ import torch
 import torch.nn as nn
 
 from ... import ops
-from ...engine import SEARaftEngine, _searaft_params
+from ...engine import SEARaftEngine
 from ...utils.registry import register_model, trainable
 from ..raft.extractor import _NATIVE_CONV1, _NATIVE_CONV2, _Encoder, _fold
 from ..raft.raft import RAFT
@@ -174,18 +174,11 @@ class SEARAFT(RAFT):
 
     # -- engine: packs init_conv, the heads and (iters > 0) the update block --------------------
     def _loop_parameters(self):
-        return _searaft_params(self)  # (no update_block at iters = 0)
+        mods = [self.init_conv, self.flow_head, self.upsample_weight] + ([self.update_block] if hasattr(self, "update_block") else [])
+        return [p for m in mods for p in m.parameters()]
 
-    def _get_engine(self, dtype: torch.dtype, device: torch.device) -> SEARaftEngine:
-        eng = self._engine
-        cls = self._engine_cls
-        if (eng is None or eng.dtype != dtype or eng.device != device or eng.impl != self.kernel_impl
-                or eng.corr_levels != self.corr_levels or eng.corr_radius != self.corr_radius or eng.signature != cls.param_signature(self)):
-            eng = cls(self, self._variant, self.hidden_dim, self.context_dim, self.corr_levels, self.corr_radius, dtype, device,
-                      impl=self.kernel_impl)
-            self._engine = eng
-        eng.fork_flow = False
-        return eng
+    def _engine_module(self) -> nn.Module:
+        return self
 
     def _check_grid(self, h8: int, w8: int) -> None:
         """The reference halves fmap2 corr_levels - 1 times and fails once a side reaches zero (e.g. an 8 x 12 grid at 64 x 96)."""
@@ -209,15 +202,15 @@ class SEARAFT(RAFT):
         _, H8, W8, _ = cnet.shape
         eng = self._get_engine(cnet.dtype, cnet.device)
         coords = ops.init_coords(B, H8, W8, cnet.device)
-        pyramid, f1 = [], None
+        pyramid, layout, f1 = [], 0, None
         if self.iters > 0:
             if self.alternate_corr:
                 pyramid, f1 = ops.feature_pyramid(fmap2, self.corr_levels), fmap1
             else:
-                pyramid = eng.build_volume(fmap1, fmap2, impl=self.kernel_impl)
+                pyramid, layout = eng.build_volume(fmap1, fmap2, impl=self.kernel_impl)
         net = torch.empty((B, H8, W8, self.dim), dtype=cnet.dtype, device=cnet.device)
         orig_h, orig_w = images.shape[-2:]
-        flow_up, flow_small = eng.refine(pyramid, net, cnet, coords, self.iters, (orig_h, orig_w), resizer.pad_top_left, fmap1=f1,
+        flow_up, flow_small = eng.refine(pyramid, layout, net, cnet, coords, self.iters, (orig_h, orig_w), resizer.pad_top_left, fmap1=f1,
                                          scratch=scratch)
         return self.postprocess_predictions(flow_up, resizer, is_flow=True), flow_small
 

@@ -10,7 +10,7 @@ from __future__ import annotations
 import contextlib
 import ctypes as C
 import threading
-from typing import List, Optional, Sequence
+from typing import List, NamedTuple, Optional, Sequence
 
 import torch
 
@@ -215,6 +215,13 @@ def corr_lookup_onthefly_tc(fmap1: torch.Tensor, fmap2_pyramid: Sequence[torch.T
 # ------------------------------------------------------------------------------------------
 # conv building block
 # ------------------------------------------------------------------------------------------
+class ConvWeights(NamedTuple):
+    """A weight / bias pair shaped like an nn.Conv2d's, for PackedConv: slices, folds and repacks of a model's parameters."""
+
+    weight: torch.Tensor
+    bias: Optional[torch.Tensor] = None
+
+
 class PackedConv:
     """One (possibly fused) conv layer: packed weight [KH*KW][Cin][Cout_pad] + fp32 bias."""
 

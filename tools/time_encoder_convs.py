@@ -22,7 +22,6 @@ import subprocess
 import sys
 import tempfile
 from argparse import Namespace
-from types import SimpleNamespace
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
@@ -118,7 +117,7 @@ def main():
             if routed:
                 packed, bias = e[cname + "_enc"]
             else:  # a layer the dispatch leaves on cuDNN: packed here from the same storage-rounded weights
-                packed = ops.PackedConv([SimpleNamespace(weight=wb[0].float(), bias=None)], dt, dev, src_channels=[wb[0].shape[1]])
+                packed = ops.PackedConv([ops.ConvWeights(wb[0].float())], dt, dev, src_channels=[wb[0].shape[1]])
                 bias = wb[1]
             cin, cout = packed.Cin, packed.Cout
             x = (torch.randn(nb, hh, ww, cin, device=dev) * 0.5).relu().to(dt)
