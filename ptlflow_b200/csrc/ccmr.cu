@@ -11,12 +11,6 @@
 
 #include "refine.cuh"
 
-#define PFB_TRY(expr)        \
-  do {                       \
-    int rc__ = (expr);       \
-    if (rc__ != PFB_OK) return rc__; \
-  } while (0)
-
 namespace pfb {
 
 constexpr int kXcaC = 128, kXcaHeads = 8, kXcaD = 16;
@@ -215,26 +209,25 @@ CcmrPlan ccmr_plan(const pfb_raft_cfg* c) {
   CcmrPlan w{};
   const size_t N = (size_t)c->H * c->W, P = (size_t)c->B * N, es = dtype_size(c->dtype), row = kXcaC * es;
   w.chunks = (int)ceil_div_sz(N, kXcaChunk);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
-  w.off_feat = take(N * 64 * es);
-  w.off_pos_c = take(N * row);
-  w.off_pos_a = take(N * row);
-  w.off_x0 = take(P * row);
-  w.off_ln = take(P * row);
-  w.off_qk = take(P * 2 * row);
-  w.off_x1 = take(P * row);
-  w.off_t = take(P * row);
-  w.off_u = take(P * row);
-  w.off_gc = take(P * row);
-  w.off_wf = take((size_t)c->B * kXcaC * row);
-  w.off_wfk = take((size_t)c->B * kXcaC * row);
-  w.off_bf = take((size_t)c->B * kXcaC * sizeof(float));
-  w.off_part = take((size_t)c->B * w.chunks * kXcaStats * sizeof(float));
-  w.off_stats = take((size_t)c->B * kXcaStats * sizeof(float));
-  w.off_gn = take(pfb_instance_norm_workspace_bytes(c->B, kXcaC));
-  w.off_up = take(P * 4 * 2 * sizeof(float));  // the padded 2x flow ahead of upflow2
-  w.total = off;
+  Carve k;
+  w.off_feat = k.take(N * 64 * es);
+  w.off_pos_c = k.take(N * row);
+  w.off_pos_a = k.take(N * row);
+  w.off_x0 = k.take(P * row);
+  w.off_ln = k.take(P * row);
+  w.off_qk = k.take(P * 2 * row);
+  w.off_x1 = k.take(P * row);
+  w.off_t = k.take(P * row);
+  w.off_u = k.take(P * row);
+  w.off_gc = k.take(P * row);
+  w.off_wf = k.take((size_t)c->B * kXcaC * row);
+  w.off_wfk = k.take((size_t)c->B * kXcaC * row);
+  w.off_bf = k.take((size_t)c->B * kXcaC * sizeof(float));
+  w.off_part = k.take((size_t)c->B * w.chunks * kXcaStats * sizeof(float));
+  w.off_stats = k.take((size_t)c->B * kXcaStats * sizeof(float));
+  w.off_gn = k.take(pfb_instance_norm_workspace_bytes(c->B, kXcaC));
+  w.off_up = k.take(P * 4 * 2 * sizeof(float));  // the padded 2x flow ahead of upflow2
+  w.total = k.total;
   return w;
 }
 
@@ -246,20 +239,12 @@ struct Xs {  // one scale's buffers
   void* at(size_t off) const { return base + off; }
 };
 
-static int conv1x1s(const Xs& x, const pfb_layer& L, int B, int H, int W, const void* src, int src_stride, int src_offset, int epi, void* out,
-                    int out_stride, int out_offset, const void* aux = nullptr, int aux_stride = 0) {
-  pfb_conv_params p{};
-  PFB_CHECK_ARG(L.weight && L.KH == 1 && L.KW == 1, "ccmr: missing 1x1 layer");
-  p.src[0].ptr = src; p.src[0].channels = L.Cin; p.src[0].stride = src_stride; p.src[0].offset = src_offset; p.src[0].is_f32 = 0;
-  p.nsrc = 1;
-  p.B = B; p.H = H; p.W = W; p.KH = 1; p.KW = 1;
-  p.Cout = L.Cout; p.Cout_pad = L.Cout_pad; p.weight = L.weight; p.bias = L.bias;
-  p.epilogue = epi; p.scale = 1.f;
-  p.out = out; p.out_stride = out_stride; p.out_offset = out_offset;
-  p.aux_h = aux; p.hidden = aux_stride;
-  p.dtype = x.c->dtype; p.impl = x.c->impl;
-  p.weight_k = L.weight_k; p.Cin_pad = L.Cin_pad; p.Cout_pad_k = L.Cout_pad_k;
-  return pfb_conv2d(&p, (pfb_stream)x.s);
+static int conv1x1s(const Xs& x, const pfb_layer& L, int B, const void* src, int src_stride, int epi, void* out, int out_stride,
+                    int out_offset, const void* aux = nullptr, int aux_stride = 0) {
+  PFB_CHECK_ARG(L.KH == 1 && L.KW == 1, "ccmr: missing 1x1 layer");
+  ConvExtras e;
+  e.aux_h = aux; e.hidden = aux_stride; e.B = B;
+  return launch_conv(x.c, x.s, L, {src_of(src, L.Cin, src_stride)}, {epi, out, out_stride, out_offset}, e);
 }
 
 // x0 (the block's residual stream, [P][128]) -> ln = LN1(x0) without affine, the folded attention (wf, wfk, bf) and, in place,
@@ -276,7 +261,7 @@ static int xcit_prepare(const Xs& x, const pfb_xcit_block& w) {
   PFB_CHECK_ARG(w.qk.Cin == kXcaC && w.qk.Cout == 2 * kXcaC, "ccmr: the q | k layer must be 128 -> 256");
   PFB_CHECK_ARG(w.v_weight && w.v_bias && w.proj_weight && w.proj_bias && w.temperature, "ccmr: null XCA weights");
   PFB_TRY(pfb_layernorm(x0, kXcaC, 0, ln, kXcaC, 0, nullptr, nullptr, P, kXcaC, w.ln_eps, c->dtype, (pfb_stream)x.s));
-  PFB_TRY(conv1x1s(x, w.qk, c->B, c->H, c->W, ln, kXcaC, 0, PFB_EPI_LINEAR, qk, 2 * kXcaC, 0));
+  PFB_TRY(conv1x1s(x, w.qk, c->B, ln, kXcaC, PFB_EPI_LINEAR, qk, 2 * kXcaC, 0));
   PFB_TRY(pfb_xca_stats(qk, 2 * kXcaC, 0, kXcaC, c->B, N, stats, x.at(x.pl.off_part), c->dtype, (pfb_stream)x.s));
   const bool kmajor = c->dtype != PFB_F32;
   PFB_TRY(pfb_xca_fold(stats, w.temperature, w.v_weight, w.v_bias, w.proj_weight, w.proj_bias, x.at(x.pl.off_wf),
@@ -296,32 +281,20 @@ static int xcit_apply(const Xs& x, const pfb_xcit_block& w, const void* v_ln, vo
   void* u = x.at(x.pl.off_u);
   // x1 = x0 + gamma1 * proj(A v): per-sample folded weights, the residual (with the folded bias) in the AXPY epilogue
   const char* wf = reinterpret_cast<const char*>(x.at(x.pl.off_wf));
+  ConvExtras e;
+  e.hidden = kXcaC;
   if (c->dtype != PFB_F32 && c->impl != 1) {
-    pfb_conv_params p{};
-    p.src[0].ptr = v_ln; p.src[0].channels = kXcaC; p.src[0].stride = kXcaC;
-    p.nsrc = 1;
-    p.B = c->B; p.H = c->H; p.W = c->W; p.KH = 1; p.KW = 1;
-    p.Cout = kXcaC; p.Cout_pad = kXcaC; p.weight = wf; p.bias = nullptr;
-    p.epilogue = PFB_EPI_AXPY; p.scale = 1.f;
-    p.out = x1; p.out_stride = kXcaC; p.out_offset = 0;
-    p.aux_h = add; p.hidden = kXcaC;
-    p.dtype = c->dtype; p.impl = 2;
-    p.weight_k = x.at(x.pl.off_wfk); p.Cin_pad = kXcaC; p.Cout_pad_k = kXcaC;
-    p.w_rows_per_sample = kXcaC;
-    PFB_TRY(pfb_conv2d(&p, st));
+    const pfb_layer fold{wf, nullptr, kXcaC, kXcaC, kXcaC, 1, 1, x.at(x.pl.off_wfk), kXcaC, kXcaC};
+    e.aux_h = add; e.impl = 2; e.w_rows_per_sample = kXcaC;
+    PFB_TRY(launch_conv(c, x.s, fold, {src_of(v_ln, kXcaC, kXcaC)}, {PFB_EPI_AXPY, x1, kXcaC, 0}, e));
   } else {
+    e.B = 1; e.impl = 1;
     for (int b = 0; b < c->B; ++b) {  // SIMT: one launch per sample with that sample's weights
       const size_t po = (size_t)b * N * kXcaC * es;
-      pfb_conv_params p{};
-      p.src[0].ptr = reinterpret_cast<const char*>(v_ln) + po; p.src[0].channels = kXcaC; p.src[0].stride = kXcaC;
-      p.nsrc = 1;
-      p.B = 1; p.H = c->H; p.W = c->W; p.KH = 1; p.KW = 1;
-      p.Cout = kXcaC; p.Cout_pad = kXcaC; p.weight = wf + (size_t)b * kXcaC * kXcaC * es; p.bias = nullptr;
-      p.epilogue = PFB_EPI_AXPY; p.scale = 1.f;
-      p.out = reinterpret_cast<char*>(x1) + po; p.out_stride = kXcaC; p.out_offset = 0;
-      p.aux_h = reinterpret_cast<char*>(add) + po; p.hidden = kXcaC;
-      p.dtype = c->dtype; p.impl = 1;
-      PFB_TRY(pfb_conv2d(&p, st));
+      const pfb_layer fold{wf + (size_t)b * kXcaC * kXcaC * es, nullptr, kXcaC, kXcaC, kXcaC, 1, 1, nullptr, 0, 0};
+      e.aux_h = reinterpret_cast<char*>(add) + po;
+      PFB_TRY(launch_conv(c, x.s, fold, {src_of(reinterpret_cast<const char*>(v_ln) + po, kXcaC, kXcaC)},
+                          {PFB_EPI_AXPY, reinterpret_cast<char*>(x1) + po, kXcaC, 0}, e));
     }
   }
   // x2 = x1 + gamma3 * LPI(LN3(x1)): LN3's affine and the group norm's are applied, not folded (the convolutions are zero padded)
@@ -332,13 +305,13 @@ static int xcit_apply(const Xs& x, const pfb_xcit_block& w, const void* v_ln, vo
   PFB_TRY(pfb_depthwise_conv3x3_ex(u, kXcaC, 0, t, kXcaC, 0, w.dw2_weight, w.dw2_bias, x1, kXcaC, 0, c->B, c->H, c->W, kXcaC, 1, c->dtype, st));
   // out = x2 + gamma2 * fc2(gelu(fc1(LN2(x2))))
   PFB_TRY(pfb_layernorm(t, kXcaC, 0, u, kXcaC, 0, nullptr, nullptr, P, kXcaC, w.ln_eps, c->dtype, st));
-  PFB_TRY(conv1x1s(x, w.fc1, c->B, c->H, c->W, u, kXcaC, 0, PFB_EPI_GELU, x1, kXcaC, 0));
-  return conv1x1s(x, w.fc2, c->B, c->H, c->W, x1, kXcaC, 0, PFB_EPI_AXPY, out, out_stride, out_offset, t, kXcaC);
+  PFB_TRY(conv1x1s(x, w.fc1, c->B, u, kXcaC, PFB_EPI_GELU, x1, kXcaC, 0));
+  return conv1x1s(x, w.fc2, c->B, x1, kXcaC, PFB_EPI_AXPY, out, out_stride, out_offset, t, kXcaC);
 }
 
 static int positional(const Xs& x, const pfb_xcit_block& w, size_t off) {
   PFB_CHECK_ARG(w.pos_proj.Cin == 64 && w.pos_proj.Cout == kXcaC, "ccmr: pos_embeder.token_projection must be 64 -> 128");
-  return conv1x1s(x, w.pos_proj, 1, x.c->H, x.c->W, x.at(x.pl.off_feat), 64, 0, PFB_EPI_LINEAR, x.at(off), kXcaC, 0);
+  return conv1x1s(x, w.pos_proj, 1, x.at(x.pl.off_feat), 64, PFB_EPI_LINEAR, x.at(off), kXcaC, 0);
 }
 
 int ccmr_scale_setup(const pfb_raft_cfg* c, const pfb_ccmr_weights* w, const void* inp, void* gc_out, bool aggregator, char* base,

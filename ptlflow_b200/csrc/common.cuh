@@ -31,6 +31,13 @@ void set_error(const char* fmt, ...);
 
 #define PFB_LAUNCH_CHECK() PFB_CUDA(cudaPeekAtLastError())
 
+// return the status of a library call unless it is PFB_OK
+#define PFB_TRY(expr)                  \
+  do {                                 \
+    int rc__ = (expr);                 \
+    if (rc__ != PFB_OK) return rc__;   \
+  } while (0)
+
 inline size_t dtype_size(pfb_dtype dt) { return dt == PFB_F32 ? 4 : 2; }
 inline bool dtype_ok(int dt) { return dt == PFB_F32 || dt == PFB_F16 || dt == PFB_BF16; }
 inline cudaStream_t as_stream(pfb_stream s) { return reinterpret_cast<cudaStream_t>(s); }

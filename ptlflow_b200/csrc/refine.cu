@@ -4,19 +4,218 @@
 // but every stage is one launch of this library's kernels on the caller's stream (so the whole
 // loop can be captured in a CUDA graph by the host), no torch.cat / permute copies exist, and
 // the mask head + upsample run once (eval returns only the last prediction, raft.py:192).
-#include <initializer_list>
-
 #include <stdlib.h>
 
 #include "refine.cuh"
 
-#define PFB_TRY(expr)        \
-  do {                       \
-    int rc__ = (expr);       \
-    if (rc__ != PFB_OK) return rc__; \
-  } while (0)
-
 namespace pfb {
+
+// ---- shared by every loop (refine.cuh) ----
+
+int launch_conv(const pfb_raft_cfg* c, cudaStream_t s, const pfb_layer& L, std::initializer_list<pfb_conv_src> srcs, const ConvOut& o,
+                const ConvExtras& e) {
+  pfb_conv_params p{};
+  int cin = 0;
+  for (const auto& src : srcs) { p.src[p.nsrc++] = src; cin += src.channels; }
+  PFB_CHECK_ARG(L.weight, "conv: a %dx%d %d -> %d layer has no packed weight", L.KH, L.KW, L.Cin, L.Cout);
+  // the lookup buffer may be wider than the layer's real Cin (zero pad columns <-> zero weight rows)
+  PFB_CHECK_ARG(cin == L.Cin, "conv: a %dx%d %d -> %d layer expects Cin=%d, sources provide %d", L.KH, L.KW, L.Cin, L.Cout, L.Cin, cin);
+  p.B = e.B > 0 ? e.B : c->B; p.H = c->H; p.W = c->W;
+  p.KH = L.KH; p.KW = L.KW; p.Cout = L.Cout; p.Cout_pad = L.Cout_pad;
+  p.weight = L.weight; p.bias = L.bias;
+  p.weight_k = L.weight_k; p.Cin_pad = L.Cin_pad; p.Cout_pad_k = L.Cout_pad_k;
+  p.epilogue = o.epi; p.scale = o.scale;
+  p.out = o.ptr; p.out_stride = o.stride; p.out_offset = o.offset;
+  p.aux_h = e.aux_h; p.aux_z = e.aux_z; p.hidden = e.hidden;
+  p.coords = e.coords; p.flow = e.flow;
+  p.addend = e.addend; p.addend_stride = e.addend_stride;
+  if (e.residual) { p.residual = e.residual->ptr; p.residual_stride = e.residual->stride; p.residual_offset = e.residual->offset; }
+  p.post_w = e.post_w; p.post_b = e.post_b;
+  p.w_rows_per_sample = e.w_rows_per_sample;
+  p.dtype = c->dtype; p.impl = e.impl >= 0 ? e.impl : c->impl;
+  return pfb_conv2d(&p, (pfb_stream)s);
+}
+
+int check_loop_cfg(const pfb_raft_cfg* c, const char* name, bool levels_fit_grid) {
+  PFB_CHECK_ARG(c, "%s: null cfg", name);
+  PFB_CHECK_ARG(dtype_ok(c->dtype), "%s: bad dtype %d", name, (int)c->dtype);
+  PFB_CHECK_ARG(c->B > 0 && c->H > 0 && c->W > 0, "%s: bad grid %dx%dx%d", name, c->B, c->H, c->W);
+  PFB_CHECK_ARG(c->corr_levels >= 1 && c->corr_levels <= PFB_MAX_LEVELS && c->corr_radius >= 0 && c->corr_radius <= 15,
+                "%s: corr_levels=%d corr_radius=%d", name, c->corr_levels, c->corr_radius);
+  if (levels_fit_grid)
+    PFB_CHECK_ARG((c->H >> (c->corr_levels - 1)) >= 1 && (c->W >> (c->corr_levels - 1)) >= 1, "%s: %dx%d grid too small for %d levels",
+                  name, c->H, c->W, c->corr_levels);
+  PFB_CHECK_ARG(c->iters >= 0, "%s: iters=%d", name, c->iters);
+  PFB_CHECK_ARG(c->volume_layout == 0 || (c->volume_layout == 1 && c->dtype != PFB_F32 && !c->alternate_corr && c->corr_levels <= 4),
+                "%s: volume_layout=%d needs f16/bf16, a materialised pyramid and <= 4 levels", name, c->volume_layout);
+  return PFB_OK;
+}
+
+int check_loop_buffers(const pfb_raft_cfg* c, const pfb_raft_buffers* buf, bool need_pyramid, size_t need, const char* name) {
+  PFB_CHECK_ARG(buf, "%s: null buffers", name);
+  PFB_CHECK_ARG(buf->net && buf->inp && buf->coords && buf->workspace, "%s: null state buffer", name);
+  if (need_pyramid) {
+    PFB_CHECK_ARG(buf->pyramid, "%s: null pyramid", name);
+    PFB_CHECK_ARG(!c->alternate_corr || (buf->fmap1 && c->feat_dim > 0), "%s: alternate_corr needs fmap1 and feat_dim", name);
+  }
+  PFB_CHECK_ARG(buf->workspace_bytes >= need, "%s: workspace %zu bytes < required %zu", name, buf->workspace_bytes, need);
+  return PFB_OK;
+}
+
+int copy_wide_state(const pfb_raft_cfg* c, const pfb_raft_buffers* buf, void* X, int x_stride, bool to_wide, cudaStream_t s) {
+  const size_t es = dtype_size(c->dtype), P = (size_t)c->B * c->H * c->W, row = 128 * es, pitch = x_stride * es;
+  char* x = reinterpret_cast<char*>(X);
+  if (!to_wide) {
+    PFB_CUDA(cudaMemcpy2DAsync(buf->net, row, x, pitch, row, P, cudaMemcpyDeviceToDevice, s));
+    return PFB_OK;
+  }
+  PFB_CUDA(cudaMemcpy2DAsync(x, pitch, buf->net, row, row, P, cudaMemcpyDeviceToDevice, s));
+  PFB_CUDA(cudaMemcpy2DAsync(x + row, pitch, buf->inp, row, row, P, cudaMemcpyDeviceToDevice, s));
+  return PFB_OK;
+}
+
+int raft_lookup(const pfb_raft_cfg* c, void* const* pyramid, const void* fmap1, const float* coords, void* out, int out_stride,
+                void* flags, cudaStream_t s, float scale) {
+  if (c->alternate_corr) {
+    static const int env_tc = getenv("PFB_ONTHEFLY_TC") ? atoi(getenv("PFB_ONTHEFLY_TC")) : 1;
+    if (env_tc && c->impl != 1 && corr_onthefly_umma_supported(c->B, c->H, c->W, c->feat_dim, c->corr_levels, c->corr_radius, c->dtype, out_stride))
+      return pfb_corr_lookup_onthefly_tc_ex(fmap1, pyramid, coords, out, flags, c->B, c->H, c->W,
+                                            c->feat_dim, c->corr_levels, c->corr_radius, scale, c->dtype, out_stride, (pfb_stream)s);
+  }
+  if (c->alternate_corr)
+    return pfb_corr_lookup_onthefly_ex(fmap1, pyramid, coords, out, c->B, c->H, c->W,
+                                       c->feat_dim, c->corr_levels, c->corr_radius, scale, c->dtype, c->dtype, 0,
+                                       out_stride, (pfb_stream)s);
+  if (c->volume_layout == 1)
+    return pfb_corr_lookup_tiled(pyramid, coords, out, c->B, c->H, c->W, c->H, c->W, c->corr_levels,
+                                 c->corr_radius, c->dtype, out_stride, (pfb_stream)s);
+  return pfb_corr_lookup(pyramid, coords, out, c->B, c->H, c->W, c->corr_levels,
+                         c->corr_radius, c->dtype, c->dtype, 0, out_stride, (pfb_stream)s);
+}
+
+int motion_encoder(const pfb_raft_cfg* c, cudaStream_t s, const ConvExtras& e, const MotionLayers& L, const MotionBuffers& m,
+                   const pfb_conv_src& corr, const ConvOut& out, cudaStream_t side, cudaEvent_t ev_join, const pfb_layer* c2f2) {
+  const int c_corflo = m.c_cor2 + m.c_flo2;
+  const cudaStream_t sf = side ? side : s;  // the flow branch's launches
+  if (L.convc2) {
+    PFB_TRY(launch_conv(c, s, *L.convc1, {corr}, {PFB_EPI_RELU, m.cor1, m.c_cor1, 0}, e));
+    if (!c2f2) PFB_TRY(launch_conv(c, s, *L.convc2, {src_of(m.cor1, m.c_cor1, m.c_cor1)}, {PFB_EPI_RELU, m.corflo, c_corflo, 0}, e));
+  } else {
+    PFB_TRY(launch_conv(c, s, *L.convc1, {corr}, {PFB_EPI_RELU, m.corflo, c_corflo, 0}, e));
+  }
+  const pfb_layer& LF = *L.convf1;
+  static const int env_fc = getenv("PFB_FLOW_CONV_UMMA") ? atoi(getenv("PFB_FLOW_CONV_UMMA")) : 1;
+  if (env_fc && LF.weight_k && LF.KH == 7 && LF.KW == 7 && LF.Cin == 2 && LF.Cout == 128 && c->dtype != PFB_F32 && c->impl != 1)
+    PFB_TRY(pfb_flow_conv7x7(e.flow, LF.weight_k, LF.bias, m.flo1, m.c_flo1, 0, c->B, c->H, c->W, c->dtype, (pfb_stream)sf));
+  else
+    PFB_TRY(launch_conv(c, sf, LF, {src_of(e.flow, 2, 2, 0, 1)}, {PFB_EPI_RELU, m.flo1, m.c_flo1, 0}, e));
+  if (c2f2)  // [cor1 | flo1] -> [cor | flo]
+    PFB_TRY(launch_conv(c, s, *c2f2, {src_of(m.cor1, m.c_cor1, m.c_cor1), src_of(m.flo1, m.c_flo1, m.c_flo1)},
+                        {PFB_EPI_RELU, m.corflo, c_corflo, 0}, e));
+  else
+    PFB_TRY(launch_conv(c, sf, *L.convf2, {src_of(m.flo1, m.c_flo1, m.c_flo1)}, {PFB_EPI_RELU, m.corflo, c_corflo, m.c_cor2}, e));
+  if (side) {  // join: `conv` reads both branches
+    PFB_CUDA(cudaEventRecord(ev_join, side));
+    PFB_CUDA(cudaStreamWaitEvent(s, ev_join, 0));
+  }
+  return launch_conv(c, s, *L.conv, {src_of(m.corflo, c_corflo, c_corflo)}, out, e);
+}
+
+int flow_head(const pfb_raft_cfg* c, cudaStream_t s, const ConvExtras& e, const pfb_layer& flow1, const pfb_layer& flow2,
+              const pfb_layer* flow2t, const pfb_conv_src& net, void* fh, int c_fh, float* taps, float* flow) {
+  PFB_TRY(launch_conv(c, s, flow1, {net}, {PFB_EPI_RELU, fh, c_fh, 0}, e));
+  if (flow2t && flow2t->weight_k && c->dtype != PFB_F32 && c->impl != 1) {
+    PFB_TRY(launch_conv(c, s, *flow2t, {src_of(fh, c_fh, c_fh)}, {PFB_EPI_LINEAR_F32, taps, 32, 0}, e));
+    return pfb_flow_tap_gather(taps, 32, flow2.bias, e.coords, flow, c->B, c->H, c->W, (pfb_stream)s);
+  }
+  return launch_conv(c, s, flow2, {src_of(fh, c_fh, c_fh)}, {PFB_EPI_FLOW, flow, 2, 0}, e);
+}
+
+int mask_head(const pfb_raft_cfg* c, cudaStream_t s, const ConvExtras& e, const pfb_layer& mask1, const pfb_layer& mask2,
+              const pfb_conv_src& net, void* mh, void* mask, int channels) {
+  PFB_TRY(launch_conv(c, s, mask1, {net}, {PFB_EPI_RELU, mh, 256, 0}, e));
+  return launch_conv(c, s, mask2, {src_of(mh, 256, 256)}, {PFB_EPI_LINEAR, mask, channels, 0, 0.25f}, e);
+}
+
+static int heads_of(const pfb_raft_cfg* c) { return c->num_heads > 0 ? c->num_heads : 1; }
+
+int gma_aggregate(const pfb_raft_cfg* c, const pfb_layer& agg_v, const pfb_layer& agg_proj, const void* attention_ptr, float gamma,
+                  void* motion, int motion_stride, int motion_offset, int out_offset, void* vbuf_ptr, void* vT_ptr, void* agg_ptr, int n_pad,
+                  cudaStream_t s) {
+  PFB_CHECK_ARG(attention_ptr, "gma: null attention");
+  const int N = c->H * c->W, heads = heads_of(c), vdim = heads * 128;
+  const size_t es = dtype_size(c->dtype);
+  const char* attention = reinterpret_cast<const char*>(attention_ptr);
+  char* vbuf = reinterpret_cast<char*>(vbuf_ptr);
+  char* vT = reinterpret_cast<char*>(vT_ptr);
+  // one head: attn @ v goes straight into the AXPY epilogue.  Several heads (gma_utils.py:101-111): every head's attn @ v
+  // lands in its 128 columns of `agg`, then project (heads*128 -> 128) carries the AXPY epilogue.
+  char* agg = heads > 1 ? reinterpret_cast<char*>(agg_ptr) : nullptr;
+  PFB_CHECK_ARG(heads == 1 || (agg_proj.weight && agg_proj.Cin == vdim),
+                "gma: num_heads=%d needs the Aggregate.project layer (%d -> 128)", heads, vdim);
+  PFB_CHECK_ARG(agg_v.weight && agg_v.Cin == 128, "gma: Aggregate.to_v layer missing");
+  {  // v = to_v(motion)
+    ConvExtras e;
+    e.hidden = c->hidden_dim;
+    PFB_TRY(launch_conv(c, s, agg_v, {src_of(motion, 128, motion_stride, motion_offset)}, {PFB_EPI_LINEAR, vbuf, vdim, 0}, e));
+  }
+  const bool tensor_path = c->dtype != PFB_F32 && c->impl != 1 && (N % 8) == 0;
+  if (tensor_path) PFB_TRY(pfb_transpose_pm(vbuf, vT, c->B, N, vdim, n_pad, c->dtype, (pfb_stream)s));
+  static const int env_batched = getenv("PFB_GMA_BATCHED") ? atoi(getenv("PFB_GMA_BATCHED")) : 1;
+  // "1x1 convolution" of head h over sample b (b < 0: all samples in one launch): pixels = queries, input channels = the N
+  // attention columns, weights = the sample's v (SIMT layout [N][vdim], columns h*128...) / v^T (K-major [vdim][n_pad], rows
+  // h*128...).  The attention is head-major, so every operand is affine in the pixel index.
+  auto attn_v = [&](int h, int b) -> int {
+    const int b0 = b < 0 ? 0 : b;
+    const pfb_layer v{vbuf + ((size_t)b0 * N * vdim + (size_t)h * 128) * es, nullptr, 128, vdim, N, 1, 1,
+                      tensor_path ? vT + ((size_t)b0 * vdim + (size_t)h * 128) * n_pad * es : nullptr, tensor_path ? n_pad : 0,
+                      tensor_path ? 128 : 0};
+    ConvExtras e;
+    e.B = b < 0 ? 0 : 1;
+    if (b < 0) {
+      // ONE launch for all samples: per-sample weights = that sample's v^T (rows b * vdim + h * 128 ...).  B x 55 row tiles
+      // fill the machine; one launch per sample left only 55 row tiles, a fraction of the machine.
+      e.impl = 2;
+      e.w_rows_per_sample = vdim;
+    }
+    const pfb_conv_src a = src_of(attention + ((size_t)h * c->B + b0) * N * N * es, N, N);
+    if (heads > 1) return launch_conv(c, s, v, {a}, {PFB_EPI_LINEAR, agg + (size_t)b0 * N * vdim * es, vdim, h * 128}, e);
+    char* mrow = reinterpret_cast<char*>(motion) + (size_t)b0 * N * motion_stride * es;
+    e.aux_h = mrow + (size_t)motion_offset * es;
+    e.hidden = motion_stride;
+    return launch_conv(c, s, v, {a}, {PFB_EPI_AXPY, mrow, motion_stride, out_offset, gamma}, e);
+  };
+  for (int h = 0; h < heads; ++h) {
+    if (tensor_path && env_batched) PFB_TRY(attn_v(h, -1));
+    else for (int b = 0; b < c->B; ++b) PFB_TRY(attn_v(h, b));
+  }
+  if (heads > 1) {  // motion_global = motion + gamma * project(out)   gma_utils.py:108-111
+    pfb_layer proj = agg_proj;
+    proj.bias = nullptr;  // Aggregate.project has no bias
+    ConvExtras e;
+    e.aux_h = reinterpret_cast<char*>(motion) + (size_t)motion_offset * es;
+    e.hidden = motion_stride;
+    PFB_TRY(launch_conv(c, s, proj, {src_of(agg, vdim, vdim)}, {PFB_EPI_AXPY, motion, motion_stride, out_offset, gamma}, e));
+  }
+  return PFB_OK;
+}
+
+int check_multiscale_args(const pfb_raft_cfg* c, const pfb_raft_buffers* buf, float corr_scale, const float* next_coords, int upflow2,
+                          const char* name) {
+  PFB_CHECK_ARG(c->iters >= 1, "%s: every scale needs at least one iteration (iters=%d)", name, c->iters);
+  PFB_CHECK_ARG(corr_scale >= 0.f, "%s: corr_scale=%g", name, (double)corr_scale);
+  PFB_CHECK_ARG(next_coords || buf->flow_up, "%s: needs next_coords (coarser scales) or flow_up (the finest)", name);
+  if (next_coords) return PFB_OK;
+  const int f = 2 << upflow2;  // the output grid is f times this scale's
+  PFB_CHECK_ARG(c->out_h > 0 && c->out_w > 0 && c->pad_top >= 0 && c->pad_left >= 0 && c->out_h + c->pad_top <= f * c->H &&
+                    c->out_w + c->pad_left <= f * c->W,
+                "%s: output window %dx%d+(%d,%d) outside %dx%d", name, c->out_h, c->out_w, c->pad_top, c->pad_left, f * c->H, f * c->W);
+  PFB_CHECK_ARG(!buf->flow_small || (c->out_h >= 16 && c->out_w >= 16), "%s: output %dx%d smaller than 16 px per side", name, c->out_h,
+                c->out_w);
+  return PFB_OK;
+}
+
+// ---- the raft / raft_small / gma / ms_raft_plus / ccmr loop ----
 
 struct Workspace {
   // element strides (channels per pixel) and byte offsets inside the caller's workspace
@@ -32,7 +231,6 @@ struct Workspace {
   int c_cor1, c_corflo, c_cor2, c_flo1, c_flo2, c_motion, c_fh;
 };
 
-static int heads_of(const pfb_raft_cfg* c) { return c->num_heads > 0 ? c->num_heads : 1; }
 // channels of the convex-upsample mask: 9 taps x 8 x 8 (raft, gma), 9 taps x 2 x 2 (ms_raft_plus, variant 5; ccmr, variant 6)
 static int mask_channels(const pfb_raft_cfg* c) { return c->variant == 5 || c->variant == 6 ? 36 : 576; }
 
@@ -53,49 +251,40 @@ static Workspace plan(const pfb_raft_cfg* c) {
     w.c_cor1 = 0; w.c_cor2 = 96; w.c_flo1 = 64; w.c_flo2 = 32; w.c_motion = 82; w.c_fh = 128;
   }
   w.c_corflo = w.c_cor2 + w.c_flo2;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
-  w.off_corr = take(P * w.corr_stride * es);
-  w.off_cor1 = take(P * (size_t)w.c_cor1 * es);
-  w.off_corflo = take(P * (size_t)w.c_corflo * es);
-  w.off_flo1 = take(P * (size_t)w.c_flo1 * es);
-  w.off_motion = take(P * (size_t)w.c_motion * es);
-  w.off_z = take(P * (size_t)c->hidden_dim * es);
-  w.off_rh = take(P * (size_t)c->hidden_dim * es);
-  w.off_fh = take(P * (size_t)w.c_fh * es);
-  w.off_mh = take(c->variant != 1 ? P * 256 * es : 0);
-  w.off_mask = take(c->variant != 1 ? P * (size_t)mask_channels(c) * es : 0);
-  w.off_flow = take(P * 2 * sizeof(float));
-  w.off_taps = take(c->variant != 1 ? P * 32 * sizeof(float) : 0);
+  Carve k;
+  w.off_corr = k.take(P * w.corr_stride * es);
+  w.off_cor1 = k.take(P * (size_t)w.c_cor1 * es);
+  w.off_corflo = k.take(P * (size_t)w.c_corflo * es);
+  w.off_flo1 = k.take(P * (size_t)w.c_flo1 * es);
+  w.off_motion = k.take(P * (size_t)w.c_motion * es);
+  w.off_z = k.take(P * (size_t)c->hidden_dim * es);
+  w.off_rh = k.take(P * (size_t)c->hidden_dim * es);
+  w.off_fh = k.take(P * (size_t)w.c_fh * es);
+  w.off_mh = k.take(c->variant != 1 ? P * 256 * es : 0);
+  w.off_mask = k.take(c->variant != 1 ? P * (size_t)mask_channels(c) * es : 0);
+  w.off_flow = k.take(P * 2 * sizeof(float));
+  w.off_taps = k.take(c->variant != 1 ? P * 32 * sizeof(float) : 0);
   w.n_pad = (int)align_up((size_t)c->H * c->W, 64);
-  w.off_vbuf = take(c->variant == 2 ? P * vdim * es : 0);
-  w.off_vT = take(c->variant == 2 ? (size_t)c->B * vdim * w.n_pad * es : 0);
-  w.off_agg = take(c->variant == 2 && vdim > 128 ? P * vdim * es : 0);
-  w.off_flags = take(c->alternate_corr ? P : 0);
+  w.off_vbuf = k.take(c->variant == 2 ? P * vdim * es : 0);
+  w.off_vT = k.take(c->variant == 2 ? (size_t)c->B * vdim * w.n_pad * es : 0);
+  w.off_agg = k.take(c->variant == 2 && vdim > 128 ? P * vdim * es : 0);
+  w.off_flags = k.take(c->alternate_corr ? P : 0);
   for (int i = 0; i < 4; ++i)
-    w.off_ctx[i] = take((c->variant != 1 && c->dtype != PFB_F32) ? P * (size_t)((i & 1) ? c->hidden_dim : 2 * c->hidden_dim) * es : 0);
-  w.total = off;
+    w.off_ctx[i] = k.take((c->variant != 1 && c->dtype != PFB_F32) ? P * (size_t)((i & 1) ? c->hidden_dim : 2 * c->hidden_dim) * es : 0);
+  w.total = k.total;
   return w;
 }
 
 // variant 5 (ms_raft_plus) only through the pfb_msraft_* entry points, 6 (ccmr) only through the pfb_ccmr_* ones, 0..2 only through
 // the pfb_raft_* ones
 static int check_cfg(const pfb_raft_cfg* c, bool msraft = false, bool ccmr = false) {
-  PFB_CHECK_ARG(c, "raft: null cfg");
+  const char* name = ccmr ? "ccmr" : msraft ? "msraft" : "raft";
+  PFB_TRY(check_loop_cfg(c, name));
   if (ccmr) PFB_CHECK_ARG(c->variant == 6, "ccmr: variant=%d (the ccmr loop is variant 6)", c->variant);
   else if (msraft) PFB_CHECK_ARG(c->variant == 5, "msraft: variant=%d (the ms_raft_plus loop is variant 5)", c->variant);
   else PFB_CHECK_ARG(c->variant >= 0 && c->variant <= 2, "raft: variant=%d", c->variant);
-  PFB_CHECK_ARG(dtype_ok(c->dtype), "raft: bad dtype");
-  PFB_CHECK_ARG(c->B > 0 && c->H > 0 && c->W > 0, "raft: bad grid %dx%dx%d", c->B, c->H, c->W);
-  PFB_CHECK_ARG(c->corr_levels >= 1 && c->corr_levels <= PFB_MAX_LEVELS && c->corr_radius >= 0 && c->corr_radius <= 15,
-                "raft: corr_levels=%d corr_radius=%d", c->corr_levels, c->corr_radius);
-  PFB_CHECK_ARG((c->H >> (c->corr_levels - 1)) >= 1 && (c->W >> (c->corr_levels - 1)) >= 1,
-                "raft: %dx%d grid too small for %d levels", c->H, c->W, c->corr_levels);
-  PFB_CHECK_ARG(c->hidden_dim > 0 && c->context_dim > 0 && c->iters >= 0, "raft: bad dims");
-  PFB_CHECK_ARG(c->num_heads >= 0 && c->num_heads <= 64 && (c->variant == 2 || heads_of(c) == 1), "raft: num_heads=%d", c->num_heads);
-  PFB_CHECK_ARG(c->volume_layout == 0 || (c->volume_layout == 1 && c->dtype != PFB_F32 && !c->alternate_corr && c->corr_levels <= 4),
-                "raft: volume_layout=%d needs f16/bf16, a materialised pyramid and <= 4 levels", c->volume_layout);
-  if (c->variant != 1) PFB_CHECK_ARG(c->hidden_dim == 128 && c->context_dim == 128, "raft/gma: the update block expects hidden=context=128");
+  PFB_CHECK_ARG(c->num_heads >= 0 && c->num_heads <= 64 && (c->variant == 2 || heads_of(c) == 1), "%s: num_heads=%d", name, c->num_heads);
+  if (c->variant != 1) PFB_CHECK_ARG(c->hidden_dim == 128 && c->context_dim == 128, "%s: the update block expects hidden=context=128", name);
   else PFB_CHECK_ARG(c->hidden_dim == 96 && c->context_dim == 64, "raft_small: SmallUpdateBlock expects hidden=96 context=64");
   return PFB_OK;
 }
@@ -107,6 +296,7 @@ struct Ctx {
   Workspace ws;
   char* base;
   cudaStream_t s;
+  ConvExtras e;            // every layer's GRU operands, coordinates and flow
   float corr_scale = 0.f;  // on-the-fly lookup scale (0: 1/sqrt(feat_dim))
   const pfb_ccmr_weights* ccmr = nullptr;  // variant 6: the XCiT blocks of the scale, and their part of the workspace
   char* ccmr_base = nullptr;
@@ -116,33 +306,11 @@ struct Ctx {
   void* at(size_t off) const { return base + off; }
 };
 
-static pfb_conv_src src_of(const void* ptr, int channels, int stride, int offset = 0, int is_f32 = 0) {
-  pfb_conv_src s;
-  s.ptr = ptr; s.channels = channels; s.stride = stride; s.offset = offset; s.is_f32 = is_f32;
-  return s;
-}
-
-static int run_conv(const Ctx& x, int layer, std::initializer_list<pfb_conv_src> srcs, int epi, void* out,
-                    int out_stride, int out_offset, float scale = 1.f, const void* addend = nullptr, int addend_stride = 0) {
-  const pfb_layer& L = x.w->layers[layer];
-  PFB_CHECK_ARG(L.weight, "raft: layer %d has no packed weight", layer);
-  pfb_conv_params p{};
-  int i = 0, cin = 0;
-  for (const auto& s : srcs) { p.src[i++] = s; cin += s.channels; }
-  p.nsrc = i;
-  // the lookup buffer may be wider than the layer's real Cin (zero pad columns <-> zero weight rows)
-  PFB_CHECK_ARG(cin == L.Cin, "raft: layer %d expects Cin=%d, sources provide %d", layer, L.Cin, cin);
-  p.B = x.c->B; p.H = x.c->H; p.W = x.c->W;
-  p.KH = L.KH; p.KW = L.KW; p.Cout = L.Cout; p.Cout_pad = L.Cout_pad;
-  p.weight = L.weight; p.bias = L.bias;
-  p.epilogue = epi; p.scale = scale;
-  p.out = out; p.out_stride = out_stride; p.out_offset = out_offset;
-  p.aux_h = x.b->net; p.aux_z = x.at(x.ws.off_z); p.hidden = x.c->hidden_dim;
-  p.coords = x.b->coords; p.flow = reinterpret_cast<const float*>(x.at(x.ws.off_flow));
-  p.dtype = x.c->dtype; p.impl = x.c->impl;
-  p.weight_k = L.weight_k; p.Cin_pad = L.Cin_pad; p.Cout_pad_k = L.Cout_pad_k;
-  p.addend = addend; p.addend_stride = addend_stride;
-  return pfb_conv2d(&p, (pfb_stream)x.s);
+static int run_conv(const Ctx& x, int layer, std::initializer_list<pfb_conv_src> srcs, const ConvOut& o, const void* addend = nullptr,
+                    int addend_stride = 0) {
+  ConvExtras e = x.e;
+  e.addend = addend; e.addend_stride = addend_stride;
+  return launch_conv(x.c, x.s, x.w->layers[layer], srcs, o, e);
 }
 
 // round-2 restructurings of the tensor-core path; PFB_GRU_CTX_SPLIT=0 / PFB_MERGE_C2F2=0 fall back to the plain layers
@@ -191,28 +359,9 @@ static int run_context_terms(const Ctx& x) {
   const int layers[4] = {PFB_L_CTX_ZR1, PFB_L_CTX_Q1, PFB_L_CTX_ZR2, PFB_L_CTX_Q2};
   for (int i = 0; i < 4; ++i) {
     const int n = (i & 1) ? hd : 2 * hd;
-    PFB_TRY(run_conv(x, layers[i], {src_of(x.b->inp, cd, cd)}, PFB_EPI_LINEAR, x.at(x.ws.off_ctx[i]), n, 0));
+    PFB_TRY(run_conv(x, layers[i], {src_of(x.b->inp, cd, cd)}, {PFB_EPI_LINEAR, x.at(x.ws.off_ctx[i]), n, 0}));
   }
   return PFB_OK;
-}
-
-int raft_lookup(const pfb_raft_cfg* c, void* const* pyramid, const void* fmap1, const float* coords, void* out, int out_stride,
-                void* flags, cudaStream_t s, float scale) {
-  if (c->alternate_corr) {
-    static const int env_tc = getenv("PFB_ONTHEFLY_TC") ? atoi(getenv("PFB_ONTHEFLY_TC")) : 1;
-    if (env_tc && c->impl != 1 && corr_onthefly_umma_supported(c->B, c->H, c->W, c->feat_dim, c->corr_levels, c->corr_radius, c->dtype, out_stride))
-      return pfb_corr_lookup_onthefly_tc_ex(fmap1, pyramid, coords, out, flags, c->B, c->H, c->W,
-                                            c->feat_dim, c->corr_levels, c->corr_radius, scale, c->dtype, out_stride, (pfb_stream)s);
-  }
-  if (c->alternate_corr)
-    return pfb_corr_lookup_onthefly_ex(fmap1, pyramid, coords, out, c->B, c->H, c->W,
-                                       c->feat_dim, c->corr_levels, c->corr_radius, scale, c->dtype, c->dtype, 0,
-                                       out_stride, (pfb_stream)s);
-  if (c->volume_layout == 1)
-    return pfb_corr_lookup_tiled(pyramid, coords, out, c->B, c->H, c->W, c->H, c->W, c->corr_levels,
-                                 c->corr_radius, c->dtype, out_stride, (pfb_stream)s);
-  return pfb_corr_lookup(pyramid, coords, out, c->B, c->H, c->W, c->corr_levels,
-                         c->corr_radius, c->dtype, c->dtype, 0, out_stride, (pfb_stream)s);
 }
 
 static int lookup(const Ctx& x) {
@@ -220,208 +369,76 @@ static int lookup(const Ctx& x) {
                      x.corr_scale);
 }
 
-int gma_aggregate(const pfb_raft_cfg* c, const pfb_layer& agg_v, const pfb_layer& agg_proj, const void* attention_ptr, float gamma,
-                  void* motion, int motion_stride, int motion_offset, int out_offset, void* vbuf_ptr, void* vT_ptr, void* agg_ptr, int n_pad,
-                  cudaStream_t s) {
-  PFB_CHECK_ARG(attention_ptr, "gma: null attention");
-  const int N = c->H * c->W, heads = heads_of(c), vdim = heads * 128;
-  const size_t es = dtype_size(c->dtype);
-  const char* attention = reinterpret_cast<const char*>(attention_ptr);
-  char* vbuf = reinterpret_cast<char*>(vbuf_ptr);
-  char* vT = reinterpret_cast<char*>(vT_ptr);
-  // one head: attn @ v goes straight into the AXPY epilogue.  Several heads (gma_utils.py:101-111): every head's attn @ v
-  // lands in its 128 columns of `agg`, then project (heads*128 -> 128) carries the AXPY epilogue.
-  char* agg = heads > 1 ? reinterpret_cast<char*>(agg_ptr) : nullptr;
-  PFB_CHECK_ARG(heads == 1 || (agg_proj.weight && agg_proj.Cin == vdim),
-                "gma: num_heads=%d needs the Aggregate.project layer (%d -> 128)", heads, vdim);
-  PFB_CHECK_ARG(agg_v.weight && agg_v.Cin == 128, "gma: Aggregate.to_v layer missing");
-  {  // v = to_v(motion)
-    pfb_conv_params p{};
-    p.src[0] = src_of(motion, 128, motion_stride, motion_offset);
-    p.nsrc = 1;
-    p.B = c->B; p.H = c->H; p.W = c->W; p.KH = agg_v.KH; p.KW = agg_v.KW;
-    p.Cout = agg_v.Cout; p.Cout_pad = agg_v.Cout_pad;
-    p.weight = agg_v.weight; p.bias = agg_v.bias;
-    p.epilogue = PFB_EPI_LINEAR; p.scale = 1.f;
-    p.out = vbuf; p.out_stride = vdim; p.out_offset = 0;
-    p.hidden = c->hidden_dim;
-    p.dtype = c->dtype; p.impl = c->impl;
-    p.weight_k = agg_v.weight_k; p.Cin_pad = agg_v.Cin_pad; p.Cout_pad_k = agg_v.Cout_pad_k;
-    PFB_TRY(pfb_conv2d(&p, (pfb_stream)s));
-  }
-  const bool tensor_path = c->dtype != PFB_F32 && c->impl != 1 && (N % 8) == 0;
-  if (tensor_path) PFB_TRY(pfb_transpose_pm(vbuf, vT, c->B, N, vdim, n_pad, c->dtype, (pfb_stream)s));
-  static const int env_batched = getenv("PFB_GMA_BATCHED") ? atoi(getenv("PFB_GMA_BATCHED")) : 1;
-  // "1x1 convolution" of head h over sample b (b < 0: all samples in one launch): pixels = queries, input channels = the N
-  // attention columns, weights = the sample's v (SIMT layout [N][vdim], columns h*128...) / v^T (K-major [vdim][n_pad], rows
-  // h*128...).  The attention is head-major, so every operand is affine in the pixel index.
-  auto attn_v = [&](int h, int b) -> int {
-    const int b0 = b < 0 ? 0 : b;
-    pfb_conv_params p{};
-    p.src[0] = src_of(attention + ((size_t)h * c->B + b0) * N * N * es, N, N);
-    p.nsrc = 1;
-    p.B = b < 0 ? c->B : 1; p.H = c->H; p.W = c->W; p.KH = 1; p.KW = 1;
-    p.Cout = 128; p.Cout_pad = vdim;
-    p.weight = vbuf + ((size_t)b0 * N * vdim + (size_t)h * 128) * es;
-    p.bias = nullptr;
-    if (heads == 1) {
-      char* mrow = reinterpret_cast<char*>(motion) + (size_t)b0 * N * motion_stride * es;
-      p.epilogue = PFB_EPI_AXPY; p.scale = gamma;
-      p.out = mrow; p.out_stride = motion_stride; p.out_offset = out_offset;
-      p.aux_h = mrow + (size_t)motion_offset * es; p.hidden = motion_stride;
-    } else {
-      p.epilogue = PFB_EPI_LINEAR; p.scale = 1.f;
-      p.out = agg + (size_t)b0 * N * vdim * es; p.out_stride = vdim; p.out_offset = h * 128;
-    }
-    p.dtype = c->dtype; p.impl = c->impl;
-    if (tensor_path) {
-      p.weight_k = vT + ((size_t)b0 * vdim + (size_t)h * 128) * n_pad * es; p.Cin_pad = n_pad; p.Cout_pad_k = 128;
-    }
-    if (b < 0) {
-      // ONE launch for all samples: per-sample weights = that sample's v^T (rows b * vdim + h * 128 ...).  B x 55 row tiles
-      // fill the machine; one launch per sample left only 55 row tiles, a fraction of the machine.
-      p.impl = 2;
-      p.w_rows_per_sample = vdim;
-    }
-    return pfb_conv2d(&p, (pfb_stream)s);
-  };
-  for (int h = 0; h < heads; ++h) {
-    if (tensor_path && env_batched) PFB_TRY(attn_v(h, -1));
-    else for (int b = 0; b < c->B; ++b) PFB_TRY(attn_v(h, b));
-  }
-  if (heads > 1) {  // motion_global = motion + gamma * project(out)   gma_utils.py:108-111
-    const pfb_layer& L = agg_proj;
-    pfb_conv_params p{};
-    p.src[0] = src_of(agg, vdim, vdim);
-    p.nsrc = 1;
-    p.B = c->B; p.H = c->H; p.W = c->W; p.KH = 1; p.KW = 1;
-    p.Cout = L.Cout; p.Cout_pad = L.Cout_pad;
-    p.weight = L.weight; p.bias = nullptr;
-    p.epilogue = PFB_EPI_AXPY; p.scale = gamma;
-    p.out = motion; p.out_stride = motion_stride; p.out_offset = out_offset;
-    p.aux_h = reinterpret_cast<char*>(motion) + (size_t)motion_offset * es; p.hidden = motion_stride;
-    p.dtype = c->dtype; p.impl = c->impl;
-    p.weight_k = L.weight_k; p.Cin_pad = L.Cin_pad; p.Cout_pad_k = L.Cout_pad_k;
-    PFB_TRY(pfb_conv2d(&p, (pfb_stream)s));
-  }
-  return PFB_OK;
-}
-
 // One BasicUpdateBlock / SmallUpdateBlock evaluation + coords update.  update.py:122-153
 static int update_iter(const Ctx& x, const void* corr_ext, void* mask_out) {
   const pfb_raft_cfg* c = x.c;
   const Workspace& ws = x.ws;
+  const pfb_layer* L = x.w->layers;
   const int hd = c->hidden_dim, cd = c->context_dim;
   const void* corr = corr_ext ? corr_ext : x.at(ws.off_corr);
   const int corr_stride = corr_ext ? ws.planes : ws.corr_stride;
-  void* corflo = x.at(ws.off_corflo);
-  void* flo1 = x.at(ws.off_flo1);
   void* motion = x.at(ws.off_motion);
   void* rh = x.at(ws.off_rh);
-  void* fh = x.at(ws.off_fh);
-  float* flow = reinterpret_cast<float*>(x.at(ws.off_flow));
+  const pfb_conv_src net = src_of(x.b->net, hd, hd);
 
-  // ---- motion encoder (update.py:76-112) ----
-  const bool merged_c2f2 = merged_c2f2_active(x);
-  Ctx xf = x;  // the flow branch's launches: the side stream when forked (the fork itself is in the caller, before the lookup)
-  if (x.side) xf.s = x.side;
-  if (c->variant != 1) {
-    void* cor1 = x.at(ws.off_cor1);
-    PFB_TRY(run_conv(x, PFB_L_CONVC1, {src_of(corr, ws.planes, corr_stride)}, PFB_EPI_RELU, cor1, ws.c_cor1, 0));
-    if (!merged_c2f2) PFB_TRY(run_conv(x, PFB_L_CONVC2, {src_of(cor1, ws.c_cor1, ws.c_cor1)}, PFB_EPI_RELU, corflo, ws.c_corflo, 0));
-  } else {
-    PFB_TRY(run_conv(x, PFB_L_CONVC1, {src_of(corr, ws.planes, corr_stride)}, PFB_EPI_RELU, corflo, ws.c_corflo, 0));
-  }
-  {
-    const pfb_layer& LF = x.w->layers[PFB_L_CONVF1];
-    static const int env_fc = getenv("PFB_FLOW_CONV_UMMA") ? atoi(getenv("PFB_FLOW_CONV_UMMA")) : 1;
-    if (env_fc && LF.weight_k && LF.KH == 7 && LF.KW == 7 && LF.Cin == 2 && LF.Cout == 128 && c->dtype != PFB_F32 && c->impl != 1)
-      PFB_TRY(pfb_flow_conv7x7(flow, LF.weight_k, LF.bias, flo1, ws.c_flo1, 0, c->B, c->H, c->W, c->dtype, (pfb_stream)xf.s));
-    else
-      PFB_TRY(run_conv(xf, PFB_L_CONVF1, {src_of(flow, 2, 2, 0, 1)}, PFB_EPI_RELU, flo1, ws.c_flo1, 0));
-  }
-  if (merged_c2f2)  // convc2 | convf2 as one block-diagonal layer: [cor1 (256) | flo1 (128)] -> [cor (192) | flo (64)]
-    PFB_TRY(run_conv(x, PFB_L_CONVC2F2, {src_of(x.at(ws.off_cor1), ws.c_cor1, ws.c_cor1), src_of(flo1, ws.c_flo1, ws.c_flo1)}, PFB_EPI_RELU,
-                     corflo, ws.c_corflo, 0));
-  else
-    PFB_TRY(run_conv(xf, PFB_L_CONVF2, {src_of(flo1, ws.c_flo1, ws.c_flo1)}, PFB_EPI_RELU, corflo, ws.c_corflo, ws.c_cor2));
-  if (x.side) {  // join: `conv` reads both branches
-    PFB_CUDA(cudaEventRecord(x.ev_join, x.side));
-    PFB_CUDA(cudaStreamWaitEvent(x.s, x.ev_join, 0));
-  }
-  PFB_TRY(run_conv(x, PFB_L_CONV, {src_of(corflo, ws.c_corflo, ws.c_corflo)}, PFB_EPI_RELU_APPEND_FLOW, motion, ws.c_motion, 0));
+  // ---- motion encoder (update.py:76-112); when forked, the fork itself is in the caller, before the lookup ----
+  const MotionLayers ml{&L[PFB_L_CONVC1], c->variant != 1 ? &L[PFB_L_CONVC2] : nullptr, &L[PFB_L_CONVF1], &L[PFB_L_CONVF2], &L[PFB_L_CONV]};
+  const MotionBuffers mb{x.at(ws.off_cor1), x.at(ws.off_corflo), x.at(ws.off_flo1), ws.c_cor1, ws.c_cor2, ws.c_flo1, ws.c_flo2};
+  PFB_TRY(motion_encoder(c, x.s, x.e, ml, mb, src_of(corr, ws.planes, corr_stride), {PFB_EPI_RELU_APPEND_FLOW, motion, ws.c_motion, 0},
+                         x.side, x.ev_join, merged_c2f2_active(x) ? &L[PFB_L_CONVC2F2] : nullptr));
 
   // ---- gma: motion_global = motion + gamma * (attention @ to_v(motion))   gma_utils.py:101-113, gma/update.py:149 ----
   if (c->variant == 2)
-    PFB_TRY(gma_aggregate(c, x.w->layers[PFB_L_AGG_V], x.w->layers[PFB_L_AGG_PROJ], x.b->attention, x.b->agg_gamma, motion, ws.c_motion, 0,
-                          128, x.at(ws.off_vbuf), x.at(ws.off_vT), x.at(ws.off_agg), ws.n_pad, x.s));
+    PFB_TRY(gma_aggregate(c, L[PFB_L_AGG_V], L[PFB_L_AGG_PROJ], x.b->attention, x.b->agg_gamma, motion, ws.c_motion, 0, 128,
+                          x.at(ws.off_vbuf), x.at(ws.off_vT), x.at(ws.off_agg), ws.n_pad, x.s));
   // ---- ccmr: motion_global = aggregator(global_context, motion)   ccmr/update.py:156-161 ----
   if (c->variant == 6) PFB_TRY(ccmr_aggregate(c, x.ccmr, motion, ws.c_motion, x.ccmr_base, x.s));
 
   // ---- GRU (update.py:24-32 ConvGRU, :58-73 SepConvGRU); x = [inp, motion (, motion_global)] ----
   const int halves = (c->variant != 1) ? 2 : 1;
   const bool split = ctx_split_active(x);
+  const pfb_conv_src mot = src_of(motion, ws.c_motion, ws.c_motion), hr = src_of(rh, hd, hd);
   for (int h = 0; h < halves; ++h) {
     if (split) {
       // conv([h | inp | motion]) = conv_inp(inp) + bias (once per forward, run_context_terms) + conv_rest([h | motion]) (here)
       const int lzr = h == 0 ? PFB_L_GRUX_ZR1 : PFB_L_GRUX_ZR2, lq = h == 0 ? PFB_L_GRUX_Q1 : PFB_L_GRUX_Q2;
-      PFB_TRY(run_conv(x, lzr, {src_of(x.b->net, hd, hd), src_of(motion, ws.c_motion, ws.c_motion)}, PFB_EPI_GRU_ZR, rh, hd, 0, 1.f,
-                       x.at(ws.off_ctx[2 * h]), 2 * hd));
-      PFB_TRY(run_conv(x, lq, {src_of(rh, hd, hd), src_of(motion, ws.c_motion, ws.c_motion)}, PFB_EPI_GRU_Q, x.b->net, hd, 0, 1.f,
-                       x.at(ws.off_ctx[2 * h + 1]), hd));
+      PFB_TRY(run_conv(x, lzr, {net, mot}, {PFB_EPI_GRU_ZR, rh, hd, 0}, x.at(ws.off_ctx[2 * h]), 2 * hd));
+      PFB_TRY(run_conv(x, lq, {hr, mot}, {PFB_EPI_GRU_Q, x.b->net, hd, 0}, x.at(ws.off_ctx[2 * h + 1]), hd));
       continue;
     }
     const int lzr = h == 0 ? PFB_L_GRU_ZR1 : PFB_L_GRU_ZR2, lq = h == 0 ? PFB_L_GRU_Q1 : PFB_L_GRU_Q2;
-    PFB_TRY(run_conv(x, lzr, {src_of(x.b->net, hd, hd), src_of(x.b->inp, cd, cd), src_of(motion, ws.c_motion, ws.c_motion)},
-                     PFB_EPI_GRU_ZR, rh, hd, 0));
-    PFB_TRY(run_conv(x, lq, {src_of(rh, hd, hd), src_of(x.b->inp, cd, cd), src_of(motion, ws.c_motion, ws.c_motion)},
-                     PFB_EPI_GRU_Q, x.b->net, hd, 0));
+    const pfb_conv_src inp = src_of(x.b->inp, cd, cd);
+    PFB_TRY(run_conv(x, lzr, {net, inp, mot}, {PFB_EPI_GRU_ZR, rh, hd, 0}));
+    PFB_TRY(run_conv(x, lq, {hr, inp, mot}, {PFB_EPI_GRU_Q, x.b->net, hd, 0}));
   }
 
   // ---- heads (update.py:6-14, :138-152) ----
-  const bool fork_mask = x.side && mask_out && c->variant != 1;
+  const bool mask = mask_out && c->variant != 1;
+  const bool fork_mask = x.side && mask;
   if (fork_mask) {  // last iteration: the mask head beside the flow head (both read the final hidden state)
     PFB_CUDA(cudaEventRecord(x.ev_fork, x.s));
     PFB_CUDA(cudaStreamWaitEvent(x.side, x.ev_fork, 0));
-    void* mh = x.at(ws.off_mh);
-    PFB_TRY(run_conv(xf, PFB_L_MASK1, {src_of(x.b->net, hd, hd)}, PFB_EPI_RELU, mh, 256, 0));
-    PFB_TRY(run_conv(xf, PFB_L_MASK2, {src_of(mh, 256, 256)}, PFB_EPI_LINEAR, mask_out, mask_channels(c), 0, 0.25f));
+    PFB_TRY(mask_head(c, x.side, x.e, L[PFB_L_MASK1], L[PFB_L_MASK2], net, x.at(ws.off_mh), mask_out, mask_channels(c)));
     PFB_CUDA(cudaEventRecord(x.ev_join, x.side));
   }
-  PFB_TRY(run_conv(x, PFB_L_FLOW1, {src_of(x.b->net, hd, hd)}, PFB_EPI_RELU, fh, ws.c_fh, 0));
-  const pfb_layer& LT = x.w->layers[PFB_L_FLOW2T];
-  if (c->variant != 1 && c->dtype != PFB_F32 && c->impl != 1 && LT.weight_k) {
-    // tensor-core form of the 3x3 -> 2 convolution: one 1x1 GEMM to the 18 (tap, output) products, then a 9-tap gather
-    float* taps = reinterpret_cast<float*>(x.at(ws.off_taps));
-    PFB_TRY(run_conv(x, PFB_L_FLOW2T, {src_of(fh, ws.c_fh, ws.c_fh)}, PFB_EPI_LINEAR_F32, taps, 32, 0));
-    PFB_TRY(pfb_flow_tap_gather(taps, 32, x.w->layers[PFB_L_FLOW2].bias, x.b->coords, flow, c->B, c->H, c->W, (pfb_stream)x.s));
-  } else {
-    PFB_TRY(run_conv(x, PFB_L_FLOW2, {src_of(fh, ws.c_fh, ws.c_fh)}, PFB_EPI_FLOW, flow, 2, 0));
-  }
-  if (fork_mask) {
-    PFB_CUDA(cudaStreamWaitEvent(x.s, x.ev_join, 0));  // the upsample reads the mask
-  } else if (mask_out && c->variant != 1) {
-    void* mh = x.at(ws.off_mh);
-    PFB_TRY(run_conv(x, PFB_L_MASK1, {src_of(x.b->net, hd, hd)}, PFB_EPI_RELU, mh, 256, 0));
-    PFB_TRY(run_conv(x, PFB_L_MASK2, {src_of(mh, 256, 256)}, PFB_EPI_LINEAR, mask_out, mask_channels(c), 0, 0.25f));
-  }
+  PFB_TRY(flow_head(c, x.s, x.e, L[PFB_L_FLOW1], L[PFB_L_FLOW2], c->variant != 1 ? &L[PFB_L_FLOW2T] : nullptr, net, x.at(ws.off_fh),
+                    ws.c_fh, reinterpret_cast<float*>(x.at(ws.off_taps)), reinterpret_cast<float*>(x.at(ws.off_flow))));
+  if (fork_mask) PFB_CUDA(cudaStreamWaitEvent(x.s, x.ev_join, 0));  // the upsample reads the mask
+  else if (mask) PFB_TRY(mask_head(c, x.s, x.e, L[PFB_L_MASK1], L[PFB_L_MASK2], net, x.at(ws.off_mh), mask_out, mask_channels(c)));
   return PFB_OK;
 }
 
 static int make_ctx(Ctx& x, const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf,
                     cudaStream_t s, bool need_pyramid, bool msraft = false, bool ccmr = false) {
   PFB_TRY(check_cfg(cfg, msraft, ccmr));
-  PFB_CHECK_ARG(w && buf, "raft: null weights/buffers");
-  PFB_CHECK_ARG(buf->net && buf->inp && buf->coords && buf->workspace, "raft: null state buffer");
-  if (need_pyramid) {
-    PFB_CHECK_ARG(buf->pyramid, "raft: null pyramid");
-    PFB_CHECK_ARG(!cfg->alternate_corr || (buf->fmap1 && cfg->feat_dim > 0), "raft: alternate_corr needs fmap1 and feat_dim");
-  }
+  const char* name = ccmr ? "ccmr" : msraft ? "msraft" : "raft";
+  PFB_CHECK_ARG(w, "%s: null weights", name);
   x.c = cfg; x.w = w; x.b = buf; x.s = s;
   x.ws = plan(cfg);
-  const size_t need = x.ws.total + (ccmr ? ccmr_plan(cfg).total : 0);
-  PFB_CHECK_ARG(buf->workspace_bytes >= need, "raft: workspace %zu bytes < required %zu", buf->workspace_bytes, need);
+  PFB_TRY(check_loop_buffers(cfg, buf, need_pyramid, x.ws.total + (ccmr ? ccmr_plan(cfg).total : 0), name));
   x.base = reinterpret_cast<char*>(buf->workspace);
+  x.e.aux_h = buf->net; x.e.aux_z = x.at(x.ws.off_z); x.e.hidden = cfg->hidden_dim;
+  x.e.coords = buf->coords; x.e.flow = reinterpret_cast<const float*>(x.at(x.ws.off_flow));
   return PFB_OK;
 }
 
@@ -511,22 +528,14 @@ extern "C" PFB_API int pfb_msraft_refine(const pfb_raft_cfg* cfg, const pfb_raft
                                          float* next_coords, pfb_stream stream) {
   Ctx x;
   PFB_TRY(make_ctx(x, cfg, w, buf, as_stream(stream), true, true));
-  PFB_CHECK_ARG(cfg->iters >= 1, "msraft_refine: every scale needs at least one iteration (iters=%d)", cfg->iters);
-  PFB_CHECK_ARG(corr_scale >= 0.f, "msraft_refine: corr_scale=%g", (double)corr_scale);
-  PFB_CHECK_ARG(next_coords || buf->flow_up, "msraft_refine: needs next_coords (coarser scales) or flow_up (the finest)");
-  if (!next_coords && buf->flow_small)
-    PFB_CHECK_ARG(cfg->out_h >= 16 && cfg->out_w >= 16, "msraft_refine: output %dx%d smaller than 16 px per side", cfg->out_h, cfg->out_w);
+  PFB_TRY(check_multiscale_args(cfg, buf, corr_scale, next_coords, 0, "msraft_refine"));
   x.corr_scale = corr_scale;
   void* mask = x.at(x.ws.off_mask);
   PFB_TRY(run_iterations(x, mask));
   if (next_coords)  // handover: the absolute coordinates, doubled and convex-upsampled with zero-padded taps (ms_raft_plus.py:198-200)
     return pfb_convex_upsample2x(buf->coords, mask, next_coords, 1, cfg->B, cfg->H, cfg->W, 0, 0, 0, 0, cfg->dtype, stream);
-  PFB_TRY(pfb_convex_upsample2x(buf->coords, mask, buf->flow_up, 0, cfg->B, cfg->H, cfg->W, cfg->out_h, cfg->out_w, cfg->pad_top,
-                                cfg->pad_left, cfg->dtype, stream));
-  if (!buf->flow_small) return PFB_OK;
   // flow_small = downflow(flow_up, 1/16) at int(h / 16) x int(w / 16) of the un-padded size (ms_raft_plus.py:22-35, 221-224)
-  const int sh = cfg->out_h / 16, sw = cfg->out_w / 16;
-  return pfb_downflow(buf->flow_up, buf->flow_small, cfg->B, cfg->out_h, cfg->out_w, sh, sw, stream);
+  return ccmr_output(cfg, buf->coords, mask, buf->flow_up, buf->flow_small, 0, nullptr, x.s);
 }
 
 // ---- a18: CCMR / CCMR+ (one call per scale of ccmr.py:179-220) ----
@@ -536,7 +545,6 @@ static int make_ccmr_ctx(Ctx& x, const pfb_raft_cfg* cfg, const pfb_ccmr_weights
                          bool need_pyramid, float corr_scale) {
   PFB_CHECK_ARG(w, "ccmr: null weights");
   PFB_TRY(make_ctx(x, cfg, &w->raft, buf, s, need_pyramid, false, true));
-  PFB_CHECK_ARG(corr_scale >= 0.f, "ccmr: corr_scale=%g", (double)corr_scale);
   PFB_CHECK_ARG(cfg->context_dim == 128, "ccmr: the XCiT blocks expect 128 context channels");
   x.corr_scale = corr_scale;
   x.ccmr = w;
@@ -557,6 +565,7 @@ extern "C" PFB_API int pfb_ccmr_update_iter(const pfb_raft_cfg* cfg, const pfb_c
                                             const void* corr, void* mask_out, float corr_scale, pfb_stream stream) {
   Ctx x;
   PFB_TRY(make_ccmr_ctx(x, cfg, w, buf, as_stream(stream), corr == nullptr, corr_scale));
+  PFB_CHECK_ARG(corr_scale >= 0.f, "ccmr_update_iter: corr_scale=%g", (double)corr_scale);
   PFB_TRY(ccmr_scale_setup(cfg, w, buf->inp, nullptr, true, x.ccmr_base, x.s));
   return update_iter_once(x, corr, mask_out);
 }
@@ -565,18 +574,8 @@ extern "C" PFB_API int pfb_ccmr_refine(const pfb_raft_cfg* cfg, const pfb_ccmr_w
                                        int upflow2, float* next_coords, pfb_stream stream) {
   Ctx x;
   PFB_TRY(make_ccmr_ctx(x, cfg, w, buf, as_stream(stream), true, corr_scale));
-  PFB_CHECK_ARG(cfg->iters >= 1, "ccmr_refine: every scale needs at least one iteration (iters=%d)", cfg->iters);
   PFB_CHECK_ARG(upflow2 == 0 || upflow2 == 1, "ccmr_refine: upflow2=%d (0 or 1)", upflow2);
-  PFB_CHECK_ARG(next_coords || buf->flow_up, "ccmr_refine: needs next_coords (coarser scales) or flow_up (the finest)");
-  if (!next_coords) {
-    const int f = 2 << upflow2;  // the output grid is f times this scale's
-    PFB_CHECK_ARG(cfg->out_h > 0 && cfg->out_w > 0 && cfg->pad_top >= 0 && cfg->pad_left >= 0 && cfg->out_h + cfg->pad_top <= f * cfg->H &&
-                      cfg->out_w + cfg->pad_left <= f * cfg->W,
-                  "ccmr_refine: output window %dx%d+(%d,%d) outside %dx%d", cfg->out_h, cfg->out_w, cfg->pad_top, cfg->pad_left, f * cfg->H,
-                  f * cfg->W);
-    if (buf->flow_small)
-      PFB_CHECK_ARG(cfg->out_h >= 16 && cfg->out_w >= 16, "ccmr_refine: output %dx%d smaller than 16 px per side", cfg->out_h, cfg->out_w);
-  }
+  PFB_TRY(check_multiscale_args(cfg, buf, corr_scale, next_coords, upflow2, "ccmr_refine"));
   PFB_TRY(ccmr_scale_setup(cfg, w, buf->inp, nullptr, true, x.ccmr_base, x.s));
   void* mask = x.at(x.ws.off_mask);
   PFB_TRY(run_iterations(x, mask));

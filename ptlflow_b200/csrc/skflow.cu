@@ -1,19 +1,14 @@
 // SKFlow's refinement loop (ptlflow/models/skflow/skflow.py:197-232, update.py:7-99): lookup -> large-kernel motion encoder ->
 // GMA aggregate -> PCBlock "GRU" -> PCBlock flow head, `iters` times, then the mask head and the convex upsample once.
 // Every stage is a launch of this library's kernels on the caller's stream, so the whole loop is one CUDA graph when the host
-// captures it.  The lookup, the attention aggregate, flow-from-coords and the upsample are the raft / gma loop's (refine.cuh).
+// captures it.  The lookup, the attention aggregate, the mask head, flow-from-coords and the upsample are the raft / gma loop's
+// (refine.cuh).
 //
 // Layout: one [P][512] buffer X = [net | inp | motion | motion_global] that every producer writes at its column offset: the
 // motion encoder's last layer writes motion (126 channels + the flow), the aggregate motion_global, the update block the new net.
 // X is at the same time the update block's input and its ffn1 residual, so no concatenation is ever copied.  Inside a PCBlock
 // the activations ping-pong between two scratch buffers; channel counts are padded to multiples of 32 whose padding stays zero.
 #include "refine.cuh"
-
-#define PFB_TRY(expr)        \
-  do {                       \
-    int rc__ = (expr);       \
-    if (rc__ != PFB_OK) return rc__; \
-  } while (0)
 
 namespace pfb {
 namespace {
@@ -38,40 +33,31 @@ SkWs plan(const pfb_raft_cfg* c) {
   const int hid_c1 = (int)align_up((size_t)(3 * w.planes) / 2, 32);
   w.hmax = hid_c1 > 3 * kX / 2 ? hid_c1 : 3 * kX / 2;
   w.n_pad = (int)align_up((size_t)c->H * c->W, 64);
-  size_t off = 0;
-  auto take = [&](size_t bytes) { size_t o = off; off = align_up(off + bytes, 256); return o; };
-  w.off_corr = take(P * w.corr_stride * es);
-  w.off_cor1 = take(P * 256 * es);
-  w.off_corflo = take(P * 256 * es);
-  w.off_flo1 = take(P * 128 * es);
-  w.off_x = take(P * kX * es);
-  w.off_a = take(P * w.cmax * es);
-  w.off_b = take(P * w.cmax * es);
-  w.off_h = take(P * w.hmax * es);
-  w.off_mh = take(P * 256 * es);
-  w.off_mask = take(P * 576 * es);
-  w.off_flow = take(P * 2 * sizeof(float));
-  w.off_vbuf = take(P * vdim * es);
-  w.off_vT = take((size_t)c->B * vdim * w.n_pad * es);
-  w.off_agg = take(vdim > 128 ? P * vdim * es : 0);
-  w.off_flags = take(c->alternate_corr ? P : 0);
-  w.total = off;
+  Carve k;
+  w.off_corr = k.take(P * w.corr_stride * es);
+  w.off_cor1 = k.take(P * 256 * es);
+  w.off_corflo = k.take(P * 256 * es);
+  w.off_flo1 = k.take(P * 128 * es);
+  w.off_x = k.take(P * kX * es);
+  w.off_a = k.take(P * w.cmax * es);
+  w.off_b = k.take(P * w.cmax * es);
+  w.off_h = k.take(P * w.hmax * es);
+  w.off_mh = k.take(P * 256 * es);
+  w.off_mask = k.take(P * 576 * es);
+  w.off_flow = k.take(P * 2 * sizeof(float));
+  w.off_vbuf = k.take(P * vdim * es);
+  w.off_vT = k.take((size_t)c->B * vdim * w.n_pad * es);
+  w.off_agg = k.take(vdim > 128 ? P * vdim * es : 0);
+  w.off_flags = k.take(c->alternate_corr ? P : 0);
+  w.total = k.total;
   return w;
 }
 
 int check_cfg(const pfb_raft_cfg* c) {
-  PFB_CHECK_ARG(c, "skflow: null cfg");
+  PFB_TRY(check_loop_cfg(c, "skflow"));
   PFB_CHECK_ARG(c->variant == 3, "skflow: variant=%d (the skflow loop is variant 3)", c->variant);
-  PFB_CHECK_ARG(dtype_ok(c->dtype), "skflow: bad dtype");
-  PFB_CHECK_ARG(c->B > 0 && c->H > 0 && c->W > 0, "skflow: bad grid %dx%dx%d", c->B, c->H, c->W);
-  PFB_CHECK_ARG(c->corr_levels >= 1 && c->corr_levels <= PFB_MAX_LEVELS && c->corr_radius >= 0 && c->corr_radius <= 15,
-                "skflow: corr_levels=%d corr_radius=%d", c->corr_levels, c->corr_radius);
-  PFB_CHECK_ARG((c->H >> (c->corr_levels - 1)) >= 1 && (c->W >> (c->corr_levels - 1)) >= 1,
-                "skflow: %dx%d grid too small for %d levels", c->H, c->W, c->corr_levels);
-  PFB_CHECK_ARG(c->hidden_dim == 128 && c->context_dim == 128 && c->iters >= 0, "skflow: the update block expects hidden=context=128");
+  PFB_CHECK_ARG(c->hidden_dim == 128 && c->context_dim == 128, "skflow: the update block expects hidden=context=128");
   PFB_CHECK_ARG(c->num_heads >= 0 && c->num_heads <= 64, "skflow: num_heads=%d", c->num_heads);
-  PFB_CHECK_ARG(c->volume_layout == 0 || (c->volume_layout == 1 && c->dtype != PFB_F32 && !c->alternate_corr && c->corr_levels <= 4),
-                "skflow: volume_layout=%d needs f16/bf16, a materialised pyramid and <= 4 levels", c->volume_layout);
   return PFB_OK;
 }
 
@@ -112,56 +98,30 @@ struct SkCtx {
   SkWs ws;
   char* base;
   cudaStream_t s;
+  ConvExtras e;  // every layer's coordinates and flow
   void* at(size_t off) const { return base + off; }
   float* flow() const { return reinterpret_cast<float*>(base + ws.off_flow); }
 };
 
-pfb_conv_src src_of(const void* ptr, int channels, int stride, int offset = 0, int is_f32 = 0) {
-  pfb_conv_src s;
-  s.ptr = ptr; s.channels = channels; s.stride = stride; s.offset = offset; s.is_f32 = is_f32;
-  return s;
-}
-
-struct Out {
-  int epi;
-  void* ptr;
-  int stride, offset;
-  float scale;
-};
-
-int conv(const SkCtx& x, const pfb_layer& L, const pfb_conv_src& src, const Out& o, const pfb_conv_src* res = nullptr,
+int conv(const SkCtx& x, const pfb_layer& L, const pfb_conv_src& src, const ConvOut& o, const pfb_conv_src* res = nullptr,
          const float* post_w = nullptr, const float* post_b = nullptr) {
-  PFB_CHECK_ARG(L.weight && src.channels == L.Cin, "skflow: layer expects Cin=%d, source provides %d", L.Cin, src.channels);
-  pfb_conv_params p{};
-  p.src[0] = src;
-  p.nsrc = 1;
-  p.B = x.c->B; p.H = x.c->H; p.W = x.c->W;
-  p.KH = L.KH; p.KW = L.KW; p.Cout = L.Cout; p.Cout_pad = L.Cout_pad;
-  p.weight = L.weight; p.bias = L.bias;
-  p.epilogue = o.epi; p.scale = o.scale;
-  p.out = o.ptr; p.out_stride = o.stride; p.out_offset = o.offset;
-  p.coords = x.b->coords; p.flow = x.flow();
-  p.dtype = x.c->dtype; p.impl = x.c->impl;
-  p.weight_k = L.weight_k; p.Cin_pad = L.Cin_pad; p.Cout_pad_k = L.Cout_pad_k;
-  if (res) {
-    p.residual = res->ptr; p.residual_stride = res->stride; p.residual_offset = res->offset;
-    p.post_w = post_w; p.post_b = post_b;
-  }
-  return pfb_conv2d(&p, (pfb_stream)x.s);
+  ConvExtras e = x.e;
+  e.residual = res; e.post_w = post_w; e.post_b = post_b;
+  return launch_conv(x.c, x.s, L, {src}, o, e);
 }
 
 // PCBlock4_Deep_nopool_res (update.py:7-41) on `in` (k.C channels); the last layer's output and epilogue are the caller's
-int pc_block(const SkCtx& x, const pfb_pc_block& k, const pfb_conv_src& in, const Out& last) {
+int pc_block(const SkCtx& x, const pfb_pc_block& k, const pfb_conv_src& in, const ConvOut& last) {
   char* h = reinterpret_cast<char*>(x.at(x.ws.off_h));
   char* cur = reinterpret_cast<char*>(x.at(x.ws.off_a));
   char* oth = reinterpret_cast<char*>(x.at(x.ws.off_b));
   const int C = k.C, hid = k.hid;
   // x = gelu(x + ffn1(x)); a leading k = 1 entry of k_conv, gelu(x + w * x + b), rides the same epilogue
-  PFB_TRY(conv(x, k.ffn1a, in, Out{PFB_EPI_GELU, h, hid, 0, 1.f}));
+  PFB_TRY(conv(x, k.ffn1a, in, ConvOut{PFB_EPI_GELU, h, hid, 0}));
   int first = 0;
   const float *pw = nullptr, *pb = nullptr;
   if (k.n_dw > 0 && k.dw_k[0] == 1) { pw = k.dw_weight[0]; pb = k.dw_bias[0]; first = 1; }
-  PFB_TRY(conv(x, k.ffn1b, src_of(h, hid, hid), Out{PFB_EPI_RESIDUAL_GELU, cur, C, 0, 1.f}, &in, pw, pb));
+  PFB_TRY(conv(x, k.ffn1b, src_of(h, hid, hid), ConvOut{PFB_EPI_RESIDUAL_GELU, cur, C, 0}, &in, pw, pb));
   // x = gelu(x + dw_k(x)) for the remaining entries of k_conv
   for (int i = first; i < k.n_dw; ++i) {
     PFB_TRY(pfb_depthwise_conv_gelu(cur, C, 0, oth, C, 0, k.dw_weight[i], k.dw_bias[i], x.c->B, x.c->H, x.c->W, C, k.dw_k[i], x.c->dtype,
@@ -170,9 +130,9 @@ int pc_block(const SkCtx& x, const pfb_pc_block& k, const pfb_conv_src& in, cons
   }
   // x = gelu(x + pw(x))
   const pfb_conv_src xs = src_of(cur, C, C);
-  PFB_TRY(conv(x, k.pw, xs, Out{PFB_EPI_RESIDUAL_GELU, oth, C, 0, 1.f}, &xs));
+  PFB_TRY(conv(x, k.pw, xs, ConvOut{PFB_EPI_RESIDUAL_GELU, oth, C, 0}, &xs));
   // out = ffn2(x)
-  PFB_TRY(conv(x, k.ffn2a, src_of(oth, C, C), Out{PFB_EPI_GELU, h, hid, 0, 1.f}));
+  PFB_TRY(conv(x, k.ffn2a, src_of(oth, C, C), ConvOut{PFB_EPI_GELU, h, hid, 0}));
   return conv(x, k.ffn2b, src_of(h, hid, hid), last);
 }
 
@@ -187,59 +147,46 @@ int update_iter(const SkCtx& x, const void* corr_ext, void* mask_out) {
   void* flo1 = x.at(ws.off_flo1);
   void* X = x.at(ws.off_x);
   // ---- motion encoder (update.py:53-61) ----
-  PFB_TRY(pc_block(x, blk[PFB_SK_CONVC1], src_of(corr, ws.corr_stride, ws.corr_stride), Out{PFB_EPI_GELU, cor1, 256, 0, 1.f}));
-  PFB_TRY(pc_block(x, blk[PFB_SK_CONVC2], src_of(cor1, 256, 256), Out{PFB_EPI_LINEAR, corflo, 256, 0, 1.f}));
-  PFB_TRY(conv(x, x.w->convf1, src_of(x.flow(), 2, 2, 0, 1), Out{PFB_EPI_LINEAR, flo1, 128, 0, 1.f}));
-  PFB_TRY(pc_block(x, blk[PFB_SK_CONVF2], src_of(flo1, 128, 128), Out{PFB_EPI_LINEAR, corflo, 256, 192, 1.f}));
-  PFB_TRY(pc_block(x, blk[PFB_SK_CONV], src_of(corflo, 256, 256), Out{PFB_EPI_LINEAR_APPEND_FLOW, X, kX, 256, 1.f}));
+  PFB_TRY(pc_block(x, blk[PFB_SK_CONVC1], src_of(corr, ws.corr_stride, ws.corr_stride), ConvOut{PFB_EPI_GELU, cor1, 256, 0}));
+  PFB_TRY(pc_block(x, blk[PFB_SK_CONVC2], src_of(cor1, 256, 256), ConvOut{PFB_EPI_LINEAR, corflo, 256, 0}));
+  PFB_TRY(conv(x, x.w->convf1, src_of(x.flow(), 2, 2, 0, 1), ConvOut{PFB_EPI_LINEAR, flo1, 128, 0}));
+  PFB_TRY(pc_block(x, blk[PFB_SK_CONVF2], src_of(flo1, 128, 128), ConvOut{PFB_EPI_LINEAR, corflo, 256, 192}));
+  PFB_TRY(pc_block(x, blk[PFB_SK_CONV], src_of(corflo, 256, 256), ConvOut{PFB_EPI_LINEAR_APPEND_FLOW, X, kX, 256}));
   // ---- motion_global = Aggregate(attention, motion) (update.py:90) ----
   PFB_TRY(gma_aggregate(c, x.w->agg_v, x.w->agg_proj, x.b->attention, x.b->agg_gamma, X, kX, 256, 384, x.at(ws.off_vbuf), x.at(ws.off_vT),
                         x.at(ws.off_agg), ws.n_pad, x.s));
   // ---- net = gru(cat[net, inp, motion, motion_global]): linear, no gates (update.py:94) ----
-  PFB_TRY(pc_block(x, blk[PFB_SK_GRU], src_of(X, kX, kX), Out{PFB_EPI_LINEAR, X, kX, 0, 1.f}));
+  PFB_TRY(pc_block(x, blk[PFB_SK_GRU], src_of(X, kX, kX), ConvOut{PFB_EPI_LINEAR, X, kX, 0}));
   // ---- delta = flow_head(net); coords += delta (update.py:96, skflow.py:218) ----
-  PFB_TRY(pc_block(x, blk[PFB_SK_FLOW_HEAD], src_of(X, 128, kX), Out{PFB_EPI_FLOW, x.flow(), 2, 0, 1.f}));
-  if (mask_out) {  // mask = 0.25 * mask(net) (update.py:98-99)
-    void* mh = x.at(ws.off_mh);
-    PFB_TRY(conv(x, x.w->mask1, src_of(X, 128, kX), Out{PFB_EPI_RELU, mh, 256, 0, 1.f}));
-    PFB_TRY(conv(x, x.w->mask2, src_of(mh, 256, 256), Out{PFB_EPI_LINEAR, mask_out, 576, 0, 0.25f}));
-  }
+  PFB_TRY(pc_block(x, blk[PFB_SK_FLOW_HEAD], src_of(X, 128, kX), ConvOut{PFB_EPI_FLOW, x.flow(), 2, 0}));
+  if (mask_out)  // mask = 0.25 * mask(net) (update.py:98-99)
+    PFB_TRY(mask_head(c, x.s, x.e, x.w->mask1, x.w->mask2, src_of(X, 128, kX), x.at(ws.off_mh), mask_out, 576));
   return PFB_OK;
 }
 
 int make_ctx(SkCtx& x, const pfb_raft_cfg* cfg, const pfb_skflow_weights* w, const pfb_raft_buffers* buf, cudaStream_t s,
              bool need_pyramid) {
   PFB_TRY(check_cfg(cfg));
-  PFB_CHECK_ARG(buf, "skflow: null buffers");
-  PFB_CHECK_ARG(buf->net && buf->inp && buf->coords && buf->workspace && buf->attention, "skflow: null state buffer / attention");
-  if (need_pyramid) {
-    PFB_CHECK_ARG(buf->pyramid, "skflow: null pyramid");
-    PFB_CHECK_ARG(!cfg->alternate_corr || (buf->fmap1 && cfg->feat_dim > 0), "skflow: alternate_corr needs fmap1 and feat_dim");
-  }
   x.c = cfg; x.w = w; x.b = buf; x.s = s;
   x.ws = plan(cfg);
+  PFB_TRY(check_loop_buffers(cfg, buf, need_pyramid, x.ws.total, "skflow"));
+  PFB_CHECK_ARG(buf->attention, "skflow: null attention");
   PFB_TRY(check_weights(cfg, w, x.ws));
-  PFB_CHECK_ARG(buf->workspace_bytes >= x.ws.total, "skflow: workspace %zu bytes < required %zu", buf->workspace_bytes, x.ws.total);
   x.base = reinterpret_cast<char*>(buf->workspace);
+  x.e.coords = buf->coords; x.e.flow = x.flow();
   return PFB_OK;
 }
 
-// net -> X[:, 0:128], inp -> X[:, 128:256]; the flow of the current coordinates; zero lookup columns past the planes
+// net | inp into X; the flow of the current coordinates; zero lookup columns past the planes
 int begin(const SkCtx& x, bool lookup_buffer) {
   const pfb_raft_cfg* c = x.c;
-  const size_t es = dtype_size(c->dtype), P = (size_t)c->B * c->H * c->W;
-  char* X = reinterpret_cast<char*>(x.at(x.ws.off_x));
-  PFB_CUDA(cudaMemcpy2DAsync(X, kX * es, x.b->net, 128 * es, 128 * es, P, cudaMemcpyDeviceToDevice, x.s));
-  PFB_CUDA(cudaMemcpy2DAsync(X + 128 * es, kX * es, x.b->inp, 128 * es, 128 * es, P, cudaMemcpyDeviceToDevice, x.s));
-  if (lookup_buffer) PFB_CUDA(cudaMemsetAsync(x.at(x.ws.off_corr), 0, P * x.ws.corr_stride * es, x.s));
+  PFB_TRY(copy_wide_state(c, x.b, x.at(x.ws.off_x), kX, true, x.s));
+  if (lookup_buffer)
+    PFB_CUDA(cudaMemsetAsync(x.at(x.ws.off_corr), 0, (size_t)c->B * c->H * c->W * x.ws.corr_stride * dtype_size(c->dtype), x.s));
   return launch_flow_from_coords(x.b->coords, x.flow(), c->B, c->H, c->W, x.s);
 }
 
-int finish(const SkCtx& x) {  // the final hidden state back to buf->net
-  const size_t es = dtype_size(x.c->dtype), P = (size_t)x.c->B * x.c->H * x.c->W;
-  PFB_CUDA(cudaMemcpy2DAsync(x.b->net, 128 * es, x.at(x.ws.off_x), kX * es, 128 * es, P, cudaMemcpyDeviceToDevice, x.s));
-  return PFB_OK;
-}
+int finish(const SkCtx& x) { return copy_wide_state(x.c, x.b, x.at(x.ws.off_x), kX, false, x.s); }  // the final hidden state
 
 int lookup(const SkCtx& x) {
   return raft_lookup(x.c, x.b->pyramid, x.b->fmap1, x.b->coords, x.at(x.ws.off_corr), x.ws.corr_stride, x.at(x.ws.off_flags), x.s);
