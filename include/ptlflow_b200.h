@@ -351,6 +351,7 @@ typedef struct {
   int variant;        /* 0 = raft (BasicUpdateBlock, SepConvGRU, convex upsample)
                          1 = raft_small (SmallUpdateBlock, ConvGRU, bilinear upflow8)
                          2 = gma (GMAUpdateBlock: raft + per-iteration attention aggregate, gma/update.py:127-160)
+                         7 = flow1d (raft's update block over the 1D lookup of a row and a column volume, see a19)
                          (3 skflow, 4 sea_raft, 5 ms_raft_plus, 6 ccmr: their own entry points only) */
   pfb_dtype dtype;
   int B, H, W;        /* 1/8-resolution grid */
@@ -604,6 +605,36 @@ PFB_API int pfb_ccmr_update_iter(const pfb_raft_cfg* cfg, const pfb_ccmr_weights
                                  void* mask_out, float corr_scale, pfb_stream stream);
 
 /* ------------------------------------------------------------------------------------
+ * a19: Flow1D (ptlflow/models/flow1d/flow1d.py:148-246): 1D cross-attention, a row and a column correlation volume, and RAFT's loop
+ * over a 1D lookup of them.  The loop is pfb_raft_refine / pfb_raft_update_iter with pfb_raft_cfg variant = 7:
+ *   corr_levels = 1, corr_radius 1..64, alternate_corr = 0, volume_layout = 0, H >= 2 and W >= 2;
+ *   buf->pyramid = {corr_x, corr_y}: corr_x [B*H*W][W] and corr_y [B*H*W][H] in the storage type (pfb_attn1d mode 1);
+ *   the lookup buffer holds 2 (2r+1) planes, [corr_x taps | corr_y taps], its pixel stride rounded up to 8 (f16 / bf16);
+ *   the layers are RAFT's BasicUpdateBlock with CONVC1.Cin = 2 (2r+1); everything else is variant 0.
+ * ---------------------------------------------------------------------------------- */
+#define PFB_ATTN1D_CORR 1
+#define PFB_ATTN1D_ATTN 2
+#define PFB_ATTN1D_MAX_L 1024
+/* Attention / correlation along one axis of pixel-major maps [B,H,W,*] (attention.py:40-78, correlation.py:77-107).  A sequence
+ * is a row (axis 0, L = W) or a column (axis 1, L = H); queries, keys and values are read in place with the given pixel strides
+ * (elements, >= C).  C a multiple of 64, at most 256; 1 <= L <= PFB_ATTN1D_MAX_L.
+ *   mode PFB_ATTN1D_CORR: out[((b*H + y)*W + x)*L + l] = scale * <q[b,y,x], k[l-th pixel of the query's sequence]>  (v unused)
+ *   mode PFB_ATTN1D_ATTN: out[b,y,x, 0..C-1] (pixel stride out_stride) = softmax_l(scale * <q, k_l>) v_l, softmax in fp32, its
+ *                         weights rounded to the storage type, fp32 accumulation; the L x L scores are never stored.
+ * impl: 0 auto (wgmma with TMA loads for f16 / bf16 when C is 64, 128 or 256, the pointers are 16-byte aligned and the pixel
+ * strides multiples of 8 elements; SIMT otherwise), 1 SIMT, 2 wgmma (an error when the operands do not qualify).
+ * Launches count as kernel class 14. */
+PFB_API int pfb_attn1d(const void* q, int q_stride, const void* k, int k_stride, const void* v, int v_stride, void* out, int out_stride,
+                       int B, int H, int W, int C, int axis, int mode, float scale, pfb_dtype dtype, int impl, pfb_stream stream);
+/* The 1D lookup of both volumes (correlation.py:21-75 with exact sample positions): for d = -r..r
+ *   out[q, r + d]          = bilinear sample of corr_x[q, 0..W-1] at coords[q].x + d
+ *   out[q, 2r + 1 + r + d] = bilinear sample of corr_y[q, 0..H-1] at coords[q].y + d
+ * each tap zero outside its row (grid_sample's zero padding, align_corners = True); channels 2 (2r+1) .. out_stride - 1 are
+ * written as zero.  coords fp32 [B,H,W,2]; out [B,H,W,out_stride]; radius 1..64.  Launches count as kernel class 2 (lookup). */
+PFB_API int pfb_corr1d_lookup(const void* corr_x, const void* corr_y, const float* coords, void* out, int B, int H, int W, int radius,
+                              pfb_dtype dtype, int out_stride, pfb_stream stream);
+
+/* ------------------------------------------------------------------------------------
  * Encoder-side kernels (SURVEY.md section 8(f) rank 1: the callers either side of the path).
  * The first 7x7 convolution and the residual blocks' stride-1 3x3 convolutions of BasicEncoder (extractor.py:122-267)
  * run here, the strided, 1x1 and bottleneck convolutions in cuDNN; pre-processing, instance norm + ReLU (+ residual)
@@ -684,11 +715,12 @@ PFB_API int pfb_bias_act(const void* x, const float* bias, const void* residual,
  * kernel_class: 0 volume, 1 pool, 2 lookup, 3 on-the-fly lookup, 4 update-block conv (wgmma / SIMT), 5 upsample,
  * 6 misc (packing, coords, softmax, transposes), 7 encoder normalise / bias / activation passes, 8 encoder instance-norm
  * statistics, 9 first encoder convolution (wgmma), 10 convf1 (7x7 on the flow, wgmma), 11 flow-head tap gather,
- * 12 depthwise convolution (SKFlow), 13 depthwise convolution + LayerNorm (SEA-RAFT); -1 = all.  pfb_profile_collect synchronises
+ * 12 depthwise convolution (SKFlow), 13 depthwise convolution + LayerNorm (SEA-RAFT), 14 1D attention / correlation (Flow1D);
+ * -1 = all.  pfb_profile_collect synchronises
  * the device, writes summed milliseconds and span counts per class (arrays of >= PFB_KERNEL_CLASSES entries) and clears the
  * recorded spans.
  * ---------------------------------------------------------------------------------- */
-#define PFB_KERNEL_CLASSES 14
+#define PFB_KERNEL_CLASSES 15
 PFB_API unsigned long long pfb_launch_count(int kernel_class);
 PFB_API int pfb_profile_enable(int on);
 PFB_API int pfb_profile_collect(double* ms, unsigned long long* n, int len);

@@ -86,7 +86,9 @@ class RaftBuffers(C.Structure):
 # SKFlow (include/ptlflow_b200.h, a15)
 PFB_SK_MAX_DW = 8
 SK_CONVC1, SK_CONVC2, SK_CONVF2, SK_CONV, SK_GRU, SK_FLOW_HEAD, SK_BLOCKS = range(7)
-KERNEL_CLASSES = 14  # PFB_KERNEL_CLASSES (12 = depthwise convolution, 13 = depthwise convolution + LayerNorm)
+KERNEL_CLASSES = 15  # PFB_KERNEL_CLASSES (12 = depthwise convolution, 13 = depthwise convolution + LayerNorm, 14 = 1D attention)
+ATTN1D_CORR, ATTN1D_ATTN = 1, 2  # pfb_attn1d modes
+ATTN1D_MAX_L = 1024  # PFB_ATTN1D_MAX_L
 
 
 class PcBlock(C.Structure):
@@ -211,6 +213,9 @@ SIGNATURES = {
     "pfb_ccmr_workspace_bytes": (C.c_size_t, [C.POINTER(RaftCfg)]),
     "pfb_ccmr_refine": (_I, [C.POINTER(RaftCfg), C.POINTER(CcmrWeights), C.POINTER(RaftBuffers), C.c_float, _I, _P, _S]),
     "pfb_ccmr_update_iter": (_I, [C.POINTER(RaftCfg), C.POINTER(CcmrWeights), C.POINTER(RaftBuffers), _P, _P, C.c_float, _S]),
+    # Flow1D (a19)
+    "pfb_attn1d": (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _I, _I, _I, _I, _I, _I, C.c_float, _I, _I, _S]),
+    "pfb_corr1d_lookup": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _S]),
 }
 
 

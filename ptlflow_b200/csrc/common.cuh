@@ -113,7 +113,7 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
 }
 
 enum KernelClass { KC_VOLUME = 0, KC_POOL, KC_LOOKUP, KC_ONTHEFLY, KC_CONV, KC_UPSAMPLE, KC_MISC,
-                   KC_ENC_AFFINE, KC_ENC_STATS, KC_ENC_CONV1, KC_FLOWCONV, KC_GATHER, KC_DEPTHWISE, KC_DW_LAYERNORM, KC_COUNT };
+                   KC_ENC_AFFINE, KC_ENC_STATS, KC_ENC_CONV1, KC_FLOWCONV, KC_GATHER, KC_DEPTHWISE, KC_DW_LAYERNORM, KC_ATTN1D, KC_COUNT };
 class ProfScope {
  public:
   ProfScope(int kc, cudaStream_t s);

@@ -36,11 +36,11 @@ int launch_conv(const pfb_raft_cfg* c, cudaStream_t s, const pfb_layer& L, std::
   return pfb_conv2d(&p, (pfb_stream)s);
 }
 
-int check_loop_cfg(const pfb_raft_cfg* c, const char* name, bool levels_fit_grid) {
+int check_loop_cfg(const pfb_raft_cfg* c, const char* name, bool levels_fit_grid, int max_radius) {
   PFB_CHECK_ARG(c, "%s: null cfg", name);
   PFB_CHECK_ARG(dtype_ok(c->dtype), "%s: bad dtype %d", name, (int)c->dtype);
   PFB_CHECK_ARG(c->B > 0 && c->H > 0 && c->W > 0, "%s: bad grid %dx%dx%d", name, c->B, c->H, c->W);
-  PFB_CHECK_ARG(c->corr_levels >= 1 && c->corr_levels <= PFB_MAX_LEVELS && c->corr_radius >= 0 && c->corr_radius <= 15,
+  PFB_CHECK_ARG(c->corr_levels >= 1 && c->corr_levels <= PFB_MAX_LEVELS && c->corr_radius >= 0 && c->corr_radius <= max_radius,
                 "%s: corr_levels=%d corr_radius=%d", name, c->corr_levels, c->corr_radius);
   if (levels_fit_grid)
     PFB_CHECK_ARG((c->H >> (c->corr_levels - 1)) >= 1 && (c->W >> (c->corr_levels - 1)) >= 1, "%s: %dx%d grid too small for %d levels",
@@ -240,10 +240,10 @@ static Workspace plan(const pfb_raft_cfg* c) {
   const size_t P = (size_t)c->B * c->H * c->W;
   const size_t es = dtype_size(c->dtype);
   const int K = 2 * c->corr_radius + 1;
-  w.planes = c->corr_levels * K * K;
+  w.planes = c->variant == 7 ? 2 * K : c->corr_levels * K * K;  // flow1d: [corr_x taps | corr_y taps]
   // 16-byte aligned rows for the tensor-core path (the TMA unit zero-fills a partial last 64-channel K chunk itself)
   w.corr_stride = (c->dtype == PFB_F32) ? w.planes : (int)align_up(w.planes, 8);
-  if (c->variant == 0 || c->variant == 2 || c->variant == 5 || c->variant == 6) {
+  if (c->variant == 0 || c->variant == 2 || c->variant == 5 || c->variant == 6 || c->variant == 7) {
     w.c_cor1 = 256; w.c_cor2 = 192; w.c_flo1 = 128; w.c_flo2 = 64; w.c_fh = 256;
     // gma and ccmr keep [motion | motion_global] side by side so the GRU still sees three sources (update.py:150-151)
     w.c_motion = c->variant == 2 || c->variant == 6 ? 256 : 128;
@@ -275,14 +275,20 @@ static Workspace plan(const pfb_raft_cfg* c) {
   return w;
 }
 
-// variant 5 (ms_raft_plus) only through the pfb_msraft_* entry points, 6 (ccmr) only through the pfb_ccmr_* ones, 0..2 only through
-// the pfb_raft_* ones
+// variant 5 (ms_raft_plus) only through the pfb_msraft_* entry points, 6 (ccmr) only through the pfb_ccmr_* ones, 0..2 and 7 (flow1d)
+// only through the pfb_raft_* ones
 static int check_cfg(const pfb_raft_cfg* c, bool msraft = false, bool ccmr = false) {
   const char* name = ccmr ? "ccmr" : msraft ? "msraft" : "raft";
-  PFB_TRY(check_loop_cfg(c, name));
+  const bool flow1d = c && c->variant == 7 && !msraft && !ccmr;
+  PFB_TRY(check_loop_cfg(c, name, true, flow1d ? 64 : 15));
   if (ccmr) PFB_CHECK_ARG(c->variant == 6, "ccmr: variant=%d (the ccmr loop is variant 6)", c->variant);
   else if (msraft) PFB_CHECK_ARG(c->variant == 5, "msraft: variant=%d (the ms_raft_plus loop is variant 5)", c->variant);
-  else PFB_CHECK_ARG(c->variant >= 0 && c->variant <= 2, "raft: variant=%d", c->variant);
+  else PFB_CHECK_ARG((c->variant >= 0 && c->variant <= 2) || flow1d, "raft: variant=%d", c->variant);
+  if (flow1d)  // two 1D volumes, looked up along rows / columns of at least two pixels (flow1d/correlation.py:41, 66)
+    PFB_CHECK_ARG(c->corr_levels == 1 && c->corr_radius >= 1 && !c->alternate_corr && c->volume_layout == 0 && c->H >= 2 && c->W >= 2,
+                  "flow1d: needs corr_levels=1, corr_radius 1..64, a materialised dense volume and a grid of at least 2x2 (got levels=%d "
+                  "radius=%d alternate_corr=%d volume_layout=%d grid %dx%d)", c->corr_levels, c->corr_radius, c->alternate_corr,
+                  c->volume_layout, c->H, c->W);
   PFB_CHECK_ARG(c->num_heads >= 0 && c->num_heads <= 64 && (c->variant == 2 || heads_of(c) == 1), "%s: num_heads=%d", name, c->num_heads);
   if (c->variant != 1) PFB_CHECK_ARG(c->hidden_dim == 128 && c->context_dim == 128, "%s: the update block expects hidden=context=128", name);
   else PFB_CHECK_ARG(c->hidden_dim == 96 && c->context_dim == 64, "raft_small: SmallUpdateBlock expects hidden=96 context=64");
@@ -365,6 +371,9 @@ static int run_context_terms(const Ctx& x) {
 }
 
 static int lookup(const Ctx& x) {
+  if (x.c->variant == 7)
+    return pfb_corr1d_lookup(x.b->pyramid[0], x.b->pyramid[1], x.b->coords, x.at(x.ws.off_corr), x.c->B, x.c->H, x.c->W, x.c->corr_radius,
+                             x.c->dtype, x.ws.corr_stride, (pfb_stream)x.s);
   return raft_lookup(x.c, x.b->pyramid, x.b->fmap1, x.b->coords, x.at(x.ws.off_corr), x.ws.corr_stride, x.at(x.ws.off_flags), x.s,
                      x.corr_scale);
 }

@@ -53,9 +53,9 @@ struct ConvExtras {
 int launch_conv(const pfb_raft_cfg* c, cudaStream_t s, const pfb_layer& L, std::initializer_list<pfb_conv_src> srcs, const ConvOut& o,
                 const ConvExtras& e = ConvExtras());
 
-// The rules every loop's cfg follows (dtype, grid, levels / radius, volume_layout, iters >= 0); with `levels_fit_grid` the
-// coarsest pyramid level must keep at least one pixel.  name: the entry point family, for the messages.
-int check_loop_cfg(const pfb_raft_cfg* c, const char* name, bool levels_fit_grid = true);
+// The rules every loop's cfg follows (dtype, grid, levels / radius <= max_radius, volume_layout, iters >= 0); with `levels_fit_grid`
+// the coarsest pyramid level must keep at least one pixel.  name: the entry point family, for the messages.
+int check_loop_cfg(const pfb_raft_cfg* c, const char* name, bool levels_fit_grid = true, int max_radius = 15);
 // The state buffers, the pyramid (and fmap1 for alternate_corr) when the call looks up, and a workspace of at least `need` bytes
 int check_loop_buffers(const pfb_raft_cfg* c, const pfb_raft_buffers* buf, bool need_pyramid, size_t need, const char* name);
 

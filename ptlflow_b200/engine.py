@@ -7,6 +7,7 @@ packing, buffers, pointer structs, CUDA-graph capture.
 from __future__ import annotations
 
 import ctypes as C
+import math
 import os
 from typing import Dict, List, Optional, Sequence, Tuple
 
@@ -78,7 +79,7 @@ class RaftEngine:
         dtype, device, variant = self.dtype, self.device, self.variant
         ub = update_block
         enc, gru, fh = ub.encoder, ub.gru, ub.flow_head
-        planes = self.corr_levels * (2 * self.corr_radius + 1) ** 2
+        planes = enc.convc1.in_channels  # levels * (2r+1)^2 planes, or flow1d's 2 (2r+1)
         hd, cd = self.hidden_dim, self.context_dim
 
         def P(srcs, *convs):  # srcs: channel counts of the concatenated inputs, in order (wgmma K-major pack)
@@ -504,3 +505,69 @@ class CCMREngine(MSRaftEngine):
             check(load().pfb_xcit_context(C.byref(cfg), C.byref(self.scale_weights[scale]), inp.data_ptr(), out.data_ptr(), ws.data_ptr(),
                                           ws.numel(), stream_ptr(self.device)), "xcit_context")
         return out
+
+
+def sine_position(H: int, W: int, C: int, device) -> torch.Tensor:
+    """PositionEmbeddingSine(C // 2) of an H x W grid (flow1d/position.py), fp32 pixel-major [H, W, C]: channels 0 .. C/2-1 from the
+    row, C/2 .. C-1 from the column; inside each half sin at even and cos at odd channels of (i + 1) / (n + 1e-6) * 2 pi / dim_t,
+    dim_t[j] = 10000 ** (2 (j // 2) / (C / 2))."""
+    npf = C // 2
+    dim_t = 10000.0 ** (2 * (torch.arange(npf, dtype=torch.float32, device=device) // 2) / npf)
+
+    def half(n: int) -> torch.Tensor:  # [n, npf]
+        e = torch.arange(1, n + 1, dtype=torch.float32, device=device) / (n + 1e-6) * (2 * math.pi)
+        p = e[:, None] / dim_t
+        return torch.stack((p[:, 0::2].sin(), p[:, 1::2].cos()), dim=2).flatten(1)
+
+    return torch.cat((half(H)[:, None, :].expand(H, W, npf), half(W)[None, :, :].expand(H, W, npf)), dim=2).contiguous()
+
+
+class Flow1DEngine(RaftEngine):
+    """Flow1D (flow1d.py:148-246): RAFT's update block over the 2 (2r+1) planes of the 1D lookup, run by pfb_raft_refine as
+    pfb_raft_cfg variant 7, and, in place of the correlation pyramid, the four 1D attentions and the two 1D volumes (build_volume).
+    The attentions' query / key 1x1 convolutions are packed here; ``x + pos`` is one add in the storage type ahead of each (the
+    reference's rounding of its half model)."""
+
+    def _pack(self, update_block: torch.nn.Module, attention: Sequence[torch.nn.Module] = ()) -> _lib.RaftWeights:
+        w = super()._pack(update_block)
+        self.proj: Dict[str, ops.PackedConv] = {}
+        for axis, mod in zip("xy", attention):
+            for sub, m in (("self_", mod.self_attn), ("", mod)):
+                for kind in ("query", "key"):
+                    conv = getattr(m, kind + "_conv")
+                    self.proj[f"{axis}.{sub}{kind}"] = ops.PackedConv([conv], self.dtype, self.device, src_channels=[conv.in_channels])
+        self._pos: Dict[Tuple[int, int, int], torch.Tensor] = {}
+        return w
+
+    def position(self, H: int, W: int, C: int) -> torch.Tensor:
+        """sine_position in the storage type (computed in fp32 and rounded once), cached per grid."""
+        key = (H, W, C)
+        pos = self._pos.get(key)
+        if pos is None:
+            if len(self._pos) >= 8:
+                self._pos.pop(next(iter(self._pos)))
+            pos = self._pos[key] = sine_position(H, W, C, self.device).to(self.dtype)
+        return pos
+
+    def attention_features(self, fmap1: torch.Tensor, fmap2: torch.Tensor, impl: int = 0):
+        """(feature2_x, feature2_y) of flow1d.py:176, 184: attn_x = column self-attention of fmap1, then its row attention into fmap2;
+        attn_y = row self-attention, then column attention (attention.py:40-78).  Pixel-major [B,H,W,C] in, out."""
+        B, H, W, C = fmap1.shape
+        pos = self.position(H, W, C)
+        f1p, f2p = fmap1 + pos, fmap2 + pos
+
+        def proj(name: str, x: torch.Tensor) -> torch.Tensor:
+            return ops.conv2d([x], self.proj[name], torch.empty_like(x), impl=impl)
+
+        def attend(prefix: str, q_in: torch.Tensor, k_in: torch.Tensor, v: torch.Tensor, axis: int) -> torch.Tensor:
+            return ops.attn1d(proj(prefix + "query", q_in), proj(prefix + "key", k_in), v, axis, impl=impl)
+
+        f2_x = attend("x.", attend("x.self_", f1p, f1p, fmap1, 1) + pos, f2p, fmap2, 0)
+        f2_y = attend("y.", attend("y.self_", f1p, f1p, fmap1, 0) + pos, f2p, fmap2, 1)
+        return f2_x, f2_y
+
+    def build_volume(self, fmap1: torch.Tensor, fmap2: torch.Tensor, impl: int = 0):
+        """([corr_x [B*H*W, W], corr_y [B*H*W, H]], layout 0): corr_x of fmap1 against feature2_y along rows, corr_y against
+        feature2_x along columns, both scaled by 1/sqrt(C) (flow1d.py:177-190, correlation.py:77-107)."""
+        f2_x, f2_y = self.attention_features(fmap1, fmap2, impl)
+        return [ops.attn1d(fmap1, f2_y, None, 0, _lib.ATTN1D_CORR, impl=impl), ops.attn1d(fmap1, f2_x, None, 1, _lib.ATTN1D_CORR, impl=impl)], 0

@@ -842,3 +842,55 @@ def convex_handover2x(coords: torch.Tensor, mask: torch.Tensor) -> torch.Tensor:
         check(load().pfb_convex_handover2x(coords.data_ptr(), mask.data_ptr(), out.data_ptr(), B, H, W, dtype_code(mask.dtype),
                                            stream_ptr(coords.device)), "convex_handover2x")
     return out
+
+
+# ------------------------------------------------------------------------------------------
+# a19: Flow1D
+# ------------------------------------------------------------------------------------------
+def _pixel_stride(t: torch.Tensor, name: str) -> int:
+    """The pixel stride (elements) of a pixel-major [B,H,W,C] view whose pixels are evenly spaced (a channel slice of a wider map)."""
+    if not t.is_cuda or t.dim() != 4 or t.stride(3) != 1:
+        raise RuntimeError(f"{name} must be a CUDA [B,H,W,C] tensor with unit channel stride")
+    B, H, W, _ = t.shape
+    s = t.stride(2)
+    if (H > 1 and t.stride(1) != W * s) or (B > 1 and t.stride(0) != H * W * s):
+        raise RuntimeError(f"{name}: pixels must be evenly spaced (a channel slice of a contiguous [B,H,W,S] map)")
+    return s
+
+
+def attn1d(q: torch.Tensor, k: torch.Tensor, v: Optional[torch.Tensor], axis: int, mode: int = _lib.ATTN1D_ATTN,
+           scale: Optional[float] = None, impl: int = 0) -> torch.Tensor:
+    """Flow1D's attention / correlation along rows (axis 0) or columns (axis 1) of pixel-major [B,H,W,C] maps (pfb_attn1d).
+    mode ATTN1D_ATTN: softmax(scale q k^T) v per sequence -> [B,H,W,C];  ATTN1D_CORR: scale q k^T -> [B*H*W, L] (L = W or H).
+    ``scale`` defaults to 1/sqrt(C).  impl: 0 auto (wgmma for f16 / bf16 where the operands qualify), 1 SIMT, 2 wgmma."""
+    B, H, W, Cc = q.shape
+    if k.shape != q.shape or k.dtype != q.dtype or (v is not None and (v.shape != q.shape or v.dtype != q.dtype)):
+        raise RuntimeError("attn1d: q, k (and v) must have equal [B,H,W,C] shapes and dtypes")
+    qs, ks = _pixel_stride(q, "q"), _pixel_stride(k, "k")
+    vs = _pixel_stride(v, "v") if v is not None else 0
+    L = W if axis == 0 else H
+    out = torch.empty((B, H, W, Cc) if mode == _lib.ATTN1D_ATTN else (B * H * W, L), dtype=q.dtype, device=q.device)
+    os_ = Cc if mode == _lib.ATTN1D_ATTN else L
+    with torch.cuda.device(q.device):
+        check(load().pfb_attn1d(q.data_ptr(), qs, k.data_ptr(), ks, v.data_ptr() if v is not None else None, vs, out.data_ptr(), os_,
+                                B, H, W, Cc, int(axis), int(mode), float(Cc ** -0.5 if scale is None else scale), dtype_code(q.dtype),
+                                int(impl), stream_ptr(q.device)), "attn1d")
+    return out
+
+
+def corr1d_lookup(corr_x: torch.Tensor, corr_y: torch.Tensor, coords: torch.Tensor, radius: int,
+                  out_stride: Optional[int] = None) -> torch.Tensor:
+    """Flow1D's lookup of corr_x [B*H*W, W] and corr_y [B*H*W, H] at coords fp32 [B,H,W,2] -> [B,H,W,out_stride] in the volumes'
+    dtype: channels [x taps d = -r..r | y taps d = -r..r], zero beyond 2 (2r+1)."""
+    require_cuda(corr_x, "corr_x"); require_cuda(corr_y, "corr_y"); require_cuda(coords, "coords")
+    if coords.dtype != torch.float32 or coords.dim() != 4:
+        raise RuntimeError("corr1d_lookup: coords must be float32 [B,H,W,2]")
+    B, H, W, _ = coords.shape
+    if tuple(corr_x.shape) != (B * H * W, W) or tuple(corr_y.shape) != (B * H * W, H) or corr_x.dtype != corr_y.dtype:
+        raise RuntimeError("corr1d_lookup: corr_x [B*H*W, W] and corr_y [B*H*W, H] of one dtype")
+    stride = 2 * (2 * radius + 1) if out_stride is None else out_stride
+    out = torch.empty((B, H, W, stride), dtype=corr_x.dtype, device=coords.device)
+    with torch.cuda.device(coords.device):
+        check(load().pfb_corr1d_lookup(corr_x.data_ptr(), corr_y.data_ptr(), coords.data_ptr(), out.data_ptr(), B, H, W, radius,
+                                       dtype_code(corr_x.dtype), stride, stream_ptr(coords.device)), "corr1d_lookup")
+    return out

@@ -20,7 +20,7 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 
 CLASSES = ["volume", "pool", "lookup", "onthefly", "conv", "upsample", "misc", "enc_affine", "enc_stats", "enc_conv1", "flowconv",
-           "gather", "depthwise", "dw_layernorm"]
+           "gather", "depthwise", "dw_layernorm", "attn1d"]
 
 
 def card():
