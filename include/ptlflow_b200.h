@@ -352,6 +352,7 @@ typedef struct {
                          1 = raft_small (SmallUpdateBlock, ConvGRU, bilinear upflow8)
                          2 = gma (GMAUpdateBlock: raft + per-iteration attention aggregate, gma/update.py:127-160)
                          7 = flow1d (raft's update block over the 1D lookup of a row and a column volume, see a19)
+                         8 = csflow (raft's update block over the 4D and the cross-strip lookup, see a20)
                          (3 skflow, 4 sea_raft, 5 ms_raft_plus, 6 ccmr: their own entry points only) */
   pfb_dtype dtype;
   int B, H, W;        /* 1/8-resolution grid */
@@ -633,6 +634,38 @@ PFB_API int pfb_attn1d(const void* q, int q_stride, const void* k, int k_stride,
  * written as zero.  coords fp32 [B,H,W,2]; out [B,H,W,out_stride]; radius 1..64.  Launches count as kernel class 2 (lookup). */
 PFB_API int pfb_corr1d_lookup(const void* corr_x, const void* corr_y, const float* coords, void* out, int B, int H, int W, int radius,
                               pfb_dtype dtype, int out_stride, pfb_stream stream);
+
+/* ------------------------------------------------------------------------------------
+ * a20: CSFlow (ptlflow/models/csflow/csflow.py:116-278, 445-493): the cross-strip correlation (CSC) as a second channel of RAFT's
+ * pyramid, and the initial flow regressed from the strips.  With f1w, f1h, g2w, g2h the four ConvBNReLU 1x1 maps (csflow.py:243-258):
+ *   kw[b, x] = mean over y of g2w[b, :, x],  kh[b, y] = mean over x of g2h[b, y, :]           (pfb_strip_means)
+ *   sw[q, x2] = <f1w[q], kw[b, x2]>,  sh[q, y2] = <f1h[q], kh[b, y2]>, unscaled               (pfb_corr_volume_build_ex, scale 1,
+ *                                                                                              target grid 1 x W / H x 1)
+ *   strip channel S[q, y2, x2] = sw[q, x2] + sh[q, y2]; level l of its 2x2-pooled pyramid = A_l[x] + B_l[y], A_0 = sw[q], B_0 = sh[q],
+ *   A_{l+1}[x] = (A_l[2x] + A_l[2x+1]) / 2 (floor sizes), so it is stored as two fp32 tables per query and never in 4D.
+ * The loop is pfb_raft_refine / pfb_raft_update_iter with pfb_raft_cfg variant = 8:
+ *   corr_levels = 4, corr_radius 0..15, alternate_corr = 0, volume_layout 0 (dense) or 1 (tiled);
+ *   buf->pyramid = {the 4 levels of RAFT's volume (of that layout), tab_w, tab_h};
+ *   the lookup buffer holds 2 L (2r+1)^2 planes, [4D taps of levels 0..L-1 | strip taps of levels 0..L-1] (the reference
+ *   interleaves [4D l | strip l] per level: CONVC1's input columns are permuted to this order), pixel stride rounded up to 8;
+ *   the layers are RAFT's BasicUpdateBlock with CONVC1.Cin = 2 L (2r+1)^2; everything else is variant 0.
+ * ---------------------------------------------------------------------------------- */
+/* sum over l < levels of n >> l: the per-query width of a strip table (0 when n >> (levels - 1) < 1). */
+PFB_API int pfb_strip_table_width(int n, int levels);
+/* gw, gh [B,H,W,C] -> kw [B,W,C] (column means of gw), kh [B,H,C] (row means of gh); fp32 sums, one rounding.  Kernel class 6. */
+PFB_API int pfb_strip_means(const void* gw, const void* gh, void* kw, void* kh, int B, int H, int W, int C, pfb_dtype dtype,
+                            pfb_stream stream);
+/* sw [B*H*W][W], sh [B*H*W][H] (storage type) -> tab_w fp32 [B*H*W][pfb_strip_table_width(W, levels)] and tab_h fp32
+ * [B*H*W][pfb_strip_table_width(H, levels)]: level l at offset sum_{m<l} n >> m.  When coords (fp32 [B,H,W,2]) is not NULL it gets
+ * the initial flow of csflow.py:176-193 added in place: x += sum over y2 of sh[q], y += sum over x2 of sw[q] (both softmax calls
+ * there run over a singleton axis, so their weights are 1).  Kernel class 6. */
+PFB_API int pfb_strip_prepare(const void* sw, const void* sh, float* tab_w, float* tab_h, float* coords, int B, int H, int W, int levels,
+                              pfb_dtype dtype, pfb_stream stream);
+/* The strip channel's taps: out[q, out_offset + l (2r+1)^2 + i (2r+1) + j] = bilinear sample (zero padding, align_corners = True) of
+ * level l at (x / 2^l + i - r, y / 2^l + j - r), coords fp32 [B,H,W,2]; out [B,H,W,out_stride] in the storage type, only those
+ * levels (2r+1)^2 channels written (any offset: no alignment assumed).  radius 0..15.  Kernel class 2 (lookup). */
+PFB_API int pfb_strip_lookup(const float* tab_w, const float* tab_h, const float* coords, void* out, int B, int H, int W, int levels,
+                             int radius, pfb_dtype dtype, int out_stride, int out_offset, pfb_stream stream);
 
 /* ------------------------------------------------------------------------------------
  * Encoder-side kernels (SURVEY.md section 8(f) rank 1: the callers either side of the path).

@@ -216,6 +216,11 @@ SIGNATURES = {
     # Flow1D (a19)
     "pfb_attn1d": (_I, [_P, _I, _P, _I, _P, _I, _P, _I, _I, _I, _I, _I, _I, _I, C.c_float, _I, _I, _S]),
     "pfb_corr1d_lookup": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _S]),
+    # CSFlow (a20)
+    "pfb_strip_table_width": (_I, [_I, _I]),
+    "pfb_strip_means": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _S]),
+    "pfb_strip_prepare": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _S]),
+    "pfb_strip_lookup": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
 }
 
 

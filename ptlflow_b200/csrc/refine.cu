@@ -240,10 +240,11 @@ static Workspace plan(const pfb_raft_cfg* c) {
   const size_t P = (size_t)c->B * c->H * c->W;
   const size_t es = dtype_size(c->dtype);
   const int K = 2 * c->corr_radius + 1;
-  w.planes = c->variant == 7 ? 2 * K : c->corr_levels * K * K;  // flow1d: [corr_x taps | corr_y taps]
+  // flow1d: [corr_x taps | corr_y taps]; csflow: [4D taps of every level | strip taps of every level]
+  w.planes = c->variant == 7 ? 2 * K : (c->variant == 8 ? 2 : 1) * c->corr_levels * K * K;
   // 16-byte aligned rows for the tensor-core path (the TMA unit zero-fills a partial last 64-channel K chunk itself)
   w.corr_stride = (c->dtype == PFB_F32) ? w.planes : (int)align_up(w.planes, 8);
-  if (c->variant == 0 || c->variant == 2 || c->variant == 5 || c->variant == 6 || c->variant == 7) {
+  if (c->variant == 0 || c->variant == 2 || c->variant == 5 || c->variant == 6 || c->variant == 7 || c->variant == 8) {
     w.c_cor1 = 256; w.c_cor2 = 192; w.c_flo1 = 128; w.c_flo2 = 64; w.c_fh = 256;
     // gma and ccmr keep [motion | motion_global] side by side so the GRU still sees three sources (update.py:150-151)
     w.c_motion = c->variant == 2 || c->variant == 6 ? 256 : 128;
@@ -275,15 +276,20 @@ static Workspace plan(const pfb_raft_cfg* c) {
   return w;
 }
 
-// variant 5 (ms_raft_plus) only through the pfb_msraft_* entry points, 6 (ccmr) only through the pfb_ccmr_* ones, 0..2 and 7 (flow1d)
-// only through the pfb_raft_* ones
+// variant 5 (ms_raft_plus) only through the pfb_msraft_* entry points, 6 (ccmr) only through the pfb_ccmr_* ones, 0..2, 7 (flow1d) and
+// 8 (csflow) only through the pfb_raft_* ones
 static int check_cfg(const pfb_raft_cfg* c, bool msraft = false, bool ccmr = false) {
   const char* name = ccmr ? "ccmr" : msraft ? "msraft" : "raft";
   const bool flow1d = c && c->variant == 7 && !msraft && !ccmr;
+  const bool csflow = c && c->variant == 8 && !msraft && !ccmr;
   PFB_TRY(check_loop_cfg(c, name, true, flow1d ? 64 : 15));
   if (ccmr) PFB_CHECK_ARG(c->variant == 6, "ccmr: variant=%d (the ccmr loop is variant 6)", c->variant);
   else if (msraft) PFB_CHECK_ARG(c->variant == 5, "msraft: variant=%d (the ms_raft_plus loop is variant 5)", c->variant);
-  else PFB_CHECK_ARG((c->variant >= 0 && c->variant <= 2) || flow1d, "raft: variant=%d", c->variant);
+  else PFB_CHECK_ARG((c->variant >= 0 && c->variant <= 2) || flow1d || csflow, "raft: variant=%d", c->variant);
+  if (csflow)  // the reference's pyramid always has 4 levels (csflow.py:158, 448) and its strips need a materialised volume
+    PFB_CHECK_ARG(c->corr_levels == 4 && !c->alternate_corr && (c->volume_layout == 0 || c->volume_layout == 1),
+                  "csflow: needs corr_levels=4 and a materialised dense or tiled volume (got levels=%d alternate_corr=%d volume_layout=%d)",
+                  c->corr_levels, c->alternate_corr, c->volume_layout);
   if (flow1d)  // two 1D volumes, looked up along rows / columns of at least two pixels (flow1d/correlation.py:41, 66)
     PFB_CHECK_ARG(c->corr_levels == 1 && c->corr_radius >= 1 && !c->alternate_corr && c->volume_layout == 0 && c->H >= 2 && c->W >= 2,
                   "flow1d: needs corr_levels=1, corr_radius 1..64, a materialised dense volume and a grid of at least 2x2 (got levels=%d "
@@ -374,8 +380,14 @@ static int lookup(const Ctx& x) {
   if (x.c->variant == 7)
     return pfb_corr1d_lookup(x.b->pyramid[0], x.b->pyramid[1], x.b->coords, x.at(x.ws.off_corr), x.c->B, x.c->H, x.c->W, x.c->corr_radius,
                              x.c->dtype, x.ws.corr_stride, (pfb_stream)x.s);
-  return raft_lookup(x.c, x.b->pyramid, x.b->fmap1, x.b->coords, x.at(x.ws.off_corr), x.ws.corr_stride, x.at(x.ws.off_flags), x.s,
-                     x.corr_scale);
+  PFB_TRY(raft_lookup(x.c, x.b->pyramid, x.b->fmap1, x.b->coords, x.at(x.ws.off_corr), x.ws.corr_stride, x.at(x.ws.off_flags), x.s,
+                      x.corr_scale));
+  if (x.c->variant != 8) return PFB_OK;
+  // csflow: the 4D lookup above wrote planes 0 .. L K^2 - 1 and zero-filled the rest; the strip taps follow (a20)
+  const int L = x.c->corr_levels, K = 2 * x.c->corr_radius + 1;
+  return pfb_strip_lookup(reinterpret_cast<const float*>(x.b->pyramid[L]), reinterpret_cast<const float*>(x.b->pyramid[L + 1]),
+                          x.b->coords, x.at(x.ws.off_corr), x.c->B, x.c->H, x.c->W, L, x.c->corr_radius, x.c->dtype, x.ws.corr_stride,
+                          L * K * K, (pfb_stream)x.s);
 }
 
 // One BasicUpdateBlock / SmallUpdateBlock evaluation + coords update.  update.py:122-153

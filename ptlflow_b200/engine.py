@@ -188,6 +188,11 @@ class RaftEngine:
             return ops.corr_volume_build_tiled(fmap1, fmap2, self.corr_levels), 1
         return ops.corr_volume_build(fmap1, fmap2, self.corr_levels, impl=impl), 0
 
+    def before_loop(self, pyramid: Sequence[torch.Tensor], coords: torch.Tensor) -> Sequence[torch.Tensor]:
+        """What the loop reads, from what build_volume returned, once the engine has adjusted the start coordinates (fp32 [B,H,W,2], in
+        place) after the volume exists.  The pyramid unchanged, and no launch, for every model but CSFlow."""
+        return pyramid
+
     def _new_workspace(self, cfg: _lib.RaftCfg) -> torch.Tensor:
         nbytes = getattr(load(), self._ws_symbol)(C.byref(cfg))
         if nbytes == 0:
@@ -571,3 +576,61 @@ class Flow1DEngine(RaftEngine):
         feature2_x along columns, both scaled by 1/sqrt(C) (flow1d.py:177-190, correlation.py:77-107)."""
         f2_x, f2_y = self.attention_features(fmap1, fmap2, impl)
         return [ops.attn1d(fmap1, f2_y, None, 0, _lib.ATTN1D_CORR, impl=impl), ops.attn1d(fmap1, f2_x, None, 1, _lib.ATTN1D_CORR, impl=impl)], 0
+
+
+def fold_conv_bn_relu(block: torch.nn.Module) -> ConvWeights:
+    """A ConvBNReLU (csflow.py:299-319: a convolution without bias, then eval-mode BatchNorm) as one convolution with bias, folded in
+    fp64: w' = w s, b' = beta - mean s, s = gamma / sqrt(var + eps).  The ReLU is the convolution's epilogue."""
+    conv, bn = block.conv, block.bn
+    s = bn.weight.detach().double() / torch.sqrt(bn.running_var.detach().double() + bn.eps)
+    w = conv.weight.detach().double() * s[:, None, None, None]
+    b = bn.bias.detach().double() - bn.running_mean.detach().double() * s
+    return ConvWeights(w.float().contiguous(), b.float())
+
+
+def csflow_convc1_permutation(levels: int, radius: int) -> torch.Tensor:
+    """Column b of the lookup buffer ([4D taps of levels 0..L-1 | strip taps of levels 0..L-1]) is input column perm[b] of the
+    reference's convc1, whose input interleaves the two channels per level ([4D l | strip l], csflow.py:488-492)."""
+    kk = (2 * radius + 1) ** 2
+    t = torch.arange(kk)
+    return torch.cat([l * 2 * kk + ch * kk + t for ch in (0, 1) for l in range(levels)])
+
+
+class CSFlowEngine(RaftEngine):
+    """CSFlow (csflow.py:116-278, 445-493): RAFT's update block over [4D taps | strip taps], run by pfb_raft_refine as pfb_raft_cfg
+    variant 8.  Packs the four ConvBNReLU blocks of the strip module (BatchNorm folded) and convc1 with its input columns permuted to the
+    lookup buffer's order; build_volume adds the strip maps to RAFT's pyramid, and before_loop turns them into the separable fp32 tables
+    the loop reads while adding the initial strip flow to the coordinates."""
+
+    def _pack(self, update_block: torch.nn.Module, strip_block: Optional[torch.nn.Module] = None) -> _lib.RaftWeights:
+        w = super()._pack(update_block)
+        c1 = update_block.encoder.convc1
+        perm = csflow_convc1_permutation(self.corr_levels, self.corr_radius).to(c1.weight.device)
+        pc = ops.PackedConv([ConvWeights(c1.weight.detach()[:, perm].contiguous(), c1.bias)], self.dtype, self.device,
+                            src_channels=[c1.in_channels])
+        self.layers[_lib.L_CONVC1] = pc
+        w.layers[_lib.L_CONVC1] = pc.layer_struct()
+        self.strip = {name: ops.PackedConv([fold_conv_bn_relu(getattr(strip_block, name))], self.dtype, self.device, src_channels=[256])
+                      for name in ("conv1_1", "conv1_2", "conv2_1", "conv2_2")}
+        return w
+
+    def strip_maps(self, fmap1: torch.Tensor, fmap2: torch.Tensor, impl: int = 0):
+        """(sw [B*H*W, 1, W], sh [B*H*W, H, 1]) of StripCrossCorrMap_v2 (csflow.py:239-278), in the storage type, unscaled."""
+        def cbr(name: str, x: torch.Tensor) -> torch.Tensor:
+            return ops.conv2d([x], self.strip[name], torch.empty_like(x), _lib.EPI_RELU, impl=impl)
+
+        kw, kh = ops.strip_means(cbr("conv2_1", fmap2), cbr("conv2_2", fmap2))
+        sw = ops.corr_volume_build_ex(cbr("conv1_1", fmap1), kw, 1, scale=1.0, impl=impl)[0]
+        sh = ops.corr_volume_build_ex(cbr("conv1_2", fmap1), kh, 1, scale=1.0, impl=impl)[0]
+        return sw, sh
+
+    def build_volume(self, fmap1: torch.Tensor, fmap2: torch.Tensor, impl: int = 0):
+        """(RaftEngine's pyramid (dense or tiled) + [sw, sh], its layout)."""
+        pyr, layout = super().build_volume(fmap1, fmap2, impl)
+        return list(pyr) + list(self.strip_maps(fmap1, fmap2, impl)), layout
+
+    def before_loop(self, pyramid: Sequence[torch.Tensor], coords: torch.Tensor) -> List[torch.Tensor]:
+        L = self.corr_levels
+        _, H, W, _ = coords.shape
+        tab_w, tab_h = ops.strip_prepare(pyramid[L], pyramid[L + 1], (H, W), L, coords)
+        return list(pyramid[:L]) + [tab_w, tab_h]

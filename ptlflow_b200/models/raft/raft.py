@@ -318,6 +318,7 @@ class RAFT(BaseModel):
             pyramid, layout, f1 = ops.feature_pyramid(fmap2, self.corr_levels), 0, fmap1
         else:
             (pyramid, layout), f1 = eng.build_volume(fmap1, fmap2, impl=self.kernel_impl), None
+            pyramid = eng.before_loop(pyramid, coords)  # csflow: the strip flow joins the start coordinates
 
         orig_h, orig_w = images.shape[-2:]
         pad_top, pad_left = resizer.pad_top_left

@@ -894,3 +894,70 @@ def corr1d_lookup(corr_x: torch.Tensor, corr_y: torch.Tensor, coords: torch.Tens
         check(load().pfb_corr1d_lookup(corr_x.data_ptr(), corr_y.data_ptr(), coords.data_ptr(), out.data_ptr(), B, H, W, radius,
                                        dtype_code(corr_x.dtype), stride, stream_ptr(coords.device)), "corr1d_lookup")
     return out
+
+
+# ------------------------------------------------------------------------------------------
+# a20: CSFlow
+# ------------------------------------------------------------------------------------------
+def strip_means(gw: torch.Tensor, gh: torch.Tensor):
+    """CSFlow's strip maps of the fmap2 branch (csflow.py:253-260): gw, gh [B,H,W,C] -> (kw [B,1,W,C] column means of gw, kh [B,H,1,C]
+    row means of gh), the target grids of the two strip correlations."""
+    require_cuda(gw, "gw"); require_cuda(gh, "gh")
+    if gw.shape != gh.shape or gw.dtype != gh.dtype or gw.dim() != 4 or not gw.is_contiguous() or not gh.is_contiguous():
+        raise RuntimeError("strip_means: gw / gh must be contiguous [B,H,W,C] of one shape and dtype")
+    B, H, W, Cc = gw.shape
+    kw = torch.empty((B, 1, W, Cc), dtype=gw.dtype, device=gw.device)
+    kh = torch.empty((B, H, 1, Cc), dtype=gw.dtype, device=gw.device)
+    with torch.cuda.device(gw.device):
+        check(load().pfb_strip_means(gw.data_ptr(), gh.data_ptr(), kw.data_ptr(), kh.data_ptr(), B, H, W, Cc, dtype_code(gw.dtype),
+                                     stream_ptr(gw.device)), "strip_means")
+    return kw, kh
+
+
+def strip_table_width(n: int, levels: int) -> int:
+    """sum over l < levels of n >> l (pfb_strip_table_width)."""
+    return sum(n >> l for l in range(levels))
+
+
+def _ptr_or_none(t: Optional[torch.Tensor]):
+    return t.data_ptr() if t is not None else None
+
+
+def strip_prepare(sw: torch.Tensor, sh: torch.Tensor, grid_hw, levels: int = 4, coords: Optional[torch.Tensor] = None):
+    """CSFlow's strip maps sw [B*H*W, W] and sh [B*H*W, H] (any view of that size, e.g. the [Q,1,W] / [Q,H,1] levels of
+    corr_volume_build_ex) -> (tab_w fp32 [B*H*W, sum_l W>>l], tab_h fp32 [B*H*W, sum_l H>>l]), the separable strip pyramid.  With
+    ``coords`` (fp32 [B,H,W,2]) the initial flow (sum of sh, sum of sw) is added to it in place (csflow.py:176-193)."""
+    require_cuda(sw, "sw"); require_cuda(sh, "sh")
+    H, W = grid_hw
+    Q = sw.numel() // W
+    if sw.numel() != Q * W or sh.numel() != Q * H or Q % (H * W) or sw.dtype != sh.dtype or not sw.is_contiguous() or not sh.is_contiguous():
+        raise RuntimeError("strip_prepare: sw [B*H*W, W] and sh [B*H*W, H], contiguous, of one dtype")
+    if coords is not None and (coords.dtype != torch.float32 or tuple(coords.shape) != (Q // (H * W), H, W, 2) or not coords.is_contiguous()):
+        raise RuntimeError("strip_prepare: coords must be contiguous float32 [B,H,W,2]")
+    tw = torch.empty((Q, strip_table_width(W, levels)), dtype=torch.float32, device=sw.device)
+    th = torch.empty((Q, strip_table_width(H, levels)), dtype=torch.float32, device=sw.device)
+    with torch.cuda.device(sw.device):
+        check(load().pfb_strip_prepare(sw.data_ptr(), sh.data_ptr(), tw.data_ptr(), th.data_ptr(), _ptr_or_none(coords), Q // (H * W), H, W,
+                                       levels, dtype_code(sw.dtype), stream_ptr(sw.device)), "strip_prepare")
+    return tw, th
+
+
+def strip_lookup(tab_w: torch.Tensor, tab_h: torch.Tensor, coords: torch.Tensor, radius: int, levels: int = 4, dtype: torch.dtype = torch.float32,
+                 out: Optional[torch.Tensor] = None, out_offset: int = 0) -> torch.Tensor:
+    """The strip channel's levels * (2r+1)^2 taps at coords fp32 [B,H,W,2] -> written into ``out`` [B,H,W,S] (a new [B,H,W,planes] tensor
+    of ``dtype`` when None) at channels out_offset .., the order of corr_lookup (level, then x offset, then y offset)."""
+    require_cuda(coords, "coords")
+    if coords.dtype != torch.float32 or coords.dim() != 4 or not coords.is_contiguous():
+        raise RuntimeError("strip_lookup: coords must be contiguous float32 [B,H,W,2]")
+    B, H, W, _ = coords.shape
+    if tab_w.dtype != torch.float32 or tab_h.dtype != torch.float32 or tuple(tab_w.shape) != (B * H * W, strip_table_width(W, levels)) \
+            or tuple(tab_h.shape) != (B * H * W, strip_table_width(H, levels)):
+        raise RuntimeError("strip_lookup: tab_w / tab_h must be the fp32 tables of strip_prepare for this grid and level count")
+    if out is None:
+        out = torch.empty((B, H, W, levels * (2 * radius + 1) ** 2), dtype=dtype, device=coords.device)
+    if tuple(out.shape[:3]) != (B, H, W) or not out.is_contiguous():
+        raise RuntimeError("strip_lookup: out must be contiguous [B,H,W,S]")
+    with torch.cuda.device(coords.device):
+        check(load().pfb_strip_lookup(tab_w.data_ptr(), tab_h.data_ptr(), coords.data_ptr(), out.data_ptr(), B, H, W, levels, radius,
+                                      dtype_code(out.dtype), out.shape[-1], out_offset, stream_ptr(coords.device)), "strip_lookup")
+    return out
