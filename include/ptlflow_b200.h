@@ -284,6 +284,10 @@ PFB_API int pfb_depthwise_conv_layernorm(const void* x, int in_stride, int in_of
 PFB_API int pfb_convex_upsample(const float* coords, const void* mask, float* out, float* flow_small, int B, int H,
                         int W, int out_h, int out_w, int pad_top, int pad_left, pfb_dtype dtype,
                         pfb_stream stream);
+/* The same with a 4x convex upsample (scv.py:186-197): mask [B,H,W,144] (channel = tap * 16 + sy * 4 + sx), out the window of the
+ * 4H x 4W result of 4 * flow. */
+PFB_API int pfb_convex_upsample4x(const float* coords, const void* mask, float* out, float* flow_small, int B, int H, int W, int out_h,
+                                  int out_w, int pad_top, int pad_left, pfb_dtype dtype, pfb_stream stream);
 PFB_API int pfb_upflow8(const float* coords, float* out, float* flow_small, int B, int H, int W, int out_h, int out_w,
                 int pad_top, int pad_left, pfb_stream stream);
 
@@ -353,10 +357,11 @@ typedef struct {
                          2 = gma (GMAUpdateBlock: raft + per-iteration attention aggregate, gma/update.py:127-160)
                          7 = flow1d (raft's update block over the 1D lookup of a row and a column volume, see a19)
                          8 = csflow (raft's update block over the 4D and the cross-strip lookup, see a20)
+                         9 = scv8, 10 = scv4 (raft's update block over SCV's sparse lookup, see a21)
                          (3 skflow, 4 sea_raft, 5 ms_raft_plus, 6 ccmr: their own entry points only) */
   pfb_dtype dtype;
   int B, H, W;        /* 1/8-resolution grid */
-  int feat_dim;       /* C of fmap1/fmap2 (on-the-fly mode) */
+  int feat_dim;       /* C of fmap1/fmap2 (on-the-fly mode); variants 9 / 10: num_k, the matches per query of the sparse table */
   int corr_levels, corr_radius;
   int hidden_dim, context_dim;
   int iters;
@@ -666,6 +671,36 @@ PFB_API int pfb_strip_prepare(const void* sw, const void* sh, float* tab_w, floa
  * levels (2r+1)^2 channels written (any offset: no alignment assumed).  radius 0..15.  Kernel class 2 (lookup). */
 PFB_API int pfb_strip_lookup(const float* tab_w, const float* tab_h, const float* coords, void* out, int B, int H, int W, int levels,
                              int radius, pfb_dtype dtype, int out_stride, int out_offset, pfb_stream stream);
+
+/* ------------------------------------------------------------------------------------
+ * a21: SCV (ptlflow/models/scv/scv.py:48-83, 248-298, utils.py:148-175): the k nearest neighbours of every query by inner product,
+ * and the sparse pyramid lookup built from them.
+ *   val[q, j] = scale <f1[q], f2[t_j]> (fp32), idx[q, j] = t_j: the num_k targets of the same sample with the largest score, ordered
+ *   by score descending, ties to the lower target (pfb_knn_topk);
+ *   table[q, j] = (ty_j + wy, tx_j + wx, val[q, j]) fp32, w = coords - grid at the start of the loop (the warm start, which the
+ *   reference's displacements do not see) (pfb_sparse_prepare);
+ *   lookup at coords1: d_j = (table_y - y1, table_x - x1); for level i = 0..4 every match is splatted bilinearly (utils.py:159-162)
+ *   onto the four integer corners of d_j / 2^i; a corner with both coordinates in [-4, 4] adds weight * val to bin
+ *   i * 81 + (cy + 4) * 9 + (cx + 4) (pfb_sparse_lookup).
+ * The loop is pfb_raft_refine / pfb_raft_update_iter with pfb_raft_cfg variant 9 (scv8: 1/8 grid, 576-channel mask, convex 8x) or 10
+ * (scv4: 1/4 grid, 144-channel mask, convex 4x): corr_levels = 5, corr_radius = 4 (405 lookup planes, pixel stride rounded up to 8
+ * in f16 / bf16), alternate_corr = 0, volume_layout = 0, feat_dim = num_k, buf->pyramid = {table}; everything else is variant 0.
+ * ---------------------------------------------------------------------------------- */
+/* f1, f2 [B, N, C] pixel-major in the storage type -> val fp32 [B*N, k], idx int32 [B*N, k] (the target pixel within its sample).
+ * 1 <= k <= 32, k <= N.  The volume is never written; deterministic (the exact top-k of the scores).  impl 0: wgmma when the operands
+ * qualify (f16 / bf16, C = 64, 128, 192 or 256, 16-byte aligned), SIMT otherwise; 1: SIMT (exact fp32 FMAs, no TF32); 2: wgmma, refusing
+ * operands that do not qualify.  When the query blocks would leave SMs idle the targets are split across CTAs and the partial lists
+ * merged: the workspace holds them (pfb_knn_topk_workspace_bytes, 0 when the targets are not split).  Kernel class 0 (volume). */
+PFB_API size_t pfb_knn_topk_workspace_bytes(const void* f1, const void* f2, int B, int N, int C, int k, pfb_dtype dtype, int impl);
+PFB_API int pfb_knn_topk(const void* f1, const void* f2, float* val, int* idx, void* workspace, size_t workspace_bytes, int B, int N, int C,
+                         int k, float scale, pfb_dtype dtype, int impl, pfb_stream stream);
+/* val, idx of pfb_knn_topk on the grid H x W, coords fp32 [B,H,W,2] (x, y) -> table fp32 [B*H*W, k, 3].  Kernel class 6. */
+PFB_API int pfb_sparse_prepare(const float* val, const int* idx, const float* coords, float* table, int B, int H, int W, int k,
+                               pfb_stream stream);
+/* table, coords fp32 [B,H,W,2] -> out [B,H,W,out_stride] in the storage type: the 405 bins, zeros up to out_stride (>= 405).
+ * Deterministic (no atomics).  Kernel class 2 (lookup). */
+PFB_API int pfb_sparse_lookup(const float* table, const float* coords, void* out, int B, int H, int W, int k, pfb_dtype dtype,
+                              int out_stride, pfb_stream stream);
 
 /* ------------------------------------------------------------------------------------
  * Encoder-side kernels (SURVEY.md section 8(f) rank 1: the callers either side of the path).

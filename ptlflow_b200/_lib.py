@@ -221,6 +221,12 @@ SIGNATURES = {
     "pfb_strip_means": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _S]),
     "pfb_strip_prepare": (_I, [_P, _P, _P, _P, _P, _I, _I, _I, _I, _I, _S]),
     "pfb_strip_lookup": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
+    # SCV (a21)
+    "pfb_knn_topk_workspace_bytes": (C.c_size_t, [_P, _P, _I, _I, _I, _I, _I, _I]),
+    "pfb_knn_topk": (_I, [_P, _P, _P, _P, _P, C.c_size_t, _I, _I, _I, _I, C.c_float, _I, _I, _S]),
+    "pfb_sparse_prepare": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _S]),
+    "pfb_sparse_lookup": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _S]),
+    "pfb_convex_upsample4x": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
 }
 
 

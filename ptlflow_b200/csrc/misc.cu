@@ -166,24 +166,25 @@ __global__ void flow_small_kernel(const float* __restrict__ coords, float* __res
   flow_small[((size_t)(b * 2 + 1) * H + y) * W + x] = coords[2 * (size_t)p + 1] - (float)y;
 }
 
-// a10, convex: one thread per (coarse pixel, sy, sx); 64 threads share a coarse pixel so the nine
-// mask reads (stride 64 channels) are fully coalesced.   raft.py:112-123
-template <typename T>
+// a10, convex: one thread per (coarse pixel, sy, sx); F * F threads share a coarse pixel so the nine
+// mask reads (stride F * F channels) are fully coalesced.   raft.py:112-123 (F = 8), scv.py:186-197 (F = 4)
+template <typename T, int F>
 __global__ void __launch_bounds__(256) convex_upsample_kernel(const float* __restrict__ coords,
                                                               const T* __restrict__ mask, float* __restrict__ out,
                                                               int B, int H, int W, int OH, int OW, int pad_top,
                                                               int pad_left) {
+  constexpr int FF = F * F;
   const int P = B * H * W;
-  const int p = blockIdx.x * 4 + (threadIdx.x >> 6);
+  const int p = blockIdx.x * (256 / FF) + threadIdx.x / FF;
   if (p >= P) return;
-  const int sub = threadIdx.x & 63;
-  const int sy = sub >> 3, sx = sub & 7;
+  const int sub = threadIdx.x % FF;
+  const int sy = sub / F, sx = sub % F;
   const int x = p % W, y = (p / W) % H, b = p / (W * H);
-  const T* m = mask + (size_t)p * 576 + sub;
+  const T* m = mask + (size_t)p * 9 * FF + sub;
   float v[9], mx = -INFINITY;
 #pragma unroll
   for (int t = 0; t < 9; ++t) {
-    v[t] = to_f32(m[t * 64]);
+    v[t] = to_f32(m[t * FF]);
     mx = fmaxf(mx, v[t]);
   }
   float sum = 0.f, ax = 0.f, ay = 0.f;
@@ -194,11 +195,11 @@ __global__ void __launch_bounds__(256) convex_upsample_kernel(const float* __res
     sum += e;
     if (ny >= 0 && ny < H && nx >= 0 && nx < W) {
       const float* c = coords + 2 * ((size_t)(b * H + ny) * W + nx);
-      ax = fmaf(e, 8.f * (c[0] - (float)nx), ax);
-      ay = fmaf(e, 8.f * (c[1] - (float)ny), ay);
+      ax = fmaf(e, (float)F * (c[0] - (float)nx), ax);
+      ay = fmaf(e, (float)F * (c[1] - (float)ny), ay);
     }
   }
-  const int oy = 8 * y + sy - pad_top, ox = 8 * x + sx - pad_left;
+  const int oy = F * y + sy - pad_top, ox = F * x + sx - pad_left;
   if (oy >= 0 && oy < OH && ox >= 0 && ox < OW) {
     const float inv = 1.f / sum;
     out[((size_t)(b * 2 + 0) * OH + oy) * OW + ox] = ax * inv;
@@ -482,23 +483,35 @@ static int write_flow_small(const float* coords, float* flow_small, int B, int H
   return PFB_OK;
 }
 
-extern "C" PFB_API int pfb_convex_upsample(const float* coords, const void* mask, float* out, float* flow_small, int B,
-                                   int H, int W, int out_h, int out_w, int pad_top, int pad_left,
-                                   pfb_dtype dtype, pfb_stream stream) {
+template <int F>
+static int convex_upsample(const float* coords, const void* mask, float* out, float* flow_small, int B, int H, int W, int out_h, int out_w,
+                           int pad_top, int pad_left, pfb_dtype dtype, pfb_stream stream) {
   PFB_CHECK_ARG(coords && mask && out, "convex_upsample: null pointer");
   PFB_CHECK_ARG(dtype_ok(dtype) && B > 0 && H > 0 && W > 0, "convex_upsample: bad arguments");
-  PFB_CHECK_ARG(out_h > 0 && out_w > 0 && pad_top >= 0 && pad_left >= 0 && out_h + pad_top <= 8 * H && out_w + pad_left <= 8 * W,
-                "convex_upsample: output window %dx%d+(%d,%d) outside %dx%d", out_h, out_w, pad_top, pad_left, 8 * H, 8 * W);
+  PFB_CHECK_ARG(out_h > 0 && out_w > 0 && pad_top >= 0 && pad_left >= 0 && out_h + pad_top <= F * H && out_w + pad_left <= F * W,
+                "convex_upsample: output window %dx%d+(%d,%d) outside %dx%d", out_h, out_w, pad_top, pad_left, F * H, F * W);
   cudaStream_t s = as_stream(stream);
   const int P = B * H * W;
   {
   ProfScope prof(KC_UPSAMPLE, s);
   PFB_DISPATCH_DTYPE(dtype, T, {
-    convex_upsample_kernel<T><<<ceil_div(P, 4), 256, 0, s>>>(coords, (const T*)mask, out, B, H, W, out_h, out_w, pad_top, pad_left);
+    convex_upsample_kernel<T, F><<<ceil_div(P, 256 / (F * F)), 256, 0, s>>>(coords, (const T*)mask, out, B, H, W, out_h, out_w, pad_top,
+                                                                            pad_left);
   });
   }
   PFB_LAUNCH_CHECK();
   return write_flow_small(coords, flow_small, B, H, W, s);
+}
+
+extern "C" PFB_API int pfb_convex_upsample(const float* coords, const void* mask, float* out, float* flow_small, int B,
+                                   int H, int W, int out_h, int out_w, int pad_top, int pad_left,
+                                   pfb_dtype dtype, pfb_stream stream) {
+  return convex_upsample<8>(coords, mask, out, flow_small, B, H, W, out_h, out_w, pad_top, pad_left, dtype, stream);
+}
+
+extern "C" PFB_API int pfb_convex_upsample4x(const float* coords, const void* mask, float* out, float* flow_small, int B, int H, int W,
+                                             int out_h, int out_w, int pad_top, int pad_left, pfb_dtype dtype, pfb_stream stream) {
+  return convex_upsample<4>(coords, mask, out, flow_small, B, H, W, out_h, out_w, pad_top, pad_left, dtype, stream);
 }
 
 extern "C" PFB_API int pfb_upflow8(const float* coords, float* out, float* flow_small, int B, int H, int W, int out_h,

@@ -231,8 +231,10 @@ struct Workspace {
   int c_cor1, c_corflo, c_cor2, c_flo1, c_flo2, c_motion, c_fh;
 };
 
-// channels of the convex-upsample mask: 9 taps x 8 x 8 (raft, gma), 9 taps x 2 x 2 (ms_raft_plus, variant 5; ccmr, variant 6)
-static int mask_channels(const pfb_raft_cfg* c) { return c->variant == 5 || c->variant == 6 ? 36 : 576; }
+// channels of the convex-upsample mask: 9 taps x 8 x 8 (raft, gma), 9 taps x 2 x 2 (ms_raft_plus, variant 5; ccmr, variant 6), 9 taps x
+// 4 x 4 (scv4, variant 10)
+static int mask_channels(const pfb_raft_cfg* c) { return c->variant == 5 || c->variant == 6 ? 36 : c->variant == 10 ? 144 : 576; }
+static bool is_scv(const pfb_raft_cfg* c) { return c->variant == 9 || c->variant == 10; }
 
 static Workspace plan(const pfb_raft_cfg* c) {
   Workspace w{};
@@ -244,7 +246,7 @@ static Workspace plan(const pfb_raft_cfg* c) {
   w.planes = c->variant == 7 ? 2 * K : (c->variant == 8 ? 2 : 1) * c->corr_levels * K * K;
   // 16-byte aligned rows for the tensor-core path (the TMA unit zero-fills a partial last 64-channel K chunk itself)
   w.corr_stride = (c->dtype == PFB_F32) ? w.planes : (int)align_up(w.planes, 8);
-  if (c->variant == 0 || c->variant == 2 || c->variant == 5 || c->variant == 6 || c->variant == 7 || c->variant == 8) {
+  if (c->variant == 0 || c->variant == 2 || (c->variant >= 5 && c->variant <= 10)) {
     w.c_cor1 = 256; w.c_cor2 = 192; w.c_flo1 = 128; w.c_flo2 = 64; w.c_fh = 256;
     // gma and ccmr keep [motion | motion_global] side by side so the GRU still sees three sources (update.py:150-151)
     w.c_motion = c->variant == 2 || c->variant == 6 ? 256 : 128;
@@ -276,16 +278,23 @@ static Workspace plan(const pfb_raft_cfg* c) {
   return w;
 }
 
-// variant 5 (ms_raft_plus) only through the pfb_msraft_* entry points, 6 (ccmr) only through the pfb_ccmr_* ones, 0..2, 7 (flow1d) and
-// 8 (csflow) only through the pfb_raft_* ones
+// variant 5 (ms_raft_plus) only through the pfb_msraft_* entry points, 6 (ccmr) only through the pfb_ccmr_* ones, 0..2, 7 (flow1d),
+// 8 (csflow) and 9 / 10 (scv8 / scv4) only through the pfb_raft_* ones
 static int check_cfg(const pfb_raft_cfg* c, bool msraft = false, bool ccmr = false) {
   const char* name = ccmr ? "ccmr" : msraft ? "msraft" : "raft";
   const bool flow1d = c && c->variant == 7 && !msraft && !ccmr;
   const bool csflow = c && c->variant == 8 && !msraft && !ccmr;
-  PFB_TRY(check_loop_cfg(c, name, true, flow1d ? 64 : 15));
+  const bool scv = c && is_scv(c) && !msraft && !ccmr;
+  PFB_TRY(check_loop_cfg(c, name, !scv, flow1d ? 64 : 15));
   if (ccmr) PFB_CHECK_ARG(c->variant == 6, "ccmr: variant=%d (the ccmr loop is variant 6)", c->variant);
   else if (msraft) PFB_CHECK_ARG(c->variant == 5, "msraft: variant=%d (the ms_raft_plus loop is variant 5)", c->variant);
-  else PFB_CHECK_ARG((c->variant >= 0 && c->variant <= 2) || flow1d || csflow, "raft: variant=%d", c->variant);
+  else PFB_CHECK_ARG((c->variant >= 0 && c->variant <= 2) || flow1d || csflow || scv, "raft: variant=%d", c->variant);
+  if (scv)  // the sparse lookup's 5 levels of 9 x 9 bins (scv.py:245-260) over a table of feat_dim = num_k matches per query
+    PFB_CHECK_ARG(c->corr_levels == 5 && c->corr_radius == 4 && !c->alternate_corr && c->volume_layout == 0 && c->feat_dim >= 1 &&
+                      c->feat_dim <= 32 && c->feat_dim <= c->H * c->W,
+                  "scv: needs corr_levels=5, corr_radius=4, the sparse table (volume_layout=0) and num_k (feat_dim) in 1..min(32, H*W) "
+                  "(got levels=%d radius=%d alternate_corr=%d volume_layout=%d num_k=%d grid %dx%d)", c->corr_levels, c->corr_radius,
+                  c->alternate_corr, c->volume_layout, c->feat_dim, c->H, c->W);
   if (csflow)  // the reference's pyramid always has 4 levels (csflow.py:158, 448) and its strips need a materialised volume
     PFB_CHECK_ARG(c->corr_levels == 4 && !c->alternate_corr && (c->volume_layout == 0 || c->volume_layout == 1),
                   "csflow: needs corr_levels=4 and a materialised dense or tiled volume (got levels=%d alternate_corr=%d volume_layout=%d)",
@@ -377,6 +386,9 @@ static int run_context_terms(const Ctx& x) {
 }
 
 static int lookup(const Ctx& x) {
+  if (is_scv(x.c))
+    return pfb_sparse_lookup(reinterpret_cast<const float*>(x.b->pyramid[0]), x.b->coords, x.at(x.ws.off_corr), x.c->B, x.c->H, x.c->W,
+                             x.c->feat_dim, x.c->dtype, x.ws.corr_stride, (pfb_stream)x.s);
   if (x.c->variant == 7)
     return pfb_corr1d_lookup(x.b->pyramid[0], x.b->pyramid[1], x.b->coords, x.at(x.ws.off_corr), x.c->B, x.c->H, x.c->W, x.c->corr_radius,
                              x.c->dtype, x.ws.corr_stride, (pfb_stream)x.s);
@@ -526,6 +538,9 @@ extern "C" PFB_API int pfb_raft_refine(const pfb_raft_cfg* cfg, const pfb_raft_w
   PFB_CHECK_ARG(cfg->variant == 1 || cfg->iters >= 1, "raft_refine: the convex upsample needs at least one iteration (mask)");
   void* mask = cfg->variant != 1 ? x.at(x.ws.off_mask) : nullptr;
   PFB_TRY(run_iterations(x, mask));
+  if (cfg->variant == 10)
+    return pfb_convex_upsample4x(buf->coords, mask, buf->flow_up, buf->flow_small, cfg->B, cfg->H, cfg->W, cfg->out_h, cfg->out_w,
+                                 cfg->pad_top, cfg->pad_left, cfg->dtype, stream);
   if (cfg->variant != 1)
     return pfb_convex_upsample(buf->coords, mask, buf->flow_up, buf->flow_small, cfg->B, cfg->H, cfg->W, cfg->out_h,
                                cfg->out_w, cfg->pad_top, cfg->pad_left, cfg->dtype, stream);

@@ -634,3 +634,28 @@ class CSFlowEngine(RaftEngine):
         _, H, W, _ = coords.shape
         tab_w, tab_h = ops.strip_prepare(pyramid[L], pyramid[L + 1], (H, W), L, coords)
         return list(pyramid[:L]) + [tab_w, tab_h]
+
+
+class SCVEngine(RaftEngine):
+    """SCV (scv.py:148-500): RAFT's BasicUpdateBlock over the 405-plane sparse lookup, run by pfb_raft_refine as pfb_raft_cfg variant 9
+    (scv8) or 10 (scv4, convex 4x).  build_volume keeps the num_k best matches of every query (pfb_knn_topk, the volume never
+    materialised); before_loop turns them into the fp32 table the loop's lookup reads, with the warm start folded in."""
+
+    def _pack(self, update_block: torch.nn.Module, num_k: int = 32) -> _lib.RaftWeights:
+        self.num_k = num_k
+        self.upsample = 4 if self.variant == 10 else 8
+        return super()._pack(update_block)
+
+    def make_cfg(self, B: int, H: int, W: int, iters: int, out_hw, pad, alternate_corr: bool, feat_dim: int, volume_layout: int = 0,
+                 fork_flow: bool = False) -> _lib.RaftCfg:
+        # feat_dim carries num_k for the sparse lookup (include/ptlflow_b200.h, a21)
+        return super().make_cfg(B, H, W, iters, out_hw, pad, False, self.num_k, 0, fork_flow)
+
+    def build_volume(self, fmap1: torch.Tensor, fmap2: torch.Tensor, impl: int = 0):
+        """([val fp32 [B*N, k], idx int32 [B*N, k]], layout 0): the k-NN of compute_sparse_corr (scv.py:48-83), scaled by 1/sqrt(C)."""
+        # fp32 features have no tensor-core path: every impl runs the exact SIMT kernel, as for the convolutions
+        impl = 1 if fmap1.dtype == torch.float32 else impl
+        return list(ops.knn_topk(fmap1, fmap2, self.num_k, 1.0 / math.sqrt(fmap1.shape[-1]), impl=impl)), 0
+
+    def before_loop(self, pyramid: Sequence[torch.Tensor], coords: torch.Tensor) -> List[torch.Tensor]:
+        return [ops.sparse_prepare(pyramid[0], pyramid[1], coords)]

@@ -26,9 +26,10 @@ def _norm(kind: str, channels: int, groups: int = 8) -> nn.Module:
 
 
 class ResidualBlock(nn.Module):
-    """3x3 -> 3x3 with identity (or strided 1x1) shortcut."""
+    """3x3 -> 3x3 with identity (or strided 1x1) shortcut.  ``project``: a 1x1 convolution + norm shortcut at stride 1 too (SCV's
+    encoders, scv/extractor.py:6-59)."""
 
-    def __init__(self, in_planes: int, planes: int, norm_fn: str = "group", stride: int = 1) -> None:
+    def __init__(self, in_planes: int, planes: int, norm_fn: str = "group", stride: int = 1, project: bool = False) -> None:
         super().__init__()
         self.conv1 = nn.Conv2d(in_planes, planes, 3, stride=stride, padding=1)
         self.conv2 = nn.Conv2d(planes, planes, 3, padding=1)
@@ -36,7 +37,7 @@ class ResidualBlock(nn.Module):
         g = planes // 8
         self.norm1, self.norm2 = _norm(norm_fn, planes, g), _norm(norm_fn, planes, g)
         self.downsample = None
-        if stride != 1:
+        if stride != 1 or project:
             self.norm3 = _norm(norm_fn, planes, g)
             # the norm is shared: state_dict carries it as both norm3.* and downsample.1.* (as upstream)
             self.downsample = nn.Sequential(nn.Conv2d(in_planes, planes, 1, stride=stride), self.norm3)
@@ -127,6 +128,8 @@ def enc_conv_eligible(conv: nn.Conv2d, dtype: torch.dtype, fused_residual: bool 
 class _Encoder(nn.Module):
     block = ResidualBlock
     widths = (64, 64, 96, 128)
+    strides = (1, 2, 2)  # of layer1..3: output at 1/8
+    project_shortcut = False  # ResidualBlock(project=True) in every block
 
     def __init__(self, output_dim: int = 128, norm_fn: str = "batch", dropout: float = 0.0) -> None:
         super().__init__()
@@ -135,9 +138,9 @@ class _Encoder(nn.Module):
         self.norm1 = _norm(norm_fn, w0, 8)
         self.conv1 = nn.Conv2d(3, w0, 7, stride=2, padding=3)
         self.relu1 = nn.ReLU(inplace=True)
-        self.layer1 = self._stage(w0, w1, 1)
-        self.layer2 = self._stage(w1, w2, 2)
-        self.layer3 = self._stage(w2, w3, 2)
+        self.layer1 = self._stage(w0, w1, self.strides[0])
+        self.layer2 = self._stage(w1, w2, self.strides[1])
+        self.layer3 = self._stage(w2, w3, self.strides[2])
         self.conv2 = nn.Conv2d(w3, output_dim, 1)
         self.dropout = nn.Dropout2d(p=dropout) if dropout > 0 else None
         for m in self.modules():
@@ -148,7 +151,8 @@ class _Encoder(nn.Module):
                 nn.init.zeros_(m.bias)
 
     def _stage(self, cin: int, cout: int, stride: int) -> nn.Sequential:
-        return nn.Sequential(self.block(cin, cout, self.norm_fn, stride=stride), self.block(cout, cout, self.norm_fn, stride=1))
+        kw = {"project": True} if self.project_shortcut else {}
+        return nn.Sequential(self.block(cin, cout, self.norm_fn, stride=stride, **kw), self.block(cout, cout, self.norm_fn, stride=1, **kw))
 
     # ---- inference path: cuDNN convs + this library's fused norm / activation / residual kernels ----
     def _signature(self, dtype, device):
@@ -207,7 +211,7 @@ class _Encoder(nn.Module):
         return prep
 
     def forward_pm(self, x: torch.Tensor) -> torch.Tensor:
-        """x: pixel-major frames [N,H,W,3] on CUDA -> features [N,H/8,W/8,C] (eval semantics of
+        """x: pixel-major frames [N,H,W,3] on CUDA -> features [N,H/8,W/8,C] (H/4 with strides (1, 2, 1)) (eval semantics of
         extractor.py:171-194 / :246-267).  Batch norm is folded into the convolutions, instance norm + ReLU
         (+ residual join) is one fused pass (pfb_instance_norm_act) instead of five PyTorch kernels."""
         if self.norm_fn not in ("instance", "batch", "none"):

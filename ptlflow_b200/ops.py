@@ -961,3 +961,80 @@ def strip_lookup(tab_w: torch.Tensor, tab_h: torch.Tensor, coords: torch.Tensor,
         check(load().pfb_strip_lookup(tab_w.data_ptr(), tab_h.data_ptr(), coords.data_ptr(), out.data_ptr(), B, H, W, levels, radius,
                                       dtype_code(out.dtype), out.shape[-1], out_offset, stream_ptr(coords.device)), "strip_lookup")
     return out
+
+
+# ------------------------------------------------------------------------------------------
+# a21: SCV
+# ------------------------------------------------------------------------------------------
+SCV_PLANES = 405  # 5 levels x 9 x 9 bins of the sparse lookup
+
+
+def knn_topk(f1: torch.Tensor, f2: torch.Tensor, k: int, scale: float = 1.0, impl: int = 0):
+    """SCV's k-NN (scv.py:48-83): f1, f2 pixel-major [B,H,W,C] (or [B,N,C]) of one dtype -> (val fp32 [B*N, k] = scale * <f1[q], f2[t]>,
+    idx int32 [B*N, k] = t, the target pixel within its sample), the k largest scores of each query, descending, ties to the lower
+    target.  1 <= k <= 32, k <= N.  impl 0: wgmma where the operands qualify (f16 / bf16, C a multiple of 64 up to 256), SIMT
+    otherwise; 1: SIMT; 2: wgmma or an error."""
+    require_cuda(f1, "f1"); require_cuda(f2, "f2")
+    if f1.shape != f2.shape or f1.dtype != f2.dtype or f1.dim() not in (3, 4) or not f1.is_contiguous() or not f2.is_contiguous():
+        raise RuntimeError("knn_topk: f1 / f2 must be contiguous pixel-major tensors of one shape and dtype")
+    B, Cc = f1.shape[0], f1.shape[-1]
+    N = f1[0].numel() // Cc
+    val = torch.empty((B * N, k), dtype=torch.float32, device=f1.device)
+    idx = torch.empty((B * N, k), dtype=torch.int32, device=f1.device)
+    lib, dt = load(), dtype_code(f1.dtype)
+    with torch.cuda.device(f1.device):
+        nbytes = lib.pfb_knn_topk_workspace_bytes(f1.data_ptr(), f2.data_ptr(), B, N, Cc, k, dt, impl)
+        ws = torch.empty(nbytes, dtype=torch.uint8, device=f1.device) if nbytes else None
+        check(lib.pfb_knn_topk(f1.data_ptr(), f2.data_ptr(), val.data_ptr(), idx.data_ptr(), _ptr_or_none(ws), nbytes, B, N, Cc, k,
+                               float(scale), dt, impl, stream_ptr(f1.device)), "knn_topk")
+    return val, idx
+
+
+def sparse_prepare(val: torch.Tensor, idx: torch.Tensor, coords: torch.Tensor) -> torch.Tensor:
+    """(val, idx) of knn_topk on the grid of coords (fp32 [B,H,W,2], after the warm start) -> the fp32 table [B*H*W, k, 3] of
+    (ty + wy, tx + wx, val), w = coords - grid."""
+    require_cuda(val, "val"); require_cuda(idx, "idx"); require_cuda(coords, "coords")
+    if coords.dtype != torch.float32 or coords.dim() != 4 or not coords.is_contiguous():
+        raise RuntimeError("sparse_prepare: coords must be contiguous float32 [B,H,W,2]")
+    B, H, W, _ = coords.shape
+    k = val.shape[-1]
+    if val.dtype != torch.float32 or idx.dtype != torch.int32 or tuple(val.shape) != (B * H * W, k) or tuple(idx.shape) != (B * H * W, k) \
+            or not val.is_contiguous() or not idx.is_contiguous():
+        raise RuntimeError("sparse_prepare: val fp32 and idx int32 [B*H*W, k], contiguous")
+    table = torch.empty((B * H * W, k, 3), dtype=torch.float32, device=coords.device)
+    with torch.cuda.device(coords.device):
+        check(load().pfb_sparse_prepare(val.data_ptr(), idx.data_ptr(), coords.data_ptr(), table.data_ptr(), B, H, W, k,
+                                        stream_ptr(coords.device)), "sparse_prepare")
+    return table
+
+
+def sparse_lookup(table: torch.Tensor, coords: torch.Tensor, dtype: torch.dtype = torch.float32,
+                  out_stride: Optional[int] = None) -> torch.Tensor:
+    """SCV's per-iteration lookup (scv.py:248-298) at coords fp32 [B,H,W,2] -> [B,H,W,out_stride] of ``dtype``: the 405 bins (level, then
+    y offset, then x offset), zero beyond."""
+    require_cuda(table, "table"); require_cuda(coords, "coords")
+    if coords.dtype != torch.float32 or coords.dim() != 4 or not coords.is_contiguous():
+        raise RuntimeError("sparse_lookup: coords must be contiguous float32 [B,H,W,2]")
+    B, H, W, _ = coords.shape
+    if table.dtype != torch.float32 or table.dim() != 3 or table.shape[0] != B * H * W or table.shape[2] != 3 or not table.is_contiguous():
+        raise RuntimeError("sparse_lookup: table must be the contiguous fp32 [B*H*W, k, 3] of sparse_prepare")
+    stride = SCV_PLANES if out_stride is None else out_stride
+    out = torch.empty((B, H, W, stride), dtype=dtype, device=coords.device)
+    with torch.cuda.device(coords.device):
+        check(load().pfb_sparse_lookup(table.data_ptr(), coords.data_ptr(), out.data_ptr(), B, H, W, table.shape[1], dtype_code(dtype), stride,
+                                       stream_ptr(coords.device)), "sparse_lookup")
+    return out
+
+
+def convex_upsample4x(coords: torch.Tensor, mask: torch.Tensor, out_hw=None, pad=(0, 0)):
+    """coords fp32 [B,H,W,2], mask [B,H,W,144] -> (flow_up fp32 [B,2,oh,ow] of the convex 4x of 4 * flow, flow_small fp32 [B,2,H,W])
+    (scv.py:186-197)."""
+    require_cuda(coords, "coords"); require_cuda(mask, "mask")
+    B, H, W, _ = coords.shape
+    oh, ow = out_hw or (4 * H, 4 * W)
+    up = torch.empty((B, 2, oh, ow), dtype=torch.float32, device=coords.device)
+    small = torch.empty((B, 2, H, W), dtype=torch.float32, device=coords.device)
+    with torch.cuda.device(coords.device):
+        check(load().pfb_convex_upsample4x(coords.data_ptr(), mask.data_ptr(), up.data_ptr(), small.data_ptr(), B, H, W, oh, ow,
+                                           pad[0], pad[1], dtype_code(mask.dtype), stream_ptr(coords.device)), "convex_upsample4x")
+    return up, small
