@@ -351,17 +351,28 @@ typedef struct {
   int Cin_pad, Cout_pad_k;
 } pfb_layer;
 
+/* The refinement loop a pfb_raft_cfg describes (its `variant`).  The pfb_raft_* entry points run RAFT, RAFT_SMALL, GMA, FLOW1D,
+ * CSFLOW, SCV8 and SCV4; every other variant has entry points of its own. */
+typedef enum {
+  PFB_VARIANT_RAFT = 0,   /* BasicUpdateBlock, SepConvGRU, convex upsample */
+  PFB_VARIANT_RAFT_SMALL, /* SmallUpdateBlock, ConvGRU, bilinear upflow8 */
+  PFB_VARIANT_GMA,        /* GMAUpdateBlock: raft + per-iteration attention aggregate, gma/update.py:127-160 */
+  PFB_VARIANT_SKFLOW,     /* pfb_skflow_* (a15) */
+  PFB_VARIANT_SEA_RAFT,   /* pfb_searaft_* (a16) */
+  PFB_VARIANT_MS_RAFT_P,  /* pfb_msraft_* (a17) */
+  PFB_VARIANT_CCMR,       /* pfb_ccmr_* (a18) */
+  PFB_VARIANT_FLOW1D,     /* raft's update block over the 1D lookup of a row and a column volume (a19) */
+  PFB_VARIANT_CSFLOW,     /* raft's update block over the 4D and the cross-strip lookup (a20) */
+  PFB_VARIANT_SCV8,       /* raft's update block over SCV's sparse lookup, convex 8x (a21) */
+  PFB_VARIANT_SCV4,       /* as SCV8 on the 1/4 grid, convex 4x (a21) */
+  PFB_VARIANT_COUNT
+} pfb_variant;
+
 typedef struct {
-  int variant;        /* 0 = raft (BasicUpdateBlock, SepConvGRU, convex upsample)
-                         1 = raft_small (SmallUpdateBlock, ConvGRU, bilinear upflow8)
-                         2 = gma (GMAUpdateBlock: raft + per-iteration attention aggregate, gma/update.py:127-160)
-                         7 = flow1d (raft's update block over the 1D lookup of a row and a column volume, see a19)
-                         8 = csflow (raft's update block over the 4D and the cross-strip lookup, see a20)
-                         9 = scv8, 10 = scv4 (raft's update block over SCV's sparse lookup, see a21)
-                         (3 skflow, 4 sea_raft, 5 ms_raft_plus, 6 ccmr: their own entry points only) */
+  int variant;        /* a pfb_variant */
   pfb_dtype dtype;
   int B, H, W;        /* 1/8-resolution grid */
-  int feat_dim;       /* C of fmap1/fmap2 (on-the-fly mode); variants 9 / 10: num_k, the matches per query of the sparse table */
+  int feat_dim;       /* C of fmap1/fmap2 (on-the-fly mode); SCV8 / SCV4: num_k, the matches per query of the sparse table */
   int corr_levels, corr_radius;
   int hidden_dim, context_dim;
   int iters;
@@ -408,7 +419,7 @@ PFB_API int pfb_raft_update_iter(const pfb_raft_cfg* cfg, const pfb_raft_weights
 /* ------------------------------------------------------------------------------------
  * a15: SKFlow's refinement loop (SKUpdateBlock6_Deep_nopoolres_AllDecoder + the GMA loop)
  *   ptlflow/models/skflow/update.py:7-99, ptlflow/models/skflow/skflow.py:197-232
- * pfb_raft_cfg with variant = 3 (accepted by the pfb_skflow_* entry points only), hidden = context = 128, any num_heads;
+ * pfb_raft_cfg with variant = PFB_VARIANT_SKFLOW (accepted by the pfb_skflow_* entry points only), hidden = context = 128, any num_heads;
  * pfb_raft_buffers as for gma (attention and agg_gamma are required).
  * ---------------------------------------------------------------------------------- */
 #define PFB_SK_MAX_DW 8
@@ -454,9 +465,9 @@ PFB_API int pfb_skflow_update_iter(const pfb_raft_cfg* cfg, const pfb_skflow_wei
 /* ------------------------------------------------------------------------------------
  * a16: SEA-RAFT's refinement loop (BasicUpdateBlock of ConvNeXt blocks + the SEARAFT.forward loop)
  *   ptlflow/models/sea_raft/update.py:18-54, layer.py:41-83, sea_raft.py:189-236
- * pfb_raft_cfg with variant = 4 (accepted by the pfb_searaft_* entry points only), hidden = context = 128.  The correlation pyramid
- * is RAFT's (SEA-RAFT's per-level volumes against a bilinearly halved fmap2 are exactly the 2x2-pooled levels), so `pyramid`,
- * `fmap1` and alternate_corr mean what they mean for pfb_raft_refine.
+ * pfb_raft_cfg with variant = PFB_VARIANT_SEA_RAFT (accepted by the pfb_searaft_* entry points only), hidden = context = 128.
+ * The correlation pyramid is RAFT's (SEA-RAFT's per-level volumes against a bilinearly halved fmap2 are exactly the 2x2-pooled
+ * levels), so `pyramid`, `fmap1` and alternate_corr mean what they mean for pfb_raft_refine.
  * ---------------------------------------------------------------------------------- */
 #define PFB_SR_MAX_BLOCKS 8
 /* One ConvNextBlock(384 -> 128) on x = [net | context | motion | flow]:
@@ -496,8 +507,8 @@ PFB_API int pfb_searaft_update_iter(const pfb_raft_cfg* cfg, const pfb_searaft_w
 /* ------------------------------------------------------------------------------------
  * a17: MS-RAFT+'s four-scale refinement (ptlflow/models/ms_raft_plus/ms_raft_plus.py:146-226)
  * The scale loop runs RAFT's update block (pfb_raft_weights with CONVC1.Cin = levels*(2r+1)^2 and MASK2.Cout = 36) once per scale
- * (1/16, 1/8, 1/4, 1/2), with pfb_raft_cfg variant = 5 (accepted by the pfb_msraft_* entry points only) describing that scale's
- * grid.  pyramid / fmap1 / alternate_corr / volume_layout mean what they mean for pfb_raft_refine.
+ * (1/16, 1/8, 1/4, 1/2), with pfb_raft_cfg variant = PFB_VARIANT_MS_RAFT_P (accepted by the pfb_msraft_* entry points only)
+ * describing that scale's grid.  pyramid / fmap1 / alternate_corr / volume_layout mean what they mean for pfb_raft_refine.
  * ---------------------------------------------------------------------------------- */
 /* out [B,2H,2W,Cs+Ck] = cat[bilinear 2x (align_corners = False, edge clamped) of src [B,H,W,Cs], skip [B,2H,2W,Ck]] along the
  * channels: TF.resize + torch.cat of the encoders' up path (extractor.py:193-210).  Cs, Ck multiples of 8 (Ck may be 0, skip
@@ -593,13 +604,13 @@ typedef struct {
 } pfb_ccmr_weights;
 
 /* The whole XCiT (xcit.py:406-427) of one scale's context: x = inp + pos; x = block(x) -> out [B,H,W,128].  cfg describes the scale
- * (variant 6); workspace: pfb_ccmr_workspace_bytes(cfg). */
+ * (PFB_VARIANT_CCMR); workspace: pfb_ccmr_workspace_bytes(cfg). */
 PFB_API int pfb_xcit_context(const pfb_raft_cfg* cfg, const pfb_ccmr_weights* w, const void* inp, void* out, void* workspace,
                              size_t workspace_bytes, pfb_stream stream);
 PFB_API size_t pfb_ccmr_workspace_bytes(const pfb_raft_cfg* cfg);
-/* One scale (pfb_raft_cfg variant 6, accepted by the pfb_ccmr_* entry points only): the global context of buf->inp and the aggregator's
- * folded attention once, the GRU context terms once, cfg->iters >= 1 iterations (lookup, motion encoder, aggregator written into the
- * motion_global columns of the GRU input, GRU, flow head), the mask head on the last one.  Then either
+/* One scale (pfb_raft_cfg variant PFB_VARIANT_CCMR, accepted by the pfb_ccmr_* entry points only): the global context of buf->inp
+ * and the aggregator's folded attention once, the GRU context terms once, cfg->iters >= 1 iterations (lookup, motion encoder,
+ * aggregator written into the motion_global columns of the GRU input, GRU, flow head), the mask head on the last one.  Then either
  *   next_coords != NULL: pfb_convex_handover2x into next_coords [B,2H,2W,2], or
  *   next_coords == NULL: the convex 2x of the flow, followed by `upflow2` (0 or 1) pfb_upflow2 steps, into buf->flow_up (cfg's window
  *                        of the result) and, if buf->flow_small != NULL, pfb_downflow of it into [B,2,out_h/16,out_w/16]. */
@@ -612,11 +623,11 @@ PFB_API int pfb_ccmr_update_iter(const pfb_raft_cfg* cfg, const pfb_ccmr_weights
 
 /* ------------------------------------------------------------------------------------
  * a19: Flow1D (ptlflow/models/flow1d/flow1d.py:148-246): 1D cross-attention, a row and a column correlation volume, and RAFT's loop
- * over a 1D lookup of them.  The loop is pfb_raft_refine / pfb_raft_update_iter with pfb_raft_cfg variant = 7:
+ * over a 1D lookup of them.  The loop is pfb_raft_refine / pfb_raft_update_iter with pfb_raft_cfg variant = PFB_VARIANT_FLOW1D:
  *   corr_levels = 1, corr_radius 1..64, alternate_corr = 0, volume_layout = 0, H >= 2 and W >= 2;
  *   buf->pyramid = {corr_x, corr_y}: corr_x [B*H*W][W] and corr_y [B*H*W][H] in the storage type (pfb_attn1d mode 1);
  *   the lookup buffer holds 2 (2r+1) planes, [corr_x taps | corr_y taps], its pixel stride rounded up to 8 (f16 / bf16);
- *   the layers are RAFT's BasicUpdateBlock with CONVC1.Cin = 2 (2r+1); everything else is variant 0.
+ *   the layers are RAFT's BasicUpdateBlock with CONVC1.Cin = 2 (2r+1); everything else is PFB_VARIANT_RAFT's.
  * ---------------------------------------------------------------------------------- */
 #define PFB_ATTN1D_CORR 1
 #define PFB_ATTN1D_ATTN 2
@@ -648,12 +659,12 @@ PFB_API int pfb_corr1d_lookup(const void* corr_x, const void* corr_y, const floa
  *                                                                                              target grid 1 x W / H x 1)
  *   strip channel S[q, y2, x2] = sw[q, x2] + sh[q, y2]; level l of its 2x2-pooled pyramid = A_l[x] + B_l[y], A_0 = sw[q], B_0 = sh[q],
  *   A_{l+1}[x] = (A_l[2x] + A_l[2x+1]) / 2 (floor sizes), so it is stored as two fp32 tables per query and never in 4D.
- * The loop is pfb_raft_refine / pfb_raft_update_iter with pfb_raft_cfg variant = 8:
+ * The loop is pfb_raft_refine / pfb_raft_update_iter with pfb_raft_cfg variant = PFB_VARIANT_CSFLOW:
  *   corr_levels = 4, corr_radius 0..15, alternate_corr = 0, volume_layout 0 (dense) or 1 (tiled);
  *   buf->pyramid = {the 4 levels of RAFT's volume (of that layout), tab_w, tab_h};
  *   the lookup buffer holds 2 L (2r+1)^2 planes, [4D taps of levels 0..L-1 | strip taps of levels 0..L-1] (the reference
  *   interleaves [4D l | strip l] per level: CONVC1's input columns are permuted to this order), pixel stride rounded up to 8;
- *   the layers are RAFT's BasicUpdateBlock with CONVC1.Cin = 2 L (2r+1)^2; everything else is variant 0.
+ *   the layers are RAFT's BasicUpdateBlock with CONVC1.Cin = 2 L (2r+1)^2; everything else is PFB_VARIANT_RAFT's.
  * ---------------------------------------------------------------------------------- */
 /* sum over l < levels of n >> l: the per-query width of a strip table (0 when n >> (levels - 1) < 1). */
 PFB_API int pfb_strip_table_width(int n, int levels);
@@ -682,9 +693,10 @@ PFB_API int pfb_strip_lookup(const float* tab_w, const float* tab_h, const float
  *   lookup at coords1: d_j = (table_y - y1, table_x - x1); for level i = 0..4 every match is splatted bilinearly (utils.py:159-162)
  *   onto the four integer corners of d_j / 2^i; a corner with both coordinates in [-4, 4] adds weight * val to bin
  *   i * 81 + (cy + 4) * 9 + (cx + 4) (pfb_sparse_lookup).
- * The loop is pfb_raft_refine / pfb_raft_update_iter with pfb_raft_cfg variant 9 (scv8: 1/8 grid, 576-channel mask, convex 8x) or 10
- * (scv4: 1/4 grid, 144-channel mask, convex 4x): corr_levels = 5, corr_radius = 4 (405 lookup planes, pixel stride rounded up to 8
- * in f16 / bf16), alternate_corr = 0, volume_layout = 0, feat_dim = num_k, buf->pyramid = {table}; everything else is variant 0.
+ * The loop is pfb_raft_refine / pfb_raft_update_iter with pfb_raft_cfg variant PFB_VARIANT_SCV8 (1/8 grid, 576-channel mask,
+ * convex 8x) or PFB_VARIANT_SCV4 (1/4 grid, 144-channel mask, convex 4x): corr_levels = 5, corr_radius = 4 (405 lookup planes,
+ * pixel stride rounded up to 8 in f16 / bf16), alternate_corr = 0, volume_layout = 0, feat_dim = num_k, buf->pyramid = {table};
+ * everything else is PFB_VARIANT_RAFT's.
  * ---------------------------------------------------------------------------------- */
 /* f1, f2 [B, N, C] pixel-major in the storage type -> val fp32 [B*N, k], idx int32 [B*N, k] (the target pixel within its sample).
  * 1 <= k <= 32, k <= N.  The volume is never written; deterministic (the exact top-k of the scores).  impl 0: wgmma when the operands

@@ -30,6 +30,9 @@ ENC_CONV_LINEAR, ENC_CONV_BIAS_RELU, ENC_CONV_BIAS_RELU_RESIDUAL = range(3)
 (L_CONVC1, L_CONVC2, L_CONVF1, L_CONVF2, L_CONV, L_GRU_ZR1, L_GRU_Q1, L_GRU_ZR2, L_GRU_Q2,
  L_FLOW1, L_FLOW2, L_MASK1, L_MASK2, L_AGG_V, L_FLOW2T,
  L_CTX_ZR1, L_CTX_Q1, L_CTX_ZR2, L_CTX_Q2, L_GRUX_ZR1, L_GRUX_Q1, L_GRUX_ZR2, L_GRUX_Q2, L_CONVC2F2, L_AGG_PROJ, L_COUNT) = range(26)
+# pfb_variant: the refinement loop a RaftCfg describes
+(VARIANT_RAFT, VARIANT_RAFT_SMALL, VARIANT_GMA, VARIANT_SKFLOW, VARIANT_SEA_RAFT, VARIANT_MS_RAFT_P, VARIANT_CCMR, VARIANT_FLOW1D,
+ VARIANT_CSFLOW, VARIANT_SCV8, VARIANT_SCV4, VARIANT_COUNT) = range(12)
 
 
 class ConvSrc(C.Structure):

@@ -215,7 +215,29 @@ int check_multiscale_args(const pfb_raft_cfg* c, const pfb_raft_buffers* buf, fl
   return PFB_OK;
 }
 
-// ---- the raft / raft_small / gma / ms_raft_plus / ccmr loop ----
+// ---- the raft / raft_small / gma / ms_raft_plus / ccmr / flow1d / csflow / scv loop ----
+
+enum LoopFamily { FAMILY_RAFT, FAMILY_MSRAFT, FAMILY_CCMR };  // the pfb_raft_*, pfb_msraft_* or pfb_ccmr_* entry points
+static const char* const kFamilyName[] = {"raft", "msraft", "ccmr"};
+enum LookupKind { LOOKUP_PYRAMID, LOOKUP_1D, LOOKUP_STRIP, LOOKUP_SPARSE };  // RAFT's, flow1d's rows / columns, csflow's strips, scv's k-NN
+enum Aggregate { AGG_NONE, AGG_GMA, AGG_CCMR };  // motion_global beside motion (a 256-channel motion buffer), and by what
+struct LoopSpec {
+  LoopFamily family; LookupKind lookup; Aggregate aggregate;
+  bool small;    // SmallUpdateBlock: 96 / 64 widths, one ConvGRU half, no context terms, flow2t or mask head, SIMT only
+  int upsample;  // the convex upsample's factor (mask of 9 taps x upsample^2 channels); 0: no mask, pfb_raft_refine ends in upflow8
+};
+// What a variant's loop is made of (every per-model decision of this file reads it); null for the variants this loop does not run
+static const LoopSpec* loop_spec(int variant) {
+  static const LoopSpec raft{FAMILY_RAFT, LOOKUP_PYRAMID, AGG_NONE, false, 8}, raft_small{FAMILY_RAFT, LOOKUP_PYRAMID, AGG_NONE, true, 0},
+      gma{FAMILY_RAFT, LOOKUP_PYRAMID, AGG_GMA, false, 8}, ms_raft_p{FAMILY_MSRAFT, LOOKUP_PYRAMID, AGG_NONE, false, 2},
+      ccmr{FAMILY_CCMR, LOOKUP_PYRAMID, AGG_CCMR, false, 2}, flow1d{FAMILY_RAFT, LOOKUP_1D, AGG_NONE, false, 8},
+      csflow{FAMILY_RAFT, LOOKUP_STRIP, AGG_NONE, false, 8}, scv8{FAMILY_RAFT, LOOKUP_SPARSE, AGG_NONE, false, 8},
+      scv4{FAMILY_RAFT, LOOKUP_SPARSE, AGG_NONE, false, 4};
+  static const LoopSpec* const by_variant[PFB_VARIANT_COUNT] = {  // in pfb_variant order
+      &raft, &raft_small, &gma, nullptr /* skflow */, nullptr /* sea_raft */, &ms_raft_p, &ccmr, &flow1d, &csflow, &scv8, &scv4};
+  return (unsigned)variant < PFB_VARIANT_COUNT ? by_variant[variant] : nullptr;
+}
+static int mask_channels(const LoopSpec& sp) { return 9 * sp.upsample * sp.upsample; }
 
 struct Workspace {
   // element strides (channels per pixel) and byte offsets inside the caller's workspace
@@ -231,25 +253,22 @@ struct Workspace {
   int c_cor1, c_corflo, c_cor2, c_flo1, c_flo2, c_motion, c_fh;
 };
 
-// channels of the convex-upsample mask: 9 taps x 8 x 8 (raft, gma), 9 taps x 2 x 2 (ms_raft_plus, variant 5; ccmr, variant 6), 9 taps x
-// 4 x 4 (scv4, variant 10)
-static int mask_channels(const pfb_raft_cfg* c) { return c->variant == 5 || c->variant == 6 ? 36 : c->variant == 10 ? 144 : 576; }
-static bool is_scv(const pfb_raft_cfg* c) { return c->variant == 9 || c->variant == 10; }
-
+// of a cfg check_cfg accepted
 static Workspace plan(const pfb_raft_cfg* c) {
+  const LoopSpec& sp = *loop_spec(c->variant);
   Workspace w{};
   const size_t vdim = (size_t)heads_of(c) * 128;
   const size_t P = (size_t)c->B * c->H * c->W;
   const size_t es = dtype_size(c->dtype);
   const int K = 2 * c->corr_radius + 1;
   // flow1d: [corr_x taps | corr_y taps]; csflow: [4D taps of every level | strip taps of every level]
-  w.planes = c->variant == 7 ? 2 * K : (c->variant == 8 ? 2 : 1) * c->corr_levels * K * K;
+  w.planes = sp.lookup == LOOKUP_1D ? 2 * K : (sp.lookup == LOOKUP_STRIP ? 2 : 1) * c->corr_levels * K * K;
   // 16-byte aligned rows for the tensor-core path (the TMA unit zero-fills a partial last 64-channel K chunk itself)
   w.corr_stride = (c->dtype == PFB_F32) ? w.planes : (int)align_up(w.planes, 8);
-  if (c->variant == 0 || c->variant == 2 || (c->variant >= 5 && c->variant <= 10)) {
+  if (!sp.small) {
     w.c_cor1 = 256; w.c_cor2 = 192; w.c_flo1 = 128; w.c_flo2 = 64; w.c_fh = 256;
     // gma and ccmr keep [motion | motion_global] side by side so the GRU still sees three sources (update.py:150-151)
-    w.c_motion = c->variant == 2 || c->variant == 6 ? 256 : 128;
+    w.c_motion = sp.aggregate != AGG_NONE ? 256 : 128;
   } else {
     w.c_cor1 = 0; w.c_cor2 = 96; w.c_flo1 = 64; w.c_flo2 = 32; w.c_motion = 82; w.c_fh = 128;
   }
@@ -263,55 +282,54 @@ static Workspace plan(const pfb_raft_cfg* c) {
   w.off_z = k.take(P * (size_t)c->hidden_dim * es);
   w.off_rh = k.take(P * (size_t)c->hidden_dim * es);
   w.off_fh = k.take(P * (size_t)w.c_fh * es);
-  w.off_mh = k.take(c->variant != 1 ? P * 256 * es : 0);
-  w.off_mask = k.take(c->variant != 1 ? P * (size_t)mask_channels(c) * es : 0);
+  w.off_mh = k.take(sp.upsample ? P * 256 * es : 0);
+  w.off_mask = k.take(P * (size_t)mask_channels(sp) * es);
   w.off_flow = k.take(P * 2 * sizeof(float));
-  w.off_taps = k.take(c->variant != 1 ? P * 32 * sizeof(float) : 0);
+  w.off_taps = k.take(!sp.small ? P * 32 * sizeof(float) : 0);
   w.n_pad = (int)align_up((size_t)c->H * c->W, 64);
-  w.off_vbuf = k.take(c->variant == 2 ? P * vdim * es : 0);
-  w.off_vT = k.take(c->variant == 2 ? (size_t)c->B * vdim * w.n_pad * es : 0);
-  w.off_agg = k.take(c->variant == 2 && vdim > 128 ? P * vdim * es : 0);
+  w.off_vbuf = k.take(sp.aggregate == AGG_GMA ? P * vdim * es : 0);
+  w.off_vT = k.take(sp.aggregate == AGG_GMA ? (size_t)c->B * vdim * w.n_pad * es : 0);
+  w.off_agg = k.take(sp.aggregate == AGG_GMA && vdim > 128 ? P * vdim * es : 0);
   w.off_flags = k.take(c->alternate_corr ? P : 0);
   for (int i = 0; i < 4; ++i)
-    w.off_ctx[i] = k.take((c->variant != 1 && c->dtype != PFB_F32) ? P * (size_t)((i & 1) ? c->hidden_dim : 2 * c->hidden_dim) * es : 0);
+    w.off_ctx[i] = k.take((!sp.small && c->dtype != PFB_F32) ? P * (size_t)((i & 1) ? c->hidden_dim : 2 * c->hidden_dim) * es : 0);
   w.total = k.total;
   return w;
 }
 
-// variant 5 (ms_raft_plus) only through the pfb_msraft_* entry points, 6 (ccmr) only through the pfb_ccmr_* ones, 0..2, 7 (flow1d),
-// 8 (csflow) and 9 / 10 (scv8 / scv4) only through the pfb_raft_* ones
-static int check_cfg(const pfb_raft_cfg* c, bool msraft = false, bool ccmr = false) {
-  const char* name = ccmr ? "ccmr" : msraft ? "msraft" : "raft";
-  const bool flow1d = c && c->variant == 7 && !msraft && !ccmr;
-  const bool csflow = c && c->variant == 8 && !msraft && !ccmr;
-  const bool scv = c && is_scv(c) && !msraft && !ccmr;
-  PFB_TRY(check_loop_cfg(c, name, !scv, flow1d ? 64 : 15));
-  if (ccmr) PFB_CHECK_ARG(c->variant == 6, "ccmr: variant=%d (the ccmr loop is variant 6)", c->variant);
-  else if (msraft) PFB_CHECK_ARG(c->variant == 5, "msraft: variant=%d (the ms_raft_plus loop is variant 5)", c->variant);
-  else PFB_CHECK_ARG((c->variant >= 0 && c->variant <= 2) || flow1d || csflow || scv, "raft: variant=%d", c->variant);
-  if (scv)  // the sparse lookup's 5 levels of 9 x 9 bins (scv.py:245-260) over a table of feat_dim = num_k matches per query
-    PFB_CHECK_ARG(c->corr_levels == 5 && c->corr_radius == 4 && !c->alternate_corr && c->volume_layout == 0 && c->feat_dim >= 1 &&
-                      c->feat_dim <= 32 && c->feat_dim <= c->H * c->W,
-                  "scv: needs corr_levels=5, corr_radius=4, the sparse table (volume_layout=0) and num_k (feat_dim) in 1..min(32, H*W) "
-                  "(got levels=%d radius=%d alternate_corr=%d volume_layout=%d num_k=%d grid %dx%d)", c->corr_levels, c->corr_radius,
-                  c->alternate_corr, c->volume_layout, c->feat_dim, c->H, c->W);
-  if (csflow)  // the reference's pyramid always has 4 levels (csflow.py:158, 448) and its strips need a materialised volume
-    PFB_CHECK_ARG(c->corr_levels == 4 && !c->alternate_corr && (c->volume_layout == 0 || c->volume_layout == 1),
-                  "csflow: needs corr_levels=4 and a materialised dense or tiled volume (got levels=%d alternate_corr=%d volume_layout=%d)",
-                  c->corr_levels, c->alternate_corr, c->volume_layout);
-  if (flow1d)  // two 1D volumes, looked up along rows / columns of at least two pixels (flow1d/correlation.py:41, 66)
-    PFB_CHECK_ARG(c->corr_levels == 1 && c->corr_radius >= 1 && !c->alternate_corr && c->volume_layout == 0 && c->H >= 2 && c->W >= 2,
-                  "flow1d: needs corr_levels=1, corr_radius 1..64, a materialised dense volume and a grid of at least 2x2 (got levels=%d "
-                  "radius=%d alternate_corr=%d volume_layout=%d grid %dx%d)", c->corr_levels, c->corr_radius, c->alternate_corr,
-                  c->volume_layout, c->H, c->W);
-  PFB_CHECK_ARG(c->num_heads >= 0 && c->num_heads <= 64 && (c->variant == 2 || heads_of(c) == 1), "%s: num_heads=%d", name, c->num_heads);
-  if (c->variant != 1) PFB_CHECK_ARG(c->hidden_dim == 128 && c->context_dim == 128, "%s: the update block expects hidden=context=128", name);
+static int check_cfg(const pfb_raft_cfg* c, LoopFamily family) {
+  const char* name = kFamilyName[family];
+  PFB_CHECK_ARG(c, "%s: null cfg", name);
+  const LoopSpec* sp = loop_spec(c->variant);
+  PFB_CHECK_ARG(sp && sp->family == family, "%s: variant=%d is not a loop of the pfb_%s_* entry points", name, c->variant, name);
+  PFB_TRY(check_loop_cfg(c, name, sp->lookup != LOOKUP_SPARSE, sp->lookup == LOOKUP_1D ? 64 : 15));
+  switch (sp->lookup) {
+    case LOOKUP_SPARSE:  // 5 levels of 9 x 9 bins (scv.py:245-260) over a table of feat_dim = num_k matches per query
+      PFB_CHECK_ARG(c->corr_levels == 5 && c->corr_radius == 4 && !c->alternate_corr && c->volume_layout == 0 && c->feat_dim >= 1 &&
+                        c->feat_dim <= 32 && c->feat_dim <= c->H * c->W,
+                    "scv: needs corr_levels=5, corr_radius=4, the sparse table (volume_layout=0) and num_k (feat_dim) in 1..min(32, H*W) "
+                    "(got levels=%d radius=%d alternate_corr=%d volume_layout=%d num_k=%d grid %dx%d)", c->corr_levels, c->corr_radius,
+                    c->alternate_corr, c->volume_layout, c->feat_dim, c->H, c->W); break;
+    case LOOKUP_STRIP:  // the reference's pyramid always has 4 levels (csflow.py:158, 448) and its strips need a materialised volume
+      PFB_CHECK_ARG(c->corr_levels == 4 && !c->alternate_corr && (c->volume_layout == 0 || c->volume_layout == 1),
+                    "csflow: needs corr_levels=4 and a materialised dense or tiled volume (got levels=%d alternate_corr=%d volume_layout=%d)",
+                    c->corr_levels, c->alternate_corr, c->volume_layout); break;
+    case LOOKUP_1D:  // two 1D volumes, looked up along rows / columns of at least two pixels (flow1d/correlation.py:41, 66)
+      PFB_CHECK_ARG(c->corr_levels == 1 && c->corr_radius >= 1 && !c->alternate_corr && c->volume_layout == 0 && c->H >= 2 && c->W >= 2,
+                    "flow1d: needs corr_levels=1, corr_radius 1..64, a materialised dense volume and a grid of at least 2x2 (got levels=%d "
+                    "radius=%d alternate_corr=%d volume_layout=%d grid %dx%d)", c->corr_levels, c->corr_radius, c->alternate_corr,
+                    c->volume_layout, c->H, c->W); break;
+    case LOOKUP_PYRAMID: break;
+  }
+  PFB_CHECK_ARG(c->num_heads >= 0 && c->num_heads <= 64 && (sp->aggregate == AGG_GMA || heads_of(c) == 1), "%s: num_heads=%d", name, c->num_heads);
+  if (!sp->small) PFB_CHECK_ARG(c->hidden_dim == 128 && c->context_dim == 128, "%s: the update block expects hidden=context=128", name);
   else PFB_CHECK_ARG(c->hidden_dim == 96 && c->context_dim == 64, "raft_small: SmallUpdateBlock expects hidden=96 context=64");
   return PFB_OK;
 }
 
 struct Ctx {
   const pfb_raft_cfg* c;
+  const LoopSpec* sp;
   const pfb_raft_weights* w;
   const pfb_raft_buffers* b;
   Workspace ws;
@@ -319,7 +337,7 @@ struct Ctx {
   cudaStream_t s;
   ConvExtras e;            // every layer's GRU operands, coordinates and flow
   float corr_scale = 0.f;  // on-the-fly lookup scale (0: 1/sqrt(feat_dim))
-  const pfb_ccmr_weights* ccmr = nullptr;  // variant 6: the XCiT blocks of the scale, and their part of the workspace
+  const pfb_ccmr_weights* ccmr = nullptr;  // ccmr: the XCiT blocks of the scale, and their part of the workspace
   char* ccmr_base = nullptr;
   // flow branch of the motion encoder on a second stream (fork_flow_branch): null when not forked
   cudaStream_t side = nullptr;
@@ -335,7 +353,7 @@ static int run_conv(const Ctx& x, int layer, std::initializer_list<pfb_conv_src>
 }
 
 // round-2 restructurings of the tensor-core path; PFB_GRU_CTX_SPLIT=0 / PFB_MERGE_C2F2=0 fall back to the plain layers
-static bool tensor_path(const Ctx& x) { return x.c->variant != 1 && x.c->dtype != PFB_F32 && x.c->impl != 1; }
+static bool tensor_path(const Ctx& x) { return !x.sp->small && x.c->dtype != PFB_F32 && x.c->impl != 1; }
 static bool ctx_split_active(const Ctx& x) {
   static const int env = getenv("PFB_GRU_CTX_SPLIT") ? atoi(getenv("PFB_GRU_CTX_SPLIT")) : 1;
   return env && tensor_path(x) && x.w->layers[PFB_L_GRUX_ZR1].weight_k && x.w->layers[PFB_L_CTX_ZR1].weight_k;
@@ -386,15 +404,15 @@ static int run_context_terms(const Ctx& x) {
 }
 
 static int lookup(const Ctx& x) {
-  if (is_scv(x.c))
+  if (x.sp->lookup == LOOKUP_SPARSE)
     return pfb_sparse_lookup(reinterpret_cast<const float*>(x.b->pyramid[0]), x.b->coords, x.at(x.ws.off_corr), x.c->B, x.c->H, x.c->W,
                              x.c->feat_dim, x.c->dtype, x.ws.corr_stride, (pfb_stream)x.s);
-  if (x.c->variant == 7)
+  if (x.sp->lookup == LOOKUP_1D)
     return pfb_corr1d_lookup(x.b->pyramid[0], x.b->pyramid[1], x.b->coords, x.at(x.ws.off_corr), x.c->B, x.c->H, x.c->W, x.c->corr_radius,
                              x.c->dtype, x.ws.corr_stride, (pfb_stream)x.s);
   PFB_TRY(raft_lookup(x.c, x.b->pyramid, x.b->fmap1, x.b->coords, x.at(x.ws.off_corr), x.ws.corr_stride, x.at(x.ws.off_flags), x.s,
                       x.corr_scale));
-  if (x.c->variant != 8) return PFB_OK;
+  if (x.sp->lookup != LOOKUP_STRIP) return PFB_OK;
   // csflow: the 4D lookup above wrote planes 0 .. L K^2 - 1 and zero-filled the rest; the strip taps follow (a20)
   const int L = x.c->corr_levels, K = 2 * x.c->corr_radius + 1;
   return pfb_strip_lookup(reinterpret_cast<const float*>(x.b->pyramid[L]), reinterpret_cast<const float*>(x.b->pyramid[L + 1]),
@@ -405,6 +423,7 @@ static int lookup(const Ctx& x) {
 // One BasicUpdateBlock / SmallUpdateBlock evaluation + coords update.  update.py:122-153
 static int update_iter(const Ctx& x, const void* corr_ext, void* mask_out) {
   const pfb_raft_cfg* c = x.c;
+  const LoopSpec& sp = *x.sp;
   const Workspace& ws = x.ws;
   const pfb_layer* L = x.w->layers;
   const int hd = c->hidden_dim, cd = c->context_dim;
@@ -415,20 +434,20 @@ static int update_iter(const Ctx& x, const void* corr_ext, void* mask_out) {
   const pfb_conv_src net = src_of(x.b->net, hd, hd);
 
   // ---- motion encoder (update.py:76-112); when forked, the fork itself is in the caller, before the lookup ----
-  const MotionLayers ml{&L[PFB_L_CONVC1], c->variant != 1 ? &L[PFB_L_CONVC2] : nullptr, &L[PFB_L_CONVF1], &L[PFB_L_CONVF2], &L[PFB_L_CONV]};
+  const MotionLayers ml{&L[PFB_L_CONVC1], !sp.small ? &L[PFB_L_CONVC2] : nullptr, &L[PFB_L_CONVF1], &L[PFB_L_CONVF2], &L[PFB_L_CONV]};
   const MotionBuffers mb{x.at(ws.off_cor1), x.at(ws.off_corflo), x.at(ws.off_flo1), ws.c_cor1, ws.c_cor2, ws.c_flo1, ws.c_flo2};
   PFB_TRY(motion_encoder(c, x.s, x.e, ml, mb, src_of(corr, ws.planes, corr_stride), {PFB_EPI_RELU_APPEND_FLOW, motion, ws.c_motion, 0},
                          x.side, x.ev_join, merged_c2f2_active(x) ? &L[PFB_L_CONVC2F2] : nullptr));
 
   // ---- gma: motion_global = motion + gamma * (attention @ to_v(motion))   gma_utils.py:101-113, gma/update.py:149 ----
-  if (c->variant == 2)
+  if (sp.aggregate == AGG_GMA)
     PFB_TRY(gma_aggregate(c, L[PFB_L_AGG_V], L[PFB_L_AGG_PROJ], x.b->attention, x.b->agg_gamma, motion, ws.c_motion, 0, 128,
                           x.at(ws.off_vbuf), x.at(ws.off_vT), x.at(ws.off_agg), ws.n_pad, x.s));
   // ---- ccmr: motion_global = aggregator(global_context, motion)   ccmr/update.py:156-161 ----
-  if (c->variant == 6) PFB_TRY(ccmr_aggregate(c, x.ccmr, motion, ws.c_motion, x.ccmr_base, x.s));
+  if (sp.aggregate == AGG_CCMR) PFB_TRY(ccmr_aggregate(c, x.ccmr, motion, ws.c_motion, x.ccmr_base, x.s));
 
   // ---- GRU (update.py:24-32 ConvGRU, :58-73 SepConvGRU); x = [inp, motion (, motion_global)] ----
-  const int halves = (c->variant != 1) ? 2 : 1;
+  const int halves = sp.small ? 1 : 2;
   const bool split = ctx_split_active(x);
   const pfb_conv_src mot = src_of(motion, ws.c_motion, ws.c_motion), hr = src_of(rh, hd, hd);
   for (int h = 0; h < halves; ++h) {
@@ -446,29 +465,29 @@ static int update_iter(const Ctx& x, const void* corr_ext, void* mask_out) {
   }
 
   // ---- heads (update.py:6-14, :138-152) ----
-  const bool mask = mask_out && c->variant != 1;
+  const bool mask = mask_out && sp.upsample;
   const bool fork_mask = x.side && mask;
   if (fork_mask) {  // last iteration: the mask head beside the flow head (both read the final hidden state)
     PFB_CUDA(cudaEventRecord(x.ev_fork, x.s));
     PFB_CUDA(cudaStreamWaitEvent(x.side, x.ev_fork, 0));
-    PFB_TRY(mask_head(c, x.side, x.e, L[PFB_L_MASK1], L[PFB_L_MASK2], net, x.at(ws.off_mh), mask_out, mask_channels(c)));
+    PFB_TRY(mask_head(c, x.side, x.e, L[PFB_L_MASK1], L[PFB_L_MASK2], net, x.at(ws.off_mh), mask_out, mask_channels(sp)));
     PFB_CUDA(cudaEventRecord(x.ev_join, x.side));
   }
-  PFB_TRY(flow_head(c, x.s, x.e, L[PFB_L_FLOW1], L[PFB_L_FLOW2], c->variant != 1 ? &L[PFB_L_FLOW2T] : nullptr, net, x.at(ws.off_fh),
+  PFB_TRY(flow_head(c, x.s, x.e, L[PFB_L_FLOW1], L[PFB_L_FLOW2], !sp.small ? &L[PFB_L_FLOW2T] : nullptr, net, x.at(ws.off_fh),
                     ws.c_fh, reinterpret_cast<float*>(x.at(ws.off_taps)), reinterpret_cast<float*>(x.at(ws.off_flow))));
   if (fork_mask) PFB_CUDA(cudaStreamWaitEvent(x.s, x.ev_join, 0));  // the upsample reads the mask
-  else if (mask) PFB_TRY(mask_head(c, x.s, x.e, L[PFB_L_MASK1], L[PFB_L_MASK2], net, x.at(ws.off_mh), mask_out, mask_channels(c)));
+  else if (mask) PFB_TRY(mask_head(c, x.s, x.e, L[PFB_L_MASK1], L[PFB_L_MASK2], net, x.at(ws.off_mh), mask_out, mask_channels(sp)));
   return PFB_OK;
 }
 
 static int make_ctx(Ctx& x, const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf,
-                    cudaStream_t s, bool need_pyramid, bool msraft = false, bool ccmr = false) {
-  PFB_TRY(check_cfg(cfg, msraft, ccmr));
-  const char* name = ccmr ? "ccmr" : msraft ? "msraft" : "raft";
+                    cudaStream_t s, bool need_pyramid, LoopFamily family) {
+  PFB_TRY(check_cfg(cfg, family));
+  const char* name = kFamilyName[family];
   PFB_CHECK_ARG(w, "%s: null weights", name);
-  x.c = cfg; x.w = w; x.b = buf; x.s = s;
+  x.c = cfg; x.sp = loop_spec(cfg->variant); x.w = w; x.b = buf; x.s = s;
   x.ws = plan(cfg);
-  PFB_TRY(check_loop_buffers(cfg, buf, need_pyramid, x.ws.total + (ccmr ? ccmr_plan(cfg).total : 0), name));
+  PFB_TRY(check_loop_buffers(cfg, buf, need_pyramid, x.ws.total + (family == FAMILY_CCMR ? ccmr_plan(cfg).total : 0), name));
   x.base = reinterpret_cast<char*>(buf->workspace);
   x.e.aux_h = buf->net; x.e.aux_z = x.at(x.ws.off_z); x.e.hidden = cfg->hidden_dim;
   x.e.coords = buf->coords; x.e.flow = reinterpret_cast<const float*>(x.at(x.ws.off_flow));
@@ -480,9 +499,9 @@ static int make_ctx(Ctx& x, const pfb_raft_cfg* cfg, const pfb_raft_weights* w, 
 using namespace pfb;
 
 // the workspace of the msraft / ccmr / raft entry points (ccmr's holds its XCiT plan after the loop's); 0 for a cfg they refuse
-static size_t workspace_bytes(const pfb_raft_cfg* cfg, bool msraft, bool ccmr) {
-  if (check_cfg(cfg, msraft, ccmr) != PFB_OK) return 0;
-  return plan(cfg).total + (ccmr ? ccmr_plan(cfg).total : 0);
+static size_t workspace_bytes(const pfb_raft_cfg* cfg, LoopFamily family) {
+  if (check_cfg(cfg, family) != PFB_OK) return 0;
+  return plan(cfg).total + (family == FAMILY_CCMR ? ccmr_plan(cfg).total : 0);
 }
 
 // one update-block evaluation from the entry coordinates, on a built context: the flow, the context terms, the lookup unless the
@@ -494,12 +513,12 @@ static int update_iter_once(Ctx& x, const void* corr, void* mask_out) {
   return update_iter(x, corr, mask_out);
 }
 
-extern "C" PFB_API size_t pfb_raft_workspace_bytes(const pfb_raft_cfg* cfg) { return workspace_bytes(cfg, false, false); }
+extern "C" PFB_API size_t pfb_raft_workspace_bytes(const pfb_raft_cfg* cfg) { return workspace_bytes(cfg, FAMILY_RAFT); }
 
 extern "C" PFB_API int pfb_raft_update_iter(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf,
                                     const void* corr, void* mask_out, pfb_stream stream) {
   Ctx x;
-  PFB_TRY(make_ctx(x, cfg, w, buf, as_stream(stream), corr == nullptr));
+  PFB_TRY(make_ctx(x, cfg, w, buf, as_stream(stream), corr == nullptr, FAMILY_RAFT));
   return update_iter_once(x, corr, mask_out);
 }
 
@@ -533,15 +552,15 @@ static int run_iterations(Ctx& x, void* mask) {
 extern "C" PFB_API int pfb_raft_refine(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf,
                                pfb_stream stream) {
   Ctx x;
-  PFB_TRY(make_ctx(x, cfg, w, buf, as_stream(stream), true));
+  PFB_TRY(make_ctx(x, cfg, w, buf, as_stream(stream), true, FAMILY_RAFT));
   PFB_CHECK_ARG(buf->flow_up, "raft_refine: null flow_up");
-  PFB_CHECK_ARG(cfg->variant == 1 || cfg->iters >= 1, "raft_refine: the convex upsample needs at least one iteration (mask)");
-  void* mask = cfg->variant != 1 ? x.at(x.ws.off_mask) : nullptr;
+  PFB_CHECK_ARG(!x.sp->upsample || cfg->iters >= 1, "raft_refine: the convex upsample needs at least one iteration (mask)");
+  void* mask = x.sp->upsample ? x.at(x.ws.off_mask) : nullptr;
   PFB_TRY(run_iterations(x, mask));
-  if (cfg->variant == 10)
+  if (x.sp->upsample == 4)
     return pfb_convex_upsample4x(buf->coords, mask, buf->flow_up, buf->flow_small, cfg->B, cfg->H, cfg->W, cfg->out_h, cfg->out_w,
                                  cfg->pad_top, cfg->pad_left, cfg->dtype, stream);
-  if (cfg->variant != 1)
+  if (x.sp->upsample == 8)
     return pfb_convex_upsample(buf->coords, mask, buf->flow_up, buf->flow_small, cfg->B, cfg->H, cfg->W, cfg->out_h,
                                cfg->out_w, cfg->pad_top, cfg->pad_left, cfg->dtype, stream);
   return pfb_upflow8(buf->coords, buf->flow_up, buf->flow_small, cfg->B, cfg->H, cfg->W, cfg->out_h, cfg->out_w,
@@ -549,12 +568,12 @@ extern "C" PFB_API int pfb_raft_refine(const pfb_raft_cfg* cfg, const pfb_raft_w
 }
 
 // ---- a17: MS-RAFT+ (one call per scale of ms_raft_plus.py:177-214) ----
-extern "C" PFB_API size_t pfb_msraft_workspace_bytes(const pfb_raft_cfg* cfg) { return workspace_bytes(cfg, true, false); }
+extern "C" PFB_API size_t pfb_msraft_workspace_bytes(const pfb_raft_cfg* cfg) { return workspace_bytes(cfg, FAMILY_MSRAFT); }
 
 extern "C" PFB_API int pfb_msraft_update_iter(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf,
                                               const void* corr, void* mask_out, float corr_scale, pfb_stream stream) {
   Ctx x;
-  PFB_TRY(make_ctx(x, cfg, w, buf, as_stream(stream), corr == nullptr, true));
+  PFB_TRY(make_ctx(x, cfg, w, buf, as_stream(stream), corr == nullptr, FAMILY_MSRAFT));
   PFB_CHECK_ARG(corr_scale >= 0.f, "msraft_update_iter: corr_scale=%g", (double)corr_scale);
   x.corr_scale = corr_scale;
   return update_iter_once(x, corr, mask_out);
@@ -563,7 +582,7 @@ extern "C" PFB_API int pfb_msraft_update_iter(const pfb_raft_cfg* cfg, const pfb
 extern "C" PFB_API int pfb_msraft_refine(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf, float corr_scale,
                                          float* next_coords, pfb_stream stream) {
   Ctx x;
-  PFB_TRY(make_ctx(x, cfg, w, buf, as_stream(stream), true, true));
+  PFB_TRY(make_ctx(x, cfg, w, buf, as_stream(stream), true, FAMILY_MSRAFT));
   PFB_TRY(check_multiscale_args(cfg, buf, corr_scale, next_coords, 0, "msraft_refine"));
   x.corr_scale = corr_scale;
   void* mask = x.at(x.ws.off_mask);
@@ -575,12 +594,12 @@ extern "C" PFB_API int pfb_msraft_refine(const pfb_raft_cfg* cfg, const pfb_raft
 }
 
 // ---- a18: CCMR / CCMR+ (one call per scale of ccmr.py:179-220) ----
-extern "C" PFB_API size_t pfb_ccmr_workspace_bytes(const pfb_raft_cfg* cfg) { return workspace_bytes(cfg, false, true); }
+extern "C" PFB_API size_t pfb_ccmr_workspace_bytes(const pfb_raft_cfg* cfg) { return workspace_bytes(cfg, FAMILY_CCMR); }
 
 static int make_ccmr_ctx(Ctx& x, const pfb_raft_cfg* cfg, const pfb_ccmr_weights* w, const pfb_raft_buffers* buf, cudaStream_t s,
                          bool need_pyramid, float corr_scale) {
   PFB_CHECK_ARG(w, "ccmr: null weights");
-  PFB_TRY(make_ctx(x, cfg, &w->raft, buf, s, need_pyramid, false, true));
+  PFB_TRY(make_ctx(x, cfg, &w->raft, buf, s, need_pyramid, FAMILY_CCMR));
   PFB_CHECK_ARG(cfg->context_dim == 128, "ccmr: the XCiT blocks expect 128 context channels");
   x.corr_scale = corr_scale;
   x.ccmr = w;
@@ -591,7 +610,7 @@ static int make_ccmr_ctx(Ctx& x, const pfb_raft_cfg* cfg, const pfb_ccmr_weights
 extern "C" PFB_API int pfb_xcit_context(const pfb_raft_cfg* cfg, const pfb_ccmr_weights* w, const void* inp, void* out, void* workspace,
                                         size_t workspace_bytes, pfb_stream stream) {
   PFB_CHECK_ARG(cfg && w && inp && out && workspace, "xcit_context: null pointer");
-  PFB_TRY(check_cfg(cfg, false, true));
+  PFB_TRY(check_cfg(cfg, FAMILY_CCMR));
   const size_t off = plan(cfg).total, need = off + ccmr_plan(cfg).total;
   PFB_CHECK_ARG(workspace_bytes >= need, "xcit_context: workspace %zu bytes < required %zu", workspace_bytes, need);
   return ccmr_scale_setup(cfg, w, inp, out, false, reinterpret_cast<char*>(workspace) + off, as_stream(stream));

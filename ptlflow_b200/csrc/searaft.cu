@@ -49,7 +49,7 @@ SrWs plan(const pfb_raft_cfg* c) {
 
 int check_cfg(const pfb_raft_cfg* c) {
   PFB_TRY(check_loop_cfg(c, "searaft", c && c->iters > 0));  // iters = 0 looks nothing up
-  PFB_CHECK_ARG(c->variant == 4, "searaft: variant=%d (the sea_raft loop is variant 4)", c->variant);
+  PFB_CHECK_ARG(c->variant == PFB_VARIANT_SEA_RAFT, "searaft: variant=%d (the sea_raft loop is PFB_VARIANT_SEA_RAFT)", c->variant);
   PFB_CHECK_ARG(c->hidden_dim == 128 && c->context_dim == 128, "searaft: the update block expects hidden=context=128");
   return PFB_OK;
 }

@@ -55,7 +55,7 @@ SkWs plan(const pfb_raft_cfg* c) {
 
 int check_cfg(const pfb_raft_cfg* c) {
   PFB_TRY(check_loop_cfg(c, "skflow"));
-  PFB_CHECK_ARG(c->variant == 3, "skflow: variant=%d (the skflow loop is variant 3)", c->variant);
+  PFB_CHECK_ARG(c->variant == PFB_VARIANT_SKFLOW, "skflow: variant=%d (the skflow loop is PFB_VARIANT_SKFLOW)", c->variant);
   PFB_CHECK_ARG(c->hidden_dim == 128 && c->context_dim == 128, "skflow: the update block expects hidden=context=128");
   PFB_CHECK_ARG(c->num_heads >= 0 && c->num_heads <= 64, "skflow: num_heads=%d", c->num_heads);
   return PFB_OK;

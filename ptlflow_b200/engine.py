@@ -87,14 +87,14 @@ class RaftEngine:
 
         layers: Dict[int, ops.PackedConv] = {}
         layers[_lib.L_CONVF1] = _pack_convf1(enc.convf1, dtype, device)
-        if variant != 1:
+        if variant != _lib.VARIANT_RAFT_SMALL:
             layers[_lib.L_CONVC1] = P([planes], enc.convc1)
             layers[_lib.L_CONVC2] = P([256], enc.convc2)
             layers[_lib.L_CONVF2] = P([128], enc.convf2)
             layers[_lib.L_CONV] = P([256], enc.conv)  # cat[cor(192), flo(64)] lives in one 256-channel buffer
             # cat[h or r*h, inp, motion (, motion_global)] -- three tensor maps, no concat copy (gma keeps
-            # motion | motion_global in one 256-channel buffer, and so does ccmr)
-            gsrc = [hd, cd, 256 if variant in (2, 6) else 128]
+            # motion | motion_global in one 256-channel buffer, and so does ccmr: the GRU's input beyond [h | inp])
+            gsrc = [hd, cd, gru.convz1.in_channels - hd - cd]
             layers[_lib.L_GRU_ZR1] = P(gsrc, gru.convz1, gru.convr1)  # z | r share the input: one GEMM, N = 2*hidden
             layers[_lib.L_GRU_Q1] = P(gsrc, gru.convq1)
             layers[_lib.L_GRU_ZR2] = P(gsrc, gru.convz2, gru.convr2)
@@ -136,7 +136,7 @@ class RaftEngine:
             layers[_lib.L_FLOW1] = P(None, fh.conv1)
             layers[_lib.L_FLOW2] = P(None, fh.conv2)
         self.att_q = self.att_k = self.att_pos = None
-        if variant == 2:
+        if variant == _lib.VARIANT_GMA:
             layers[_lib.L_AGG_V], proj = self._pack_attention(ub.aggregator, attention_module)
             if proj is not None:
                 layers[_lib.L_AGG_PROJ] = proj
@@ -261,7 +261,8 @@ class RaftEngine:
         up = self.upsample
         cfg = self.make_cfg(B, H, W, 1, (up * H, up * W), (0, 0), fmap1 is not None, fmap1.shape[-1] if fmap1 is not None else 0)
         ws = self.workspace(cfg)
-        mask = torch.empty((B, H, W, 9 * up * up), dtype=self.dtype, device=self.device) if want_mask and self.variant != 1 else None
+        has_mask = want_mask and self.variant != _lib.VARIANT_RAFT_SMALL  # SmallUpdateBlock has no mask head
+        mask = torch.empty((B, H, W, 9 * up * up), dtype=self.dtype, device=self.device) if has_mask else None
         self._call(self._iter_symbol, cfg, self._scale_weights(scale), ws, pyramid, net, inp, coords, _ptr(corr), _ptr(mask),
                    *self._iter_args(corr_scale), fmap1=fmap1, attention=attention)
         return mask
@@ -395,7 +396,7 @@ class SEARaftEngine(RaftEngine):
 class MSRaftEngine(RaftEngine):
     """MS-RAFT+'s update block (ms_raft_plus/update.py:119-153: RAFT's BasicUpdateBlock with convc1 over levels * (2r+1)^2 planes and
     a 36-channel mask head) packed exactly as RaftEngine packs raft's, driven one scale at a time through pfb_msraft_refine
-    (pfb_raft_cfg variant 5)."""
+    (pfb_raft_cfg variant VARIANT_MS_RAFT_P, 5)."""
 
     _ws_symbol, _refine_symbol, _iter_symbol = "pfb_msraft_workspace_bytes", "pfb_msraft_refine", "pfb_msraft_update_iter"
     upsample = 2
@@ -430,7 +431,7 @@ class CCMREngine(MSRaftEngine):
     as RaftEngine packs gma's, plus per scale the XCiT of the context (``xcit[i]``) and the aggregator (``update_block.aggregator[i]``)
     as pfb_xcit_block descriptors, folded in fp64 (xcit.py:242-300): norm1's affine into q | k and v, gamma1 into proj, gamma3 into
     LPI's second convolution, norm2's affine into fc1 and gamma2 into fc2.  Driven one scale at a time through pfb_ccmr_refine
-    (pfb_raft_cfg variant 6)."""
+    (pfb_raft_cfg variant VARIANT_CCMR, 6)."""
 
     _ws_symbol, _refine_symbol, _iter_symbol = "pfb_ccmr_workspace_bytes", "pfb_ccmr_refine", "pfb_ccmr_update_iter"
 
@@ -529,7 +530,8 @@ def sine_position(H: int, W: int, C: int, device) -> torch.Tensor:
 
 class Flow1DEngine(RaftEngine):
     """Flow1D (flow1d.py:148-246): RAFT's update block over the 2 (2r+1) planes of the 1D lookup, run by pfb_raft_refine as
-    pfb_raft_cfg variant 7, and, in place of the correlation pyramid, the four 1D attentions and the two 1D volumes (build_volume).
+    pfb_raft_cfg variant VARIANT_FLOW1D (7), and, in place of the correlation pyramid, the four 1D attentions and the two 1D volumes
+    (build_volume).
     The attentions' query / key 1x1 convolutions are packed here; ``x + pos`` is one add in the storage type ahead of each (the
     reference's rounding of its half model)."""
 
@@ -598,9 +600,9 @@ def csflow_convc1_permutation(levels: int, radius: int) -> torch.Tensor:
 
 class CSFlowEngine(RaftEngine):
     """CSFlow (csflow.py:116-278, 445-493): RAFT's update block over [4D taps | strip taps], run by pfb_raft_refine as pfb_raft_cfg
-    variant 8.  Packs the four ConvBNReLU blocks of the strip module (BatchNorm folded) and convc1 with its input columns permuted to the
-    lookup buffer's order; build_volume adds the strip maps to RAFT's pyramid, and before_loop turns them into the separable fp32 tables
-    the loop reads while adding the initial strip flow to the coordinates."""
+    variant VARIANT_CSFLOW (8).  Packs the four ConvBNReLU blocks of the strip module (BatchNorm folded) and convc1 with its input
+    columns permuted to the lookup buffer's order; build_volume adds the strip maps to RAFT's pyramid, and before_loop turns them into
+    the separable fp32 tables the loop reads while adding the initial strip flow to the coordinates."""
 
     def _pack(self, update_block: torch.nn.Module, strip_block: Optional[torch.nn.Module] = None) -> _lib.RaftWeights:
         w = super()._pack(update_block)
@@ -637,13 +639,13 @@ class CSFlowEngine(RaftEngine):
 
 
 class SCVEngine(RaftEngine):
-    """SCV (scv.py:148-500): RAFT's BasicUpdateBlock over the 405-plane sparse lookup, run by pfb_raft_refine as pfb_raft_cfg variant 9
-    (scv8) or 10 (scv4, convex 4x).  build_volume keeps the num_k best matches of every query (pfb_knn_topk, the volume never
-    materialised); before_loop turns them into the fp32 table the loop's lookup reads, with the warm start folded in."""
+    """SCV (scv.py:148-500): RAFT's BasicUpdateBlock over the 405-plane sparse lookup, run by pfb_raft_refine as pfb_raft_cfg variant
+    VARIANT_SCV8 (9) or VARIANT_SCV4 (10, convex 4x).  build_volume keeps the num_k best matches of every query (pfb_knn_topk, the
+    volume never materialised); before_loop turns them into the fp32 table the loop's lookup reads, with the warm start folded in."""
 
     def _pack(self, update_block: torch.nn.Module, num_k: int = 32) -> _lib.RaftWeights:
         self.num_k = num_k
-        self.upsample = 4 if self.variant == 10 else 8
+        self.upsample = 4 if self.variant == _lib.VARIANT_SCV4 else 8
         return super()._pack(update_block)
 
     def make_cfg(self, B: int, H: int, W: int, iters: int, out_hw, pad, alternate_corr: bool, feat_dim: int, volume_layout: int = 0,

@@ -19,6 +19,7 @@ from typing import Sequence
 import torch
 import torch.nn as nn
 
+from ... import _lib
 from ...engine import CCMREngine
 from ...utils.registry import register_model, trainable
 from ..ms_raft_plus.ms_raft_plus import MSRAFTPlus, _PyramidEncoder
@@ -132,7 +133,7 @@ class CCMR(MSRAFTPlus):
         "kitti": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/ccmr-kitti-612444b9.ckpt",
         "sintel": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/ccmr-sintel-e1760f37.ckpt",
     }
-    _variant = 6
+    _variant = _lib.VARIANT_CCMR
     _engine_cls = CCMREngine
     _name = "ccmr"
 

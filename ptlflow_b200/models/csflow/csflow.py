@@ -10,7 +10,7 @@ Kernel mapping (DESIGN.md section 1, row a20): the encoders, pre-processing, CUD
 RAFT's.  CSFlowEngine adds the strip module: its four ConvBNReLU 1x1 convolutions on the wgmma (f16 / bf16) or SIMT (fp32)
 convolution, pfb_strip_means, the two strip correlations on pfb_corr_volume_build_ex, and pfb_strip_prepare, which stores the strip
 channel's pyramid as separable fp32 tables and adds the initial strip flow to the coordinates.  The loop is pfb_raft_refine with variant
-8, whose lookup is RAFT's followed by pfb_strip_lookup.
+PFB_VARIANT_CSFLOW (8), whose lookup is RAFT's followed by pfb_strip_lookup.
 """
 from __future__ import annotations
 
@@ -18,6 +18,7 @@ from typing import Dict
 
 import torch.nn as nn
 
+from ... import _lib
 from ...engine import CSFlowEngine
 from ...utils.registry import register_model, trainable
 from ..raft.extractor import BasicEncoder
@@ -56,7 +57,7 @@ class CSFlow(RAFT):
         "things": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/csflow-things-ebdd403b.ckpt",
         "kitti": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/csflow-kitti-dc66357a.ckpt",
     }
-    _variant = 8
+    _variant = _lib.VARIANT_CSFLOW
     _engine_cls = CSFlowEngine
     min_grid = 16  # 1/8-resolution pixels per side: the coarsest of the 4 levels keeps 2, below that the reference divides by 0
 

@@ -9,7 +9,7 @@ state_dict keys (``fnet.*``, ``cnet.*`` as RAFT's BasicEncoder, ``attn_x.*`` / `
 Kernel mapping (DESIGN.md section 1, row a19): the encoders, pre-processing, CUDA-graph capture and warm start are RAFT's.  The
 correlation pyramid is replaced by Flow1DEngine.build_volume: the attentions' 1x1 query / key projections on the wgmma (f16 / bf16)
 or SIMT (fp32) convolution, four pfb_attn1d attentions and two pfb_attn1d correlations, which store a row volume [B*H*W, W] and a
-column volume [B*H*W, H].  The loop is pfb_raft_refine with variant 7, whose lookup is pfb_corr1d_lookup.
+column volume [B*H*W, H].  The loop is pfb_raft_refine with variant PFB_VARIANT_FLOW1D (7), whose lookup is pfb_corr1d_lookup.
 """
 from __future__ import annotations
 
@@ -51,7 +51,7 @@ class Flow1D(RAFT):
         "kitti": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/flow1d-kitti-803a0181.ckpt",
         "highres": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/flow1d-highres-7ab476dc.ckpt",
     }
-    _variant = 7
+    _variant = _lib.VARIANT_FLOW1D
     _engine_cls = Flow1DEngine
 
     def __init__(self, downsample_factor: int = 8, feature_channels: int = 256, hidden_dim: int = 128, context_dim: int = 128,

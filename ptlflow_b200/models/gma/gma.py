@@ -14,7 +14,7 @@ and any num_heads; the attention is head-major [heads * B * N, N]:
     pfb_attention_softmax_relpos, which also normalises the rows.  Grids above max_pos_size (160) per side raise ValueError;
   * per iteration  motion + gamma * project(attn_h @ to_v(motion)_h)  == one 1x1 convolution per head over the N attention
     columns with the sample's v as weights, then project with an AXPY epilogue (one head: no project, AXPY directly), inside
-    pfb_raft_refine (variant 2).
+    pfb_raft_refine (variant PFB_VARIANT_GMA).
 """
 from __future__ import annotations
 
@@ -86,7 +86,7 @@ class GMA(RAFT):
         "sintel": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/gma-sintel-98d6f3d0.ckpt",
         "kitti": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/gma-kitti-8ca3ec80.ckpt",
     }
-    _variant = 2
+    _variant = _lib.VARIANT_GMA
 
     def __init__(self, corr_levels: int = 4, corr_radius: int = 4, dropout: float = 0.0, gamma: float = 0.8,
                  max_flow: float = 400, iters: int = 32, num_heads: int = 1, position_only: bool = False,

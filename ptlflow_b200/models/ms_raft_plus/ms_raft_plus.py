@@ -20,7 +20,7 @@ import torch
 import torch.nn as nn
 import torch.nn.functional as F
 
-from ... import ops
+from ... import _lib, ops
 from ...engine import MSRaftEngine
 from ...utils.registry import register_model, trainable
 from ..raft.extractor import _NATIVE_CONV1, _Encoder, _conv_pm
@@ -203,7 +203,7 @@ class MSRAFTPlus(RAFT):
     pretrained_checkpoints = {
         "mixed": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/ms_raft_plus-mixed-2bb01f62.ckpt"
     }
-    _variant = 5
+    _variant = _lib.VARIANT_MS_RAFT_P
     _engine_cls = MSRaftEngine
     _name = "ms_raft_p"
     num_scales = 4  # 1/16, 1/8, 1/4, 1/2

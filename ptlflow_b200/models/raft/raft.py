@@ -17,7 +17,7 @@ import threading
 import torch
 import torch.nn as nn
 
-from ... import ops
+from ... import _lib, ops
 from ...engine import RaftEngine
 from ...utils.registry import ptlflow_trained, register_model, trainable
 from ..base_model.base_model import BaseModel
@@ -122,7 +122,7 @@ class RAFT(BaseModel):
         "sintel": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/raft-sintel-fb44381e.ckpt",
         "kitti": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/raft-kitti-3a831a4b.ckpt",
     }
-    _variant = 0  # pfb_raft_cfg.variant
+    _variant = _lib.VARIANT_RAFT  # pfb_raft_cfg.variant
     _engine_cls = RaftEngine  # packs the update block and runs its loop (SKFlow brings its own)
 
     def __init__(self, corr_levels: int = 4, corr_radius: int = 4, dropout: float = 0.0, gamma: float = 0.8,
@@ -441,7 +441,7 @@ class RAFTSmall(RAFT):
     pretrained_checkpoints = {
         "things": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/raft_small-things-b7d9f997.ckpt"
     }
-    _variant = 1
+    _variant = _lib.VARIANT_RAFT_SMALL
 
     def __init__(self, corr_levels: int = 4, corr_radius: int = 3, dropout: float = 0.0, gamma: float = 0.8,
                  max_flow: float = 400, iters: int = 32, alternate_corr: bool = False, **kwargs) -> None:

@@ -9,7 +9,8 @@ state_dict keys (``fnet.*`` / ``cnet.*`` as the reference's encoders, whose resi
 
 Kernel mapping (DESIGN.md section 1, row a21): the encoders, pre-processing, CUDA-graph capture and warm start are RAFT's.  SCVEngine
 keeps the num_k best matches of every query with pfb_knn_topk (the all-pairs volume is never materialised), folds them and the warm
-start into a per-query table with pfb_sparse_prepare, and runs pfb_raft_refine with variant 9 / 10, whose lookup is pfb_sparse_lookup.
+start into a per-query table with pfb_sparse_prepare, and runs pfb_raft_refine with variant PFB_VARIANT_SCV8 / PFB_VARIANT_SCV4,
+whose lookup is pfb_sparse_lookup.
 """
 from __future__ import annotations
 
@@ -17,6 +18,7 @@ from typing import Dict
 
 import torch.nn as nn
 
+from ... import _lib
 from ...engine import SCVEngine
 from ...utils.registry import register_model, trainable
 from ..raft.extractor import BasicEncoder
@@ -96,7 +98,7 @@ class SCVQuarter(SCVBase):
         "sintel": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/scv-quarter-sintel-2d9b4a05.ckpt",
         "things": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/scv-quarter-things-0dac9b66.ckpt",
     }
-    _variant = 10
+    _variant = _lib.VARIANT_SCV4
     _encoder_cls = SCVEncoderQuarter
     _mask_channels = 144  # 9 taps x 4 x 4 (scv/update.py:161-165)
     grid_stride = 4
@@ -107,7 +109,7 @@ class SCVEighth(SCVBase):
         "chairs": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/scv-eighth-chairs-8ba57294.ckpt",
         "things": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/scv-eighth-things-9c893323.ckpt",
     }
-    _variant = 9
+    _variant = _lib.VARIANT_SCV8
 
 
 @register_model

@@ -19,7 +19,7 @@ from typing import Optional, Sequence
 import torch
 import torch.nn as nn
 
-from ... import ops
+from ... import _lib, ops
 from ...engine import SEARaftEngine
 from ...utils.registry import register_model, trainable
 from ..raft.extractor import _NATIVE_CONV1, _NATIVE_CONV2, _Encoder, _fold
@@ -139,7 +139,7 @@ class SEAUpdateBlock(nn.Module):
 
 class SEARAFT(RAFT):
     pretrained_checkpoints: dict = {}
-    _variant = 4
+    _variant = _lib.VARIANT_SEA_RAFT
     _engine_cls = SEARaftEngine
 
     def __init__(self, corr_levels: int = 4, corr_radius: int = 4, dim: int = 128, initial_dim: int = 64, num_blocks: int = 2,

@@ -18,6 +18,7 @@ from typing import Sequence
 
 import torch.nn as nn
 
+from ... import _lib
 from ...engine import SKFlowEngine
 from ...utils.registry import register_model, trainable
 from ..gma.gma import GMA, Aggregate, Attention
@@ -80,7 +81,7 @@ class SKFlow(GMA):
         "sintel": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/skflow-sintel-98fb67cf.ckpt",
         "things": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/skflow-things-f84e6538.ckpt",
     }
-    _variant = 3
+    _variant = _lib.VARIANT_SKFLOW
     _engine_cls = SKFlowEngine
 
     def __init__(self, corr_levels: int = 4, corr_radius: int = 4, dropout: float = 0.0, gamma: float = 0.8, max_flow: float = 400,

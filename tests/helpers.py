@@ -33,3 +33,18 @@ def load_golden_arrays(name):
     """A golden file without a recipe: every array it holds."""
     z = np.load(os.path.join(GOLDEN, name + ".npz"))
     return {k: z[k] for k in z.files}
+
+
+def lib():
+    """The ctypes binding (ptlflow_b200._lib), with the library built first where it is missing."""
+    from ptlflow_b200 import _lib as L
+    from ptlflow_b200.csrc import build as B
+
+    if not os.path.exists(L.LIB_PATH):
+        B.build()
+    return L
+
+
+def raft_cfg(L, defaults, **overrides):
+    """A pfb_raft_cfg of the fields in ``defaults``, then ``overrides``, by field name; every other field 0."""
+    return L.RaftCfg(**{**defaults, **overrides})

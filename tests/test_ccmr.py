@@ -15,17 +15,9 @@ sys.path.insert(0, HERE)
 sys.path.insert(0, os.path.dirname(HERE))
 
 import ccmr_oracle as CC  # noqa: E402
+from helpers import lib as _lib, raft_cfg  # noqa: E402
 
 GOLDEN = os.path.join(HERE, "golden")
-
-
-def _lib():
-    from ptlflow_b200 import _lib as L
-    from ptlflow_b200.csrc import build as B
-
-    if not os.path.exists(L.LIB_PATH):
-        B.build()
-    return L
 
 
 @pytest.mark.parametrize("name", CC.E2E)
@@ -127,29 +119,27 @@ def test_grid_warm_start_and_volume_checks_on_the_host():
     v._check_volume(torch.zeros(1, 2, 3, 64, 96))
 
 
-def _cfg(L, variant, **kw):
-    a = dict(dtype=L.BF16, B=2, H=16, W=24, feat=128, levels=2, radius=4, iters=4, alt=1)
-    a.update(kw)
-    return L.RaftCfg(variant, a["dtype"], a["B"], a["H"], a["W"], a["feat"], a["levels"], a["radius"], 128, 128, a["iters"], a["alt"],
-                     2 * a["H"], 2 * a["W"], 0, 0, 0, 0, 0, 1)
+CFG = dict(dtype=2, B=2, H=16, W=24, feat_dim=128, corr_levels=2, corr_radius=4, hidden_dim=128, context_dim=128, iters=4,
+           alternate_corr=1, out_h=32, out_w=48, num_heads=1)  # bf16
 
 
 def test_ccmr_entry_points_check_their_arguments():
     L = _lib()
     lib = L.load()
-    n6 = lib.pfb_ccmr_workspace_bytes(C.byref(_cfg(L, 6)))
-    assert n6 > lib.pfb_msraft_workspace_bytes(C.byref(_cfg(L, 5))) > 0
-    assert lib.pfb_ccmr_workspace_bytes(C.byref(_cfg(L, 5))) == 0  # variant 6 only
+    cfg = lambda variant, **kw: C.byref(raft_cfg(L, CFG, variant=variant, **kw))  # noqa: E731
+    n6 = lib.pfb_ccmr_workspace_bytes(cfg(L.VARIANT_CCMR))
+    assert n6 > lib.pfb_msraft_workspace_bytes(cfg(L.VARIANT_MS_RAFT_P)) > 0
+    assert lib.pfb_ccmr_workspace_bytes(cfg(L.VARIANT_MS_RAFT_P)) == 0  # VARIANT_CCMR only
     for fn in (lib.pfb_raft_workspace_bytes, lib.pfb_msraft_workspace_bytes, lib.pfb_skflow_workspace_bytes, lib.pfb_searaft_workspace_bytes):
-        assert fn(C.byref(_cfg(L, 6))) == 0  # every other loop refuses it
+        assert fn(cfg(L.VARIANT_CCMR)) == 0  # every other loop refuses it
     buf, w = L.RaftBuffers(), L.CcmrWeights()
-    assert lib.pfb_ccmr_refine(C.byref(_cfg(L, 5)), C.byref(w), C.byref(buf), 0.0, 0, None, None) == -1
+    assert lib.pfb_ccmr_refine(cfg(L.VARIANT_MS_RAFT_P), C.byref(w), C.byref(buf), 0.0, 0, None, None) == -1
     assert b"variant" in lib.pfb_last_error()
-    assert lib.pfb_ccmr_refine(C.byref(_cfg(L, 6)), None, C.byref(buf), 0.0, 0, None, None) == -1
-    assert lib.pfb_ccmr_update_iter(C.byref(_cfg(L, 0)), C.byref(w), C.byref(buf), None, None, 0.0, None) == -1
-    assert lib.pfb_xcit_context(C.byref(_cfg(L, 6)), C.byref(w), 16, 16, 16, 16, None) == -1  # workspace too small
+    assert lib.pfb_ccmr_refine(cfg(L.VARIANT_CCMR), None, C.byref(buf), 0.0, 0, None, None) == -1
+    assert lib.pfb_ccmr_update_iter(cfg(L.VARIANT_RAFT), C.byref(w), C.byref(buf), None, None, 0.0, None) == -1
+    assert lib.pfb_xcit_context(cfg(L.VARIANT_CCMR), C.byref(w), 16, 16, 16, 16, None) == -1  # workspace too small
     assert b"workspace" in lib.pfb_last_error()
-    assert lib.pfb_msraft_refine(C.byref(_cfg(L, 6)), C.byref(w.raft), C.byref(buf), 0.0, None, None) == -1
+    assert lib.pfb_msraft_refine(cfg(L.VARIANT_CCMR), C.byref(w.raft), C.byref(buf), 0.0, None, None) == -1
 
 
 def test_new_kernels_check_their_arguments():

@@ -1,6 +1,6 @@
 """CPU: CSFlow -- the fp32 oracle against the reference's fixtures (and the live reference where its checkout exists), the state-dict
 contract, the constructor and grid checks, the convc1 permutation, and the C-ABI argument checks of the a20 entry points and loop
-variant 8."""
+variant VARIANT_CSFLOW."""
 import ctypes as C
 import json
 import os
@@ -16,17 +16,9 @@ sys.path.insert(0, os.path.dirname(HERE))
 
 import csflow_oracle as CS  # noqa: E402
 from oracle import ref_shim  # noqa: E402
+from helpers import lib as _lib, raft_cfg  # noqa: E402
 
 GOLDEN = os.path.join(HERE, "golden")
-
-
-def _lib():
-    from ptlflow_b200 import _lib as L
-    from ptlflow_b200.csrc import build as B
-
-    if not os.path.exists(L.LIB_PATH):
-        B.build()
-    return L
 
 
 @pytest.mark.parametrize("name", CS.E2E)
@@ -144,29 +136,27 @@ def test_convc1_permutation_round_trips(radius):
     torch.testing.assert_close(torch.nn.functional.conv2d(buf, w[:, perm]), torch.nn.functional.conv2d(ref_corr, w), rtol=1e-12, atol=1e-12)
 
 
-def _cfg(L, **kw):
-    c = dict(variant=8, dtype=1, B=1, H=16, W=20, feat_dim=0, corr_levels=4, corr_radius=4, hidden_dim=128, context_dim=128, iters=2,
-             alternate_corr=0, out_h=128, out_w=160, pad_top=0, pad_left=0, impl=0, volume_layout=1, fork_flow=0, num_heads=1)
-    c.update(kw)
-    return L.RaftCfg(*[c[n] for n, _ in L.RaftCfg._fields_])
+CFG = dict(dtype=1, B=1, H=16, W=20, feat_dim=0, corr_levels=4, corr_radius=4, hidden_dim=128, context_dim=128, iters=2,
+           alternate_corr=0, out_h=128, out_w=160, pad_top=0, pad_left=0, impl=0, volume_layout=1, fork_flow=0, num_heads=1)
 
 
 def test_loop_variant8_workspace_and_refusals():
     L = _lib()
     lib = L.load()
-    ws = lambda **kw: lib.pfb_raft_workspace_bytes(C.byref(_cfg(L, **kw)))  # noqa: E731
+    cfg = dict(CFG, variant=L.VARIANT_CSFLOW)
+    ws = lambda **kw: lib.pfb_raft_workspace_bytes(C.byref(raft_cfg(L, cfg, **kw)))  # noqa: E731
     assert ws() > 0 and ws(volume_layout=0) == ws() and ws(corr_radius=15) > ws() and ws(corr_radius=0) > 0
     for bad in (dict(corr_levels=3), dict(corr_levels=5), dict(alternate_corr=1), dict(volume_layout=2), dict(corr_radius=16),
                 dict(hidden_dim=96), dict(volume_layout=1, dtype=0)):
         assert ws(**bad) == 0, bad
-    # variant 8 is a pfb_raft loop only
+    # VARIANT_CSFLOW is a pfb_raft loop only
     for sym in ("pfb_msraft_workspace_bytes", "pfb_ccmr_workspace_bytes", "pfb_skflow_workspace_bytes", "pfb_searaft_workspace_bytes"):
-        assert getattr(lib, sym)(C.byref(_cfg(L))) == 0, sym
-    # the lookup buffer: 2 x 4 x 81 = 648 planes (already a multiple of 8); the rest of the workspace is variant 0's (324 planes)
-    ref0 = ws(variant=0)
+        assert getattr(lib, sym)(C.byref(raft_cfg(L, cfg))) == 0, sym
+    # the lookup buffer: 2 x 4 x 81 = 648 planes (already a multiple of 8); the rest of the workspace is VARIANT_RAFT's (324 planes)
+    ref0 = ws(variant=L.VARIANT_RAFT)
     P = 16 * 20
     assert ws() - ref0 == (P * 648 * 2 + 255) // 256 * 256 - (P * 328 * 2 + 255) // 256 * 256
-    assert ws(dtype=0, volume_layout=0) - ws(variant=0, dtype=0, volume_layout=0) == (P * 648 * 4 + 255) // 256 * 256 - (P * 324 * 4 + 255) // 256 * 256
+    assert ws(dtype=0, volume_layout=0) - ws(variant=L.VARIANT_RAFT, dtype=0, volume_layout=0) == (P * 648 * 4 + 255) // 256 * 256 - (P * 324 * 4 + 255) // 256 * 256
 
 
 def test_strip_argument_checks():

@@ -1,5 +1,5 @@
 """CPU: Flow1D -- the fp32 oracle against the reference's fixtures (and the live reference where its checkout exists), the state-dict
-contract, the constructor and grid checks, and the C-ABI argument checks of the a19 entry points and loop variant 7."""
+contract, the constructor and grid checks, and the C-ABI argument checks of the a19 entry points and loop variant VARIANT_FLOW1D."""
 import ctypes as C
 import json
 import os
@@ -15,17 +15,9 @@ sys.path.insert(0, os.path.dirname(HERE))
 
 import flow1d_oracle as FD  # noqa: E402
 from oracle import ref_shim  # noqa: E402
+from helpers import lib as _lib, raft_cfg  # noqa: E402
 
 GOLDEN = os.path.join(HERE, "golden")
-
-
-def _lib():
-    from ptlflow_b200 import _lib as L
-    from ptlflow_b200.csrc import build as B
-
-    if not os.path.exists(L.LIB_PATH):
-        B.build()
-    return L
 
 
 @pytest.mark.parametrize("name", FD.E2E)
@@ -132,26 +124,24 @@ def test_grid_limits_raise_before_any_launch(h, w):
     m._check_grid(2, _lib().ATTN1D_MAX_L)
 
 
-def _cfg(L, **kw):
-    c = dict(variant=7, dtype=1, B=1, H=8, W=12, feat_dim=0, corr_levels=1, corr_radius=32, hidden_dim=128, context_dim=128, iters=2,
-             alternate_corr=0, out_h=64, out_w=96, pad_top=0, pad_left=0, impl=0, volume_layout=0, fork_flow=0, num_heads=1)
-    c.update(kw)
-    return L.RaftCfg(*[c[n] for n, _ in L.RaftCfg._fields_])
+CFG = dict(dtype=1, B=1, H=8, W=12, feat_dim=0, corr_levels=1, corr_radius=32, hidden_dim=128, context_dim=128, iters=2,
+           alternate_corr=0, out_h=64, out_w=96, pad_top=0, pad_left=0, impl=0, volume_layout=0, fork_flow=0, num_heads=1)
 
 
 def test_loop_variant7_workspace_and_refusals():
     L = _lib()
     lib = L.load()
-    ws = lambda **kw: lib.pfb_raft_workspace_bytes(C.byref(_cfg(L, **kw)))  # noqa: E731
+    cfg = dict(CFG, variant=L.VARIANT_FLOW1D)
+    ws = lambda **kw: lib.pfb_raft_workspace_bytes(C.byref(raft_cfg(L, cfg, **kw)))  # noqa: E731
     assert ws() > 0 and ws(corr_radius=64) > ws() and ws(corr_radius=1) > 0
     for bad in (dict(corr_radius=65), dict(corr_levels=2), dict(alternate_corr=1), dict(volume_layout=1), dict(H=1), dict(W=1),
                 dict(hidden_dim=96)):
         assert ws(**bad) == 0, bad
-    # the radius limit of the other loops is unchanged; variant 7 is not a pfb_msraft / pfb_ccmr loop
-    assert ws(variant=0, corr_levels=4, corr_radius=16) == 0 and ws(variant=0, corr_levels=4, corr_radius=4) > 0
-    assert lib.pfb_msraft_workspace_bytes(C.byref(_cfg(L))) == 0 and lib.pfb_ccmr_workspace_bytes(C.byref(_cfg(L))) == 0
-    # the lookup buffer: 2 (2r+1) = 130 planes, stride 136 in f16 (the rest of the workspace is variant 0's)
-    ref0 = ws(variant=0, corr_levels=1, corr_radius=4)  # 81 planes, stride 88
+    # the radius limit of the other loops is unchanged; VARIANT_FLOW1D is not a pfb_msraft / pfb_ccmr loop
+    assert ws(variant=L.VARIANT_RAFT, corr_levels=4, corr_radius=16) == 0 and ws(variant=L.VARIANT_RAFT, corr_levels=4, corr_radius=4) > 0
+    assert lib.pfb_msraft_workspace_bytes(C.byref(raft_cfg(L, cfg))) == 0 and lib.pfb_ccmr_workspace_bytes(C.byref(raft_cfg(L, cfg))) == 0
+    # the lookup buffer: 2 (2r+1) = 130 planes, stride 136 in f16 (the rest of the workspace is VARIANT_RAFT's)
+    ref0 = ws(variant=L.VARIANT_RAFT, corr_levels=1, corr_radius=4)  # 81 planes, stride 88
     P = 8 * 12
     assert ws() - ref0 == (P * 136 * 2 + 255) // 256 * 256 - (P * 88 * 2 + 255) // 256 * 256
 

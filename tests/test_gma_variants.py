@@ -118,13 +118,13 @@ def test_workspace_grows_with_heads():
     lib = _lib.load()
     sizes = []
     for heads in (0, 1, 4):
-        cfg = _lib.RaftCfg(2, _lib.BF16, 4, 55, 128, 256, 4, 4, 128, 128, 12, 0, 436, 1024, 2, 0, 0, 1, 0, heads)
+        cfg = _lib.RaftCfg(_lib.VARIANT_GMA, _lib.BF16, 4, 55, 128, 256, 4, 4, 128, 128, 12, 0, 436, 1024, 2, 0, 0, 1, 0, heads)
         sizes.append(lib.pfb_raft_workspace_bytes(C.byref(cfg)))
     assert sizes[0] == sizes[1] > 0
     P, N = 4 * 55 * 128, 55 * 128
     # v and its transpose for 3 more heads, and the concatenated per-head outputs of 4 heads
     assert sizes[2] - sizes[1] >= (P * 3 * 128 + 4 * 3 * 128 * N + P * 4 * 128) * 2
-    bad = _lib.RaftCfg(0, _lib.BF16, 1, 16, 32, 256, 4, 4, 128, 128, 4, 0, 128, 256, 0, 0, 0, 0, 0, 2)  # heads on raft
+    bad = _lib.RaftCfg(_lib.VARIANT_RAFT, _lib.BF16, 1, 16, 32, 256, 4, 4, 128, 128, 4, 0, 128, 256, 0, 0, 0, 0, 0, 2)  # heads on raft
     assert lib.pfb_raft_workspace_bytes(C.byref(bad)) == 0
 
 

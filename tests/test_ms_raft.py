@@ -15,18 +15,9 @@ import torch
 
 import ptlflow_b200  # noqa: F401  (before the reference shim below can put its own lightning stand-in into sys.modules)
 import ms_raft_oracle as MS
-from helpers import GOLDEN, load_golden
+from helpers import GOLDEN, load_golden, lib as _lib, raft_cfg
 from oracle import raft_oracle as O
 from oracle import ref_shim
-
-
-def _lib():
-    from ptlflow_b200 import _lib as L
-    from ptlflow_b200.csrc import build as B
-
-    if not os.path.exists(L.LIB_PATH):
-        B.build()
-    return L
 
 
 @pytest.mark.parametrize("name", MS.E2E)
@@ -144,28 +135,26 @@ def test_c_abi_exports():
         assert hasattr(lib, sym) and sym in L.SIGNATURES, sym
 
 
-def _cfg(L, variant, **kw):
-    a = dict(dtype=L.BF16, B=2, H=16, W=24, feat=256, levels=2, radius=4, iters=4, alt=1)
-    a.update(kw)
-    return L.RaftCfg(variant, a["dtype"], a["B"], a["H"], a["W"], a["feat"], a["levels"], a["radius"], 128, 128, a["iters"], a["alt"],
-                     2 * a["H"], 2 * a["W"], 0, 0, 0, 0, 0, 1)
+CFG = dict(dtype=2, B=2, H=16, W=24, feat_dim=256, corr_levels=2, corr_radius=4, hidden_dim=128, context_dim=128, iters=4,
+           alternate_corr=1, out_h=32, out_w=48, num_heads=1)  # bf16
 
 
 def test_msraft_entry_points_check_their_arguments():
     L = _lib()
     lib = L.load()
-    n5 = lib.pfb_msraft_workspace_bytes(C.byref(_cfg(L, 5)))
+    cfg = lambda variant, **kw: C.byref(raft_cfg(L, CFG, variant=variant, **kw))  # noqa: E731
+    n5 = lib.pfb_msraft_workspace_bytes(cfg(L.VARIANT_MS_RAFT_P))
     assert n5 > 0
-    assert lib.pfb_msraft_workspace_bytes(C.byref(_cfg(L, 0))) == 0  # variant 5 only
-    assert lib.pfb_raft_workspace_bytes(C.byref(_cfg(L, 5))) == 0  # the raft, skflow and sea_raft loops refuse it
-    assert lib.pfb_skflow_workspace_bytes(C.byref(_cfg(L, 5))) == 0
-    assert lib.pfb_searaft_workspace_bytes(C.byref(_cfg(L, 5))) == 0
-    assert lib.pfb_raft_workspace_bytes(C.byref(_cfg(L, 0))) > n5  # a 576-channel mask against a 36-channel one
+    assert lib.pfb_msraft_workspace_bytes(cfg(L.VARIANT_RAFT)) == 0  # VARIANT_MS_RAFT_P only
+    assert lib.pfb_raft_workspace_bytes(cfg(L.VARIANT_MS_RAFT_P)) == 0  # the raft, skflow and sea_raft loops refuse it
+    assert lib.pfb_skflow_workspace_bytes(cfg(L.VARIANT_MS_RAFT_P)) == 0
+    assert lib.pfb_searaft_workspace_bytes(cfg(L.VARIANT_MS_RAFT_P)) == 0
+    assert lib.pfb_raft_workspace_bytes(cfg(L.VARIANT_RAFT)) > n5  # a 576-channel mask against a 36-channel one
     buf, w = L.RaftBuffers(), L.RaftWeights()
-    assert lib.pfb_msraft_refine(C.byref(_cfg(L, 0)), C.byref(w), C.byref(buf), 0.0, None, None) == -1
+    assert lib.pfb_msraft_refine(cfg(L.VARIANT_RAFT), C.byref(w), C.byref(buf), 0.0, None, None) == -1
     assert b"variant" in lib.pfb_last_error()
-    assert lib.pfb_raft_refine(C.byref(_cfg(L, 5)), C.byref(w), C.byref(buf), None) == -1
-    assert lib.pfb_msraft_update_iter(C.byref(_cfg(L, 1)), C.byref(w), C.byref(buf), None, None, 0.0, None) == -1
+    assert lib.pfb_raft_refine(cfg(L.VARIANT_MS_RAFT_P), C.byref(w), C.byref(buf), None) == -1
+    assert lib.pfb_msraft_update_iter(cfg(L.VARIANT_RAFT_SMALL), C.byref(w), C.byref(buf), None, None, 0.0, None) == -1
 
 
 def test_new_kernels_check_their_arguments():

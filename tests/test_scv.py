@@ -1,6 +1,6 @@
 """CPU: SCV -- the fp32 oracle against the reference's fixtures (and the live reference where its checkout exists), the state-dict
 contracts of scv4 / scv8, the constructor and grid checks, the encoders' projected shortcuts, and the C-ABI argument checks of the a21
-entry points and loop variants 9 / 10."""
+entry points and loop variants VARIANT_SCV8 / VARIANT_SCV4."""
 import ctypes as C
 import json
 import os
@@ -16,17 +16,9 @@ sys.path.insert(0, os.path.dirname(HERE))
 
 import scv_oracle as S  # noqa: E402
 from oracle import ref_shim  # noqa: E402
+from helpers import lib as _lib, raft_cfg  # noqa: E402
 
 GOLDEN = os.path.join(HERE, "golden")
-
-
-def _lib():
-    from ptlflow_b200 import _lib as L
-    from ptlflow_b200.csrc import build as B
-
-    if not os.path.exists(L.LIB_PATH):
-        B.build()
-    return L
 
 
 @pytest.mark.parametrize("name", S.E2E)
@@ -144,31 +136,29 @@ def test_grid_smaller_than_num_k_raises():
     m8._check_grid(2, 4)
 
 
-def _cfg(L, **kw):
-    c = dict(variant=9, dtype=1, B=1, H=12, W=16, feat_dim=32, corr_levels=5, corr_radius=4, hidden_dim=128, context_dim=128, iters=2,
-             alternate_corr=0, out_h=96, out_w=128, pad_top=0, pad_left=0, impl=0, volume_layout=0, fork_flow=0, num_heads=1)
-    c.update(kw)
-    return L.RaftCfg(*[c[n] for n, _ in L.RaftCfg._fields_])
+CFG = dict(dtype=1, B=1, H=12, W=16, feat_dim=32, corr_levels=5, corr_radius=4, hidden_dim=128, context_dim=128, iters=2,
+           alternate_corr=0, out_h=96, out_w=128, pad_top=0, pad_left=0, impl=0, volume_layout=0, fork_flow=0, num_heads=1)
 
 
 def test_loop_variants_9_10_workspace_and_refusals():
     L = _lib()
     lib = L.load()
-    ws = lambda **kw: lib.pfb_raft_workspace_bytes(C.byref(_cfg(L, **kw)))  # noqa: E731
-    assert ws() > 0 and ws(variant=10) > 0 and ws(feat_dim=1) == ws()
+    cfg = dict(CFG, variant=L.VARIANT_SCV8)
+    ws = lambda **kw: lib.pfb_raft_workspace_bytes(C.byref(raft_cfg(L, cfg, **kw)))  # noqa: E731
+    assert ws() > 0 and ws(variant=L.VARIANT_SCV4) > 0 and ws(feat_dim=1) == ws()
     for bad in (dict(corr_levels=4), dict(corr_radius=3), dict(alternate_corr=1), dict(volume_layout=1), dict(feat_dim=0),
                 dict(feat_dim=33), dict(H=4, W=7), dict(hidden_dim=96)):
         assert ws(**bad) == 0, bad
-        assert ws(variant=10, **bad) == 0, bad
+        assert ws(variant=L.VARIANT_SCV4, **bad) == 0, bad
     assert ws(H=4, W=8) > 0 and ws(H=1, W=1, feat_dim=1) > 0  # no pyramid levels to fit: any grid with num_k pixels
     for sym in ("pfb_msraft_workspace_bytes", "pfb_ccmr_workspace_bytes", "pfb_skflow_workspace_bytes", "pfb_searaft_workspace_bytes"):
-        assert getattr(lib, sym)(C.byref(_cfg(L))) == 0, sym
+        assert getattr(lib, sym)(C.byref(raft_cfg(L, cfg))) == 0, sym
     # the lookup buffer: 405 planes, 408 in f16 (rows of 16 bytes), 405 in fp32; scv4's mask has 144 channels, scv8's 576
     P = 12 * 16
     r = lambda n: (n + 255) // 256 * 256  # noqa: E731
-    assert ws() - ws(variant=0, feat_dim=0, corr_levels=4) == r(P * 408 * 2) - r(P * 328 * 2)
-    assert ws(dtype=0) - ws(variant=0, feat_dim=0, corr_levels=4, dtype=0) == r(P * 405 * 4) - r(P * 324 * 4)
-    assert ws() - ws(variant=10) == r(P * 576 * 2) - r(P * 144 * 2)
+    assert ws() - ws(variant=L.VARIANT_RAFT, feat_dim=0, corr_levels=4) == r(P * 408 * 2) - r(P * 328 * 2)
+    assert ws(dtype=0) - ws(variant=L.VARIANT_RAFT, feat_dim=0, corr_levels=4, dtype=0) == r(P * 405 * 4) - r(P * 324 * 4)
+    assert ws() - ws(variant=L.VARIANT_SCV4) == r(P * 576 * 2) - r(P * 144 * 2)
 
 
 def test_scv_argument_checks():

@@ -17,20 +17,11 @@ import torch
 
 import ptlflow_b200  # noqa: F401  (before the reference shim below can put its own lightning stand-in into sys.modules)
 import sea_raft_oracle as SR
-from helpers import GOLDEN, load_golden
+from helpers import GOLDEN, load_golden, lib as _lib, raft_cfg
 from oracle import raft_oracle as O
 from oracle import ref_shim, synth
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _lib():
-    from ptlflow_b200 import _lib as L
-    from ptlflow_b200.csrc import build as B
-
-    if not os.path.exists(L.LIB_PATH):
-        B.build()
-    return L
 
 
 @pytest.mark.parametrize("name", SR.E2E)
@@ -155,26 +146,24 @@ def test_c_abi_exports_and_mirrors():
     assert int(re.search(r"#define\s+PFB_SR_MAX_BLOCKS\s+(\d+)", text).group(1)) == L.PFB_SR_MAX_BLOCKS
 
 
-def _cfg(L, variant, **kw):
-    a = dict(dtype=L.BF16, B=2, H=16, W=24, feat=256, levels=4, radius=4, iters=4, alt=0)
-    a.update(kw)
-    return L.RaftCfg(variant, a["dtype"], a["B"], a["H"], a["W"], a["feat"], a["levels"], a["radius"], 128, 128, a["iters"], a["alt"],
-                     8 * a["H"], 8 * a["W"], 0, 0, 0, 0, 0, 1)
+CFG = dict(dtype=2, B=2, H=16, W=24, feat_dim=256, corr_levels=4, corr_radius=4, hidden_dim=128, context_dim=128, iters=4, out_h=128,
+           out_w=192, num_heads=1)  # bf16
 
 
 def test_searaft_entry_points_check_their_arguments():
     L = _lib()
     lib = L.load()
-    assert lib.pfb_searaft_workspace_bytes(C.byref(_cfg(L, 4))) > 0
-    assert 0 < lib.pfb_searaft_workspace_bytes(C.byref(_cfg(L, 4, iters=0))) < lib.pfb_searaft_workspace_bytes(C.byref(_cfg(L, 4)))
-    assert lib.pfb_searaft_workspace_bytes(C.byref(_cfg(L, 3))) == 0  # variant 4 only
-    assert lib.pfb_raft_workspace_bytes(C.byref(_cfg(L, 4))) == 0  # the raft and skflow loops keep refusing it
-    assert lib.pfb_skflow_workspace_bytes(C.byref(_cfg(L, 4))) == 0
+    cfg = lambda variant, **kw: C.byref(raft_cfg(L, CFG, variant=variant, **kw))  # noqa: E731
+    assert lib.pfb_searaft_workspace_bytes(cfg(L.VARIANT_SEA_RAFT)) > 0
+    assert 0 < lib.pfb_searaft_workspace_bytes(cfg(L.VARIANT_SEA_RAFT, iters=0)) < lib.pfb_searaft_workspace_bytes(cfg(L.VARIANT_SEA_RAFT))
+    assert lib.pfb_searaft_workspace_bytes(cfg(L.VARIANT_SKFLOW)) == 0  # VARIANT_SEA_RAFT only
+    assert lib.pfb_raft_workspace_bytes(cfg(L.VARIANT_SEA_RAFT)) == 0  # the raft and skflow loops keep refusing it
+    assert lib.pfb_skflow_workspace_bytes(cfg(L.VARIANT_SEA_RAFT)) == 0
     buf, w = L.RaftBuffers(), L.SearaftWeights()
-    assert lib.pfb_searaft_refine(C.byref(_cfg(L, 3)), C.byref(w), C.byref(buf), None) == -1
+    assert lib.pfb_searaft_refine(cfg(L.VARIANT_SKFLOW), C.byref(w), C.byref(buf), None) == -1
     assert b"variant" in lib.pfb_last_error()
-    assert lib.pfb_raft_refine(C.byref(_cfg(L, 4)), C.byref(L.RaftWeights()), C.byref(buf), None) == -1
-    assert lib.pfb_skflow_refine(C.byref(_cfg(L, 4)), C.byref(L.SkflowWeights()), C.byref(buf), None) == -1
+    assert lib.pfb_raft_refine(cfg(L.VARIANT_SEA_RAFT), C.byref(L.RaftWeights()), C.byref(buf), None) == -1
+    assert lib.pfb_skflow_refine(cfg(L.VARIANT_SEA_RAFT), C.byref(L.SkflowWeights()), C.byref(buf), None) == -1
 
 
 def test_depthwise_layernorm_argument_checks():

@@ -15,19 +15,10 @@ import pytest
 import torch
 
 import skflow_oracle as SO
-from helpers import GOLDEN, load_golden
+from helpers import GOLDEN, load_golden, lib as _lib, raft_cfg
 from oracle import ref_shim
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-
-
-def _lib():
-    from ptlflow_b200 import _lib as L
-    from ptlflow_b200.csrc import build as B
-
-    if not os.path.exists(L.LIB_PATH):
-        B.build()
-    return L
 
 
 def _header() -> str:
@@ -147,26 +138,24 @@ def test_header_mirrors():
     assert L.L_COUNT == 25
 
 
-def _cfg(L, variant, **kw):
-    a = dict(dtype=L.BF16, B=2, H=16, W=24, feat=256, levels=4, radius=4, iters=4, alt=0, heads=1)
-    a.update(kw)
-    return L.RaftCfg(variant, a["dtype"], a["B"], a["H"], a["W"], a["feat"], a["levels"], a["radius"], 128, 128, a["iters"], a["alt"],
-                     8 * a["H"], 8 * a["W"], 0, 0, 0, 0, 0, a["heads"])
+CFG = dict(dtype=2, B=2, H=16, W=24, feat_dim=256, corr_levels=4, corr_radius=4, hidden_dim=128, context_dim=128, iters=4, out_h=128,
+           out_w=192, num_heads=1)  # bf16
 
 
 def test_skflow_entry_points_check_their_arguments():
     L = _lib()
     lib = L.load()
-    assert lib.pfb_skflow_workspace_bytes(C.byref(_cfg(L, 3))) > 0
-    assert lib.pfb_skflow_workspace_bytes(C.byref(_cfg(L, 2))) == 0  # variant 3 only
-    assert lib.pfb_raft_workspace_bytes(C.byref(_cfg(L, 3))) == 0  # the raft loop keeps refusing it
+    cfg = lambda variant, **kw: C.byref(raft_cfg(L, CFG, variant=variant, **kw))  # noqa: E731
+    assert lib.pfb_skflow_workspace_bytes(cfg(L.VARIANT_SKFLOW)) > 0
+    assert lib.pfb_skflow_workspace_bytes(cfg(L.VARIANT_GMA)) == 0  # VARIANT_SKFLOW only
+    assert lib.pfb_raft_workspace_bytes(cfg(L.VARIANT_SKFLOW)) == 0  # the raft loop keeps refusing it
     P = 2 * 16 * 24
-    big = lib.pfb_skflow_workspace_bytes(C.byref(_cfg(L, 3, heads=4)))
-    assert big - lib.pfb_skflow_workspace_bytes(C.byref(_cfg(L, 3))) >= (P * 3 * 128 + P * 4 * 128) * 2
+    big = lib.pfb_skflow_workspace_bytes(cfg(L.VARIANT_SKFLOW, num_heads=4))
+    assert big - lib.pfb_skflow_workspace_bytes(cfg(L.VARIANT_SKFLOW)) >= (P * 3 * 128 + P * 4 * 128) * 2
     buf = L.RaftBuffers()
     w = L.SkflowWeights()
-    assert lib.pfb_skflow_refine(C.byref(_cfg(L, 3)), C.byref(w), C.byref(buf), None) == -1
-    assert lib.pfb_raft_refine(C.byref(_cfg(L, 3)), C.byref(L.RaftWeights()), C.byref(buf), None) == -1
+    assert lib.pfb_skflow_refine(cfg(L.VARIANT_SKFLOW), C.byref(w), C.byref(buf), None) == -1
+    assert lib.pfb_raft_refine(cfg(L.VARIANT_SKFLOW), C.byref(L.RaftWeights()), C.byref(buf), None) == -1
     assert b"variant" in lib.pfb_last_error()
 
 
