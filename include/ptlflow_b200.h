@@ -236,6 +236,11 @@ typedef struct {
 } pfb_conv_params;
 
 PFB_API int pfb_conv2d(const pfb_conv_params* p, pfb_stream stream);
+/* Host only, no device needed: the launch plan pfb_conv2d's wgmma path (impl 0 / 2, f16 / bf16) makes for p.  pixels_per_item
+ * is 256 for the two-row work item of the 3x3 ReLU layers (csrc/conv_umma.cu, conv_wide_kernel) and 128 otherwise, n_tile
+ * the output channels per work item, smem_bytes the dynamic shared memory of the launch; all 0 when the wgmma path
+ * declines the layer. */
+PFB_API int pfb_conv2d_umma_plan(const pfb_conv_params* p, int* pixels_per_item, int* n_tile, size_t* smem_bytes);
 
 /* torch-layout weight [Cout][Cin][KH][KW] (src_dtype) -> packed [KH*KW][Cin][Cout_pad] (dst_dtype),
  * written at column `col_offset` (so convz|convr share one packed matrix).  Columns outside

@@ -157,6 +157,7 @@ SIGNATURES = {
     "pfb_alt_corr_forward": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
     "pfb_avg_pool2x2_nhwc": (_I, [_P, _P, _I, _I, _I, _I, _I, _S]),
     "pfb_conv2d": (_I, [C.POINTER(ConvParams), _S]),
+    "pfb_conv2d_umma_plan": (_I, [C.POINTER(ConvParams), C.POINTER(_I), C.POINTER(_I), C.POINTER(C.c_size_t)]),
     "pfb_pack_conv_weight": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
     "pfb_pack_bias": (_I, [_P, _P, _I, _I, _I, _S]),
     "pfb_pack_conv_weight_kmajor": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, C.POINTER(C.c_int), _I, _I, _I, _I, _S]),

@@ -20,6 +20,8 @@
 // operands are requested before the accumulator wait.  Launched with programmatic stream serialization: the
 // prologue (barriers, bias, tensor-map prefetch) overlaps the previous kernel's drain (pdl_wait below).
 // PFB_CONV_TRACE=<file> records a per-CTA timeline of every launch (tools/conv_trace_report.py).
+// The 3x3 ReLU layers run on a second kernel with 256-pixel work items that halve their weight traffic (conv_wide_kernel
+// below); plan_conv_wide picks the layers it takes.
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -220,6 +222,74 @@ __device__ __forceinline__ void conv_mma_role(const ConvUmmaArgs& a, ConvBars* b
   }
 }
 
+// work item j -> (n tile, image, tile row, tile col); n-tile major so concurrent CTAs share the weight tile in L2
+__device__ __forceinline__ void conv_decode(const ConvUmmaArgs& a, int j, int& n0, int& b, int& y0, int& x0) {
+  const int tiles_m = a.tiles_x * a.tiles_y * a.B;
+  const int nt = j / tiles_m;
+  int m = j - nt * tiles_m;
+  const int px = m % a.tiles_x;
+  m /= a.tiles_x;
+  const int py = m % a.tiles_y;
+  b = m / a.tiles_y;
+  n0 = nt * a.NT;
+  y0 = py * a.TH;
+  x0 = px * a.TW;
+}
+
+// The TMA producer of both convolution kernels (one warp: warp-uniform loop, one elected lane issues).  It walks this
+// CTA's work items and streams their activation patches (box: the patch of the M tile, TW + KW - 1 x TH rows with the x
+// halo) and weight stages into the two rings.
+__device__ __forceinline__ void conv_produce(const ConvUmmaArgs& a, ConvBars* bars, uint8_t* smemA, uint8_t* smemB, const CUtensorMap* tm0,
+                                             const CUtensorMap* tm1, const CUtensorMap* tm2, const CUtensorMap* tmW) {
+  const int lane = threadIdx.x & 31;
+  const int ph2 = a.KH >> 1, pw2 = a.KW >> 1;
+  const uint32_t btx = a.NT * 128;  // bytes of one weight tap
+  // ring positions advance incrementally (stage index + phase bit): no integer division on the issue path
+  int sta = 0, stb = 0, bg = 0;
+  uint32_t pha = 0, phb = 0;
+  PFB_TR(3);
+  for (int w = blockIdx.x; w < a.n_work; w += gridDim.x) {
+    int n0, b, y0, x0;
+    conv_decode(a, w, n0, b, y0, x0);
+    int kidx = 0;
+    const int wrow0 = b * a.w_rows_per_sample;  // per-sample weights (GMA aggregate: the sample's v^T)
+    for (int s = 0; s < a.nsrc; ++s) {
+      const CUtensorMap* tm = s == 0 ? tm0 : (s == 1 ? tm1 : tm2);
+      for (int c = 0; c < a.src_chunks[s]; ++c, ++kidx) {
+        int wrow = wrow0;  // + (ky * KW + kx) * Cout_pad_k
+        for (int ky = 0; ky < a.KH; ++ky) {
+          for (int kx = 0; kx < a.KW; ++kx) {
+            // activation patch: once per (chunk, ky) with the x halo, once per chunk with the y halo, else per tap
+            if (a.halo == 0 || (a.halo == 1 && kx == 0) || (a.halo == 2 && ky == 0)) {
+              mbar_wait(&bars->a_empty[sta], pha ^ 1);
+              if (elect_one()) {
+                mbar_arrive_expect_tx(&bars->a_full[sta], a.a_tx_bytes);
+                tma_load_4d(smemA + sta * a.a_slot_bytes, tm, &bars->a_full[sta], a.src_coff[s] + c * 64,
+                            x0 - pw2 + (a.halo ? 0 : kx), y0 + ky - ph2, b);
+              }
+              __syncwarp();
+              if (++sta == a.a_stages) { sta = 0; pha ^= 1; }
+            }
+            // weight stage: b_group consecutive taps of this patch share one barrier (fewer, larger pipeline steps)
+            if (bg == 0) mbar_wait(&bars->b_empty[stb], phb ^ 1);
+            if (elect_one()) {
+              if (bg == 0) mbar_arrive_expect_tx(&bars->b_full[stb], btx * a.b_group);
+              tma_load_2d(smemB + stb * a.b_slot_bytes + bg * a.b_tap_bytes, tmW, &bars->b_full[stb], kidx * 64, wrow + n0);
+            }
+            __syncwarp();
+            wrow += a.Cout_pad_k;
+            if (++bg == a.b_group) {
+              bg = 0;
+              if (++stb == a.b_stages) { stb = 0; phb ^= 1; }
+            }
+          }
+        }
+      }
+    }
+  }
+  PFB_TR(4);
+}
+
 // Four warpgroups: warps 0-3 the epilogue (thread = pixel row, all NT columns), 4-11 the two MMA warpgroups, 12-15 the
 // producer warpgroup (warp 12 issues the TMA loads; 13-15 only give their registers away).
 // EPI (the pfb_epilogue) is a template parameter: with a run-time switch the register allocation of every epilogue was the
@@ -260,7 +330,6 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
   }
   int chunks = 0;
   for (int s = 0; s < a.nsrc; ++s) chunks += a.src_chunks[s];
-  const int tiles_m = a.tiles_x * a.tiles_y * a.B;
   const int group0 = blockIdx.x, group_stride = gridDim.x;
 
   if (threadIdx.x == 0) {
@@ -290,71 +359,11 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
   pdl_trigger();
   if (warp == 0) PFB_TR(2);
 
-  // work item j -> (n tile, image, tile row, tile col) of THIS CTA; n-tile major so concurrent CTAs share the weight
-  // tile in L2
-  auto decode = [&](int j, int& n0, int& b, int& y0, int& x0) {
-    const int nt = j / tiles_m;
-    int m = j - nt * tiles_m;
-    const int px = m % a.tiles_x;
-    m /= a.tiles_x;
-    const int py = m % a.tiles_y;
-    b = m / a.tiles_y;
-    n0 = nt * a.NT;
-    y0 = py * a.TH;
-    x0 = px * a.TW;
-  };
+  auto decode = [&](int j, int& n0, int& b, int& y0, int& x0) { conv_decode(a, j, n0, b, y0, x0); };
 
   if (warp >= kProducerWarp) {
     setmaxnreg_dec<kProducerRegs>();
-    if (warp == kProducerWarp) {
-      // ================= TMA producer (warp-uniform loop, one elected lane issues) =================
-      const int ph2 = a.KH >> 1, pw2 = a.KW >> 1;
-      const uint32_t btx = a.NT * 128;  // bytes of one weight tap
-      // ring positions advance incrementally (stage index + phase bit): no integer division on the issue path
-      int sta = 0, stb = 0, bg = 0;
-      uint32_t pha = 0, phb = 0;
-      PFB_TR(3);
-      for (int w = group0; w < a.n_work; w += group_stride) {
-        int n0, b, y0, x0;
-        decode(w, n0, b, y0, x0);
-        int kidx = 0;
-        const int wrow0 = b * a.w_rows_per_sample;  // per-sample weights (GMA aggregate: the sample's v^T)
-        for (int s = 0; s < a.nsrc; ++s) {
-          const CUtensorMap* tm = s == 0 ? &tm0 : (s == 1 ? &tm1 : &tm2);
-          for (int c = 0; c < a.src_chunks[s]; ++c, ++kidx) {
-            int wrow = wrow0;  // + (ky * KW + kx) * Cout_pad_k
-            for (int ky = 0; ky < a.KH; ++ky) {
-              for (int kx = 0; kx < a.KW; ++kx) {
-                // activation patch: once per (chunk, ky) with the x halo, once per chunk with the y halo, else per tap
-                if (a.halo == 0 || (a.halo == 1 && kx == 0) || (a.halo == 2 && ky == 0)) {
-                  mbar_wait(&bars->a_empty[sta], pha ^ 1);
-                  if (elect_one()) {
-                    mbar_arrive_expect_tx(&bars->a_full[sta], a.a_tx_bytes);
-                    tma_load_4d(smemA + sta * a.a_slot_bytes, tm, &bars->a_full[sta], a.src_coff[s] + c * 64,
-                                x0 - pw2 + (a.halo ? 0 : kx), y0 + ky - ph2, b);
-                  }
-                  __syncwarp();
-                  if (++sta == a.a_stages) { sta = 0; pha ^= 1; }
-                }
-                // weight stage: b_group consecutive taps of this patch share one barrier (fewer, larger pipeline steps)
-                if (bg == 0) mbar_wait(&bars->b_empty[stb], phb ^ 1);
-                if (elect_one()) {
-                  if (bg == 0) mbar_arrive_expect_tx(&bars->b_full[stb], btx * a.b_group);
-                  tma_load_2d(smemB + stb * a.b_slot_bytes + bg * a.b_tap_bytes, &tmW, &bars->b_full[stb], kidx * 64, wrow + n0);
-                }
-                __syncwarp();
-                wrow += a.Cout_pad_k;
-                if (++bg == a.b_group) {
-                  bg = 0;
-                  if (++stb == a.b_stages) { stb = 0; phb ^= 1; }
-                }
-              }
-            }
-          }
-        }
-      }
-      PFB_TR(4);
-    }
+    if (warp == kProducerWarp) conv_produce(a, bars, smemA, smemB, &tm0, &tm1, &tm2, &tmW);
   } else if (warp >= kMmaWarp0) {
     // ================= MMA warpgroups (kMmaRegs: the launch budget) =================
     switch (a.NT) {
@@ -641,6 +650,232 @@ conv_umma_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant_
 }
 
 // ------------------------------------------------------------------------------------------------
+// The 256-pixel work item: the plain epilogues of the update block's 3x3 layers.
+//
+// The 128-pixel kernel above streams every weight tap once per 128 pixels; on the 3x3 layers its implied L2 -> SM traffic
+// sits at 5.0-5.6 TB/s, about 70 % of it weights (DESIGN.md §5).  Here a work item is two adjacent image rows of 128
+// pixels x NT output channels, and the two MMA warpgroups, one row each, consume the same weight stage: each weight byte
+// leaves L2 once per 256 pixels.  Three warpgroups: 0 the TMA producer (conv_produce; one warp issues), 1 and 2 the MMA
+// warpgroups, each holding its 128 pixels x NT channels as two m64nNT accumulators (NT fp32 registers per thread).  The
+// activation patch of a (64-channel chunk, ky) is 2 rows x (128 + KW - 1) pixels; warpgroup r reads row r of it, and tap kx
+// through a descriptor advanced by kx pixel rows, as in the x-halo mode.  The MMA warpgroups run the epilogue from their
+// registers (fp32, rounded once): bias + ReLU (+ the two flow columns), stmatrix into a swizzled [128 pixels][64 channels]
+// staging tile per warpgroup, one TMA store per 64-channel block, clipped at the image edges and at the last column.  A
+// 32-channel last block (NT = 96) leaves the staging tile with 16-byte stores.  The epilogue does not overlap the
+// warpgroup's own MMAs (enc_conv_umma.cu explains why); the producer keeps filling the rings for the next item meanwhile.
+constexpr int kWideThreads = 3 * 128;
+constexpr int kWideTW = 128;  // pixels per MMA warpgroup: one image row
+// Register budget per role: 384 threads at one CTA per SM launch with 168 each (64512 for the CTA); the producer keeps 48
+// (conv_produce spills at 40), the MMA warpgroups (two accumulators of NT / 2 fp32 + addressing and the epilogue) take 224.
+// setmaxnreg.inc waits until the registers it asks for are free in the CTA's allocation, so the roles must fit the launch
+// allocation, not merely the register file.
+constexpr int kWideLaunchRegs = 65536 / kWideThreads / 8 * 8;
+constexpr int kWideProducerRegs = 48, kWideMmaRegs = 224;
+static_assert(128 * (kWideProducerRegs + 2 * kWideMmaRegs) <= kWideThreads * kWideLaunchRegs, "register budget exceeds the launch allocation");
+
+// stmatrix of four 8x8 b16 matrices: lane l gives the address of row l & 7 of matrix l >> 3; register i holds (row =
+// lane >> 2, columns 2 (lane & 3), +1) of matrix i -- the accumulator fragment order, pixel-major rows
+__device__ __forceinline__ void stmatrix_x4(uint32_t addr, const uint32_t (&r)[4]) {
+  asm volatile("stmatrix.sync.aligned.m8n8.x4.shared.b16 [%0], {%1, %2, %3, %4};" ::"r"(addr), "r"(r[0]), "r"(r[1]), "r"(r[2]),
+               "r"(r[3]) : "memory");
+}
+
+// G taps of one pipeline step into both accumulators (pixels 0-63 and 64-127 of the warpgroup's row, 8 KB apart)
+template <int NT, bool BF16, int G>
+__device__ __forceinline__ void wide_issue(float (&d0)[NT / 2], float (&d1)[NT / 2], uint32_t a_lo, uint32_t b_lo, uint32_t b_tap16,
+                                           uint32_t acc) {
+  wgmma_fence();
+#pragma unroll
+  for (int g = 0; g < G; ++g) {
+#pragma unroll
+    for (int kk = 0; kk < 4; ++kk) {
+      const uint32_t en = (g == 0 && kk == 0) ? acc : 1u;
+      const uint64_t bd = gdesc(b_lo + g * b_tap16 + 2 * kk, kDescHiSw128);
+      wgmma<NT, BF16>(d0, gdesc(a_lo + g * 8 + 2 * kk, kDescHiSw128), bd, en);
+      wgmma<NT, BF16>(d1, gdesc(a_lo + 512 + g * 8 + 2 * kk, kDescHiSw128), bd, en);
+    }
+  }
+  wgmma_commit();
+}
+
+// One warpgroup's row of the item: 128 pixels from x0 of image row y, channels n0 .. n0 + NT - 1.
+template <typename T, int EPI, int NT>
+__device__ __forceinline__ void wide_epilogue(const ConvUmmaArgs& a, const float (&d0)[NT / 2], const float (&d1)[NT / 2], uint8_t* stage,
+                                              const CUtensorMap* tmO, int wg, int n0, int b, int y, int x0) {
+  const int tid = threadIdx.x & 127, lane = tid & 31, wq = tid >> 5;
+  if (y >= a.H) return;  // the second row of an item below the image (warpgroup-uniform)
+  const uint32_t st = smem_u32(stage);
+  const int ncols = EPI == PFB_EPI_RELU_APPEND_FLOW ? a.Cout + 2 : a.Cout;
+#pragma unroll
+  for (int nb = 0; nb < (NT + 63) / 64; ++nb) {
+    // the previous block's store has read the staging tile before anybody overwrites it
+    if (tid == 0) tma_store_wait_read();
+    named_barrier_sync(1 + wg, 128);
+#pragma unroll
+    for (int m = 0; m < 2; ++m) {
+      const float(&d)[NT / 2] = m ? d1 : d0;
+#pragma unroll
+      for (int jj = 0; jj < 8; jj += 2) {
+        const int j = nb * 8 + jj;  // 8-column group of the accumulator; v[q] is column 8 (j + (q >> 2)) + 2 (lane & 3) + (q & 1)
+        if (j < NT / 8) {           // of row (lane >> 2) + 8 ((q >> 1) & 1)
+          float v[8];
+          const float2 b0 = __ldg(reinterpret_cast<const float2*>(a.bias + n0 + 8 * j + 2 * (lane & 3)));
+          const float2 b1 = __ldg(reinterpret_cast<const float2*>(a.bias + n0 + 8 * j + 8 + 2 * (lane & 3)));
+#pragma unroll
+          for (int q = 0; q < 8; ++q) v[q] = fmaxf(d[4 * j + q] + ((q & 4) ? ((q & 1) ? b1.y : b1.x) : ((q & 1) ? b0.y : b0.x)), 0.f);
+          if (EPI == PFB_EPI_RELU_APPEND_FLOW) {
+#pragma unroll
+            for (int q = 0; q < 8; q += 2) {
+              if (n0 + 8 * (j + (q >> 2)) + 2 * (lane & 3) == a.Cout) {  // the two columns after the last real channel
+                const int x = x0 + 64 * m + 16 * wq + (lane >> 2) + 8 * ((q >> 1) & 1);
+                if (x < a.W) {
+                  const float2 f = __ldg(reinterpret_cast<const float2*>(a.flow) + ((size_t)b * a.H + y) * a.W + x);
+                  v[q] = f.x;
+                  v[q + 1] = f.y;
+                }
+              }
+            }
+          }
+          uint32_t r[4];
+#pragma unroll
+          for (int q = 0; q < 4; ++q) r[q] = pack2<T>(v[2 * q], v[2 * q + 1]);
+          const int mi = lane >> 3;
+          const int px = 64 * m + 16 * wq + 8 * (mi & 1) + (lane & 7);
+          const int piece = jj + (mi >> 1);  // 16-byte piece q of row p lives at piece q ^ (p & 7)
+          stmatrix_x4(st + px * 128 + ((piece ^ (px & 7)) << 4), r);
+        }
+      }
+    }
+    fence_proxy_async();
+    named_barrier_sync(1 + wg, 128);
+    const int col = n0 + 64 * nb;
+    if (64 * nb + 64 <= NT) {
+      if (tid == 0) {
+        tma_store_4d(tmO, stage, a.out_offset + col, x0, y, b);
+        tma_store_commit();
+      }
+    } else if (x0 + tid < a.W) {  // 32-channel last block: thread = pixel, four 16-byte pieces
+      T* o = reinterpret_cast<T*>(a.out) + (((size_t)b * a.H + y) * a.W + x0 + tid) * a.out_stride + a.out_offset + col;
+      const int valid = ncols - col;
+#pragma unroll
+      for (int q = 0; q < 4; ++q) {
+        const uint4 u = *reinterpret_cast<const uint4*>(stage + tid * 128 + ((q ^ (tid & 7)) << 4));
+        if (valid >= 8 * q + 8) {
+          reinterpret_cast<uint4*>(o)[q] = u;
+        } else {
+          const T* h = reinterpret_cast<const T*>(&u);
+#pragma unroll
+          for (int e = 0; e < 8; ++e)
+            if (8 * q + e < valid) o[8 * q + e] = h[e];
+        }
+      }
+    }
+  }
+}
+
+template <typename T, int EPI, int NT>
+__global__ void __launch_bounds__(kWideThreads, 1)
+conv_wide_kernel(const __grid_constant__ CUtensorMap tm0, const __grid_constant__ CUtensorMap tm1, const __grid_constant__ CUtensorMap tm2,
+                 const __grid_constant__ CUtensorMap tmW, const __grid_constant__ CUtensorMap tmO, const ConvUmmaArgs a) {
+  constexpr bool kBF16 = std::is_same<T, __nv_bfloat16>::value;
+  extern __shared__ __align__(1024) uint8_t smem_raw[];
+  uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
+  uint8_t* smemA = smem;
+  uint8_t* smemB = smemA + a.a_stages * a.a_slot_bytes;
+  uint8_t* smemO = smemB + a.b_stages * a.b_slot_bytes;  // two staging tiles, one per MMA warpgroup
+  ConvBars* bars = reinterpret_cast<ConvBars*>(smemO + 2 * kATileBytes);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (a.trace && threadIdx.x == 0) {
+    a.trace[blockIdx.x * 32 + 0] = global_timer_ns();
+    a.trace[blockIdx.x * 32 + 1] = clock64();
+  }
+  int chunks = 0;
+  for (int s = 0; s < a.nsrc; ++s) chunks += a.src_chunks[s];
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < a.a_stages; ++s) {
+      mbar_init(&bars->a_full[s], 1);
+      mbar_init(&bars->a_empty[s], 8);  // one arrival per MMA warp
+    }
+    for (int s = 0; s < a.b_stages; ++s) {
+      mbar_init(&bars->b_full[s], 1);
+      mbar_init(&bars->b_empty[s], 8);
+    }
+    fence_barrier_init();
+  }
+  if (warp == 0 && lane == 0) {
+    prefetch_tmap(&tm0);
+    prefetch_tmap(&tmW);
+    prefetch_tmap(&tmO);
+  }
+  __syncthreads();
+  pdl_wait();
+  pdl_trigger();
+  if (warp == 0) PFB_TR(2);
+
+  if (warp < 4) {
+    setmaxnreg_dec<kWideProducerRegs>();
+    if (warp == 0) conv_produce(a, bars, smemA, smemB, &tm0, &tm1, &tm2, &tmW);
+  } else {
+    setmaxnreg_inc<kWideMmaRegs>();
+    // ================= MMA + epilogue warpgroups: warpgroup wg computes image row y0 + wg of the item =================
+    const int wg = (threadIdx.x >> 7) - 1;
+    const uint32_t a_slot16 = (uint32_t)a.a_slot_bytes >> 4, b_slot16 = (uint32_t)a.b_slot_bytes >> 4;
+    const uint32_t a_lo0 = gdesc_lo(smem_u32(smemA) + wg * (a.TW + a.KW - 1) * 128, 16);  // row wg of the patch
+    const uint32_t b_lo0 = gdesc_lo(smem_u32(smemB), 16);
+    const uint32_t bar_a_full = smem_u32(&bars->a_full[0]);
+    const uint32_t bar_b_full = smem_u32(&bars->b_full[0]);
+    const uint32_t b_tap16 = (uint32_t)a.b_tap_bytes >> 4;
+    const int groups = chunks * a.KH;  // patches per item
+    int sa = 0, sb = 0;
+    uint32_t pha = 0, phb = 0;
+    uint32_t a_lo = a_lo0, b_lo = b_lo0;
+    int held_b = -1, held_a = -1;  // slots of the step still in flight (as in conv_mma_role)
+    auto release_held = [&]() {
+      __syncwarp();
+      if (lane == 0 && held_b >= 0) {
+        mbar_arrive(&bars->b_empty[held_b]);
+        if (held_a >= 0) mbar_arrive(&bars->a_empty[held_a]);
+      }
+    };
+    float d0[NT / 2], d1[NT / 2];
+    for (int w = blockIdx.x; w < a.n_work; w += gridDim.x) {
+      int n0, b, y0, x0;
+      conv_decode(a, w, n0, b, y0, x0);
+      uint32_t acc = 0;  // the first MMA of the item overwrites the accumulators
+      for (int g = 0; g < groups; ++g) {
+        mbar_wait_uniform(bar_a_full + 8 * sa, pha);
+        for (int kx = 0; kx < a.KW; kx += a.b_group) {
+          mbar_wait_uniform(bar_b_full + 8 * sb, phb);
+          const uint32_t al = a_lo + 8u * kx;  // tap kx: +1 pixel row (128 B) per tap
+          if (a.b_group == 3) wide_issue<NT, kBF16, 3>(d0, d1, al, b_lo, b_tap16, acc);
+          else wide_issue<NT, kBF16, 1>(d0, d1, al, b_lo, b_tap16, acc);
+          wgmma_wait<1>();
+          reg_fence(d0);
+          reg_fence(d1);
+          release_held();
+          held_b = sb;
+          held_a = kx + a.b_group >= a.KW ? sa : -1;
+          acc = 1;
+          b_lo += b_slot16;
+          if (++sb == a.b_stages) { sb = 0; phb ^= 1; b_lo = b_lo0; }
+        }
+        a_lo += a_slot16;
+        if (++sa == a.a_stages) { sa = 0; pha ^= 1; a_lo = a_lo0; }
+      }
+      wgmma_wait<0>();
+      reg_fence(d0);
+      reg_fence(d1);
+      release_held();
+      held_b = -1;
+      wide_epilogue<T, EPI, NT>(a, d0, d1, smemO + wg * kATileBytes, &tmO, wg, n0, b, y0 + wg, x0);
+    }
+    if ((threadIdx.x & 127) == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");  // stores complete
+  }
+  __syncthreads();
+  if (warp == 0) PFB_TR(18);
+  if (a.trace && threadIdx.x == 0) a.trace[blockIdx.x * 32 + 20] = global_timer_ns();
+}
+
 static int eff_channels(const pfb_conv_src& s) { return (int)align_up((size_t)s.channels, 64); }
 
 // N tiling: the fewest equal tiles of <= 128 columns that are multiples of 32 (epilogue chunk); 0 if there is none
@@ -851,9 +1086,76 @@ static bool plan_conv_umma(const pfb_conv_params* p, ConvUmmaArgs& a) {
   return false;
 }
 
+// The 256-pixel kernel's plan (conv_wide_kernel), or false: the layer then runs on the 128-pixel kernel.  Taken by the 3x3
+// layers with at least 128 input channels, an N tile of 96 or 128 and a plain ReLU epilogue -- in RAFT's update block conv,
+// convc2, flow1 and mask1 -- on grids whose 128-pixel rows waste at most 30 % of the width.  The other layers lost or were
+// not built: DESIGN.md §5 lists them with their times.
+static bool plan_conv_wide(const pfb_conv_params* p, ConvUmmaArgs& a) {
+  if (p->epilogue != PFB_EPI_RELU && p->epilogue != PFB_EPI_RELU_APPEND_FLOW) return false;
+  if (p->KH != 3 || p->KW != 3 || p->Cin_pad < 128) return false;
+  if (p->addend || p->w_rows_per_sample || !p->bias || (reinterpret_cast<uintptr_t>(p->bias) & 7)) return false;
+  if (p->epilogue == PFB_EPI_RELU_APPEND_FLOW && (p->Cout % 2 || (reinterpret_cast<uintptr_t>(p->flow) & 7))) return false;
+  if ((long)ceil_div(p->W, kWideTW) * kWideTW * 10 > (long)p->W * 13) return false;
+  a.n_tiles = conv_n_tiles(p->Cout_pad_k);
+  if (a.n_tiles == 0) return false;
+  a.NT = p->Cout_pad_k / a.n_tiles;
+  if (a.NT != 96 && a.NT != 128) return false;
+  a.b_tap_bytes = a.NT * 128;
+  a.tma_out = 1;
+  a.TW = kWideTW; a.TH = 2; a.halo = 1; a.tw_shift = 7;
+  // 227 KB less the two staging tiles, the barriers and the alignment slack
+  if (!plan_rings(p, a, 227 * 1024 - 2 * kATileBytes - (int)sizeof(ConvBars) - 1024)) return false;
+  a.tiles_x = ceil_div(p->W, a.TW);
+  a.tiles_y = ceil_div(p->H, a.TH);
+  a.n_work = a.tiles_x * a.tiles_y * p->B * a.n_tiles;
+  return true;
+}
+
+template <typename T, int EPI, int NT>
+static int launch_conv_wide_e(const CUtensorMap* tms, const CUtensorMap& tmW, const CUtensorMap& tmO, const ConvUmmaArgs& a, int grid,
+                              size_t smem, cudaStream_t s) {
+  static std::atomic<unsigned long long> attr_done{0};  // once per (instantiation, device)
+  int dev = 0;
+  PFB_CUDA(cudaGetDevice(&dev));
+  if (!(attr_done.load(std::memory_order_acquire) & (1ull << (dev & 63)))) {
+    PFB_CUDA(cudaFuncSetAttribute(conv_wide_kernel<T, EPI, NT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024));
+    attr_done.fetch_or(1ull << (dev & 63), std::memory_order_release);
+  }
+  PFB_CUDA(launch_pdl(conv_wide_kernel<T, EPI, NT>, dim3(grid), dim3(kWideThreads), smem, s, tms[0], tms[1], tms[2], tmW, tmO, a));
+  return PFB_OK;
+}
+
+template <typename T>
+static int launch_conv_wide(const CUtensorMap* tms, const CUtensorMap& tmW, const CUtensorMap& tmO, const ConvUmmaArgs& a, int grid,
+                            size_t smem, cudaStream_t s) {
+  const bool flow = a.epilogue == PFB_EPI_RELU_APPEND_FLOW;
+  if (a.NT == 96)
+    return flow ? launch_conv_wide_e<T, PFB_EPI_RELU_APPEND_FLOW, 96>(tms, tmW, tmO, a, grid, smem, s)
+                : launch_conv_wide_e<T, PFB_EPI_RELU, 96>(tms, tmW, tmO, a, grid, smem, s);
+  return flow ? launch_conv_wide_e<T, PFB_EPI_RELU_APPEND_FLOW, 128>(tms, tmW, tmO, a, grid, smem, s)
+              : launch_conv_wide_e<T, PFB_EPI_RELU, 128>(tms, tmW, tmO, a, grid, smem, s);
+}
+
+// dynamic shared memory of a planned launch (the 1024-byte alignment slack included)
+static size_t conv_smem_bytes(const ConvUmmaArgs& a, bool wide) {
+  const size_t rings = (size_t)a.a_stages * a.a_slot_bytes + (size_t)a.b_stages * a.b_slot_bytes;
+  if (wide) return rings + 2 * kATileBytes + sizeof(ConvBars) + 1024;
+  return rings + (a.tma_out ? kATileBytes : 0) + acc_tile_bytes(a.NT) + kMaxBias * sizeof(float) + sizeof(ConvBars) + 1024;
+}
+
+// The launch plan of a layer: the 256-pixel kernel where plan_conv_wide takes it, else the 128-pixel kernel.
+static bool plan_conv(const pfb_conv_params* p, ConvUmmaArgs& a, bool& wide) {
+  a = ConvUmmaArgs{};
+  wide = plan_conv_wide(p, a);
+  if (wide) return true;
+  a = ConvUmmaArgs{};
+  return plan_conv_umma(p, a);
+}
+
 int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
   ConvUmmaArgs a{};
-  if (!plan_conv_umma(p, a)) {
+  bool wide = false;
+  if (!plan_conv(p, a, wide)) {
     set_error("conv_umma: no tile and ring plan fits in shared memory");
     return PFB_ERR_UNSUPPORTED;
   }
@@ -894,7 +1196,7 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
       const int ncols = zr ? p->hidden : (append ? p->Cout + 2 : p->Cout);
       uint64_t dims[4] = {(uint64_t)(p->out_offset + ncols), (uint64_t)p->W, (uint64_t)p->H, (uint64_t)p->B};
       uint64_t str[3] = {(uint64_t)p->out_stride * 2, (uint64_t)p->W * p->out_stride * 2, (uint64_t)p->H * p->W * p->out_stride * 2};
-      uint32_t box[4] = {64, (uint32_t)a.TW, (uint32_t)a.TH, 1};
+      uint32_t box[4] = {64, (uint32_t)a.TW, wide ? 1u : (uint32_t)a.TH, 1};  // (wide: one store per image row)
       int rc = make_tensor_map(&tmO[0], p->out, p->dtype, 4, dims, str, box);
       if (rc) return rc;
       if (zr) {
@@ -913,25 +1215,29 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
   a.post_w = p->post_w; a.post_b = p->post_b;
   a.w_rows_per_sample = p->w_rows_per_sample;
   a.ab_fmt = p->dtype == PFB_F16 ? 0 : 1;
-  const size_t smem = (size_t)a.a_stages * a.a_slot_bytes + (size_t)a.b_stages * a.b_slot_bytes + (a.tma_out ? kATileBytes : 0) +
-                      acc_tile_bytes(a.NT) + kMaxBias * sizeof(float) + sizeof(ConvBars) + 1024;
+  const size_t smem = conv_smem_bytes(a, wide);
   int grid = sm_count();
   if (grid > a.n_work) grid = a.n_work;
+  auto launch = [&]() {
+    if (wide) return p->dtype == PFB_F16 ? launch_conv_wide<__half>(tms, tmW, tmO[0], a, grid, smem, s)
+                                         : launch_conv_wide<__nv_bfloat16>(tms, tmW, tmO[0], a, grid, smem, s);
+    return p->dtype == PFB_F16 ? launch_conv_umma<__half>(tms, tmW, tmO, a, grid, smem, s)
+                               : launch_conv_umma<__nv_bfloat16>(tms, tmW, tmO, a, grid, smem, s);
+  };
   static const char* env_trace = getenv("PFB_CONV_TRACE");  // debug: per-CTA timeline of every launch -> JSON lines
   if (env_trace) {
     static unsigned long long* dbuf = nullptr;
     if (!dbuf) PFB_CUDA(cudaMalloc(&dbuf, 256 * 32 * 8));
     PFB_CUDA(cudaMemsetAsync(dbuf, 0, 256 * 32 * 8, s));
     a.trace = dbuf;
-    int rc;
-    rc = p->dtype == PFB_F16 ? launch_conv_umma<__half>(tms, tmW, tmO, a, grid, smem, s) : launch_conv_umma<__nv_bfloat16>(tms, tmW, tmO, a, grid, smem, s);
+    const int rc = launch();
     if (rc) return rc;
     PFB_CUDA(cudaStreamSynchronize(s));
     static unsigned long long host[256 * 32];
     PFB_CUDA(cudaMemcpy(host, dbuf, sizeof(host), cudaMemcpyDeviceToHost));
     if (FILE* f = fopen(env_trace, "a")) {
-      fprintf(f, "{\"KH\":%d,\"KW\":%d,\"NT\":%d,\"Cin_pad\":%d,\"halo\":%d,\"TW\":%d,\"TH\":%d,\"epi\":%d,\"grid\":%d,\"n_work\":%d,\"a_stages\":%d,\"b_stages\":%d,\"b_group\":%d,\"t\":[",
-              a.KH, a.KW, a.NT, p->Cin_pad, a.halo, a.TW, a.TH, a.epilogue, grid, a.n_work, a.a_stages, a.b_stages, a.b_group);
+      fprintf(f, "{\"KH\":%d,\"KW\":%d,\"NT\":%d,\"Cin_pad\":%d,\"halo\":%d,\"TW\":%d,\"TH\":%d,\"epi\":%d,\"grid\":%d,\"n_work\":%d,\"a_stages\":%d,\"b_stages\":%d,\"b_group\":%d,\"wide\":%d,\"t\":[",
+              a.KH, a.KW, a.NT, p->Cin_pad, a.halo, a.TW, a.TH, a.epilogue, grid, a.n_work, a.a_stages, a.b_stages, a.b_group, wide ? 1 : 0);
       for (int i = 0; i < grid * 32; ++i) fprintf(f, "%s%llu", i ? "," : "", host[i]);
       fprintf(f, "]}\n");
       fclose(f);
@@ -939,8 +1245,22 @@ int conv2d_umma(const pfb_conv_params* p, cudaStream_t s) {
     return PFB_OK;
   }
   ProfScope prof(KC_CONV, s);
-  if (p->dtype == PFB_F16) return launch_conv_umma<__half>(tms, tmW, tmO, a, grid, smem, s);
-  return launch_conv_umma<__nv_bfloat16>(tms, tmW, tmO, a, grid, smem, s);
+  return launch();
 }
 
 }  // namespace pfb
+
+extern "C" PFB_API int pfb_conv2d_umma_plan(const pfb_conv_params* p, int* pixels_per_item, int* n_tile, size_t* smem_bytes) {
+  using namespace pfb;
+  PFB_CHECK_ARG(p && pixels_per_item && n_tile && smem_bytes, "conv2d_umma_plan: null pointer");
+  *pixels_per_item = *n_tile = 0;
+  *smem_bytes = 0;
+  if (!conv2d_umma_supported(p)) return PFB_OK;
+  ConvUmmaArgs a{};
+  bool wide = false;
+  if (!plan_conv(p, a, wide)) return PFB_OK;
+  *pixels_per_item = a.TW * a.TH;
+  *n_tile = a.NT;
+  *smem_bytes = conv_smem_bytes(a, wide);
+  return PFB_OK;
+}
