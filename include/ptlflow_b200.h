@@ -720,6 +720,39 @@ PFB_API int pfb_sparse_lookup(const float* table, const float* coords, void* out
                               int out_stride, pfb_stream stream);
 
 /* ------------------------------------------------------------------------------------
+ * a22: LLA-Flow (ptlflow/models/llaflow/llaflow.py:140-217, aggregate.py, corr.py): local 5 x 5 similarity attention, the local
+ * aggregation of fmap2 and the shift-aggregated correlation term.  delta_l = (l / 5 - 2, l % 5 - 2) as (dy, dx), l = 0..24,
+ * clamp() = replicate padding (PatchExtra / ImgShift).  Features are pixel-major with 256 channels, the attention tables fp32
+ * [B*H*W, 25].
+ *   a[n, l] = softmax_l(<q[n], k[clamp(n + delta_l)]> / sqrt(128))                          (pfb_local_similar)
+ *   fmap2'  = fmap2 + lsa_gamma sum_l a2[n, l] v[clamp(n + delta_l)]                         (pfb_local_aggregate)
+ *   volume[n, m] = <fmap1[n], fmap2'[m]> / 16 + gamma sum_l a1[n, l] <f1'[clamp(n + delta_l)], f2''[clamp(m + delta_l)]> / 16
+ *                = <A'[n], B'[m]> with K = 26 x 256 = 6656:
+ *   A'[n] = [fmap1[n] / 16 | gamma a1[n, l] f1'[clamp(n + delta_l)] / 16 for l = 0..24],  B'[m] = [fmap2'[m] | f2''[clamp(m + delta_l)]]
+ * The volume and its pyramid go to the refinement loop as RAFT's: tiled (pfb_shift_volume_tiled, layout 1) or dense
+ * (pfb_corr_volume_build_ex over A' and B' with C = 6656, scale 1, layout 0).
+ * ---------------------------------------------------------------------------------- */
+/* qk [B,H,W,512] = [q1 | k1 | q2 | k2] (128 channels each: the two LocalSimilar to_qk convolutions stacked) -> a1, a2 fp32
+ * [B*H*W, 25].  Dot products and softmax in fp32.  Kernel class 6. */
+PFB_API int pfb_local_similar(const void* qk, float* a1, float* a2, int B, int H, int W, pfb_dtype dtype, pfb_stream stream);
+/* fmap2, v [B,H,W,256], a2 fp32 [B*H*W, 25] -> out [B,H,W,256] = fmap2 + gamma sum_l a2[n, l] v[clamp(n + delta_l)]; fp32 sums, one
+ * rounding.  Kernel class 6. */
+PFB_API int pfb_local_aggregate(const void* fmap2, const void* v, const float* a2, float gamma, void* out, int B, int H, int W,
+                                pfb_dtype dtype, pfb_stream stream);
+/* The volume's operands, each written when its pointer is not NULL:
+ *   a_pack [B*H*W, 6656] = A' (from fmap1, f1 = f1' [B,H,W,256] and a1; gamma and 1/16 folded in, one rounding);
+ *   b_pad  [B, H+4, W+4, 512] = [fmap2' | f2''] replicate-padded by 2 pixels (fmap2 = fmap2', f2 = f2'');
+ *   b_pack [B*H*W, 6656] = B'.
+ * Kernel class 6. */
+PFB_API int pfb_shift_pack(const void* fmap1, const void* f1, const float* a1, const void* fmap2, const void* f2, float gamma,
+                           void* a_pack, void* b_pad, void* b_pack, int B, int H, int W, pfb_dtype dtype, pfb_stream stream);
+/* The volume <A'[n], B'[m]> of the H x W grid from a_pack and b_pad (f16 / bf16, 16-byte aligned) as the tiled pyramid of
+ * pfb_corr_volume_build_tiled (levels 1..4, pyramid[l] sized by pfb_corr_level_bytes_tiled(B, H, W, H, W, l)): wgmma over 104
+ * K chunks of 64, the B tiles read as boxes of b_pad shifted by delta_l.  Kernel class 0 (volume). */
+PFB_API int pfb_shift_volume_tiled(const void* a_pack, const void* b_pad, void* const* pyramid, int B, int H, int W, int levels,
+                                   pfb_dtype dtype, pfb_stream stream);
+
+/* ------------------------------------------------------------------------------------
  * Encoder-side kernels (SURVEY.md section 8(f) rank 1: the callers either side of the path).
  * The first 7x7 convolution and the residual blocks' stride-1 3x3 convolutions of BasicEncoder (extractor.py:122-267)
  * run here, the strided, 1x1 and bottleneck convolutions in cuDNN; pre-processing, instance norm + ReLU (+ residual)

@@ -231,6 +231,11 @@ SIGNATURES = {
     "pfb_sparse_prepare": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _S]),
     "pfb_sparse_lookup": (_I, [_P, _P, _P, _I, _I, _I, _I, _I, _I, _S]),
     "pfb_convex_upsample4x": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
+    # LLA-Flow (a22)
+    "pfb_local_similar": (_I, [_P, _P, _P, _I, _I, _I, _I, _S]),
+    "pfb_local_aggregate": (_I, [_P, _P, _P, C.c_float, _P, _I, _I, _I, _I, _S]),
+    "pfb_shift_pack": (_I, [_P, _P, _P, _P, _P, C.c_float, _P, _P, _P, _I, _I, _I, _I, _S]),
+    "pfb_shift_volume_tiled": (_I, [_P, _P, _PP, _I, _I, _I, _I, _I, _S]),
 }
 
 

@@ -19,7 +19,7 @@ LIB_DIR = os.path.join(PKG, "lib")
 OBJ_DIR = os.path.join(HERE, "build")
 LIB_PATH = os.path.join(LIB_DIR, "libptlflow_b200.so")
 
-SOURCES = ["misc.cu", "prof.cu", "corr.cu", "conv_simt.cu", "refine.cu", "conv_umma.cu", "corr_umma.cu", "corr_tiled.cu", "corr_onthefly_umma.cu", "conv_special.cu", "tmap.cu", "encoder.cu", "first_conv.cu", "depthwise.cu", "skflow.cu", "searaft.cu", "msraft.cu", "ccmr.cu", "enc_conv_umma.cu", "attn1d.cu", "csflow.cu", "scv.cu", "knn_umma.cu"]
+SOURCES = ["misc.cu", "prof.cu", "corr.cu", "conv_simt.cu", "refine.cu", "conv_umma.cu", "corr_umma.cu", "corr_tiled.cu", "corr_onthefly_umma.cu", "conv_special.cu", "tmap.cu", "encoder.cu", "first_conv.cu", "depthwise.cu", "skflow.cu", "searaft.cu", "msraft.cu", "ccmr.cu", "enc_conv_umma.cu", "attn1d.cu", "csflow.cu", "scv.cu", "knn_umma.cu", "llaflow.cu"]
 NVCC_FLAGS = [
     "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-lineinfo", "-std=c++17",

@@ -14,9 +14,7 @@
 // so the epilogue of patch i overlaps the MMAs of patch i+1.
 #include <stdlib.h>
 
-#include <type_traits>
-
-#include "umma.cuh"
+#include "corr_umma.cuh"
 
 namespace pfb {
 using namespace sm90;
@@ -25,7 +23,6 @@ struct PyrOut {
   void* ptr[4];
 };
 
-constexpr int kTileBytes = 128 * 128;  // 128 rows x 64 halves
 constexpr int kMaxKChunks = 4;
 
 struct __align__(8) CorrBars {
@@ -35,30 +32,6 @@ struct __align__(8) CorrBars {
   uint64_t acc_full;
   uint64_t acc_empty;
 };
-
-constexpr int kCorrThreads = 13 * 32;
-
-// The MMA warpgroups of both volume kernels: D[128 queries][128 targets] of one patch, rows 64 * wg .. 64 * wg + 63 per
-// warpgroup.  `stage_of(i, k)` gives the ring stage holding chunk k of item i; the ring slot is released per item
-// (whole-K B stages, single_chunk = false) or per chunk (single_chunk = true).
-template <bool BF16>
-__device__ __forceinline__ void corr_mma_k(float (&d)[64], uint32_t a_base, uint32_t b_base, int kchunks_here, bool first) {
-  const int wg = (threadIdx.x >> 7) - 1;
-#pragma unroll 1
-  for (int k = 0; k < kchunks_here; ++k) {
-    const uint32_t al = gdesc_lo(a_base + k * kTileBytes + wg * 64 * 128, 16), bl = gdesc_lo(b_base + k * kTileBytes, 16);
-#pragma unroll
-    for (int kk = 0; kk < 4; ++kk)
-      wgmma<128, BF16>(d, gdesc(al + 2 * kk, kDescHiSw128), gdesc(bl + 2 * kk, kDescHiSw128), (first && k == 0 && kk == 0) ? 0u : 1u);
-  }
-}
-__device__ __forceinline__ void corr_acc_handoff(float (&d)[64], float* sacc, uint64_t* acc_empty, uint64_t* acc_full, int i) {
-  const int wg = (threadIdx.x >> 7) - 1;
-  mbar_wait(acc_empty, (i & 1) ^ 1);
-  acc_store<128>(sacc, d, wg * 64, threadIdx.x & 127);
-  __syncwarp();
-  if ((threadIdx.x & 31) == 0) mbar_arrive(acc_full);
-}
 
 template <typename T>
 __device__ __forceinline__ float rt(float v) { return to_f32(from_f32<T>(v)); }
@@ -274,29 +247,10 @@ struct __align__(8) CorrTBars {
   uint64_t acc_empty;
 };
 
-struct TiledOut {
-  void* ptr[4];
-  int h[4], w[4], tiles_x[4];
-  unsigned map_elems[4];
-};
-
 __device__ __forceinline__ void tma_store_5d(const CUtensorMap* m, const void* src, int c0, int c1, int c2, int c3, int c4) {
   asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];"
                ::"l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(src)), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
                : "memory");
-}
-
-template <typename T>
-__device__ __forceinline__ uint32_t cvt_pack2(float lo, float hi);
-template <>
-__device__ __forceinline__ uint32_t cvt_pack2<__half>(float lo, float hi) {
-  __half2 h = __floats2half2_rn(lo, hi);
-  return *reinterpret_cast<uint32_t*>(&h);
-}
-template <>
-__device__ __forceinline__ uint32_t cvt_pack2<__nv_bfloat16>(float lo, float hi) {
-  __nv_bfloat162 h = __floats2bfloat162_rn(lo, hi);
-  return *reinterpret_cast<uint32_t*>(&h);
 }
 
 template <typename T>
@@ -315,8 +269,7 @@ corr_volume_tiled_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int m_tile = blockIdx.x, b = blockIdx.z;
   const int PW = (W + 15) / 16, PH = (H + 7) / 8;
-  const int n_patches = PW * PH;
-  const int n_items = n_patches;
+  const int n_items = PW * PH;
 
   if (threadIdx.x == 0) {
     mbar_init(&bars->a_full, 1);
@@ -374,7 +327,7 @@ corr_volume_tiled_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
     }
   } else {
     // ================= epilogue: 4 warps, thread <-> query row =================
-    const int quarter = warp & 3, grp = 0;
+    const int quarter = warp & 3;
     const int row = quarter * 32 + lane;
     const int n1 = m_tile * 128 + row;
     const bool row_ok = n1 < N1;
@@ -383,100 +336,11 @@ corr_volume_tiled_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_c
     T* o1 = levels > 1 ? reinterpret_cast<T*>(out.ptr[1]) + q * out.map_elems[1] : nullptr;
     T* o2 = levels > 2 ? reinterpret_cast<T*>(out.ptr[2]) + q * out.map_elems[2] : nullptr;
     T* o3 = levels > 3 ? reinterpret_cast<T*>(out.ptr[3]) + q * out.map_elems[3] : nullptr;
-    const float s1 = 0.25f * scale, s2 = 0.0625f * scale, s3 = 0.015625f * scale;
-    const bool leader = (row == 0);
     for (int i = 0; i < n_items; ++i) {
-      const int p = i;
-      const bool p_ok = p < n_patches;
-      const int ph = p / PW, pw = p - ph * PW;
-      mbar_wait(&bars->acc_full, i & 1);
-      float l2acc[4], l3acc[2];
-#pragma unroll
-      for (int c = 0; c < 4; ++c) {  // 32 accumulator columns = patch rows 2c, 2c+1 (16 columns each)
-        uint32_t r[32];
-        acc_ld32(sacc, row, c * 32, r);
-        if (c == 0 && i > 0) {  // the previous bulk store of this group must have drained the staging buffer
-          if (leader) tma_store_wait_read();
-          named_barrier_sync(1 + grp, 128);
-        }
-        // ---- level 0: scale, pack, stage.  patch row rr -> tile row rr >> 2, row-in-tile rr & 3; columns 0-7 / 8-15 -> tile column 0 / 1
-#pragma unroll
-        for (int e = 0; e < 2; ++e) {
-          const int rr = 2 * c + e;
-#pragma unroll
-          for (int txh = 0; txh < 2; ++txh) {
-            uint4 u;
-            u.x = cvt_pack2<T>(__uint_as_float(r[e * 16 + txh * 8 + 0]) * scale, __uint_as_float(r[e * 16 + txh * 8 + 1]) * scale);
-            u.y = cvt_pack2<T>(__uint_as_float(r[e * 16 + txh * 8 + 2]) * scale, __uint_as_float(r[e * 16 + txh * 8 + 3]) * scale);
-            u.z = cvt_pack2<T>(__uint_as_float(r[e * 16 + txh * 8 + 4]) * scale, __uint_as_float(r[e * 16 + txh * 8 + 5]) * scale);
-            u.w = cvt_pack2<T>(__uint_as_float(r[e * 16 + txh * 8 + 6]) * scale, __uint_as_float(r[e * 16 + txh * 8 + 7]) * scale);
-            // staging = TMA box [tile row 2][query 128][128 bytes = the two tiles of that tile row], 128-byte swizzle:
-            // 16-byte chunk (tile column txh, row-in-tile rr & 3) of query `row` sits at chunk index ^ (row & 7)
-            const int cidx = (txh * 4 + (rr & 3)) ^ (row & 7);
-            *reinterpret_cast<uint4*>(sCg + (((rr >> 2) * 128 + row) * 128 + cidx * 16)) = u;
-          }
-        }
-        // ---- pooled levels from the fp32 accumulators (one rounding per stored value) ----
-        float l1[8];
-#pragma unroll
-        for (int j = 0; j < 8; ++j)
-          l1[j] = (__uint_as_float(r[2 * j]) + __uint_as_float(r[2 * j + 1])) + (__uint_as_float(r[16 + 2 * j]) + __uint_as_float(r[16 + 2 * j + 1]));
-        if (o1 && row_ok && p_ok) {
-          const int i1 = ph * 4 + c, j1 = pw * 8;
-          if (i1 < out.h[1] && j1 < out.w[1]) {
-            const int valid = out.w[1] - j1;  // columns of this tile inside the map; the rest are pad columns = 0
-            uint4 u;
-            u.x = cvt_pack2<T>(valid > 0 ? l1[0] * s1 : 0.f, valid > 1 ? l1[1] * s1 : 0.f);
-            u.y = cvt_pack2<T>(valid > 2 ? l1[2] * s1 : 0.f, valid > 3 ? l1[3] * s1 : 0.f);
-            u.z = cvt_pack2<T>(valid > 4 ? l1[4] * s1 : 0.f, valid > 5 ? l1[5] * s1 : 0.f);
-            u.w = cvt_pack2<T>(valid > 6 ? l1[6] * s1 : 0.f, valid > 7 ? l1[7] * s1 : 0.f);
-            *reinterpret_cast<uint4*>(o1 + (size_t)(ph * out.tiles_x[1] + pw) * 32 + c * 8) = u;
-          }
-        }
-        if ((c & 1) == 0) {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) l2acc[j] = l1[2 * j] + l1[2 * j + 1];
-        } else {
-#pragma unroll
-          for (int j = 0; j < 4; ++j) l2acc[j] += l1[2 * j] + l1[2 * j + 1];
-          if (o2 && row_ok && p_ok) {
-            const int i2 = ph * 2 + (c >> 1), j2 = pw * 4;
-            if (i2 < out.h[2] && j2 < out.w[2]) {
-              const int valid = out.w[2] - j2;
-              uint2 u;
-              u.x = cvt_pack2<T>(valid > 0 ? l2acc[0] * s2 : 0.f, valid > 1 ? l2acc[1] * s2 : 0.f);
-              u.y = cvt_pack2<T>(valid > 2 ? l2acc[2] * s2 : 0.f, valid > 3 ? l2acc[3] * s2 : 0.f);
-              *reinterpret_cast<uint2*>(o2 + (size_t)((i2 >> 2) * out.tiles_x[2] + (pw >> 1)) * 32 + (i2 & 3) * 8 + (pw & 1) * 4) = u;
-            }
-          }
-          if (c == 1) {
-            l3acc[0] = l2acc[0] + l2acc[1];
-            l3acc[1] = l2acc[2] + l2acc[3];
-          } else {
-            l3acc[0] += l2acc[0] + l2acc[1];
-            l3acc[1] += l2acc[2] + l2acc[3];
-            if (o3 && row_ok && p_ok) {
-              const int i3 = ph, j3 = pw * 2;
-              if (i3 < out.h[3] && j3 < out.w[3]) {
-                const int valid = out.w[3] - j3;
-                const uint32_t u = cvt_pack2<T>(l3acc[0] * s3, valid > 1 ? l3acc[1] * s3 : 0.f);
-                *reinterpret_cast<uint32_t*>(o3 + (size_t)((i3 >> 2) * out.tiles_x[3] + (pw >> 2)) * 32 + (i3 & 3) * 8 + (pw & 3) * 2) = u;
-              }
-            }
-          }
-        }
-      }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&bars->acc_empty);
-      fence_proxy_async();               // generic-proxy writes -> visible to the async (TMA) proxy
-      named_barrier_sync(1 + grp, 128);  // the four warps of this group
-      if (leader && p_ok) {
-        // dims (element along the tile row, query, tile row, sample): clipped at the map / N1 by the TMA unit
-        tma_store_4d(&tmO, sCg, pw * 64, m_tile * 128, ph * 2, b);
-        tma_store_commit();
-      }
+      const int ph = i / PW, pw = i - ph * PW;
+      tiled_epilogue_item<T>(sacc, sCg, &tmO, out, row, row_ok, o1, o2, o3, i, ph, pw, m_tile, b, scale, &bars->acc_full, &bars->acc_empty);
     }
-    if (leader) tma_store_wait_read();
+    if (row == 0) tma_store_wait_read();
   }
 }
 
@@ -560,6 +424,25 @@ bool corr_volume_tiled_supported(int B, int H, int W, int C, int L, pfb_dtype dt
   return true;
 }
 
+int tiled_out_maps(void* const* pyr, int B, int N1, int H, int W, int L, pfb_dtype dt, TiledOut* out, CUtensorMap* tmO) {
+  for (int l = 0; l < L; ++l) {
+    out->ptr[l] = pyr[l];
+    out->h[l] = H >> l;
+    out->w[l] = W >> l;
+    out->tiles_x[l] = (out->w[l] + 7) >> 3;
+    out->map_elems[l] = (unsigned)(((out->h[l] + 3) >> 2) * out->tiles_x[l] * 32);
+  }
+  // level-0 store map: a tile row of a query's map is tiles_x * 64 contiguous bytes, so the two tiles a patch owns in one
+  // tile row are ONE 128-byte run: box = [2 tile rows][128 queries][128 bytes], swizzled like an operand tile so that
+  // the per-thread 16-byte staging stores are conflict-free.  (The first version used 16-byte inner rows -- 2048 TMA
+  // requests per 32 KB box -- and ran at 1.56 TB/s; ncu r02b.)
+  const uint64_t tx0 = (uint64_t)out->tiles_x[0], ty0 = (uint64_t)((H + 3) >> 2), map_bytes = ty0 * tx0 * 64;
+  uint64_t dims[4] = {32 * tx0, (uint64_t)N1, ty0, (uint64_t)B};
+  uint64_t str[3] = {map_bytes, 64 * tx0, (uint64_t)N1 * map_bytes};
+  uint32_t box[4] = {64, 128, 2, 1};
+  return make_tensor_map(tmO, pyr[0], dt, 4, dims, str, box);
+}
+
 int corr_volume_tiled(const void* f1, const void* f2, void* const* pyr, int B, int N1, int H, int W, int C, int L, float scale,
                       pfb_dtype dt, cudaStream_t s) {
   const int kchunks = C / 64;
@@ -579,25 +462,7 @@ int corr_volume_tiled(const void* f1, const void* f2, void* const* pyr, int B, i
     if (rc) return rc;
   }
   TiledOut out{};
-  for (int l = 0; l < L; ++l) {
-    out.ptr[l] = pyr[l];
-    out.h[l] = H >> l;
-    out.w[l] = W >> l;
-    out.tiles_x[l] = (out.w[l] + 7) >> 3;
-    out.map_elems[l] = (unsigned)(((out.h[l] + 3) >> 2) * out.tiles_x[l] * 32);
-  }
-  {
-    // level-0 store map: a tile row of a query's map is tiles_x * 64 contiguous bytes, so the two tiles a patch owns in one
-    // tile row are ONE 128-byte run: box = [2 tile rows][128 queries][128 bytes], swizzled like an operand tile so that
-    // the per-thread 16-byte staging stores are conflict-free.  (The first version used 16-byte inner rows -- 2048 TMA
-    // requests per 32 KB box -- and ran at 1.56 TB/s; ncu r02b.)
-    const uint64_t tx0 = (uint64_t)out.tiles_x[0], ty0 = (uint64_t)((H + 3) >> 2), map_bytes = ty0 * tx0 * 64;
-    uint64_t dims[4] = {32 * tx0, (uint64_t)N1, ty0, (uint64_t)B};
-    uint64_t str[3] = {map_bytes, 64 * tx0, (uint64_t)N1 * map_bytes};
-    uint32_t box[4] = {64, 128, 2, 1};
-    int rc = make_tensor_map(&tmO, pyr[0], dt, 4, dims, str, box);
-    if (rc) return rc;
-  }
+  PFB_TRY(tiled_out_maps(pyr, B, N1, H, W, L, dt, &out, &tmO));
   const int m_tiles = ceil_div(N1, 128);
   const size_t smem = (size_t)kchunks * kTileBytes + 3 * kTileBytes + acc_tile_bytes(128) + 2 * kTileBytes + sizeof(CorrTBars) + 1024;
   dim3 grid(m_tiles, 1, B);

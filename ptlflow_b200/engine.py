@@ -180,11 +180,16 @@ class RaftEngine:
                             self.hidden_dim, self.context_dim, iters, int(alternate_corr), out_hw[0], out_hw[1], pad[0], pad[1],
                             self.impl, 0 if alternate_corr else int(volume_layout), int(fork_flow), self.num_heads)
 
+    def volume_tiled(self, fmap1: torch.Tensor, impl: int = 0) -> bool:
+        """Whether build_volume gives the tiled pyramid for these features: f16 / bf16 with tensor-core-shaped features and a
+        (radius, levels) pair the tiled lookup is instantiated for."""
+        return _TILED and impl != 1 and self.corr_radius in (3, 4) and ops.tiled_supported(fmap1, self.corr_levels) \
+            and (self.corr_radius, self.corr_levels) in ((4, 4), (4, 3), (4, 2), (4, 1), (3, 4), (3, 3))
+
     def build_volume(self, fmap1: torch.Tensor, fmap2: torch.Tensor, impl: int = 0):
-        """(a1 + a2 pyramid, its layout) for the refinement loop of this engine.  f16 / bf16 with tensor-core-shaped features get
-        the tiled pyramid (layout 1: 64-byte tiles, csrc/corr_tiled.cu); everything else the dense one (layout 0)."""
-        if _TILED and impl != 1 and self.corr_radius in (3, 4) and ops.tiled_supported(fmap1, self.corr_levels) \
-                and (self.corr_radius, self.corr_levels) in ((4, 4), (4, 3), (4, 2), (4, 1), (3, 4), (3, 3)):
+        """(a1 + a2 pyramid, its layout) for the refinement loop of this engine: the tiled pyramid (layout 1: 64-byte tiles,
+        csrc/corr_tiled.cu) where volume_tiled says so, else the dense one (layout 0)."""
+        if self.volume_tiled(fmap1, impl):
             return ops.corr_volume_build_tiled(fmap1, fmap2, self.corr_levels), 1
         return ops.corr_volume_build(fmap1, fmap2, self.corr_levels, impl=impl), 0
 
@@ -661,3 +666,39 @@ class SCVEngine(RaftEngine):
 
     def before_loop(self, pyramid: Sequence[torch.Tensor], coords: torch.Tensor) -> List[torch.Tensor]:
         return [ops.sparse_prepare(pyramid[0], pyramid[1], coords)]
+
+
+class LLAFlowEngine(RaftEngine):
+    """LLA-Flow (llaflow.py:140-217): GMA's loop (PFB_VARIANT_GMA, llaflow) or RAFT's (PFB_VARIANT_RAFT, llaflow_raft) over a volume with
+    the local-attention terms of aggregate.py.  Packs the stacked ls1 | ls2 query / key convolution (N = 512), lsa.to_v and s_lsa.to_f1 /
+    to_f2, and reads both gammas once; lla_volume builds the volume from (fmap1, fmap2, inp) as one K = 6656 GEMM (csrc/llaflow.cu)."""
+
+    def _pack(self, update_block: torch.nn.Module, attention_module: Optional[torch.nn.Module] = None, local=None) -> _lib.RaftWeights:
+        w = super()._pack(update_block, attention_module)
+        ls1, ls2, lsa, s_lsa, gamma = local
+
+        def P(convs, cin: int) -> ops.PackedConv:
+            return ops.PackedConv(convs, self.dtype, self.device, src_channels=[cin])
+
+        self.ls_qk = P([ls1.to_qk, ls2.to_qk], ls1.to_qk.in_channels)
+        self.lsa_v, self.to_f1, self.to_f2 = P([lsa.to_v], 256), P([s_lsa.to_f1], 256), P([s_lsa.to_f2], 256)
+        self.lsa_gamma = float(lsa.gamma.detach().float().cpu().item())
+        self.gamma = float(gamma.detach().float().cpu().item())
+        return w
+
+    def lla_volume(self, fmap1: torch.Tensor, fmap2: torch.Tensor, inp: torch.Tensor, impl: int = 0):
+        """(pyramid, layout) of corr.py:13-27 with corr2 of ShiftLSA: the tiled pyramid from pfb_shift_volume_tiled where RaftEngine's
+        volume_tiled holds for fmap1, else the dense pyramid of A' and the materialised B' on pfb_corr_volume_build_ex (SIMT: the
+        tensor-core volume takes C <= 256)."""
+        B, H, W, C = fmap1.shape
+
+        def conv(packed: ops.PackedConv, x: torch.Tensor) -> torch.Tensor:
+            return ops.conv2d([x], packed, torch.empty((B, H, W, packed.Cout), dtype=x.dtype, device=x.device), impl=impl)
+
+        a1, a2 = ops.local_similar(conv(self.ls_qk, inp))
+        fmap2p = ops.local_aggregate(fmap2, conv(self.lsa_v, fmap2), a2, self.lsa_gamma)
+        tiled = self.volume_tiled(fmap1, impl)
+        a, b = ops.shift_pack(fmap1, conv(self.to_f1, fmap1), a1, fmap2p, conv(self.to_f2, fmap2p), self.gamma, padded=tiled)
+        if tiled:
+            return ops.shift_volume_tiled(a, b, self.corr_levels), 1
+        return ops.corr_volume_build_ex(a, b, self.corr_levels, scale=1.0, impl=1), 0

@@ -197,6 +197,14 @@ class RAFT(BaseModel):
     def _attention(self, inp: torch.Tensor, eng):
         return None
 
+    def _correlation(self, fmap1: torch.Tensor, fmap2: torch.Tensor, inp: torch.Tensor, coords: torch.Tensor, eng):
+        """(pyramid, layout, fmap1 or None) that the refinement loop reads: with alternate_corr fmap2's feature pyramid for the
+        on-the-fly lookup, else the engine's volume after its before_loop.  ``inp``: the context features (llaflow's volume needs them)."""
+        if self.alternate_corr:
+            return ops.feature_pyramid(fmap2, self.corr_levels), 0, fmap1
+        pyramid, layout = eng.build_volume(fmap1, fmap2, impl=self.kernel_impl)
+        return eng.before_loop(pyramid, coords), layout, None  # csflow: the strip flow joins the start coordinates
+
     def _check_grid(self, h8: int, w8: int) -> None:
         """Raises ValueError, before anything is launched, for a 1/8-resolution grid (after padding) the model cannot run."""
 
@@ -314,11 +322,7 @@ class RAFT(BaseModel):
         net, inp = ops.context_split(cnet, self.hidden_dim, self.context_dim)
         coords = ops.init_coords(B, H8, W8, fmap1.device, flow_init)
 
-        if self.alternate_corr:
-            pyramid, layout, f1 = ops.feature_pyramid(fmap2, self.corr_levels), 0, fmap1
-        else:
-            (pyramid, layout), f1 = eng.build_volume(fmap1, fmap2, impl=self.kernel_impl), None
-            pyramid = eng.before_loop(pyramid, coords)  # csflow: the strip flow joins the start coordinates
+        pyramid, layout, f1 = self._correlation(fmap1, fmap2, inp, coords, eng)
 
         orig_h, orig_w = images.shape[-2:]
         pad_top, pad_left = resizer.pad_top_left

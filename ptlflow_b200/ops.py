@@ -1038,3 +1038,78 @@ def convex_upsample4x(coords: torch.Tensor, mask: torch.Tensor, out_hw=None, pad
         check(load().pfb_convex_upsample4x(coords.data_ptr(), mask.data_ptr(), up.data_ptr(), small.data_ptr(), B, H, W, oh, ow,
                                            pad[0], pad[1], dtype_code(mask.dtype), stream_ptr(coords.device)), "convex_upsample4x")
     return up, small
+
+
+# ------------------------------------------------------------------------------------------
+# a22: LLA-Flow
+# ------------------------------------------------------------------------------------------
+LLA_TAPS, LLA_K = 25, 26 * 256  # the 5 x 5 local window; K of the shifted volume GEMM
+
+
+def local_similar(qk: torch.Tensor):
+    """qk [B,H,W,512] = [q1 | k1 | q2 | k2] -> (a1, a2) fp32 [B*H*W, 25]: softmax over the 5 x 5 clamped window of <q, k> / sqrt(128)."""
+    require_cuda(qk, "qk")
+    B, H, W, Cc = qk.shape
+    if Cc != 512:
+        raise RuntimeError(f"local_similar: qk must have 512 channels ([q1 | k1 | q2 | k2]), got {Cc}")
+    a1 = torch.empty((B * H * W, LLA_TAPS), dtype=torch.float32, device=qk.device)
+    a2 = torch.empty_like(a1)
+    with torch.cuda.device(qk.device):
+        check(load().pfb_local_similar(qk.data_ptr(), a1.data_ptr(), a2.data_ptr(), B, H, W, dtype_code(qk.dtype), stream_ptr(qk.device)),
+              "local_similar")
+    return a1, a2
+
+
+def _lla_check(name: str, *ts: torch.Tensor) -> None:
+    for i, t in enumerate(ts):
+        require_cuda(t, f"{name} arg {i}")
+        if t.shape != ts[0].shape or t.dtype != ts[0].dtype or t.dim() != 4 or t.shape[-1] != 256:
+            raise RuntimeError(f"{name}: features must be [B,H,W,256] of one shape and dtype")
+
+
+def local_aggregate(fmap2: torch.Tensor, v: torch.Tensor, a2: torch.Tensor, gamma: float) -> torch.Tensor:
+    """fmap2 + gamma * sum_l a2[:, l] v[clamp(n + delta_l)] -> [B,H,W,256] in the storage type."""
+    _lla_check("local_aggregate", fmap2, v)
+    require_cuda(a2, "a2")
+    B, H, W, _ = fmap2.shape
+    out = torch.empty_like(fmap2)
+    with torch.cuda.device(fmap2.device):
+        check(load().pfb_local_aggregate(fmap2.data_ptr(), v.data_ptr(), a2.data_ptr(), float(gamma), out.data_ptr(), B, H, W,
+                                         dtype_code(fmap2.dtype), stream_ptr(fmap2.device)), "local_aggregate")
+    return out
+
+
+def shift_pack(fmap1: torch.Tensor, f1: torch.Tensor, a1: torch.Tensor, fmap2p: torch.Tensor, f2: torch.Tensor, gamma: float,
+               padded: bool = True):
+    """The shifted volume's operands: (A' [B,H,W,6656], [fmap2' | f2''] replicate-padded [B,H+4,W+4,512]) when ``padded``, else
+    (A', B' [B,H,W,6656])."""
+    _lla_check("shift_pack", fmap1, f1, fmap2p, f2)
+    require_cuda(a1, "a1")
+    B, H, W, _ = fmap1.shape
+    a = torch.empty((B, H, W, LLA_K), dtype=fmap1.dtype, device=fmap1.device)
+    b = torch.empty((B, H + 4, W + 4, 512) if padded else (B, H, W, LLA_K), dtype=fmap1.dtype, device=fmap1.device)
+    with torch.cuda.device(fmap1.device):
+        check(load().pfb_shift_pack(fmap1.data_ptr(), f1.data_ptr(), a1.data_ptr(), fmap2p.data_ptr(), f2.data_ptr(), float(gamma),
+                                    a.data_ptr(), b.data_ptr() if padded else None, None if padded else b.data_ptr(), B, H, W,
+                                    dtype_code(fmap1.dtype), stream_ptr(fmap1.device)), "shift_pack")
+    return a, b
+
+
+def shift_volume_tiled(a_pack: torch.Tensor, b_pad: torch.Tensor, levels: int = 4) -> List[torch.Tensor]:
+    """A' [B,H,W,6656], padded [fmap2' | f2''] [B,H+4,W+4,512] (f16 / bf16) -> the tiled pyramid of <A'[n], B'[m]> (as
+    corr_volume_build_tiled returns it)."""
+    require_cuda(a_pack, "a_pack"); require_cuda(b_pad, "b_pad")
+    B, H, W, K = a_pack.shape
+    if K != LLA_K or tuple(b_pad.shape) != (B, H + 4, W + 4, 512) or b_pad.dtype != a_pack.dtype:
+        raise RuntimeError("shift_volume_tiled: a_pack [B,H,W,6656] and b_pad [B,H+4,W+4,512] of one dtype")
+    lib = load()
+    pyr = []
+    for l in range(levels):
+        nbytes = lib.pfb_corr_level_bytes_tiled(B, H, W, H, W, l)
+        if nbytes == 0:
+            raise RuntimeError(f"shift_volume_tiled: {H}x{W} grid too small for {levels} levels")
+        pyr.append(torch.empty((B * H * W, nbytes // (2 * B * H * W)), dtype=a_pack.dtype, device=a_pack.device))
+    with torch.cuda.device(a_pack.device):
+        check(lib.pfb_shift_volume_tiled(a_pack.data_ptr(), b_pad.data_ptr(), ptr_array(pyr), B, H, W, levels, dtype_code(a_pack.dtype),
+                                         stream_ptr(a_pack.device)), "shift_volume_tiled")
+    return pyr
