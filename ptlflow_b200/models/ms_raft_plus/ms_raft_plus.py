@@ -23,7 +23,7 @@ import torch.nn.functional as F
 from ... import _lib, ops
 from ...engine import MSRaftEngine
 from ...utils.registry import register_model, trainable
-from ..raft.extractor import _NATIVE_CONV1, _Encoder, _conv_pm
+from ..raft.extractor import _Encoder, _EncConv, _block, _run
 from ..raft.raft import RAFT, _cudnn_flags
 from ..raft.update import BasicUpdateBlock, _no_forward
 
@@ -100,89 +100,34 @@ class _PyramidEncoder(_Encoder):
         self.in_planes = dim
         return nn.Sequential(*layers)
 
-    # ---- inference path: cuDNN convolutions + this library's group norm / resize kernels ----
-    def _prepare_locked(self, sig, dtype, device):
-        f32 = lambda t: t.detach().to(device=device, dtype=torch.float32).contiguous()  # noqa: E731
+    # ---- inference path: planned convolutions (_EncConv) and this library's resize kernel ----
+    def _plan(self, dtype, device):
+        """(first convolution, [layer1..4 blocks], conv2, [(up layer's blocks, its after-up convolution or None)]) as steps.  The
+        3x3s stay on cuDNN: pfb_enc_conv3x3 has no group-norm epilogue."""
+        def blocks(name):  # a block that changes the channel count at stride 1 returns its branch without the residual
+            return [_block(blk.downsample, [(blk.conv1, blk.norm1), (blk.conv2, blk.norm2)], dtype, device,
+                           join=blk.conv1.in_channels == blk.conv2.out_channels or blk.downsample is not None) for blk in getattr(self, name)]
 
-        def conv(c: nn.Conv2d, norm: Optional[nn.GroupNorm]):
-            e = {"w": c.weight.detach().to(device=device, dtype=dtype).contiguous(memory_format=torch.channels_last), "b": f32(c.bias),
-                 "stride": c.stride[0], "padding": c.padding[0]}
-            if norm is not None:
-                e["gamma"], e["beta"], e["eps"] = f32(norm.weight), f32(norm.bias), float(norm.eps)
-                e["group"] = c.out_channels // norm.num_groups
-            return e
+        def linear(conv):  # conv2 and CCMR's after-up 1x1s: convolution + bias
+            return _EncConv(conv, None, dtype, device, relu=False)
 
-        prep = {"conv1": conv(self.conv1, self.norm1), "conv2": conv(self.conv2, None), "layers": {}, "after": {}}
-        ups = [f"up_layer{k}" for k in range(2, 2 - self.num_up, -1)]
-        for name in ups:
-            after = getattr(self, f"after_{name}_conv", None)
-            if after is not None:
-                prep["after"][name] = conv(after, None)
-        for name in ["layer1", "layer2", "layer3", "layer4"] + ups:
-            blocks = []
-            for blk in getattr(self, name):
-                e = {"conv1": conv(blk.conv1, blk.norm1), "conv2": conv(blk.conv2, blk.norm2),
-                     "residual": blk.conv1.in_channels == blk.conv2.out_channels or blk.downsample is not None}
-                if blk.downsample is not None:
-                    e["down"] = conv(blk.downsample[0], blk.downsample[1])
-                blocks.append(e)
-            prep["layers"][name] = blocks
-        if _NATIVE_CONV1 and dtype in (torch.float16, torch.bfloat16) and tuple(self.conv1.weight.shape) == (64, 3, 7, 7):
-            prep["conv1_native"] = ops.pack_first_conv(self.conv1.weight.detach().to(device).float(), dtype)
-        torch.cuda.current_stream(device).synchronize()  # the casts / pack ran on this thread's stream: finish before others see them
-        self._prep_cache = (sig, prep)
-        return prep
-
-    @staticmethod
-    def _conv_gn(x: torch.Tensor, e: dict, relu: bool = True, residual: Optional[torch.Tensor] = None) -> torch.Tensor:
-        # the convolution without its bias; the group norm folds the bias into its statistics (unlike instance norm, a bias that
-        # differs between the channels of a group is not removed by the group mean)
-        y = _conv_pm(x, (e["w"],), e["stride"], e["padding"])
-        return ops.group_norm_act(y, e["gamma"], e["beta"], e["group"], bias=e["b"], relu=relu, residual=residual, eps=e["eps"], out=y)
-
-    def _layer(self, x: torch.Tensor, blocks) -> torch.Tensor:
-        for e in blocks:
-            xs = x
-            if "down" in e:
-                xs = self._conv_gn(x, e["down"], relu=False)
-            y = self._conv_gn(x, e["conv1"])
-            x = self._conv_gn(y, e["conv2"], relu=True, residual=xs if e["residual"] else None)
-        return x
+        ups = []
+        for k in range(2, 2 - self.num_up, -1):
+            after = getattr(self, f"after_up_layer{k}_conv", None)
+            ups.append((blocks(f"up_layer{k}"), None if after is None else linear(after)))
+        return (_EncConv(self.conv1, self.norm1, dtype, device, native="first_conv7x7s2"), [blocks(f"layer{k}") for k in range(1, 5)],
+                linear(self.conv2), ups)
 
     def forward_pm(self, x: torch.Tensor):
         """x: pixel-major frames [N,H,W,Cf] (H, W multiples of 16; channels past RGB zero) -> [1/16, 1/8, 1/4, 1/2] features."""
-        prep = self._prepared(x.dtype, x.device)
-        c1 = prep["conv1"]
-        if "conv1_native" in prep and x.shape[-1] == 4 and x.is_contiguous():
-            # wgmma first convolution: its epilogue accumulates the per-(image, channel) sums the group norm combines
-            ws = ops.instance_norm_workspace((x.shape[0], 0, 0, 64), x.device)
-            y = ops.first_conv7x7s2(x, prep["conv1_native"], None, relu=False, stats_ws=ws)
-            x = ops.group_norm_act(y, c1["gamma"], c1["beta"], c1["group"], bias=c1["b"], relu=True, eps=c1["eps"], out=y, stats_ws=ws)
-        else:
-            if x.shape[-1] != c1["w"].shape[1]:  # zero frame channels beyond RGB: pad the filter to match
-                key = ("conv1_pad", x.shape[-1])
-                if key not in prep:
-                    w = torch.zeros((64, x.shape[-1], 7, 7), dtype=c1["w"].dtype, device=c1["w"].device)
-                    w[:, :3] = c1["w"]
-                    prep[key] = dict(c1, w=w.contiguous(memory_format=torch.channels_last))
-                c1 = prep[key]
-            x = self._conv_gn(x, c1)
-        L = prep["layers"]
-        e1 = self._layer(x, L["layer1"])
-        e2 = self._layer(e1, L["layer2"])
-        e3 = self._layer(e2, L["layer3"])
-        x = self._layer(e3, L["layer4"])
-        y = _conv_pm(x, (prep["conv2"]["w"],), 1, 0)
-        e4 = ops.bias_act(y, prep["conv2"]["b"], relu=False, out=y)
-        outs = [e4]
-        for k, skip in zip(range(2, 2 - self.num_up, -1), (e3, e2, e1)):
-            name = f"up_layer{k}"
-            u = self._layer(ops.upsample2x_concat(outs[-1], skip), L[name])
-            a = prep["after"].get(name)
-            if a is not None:  # CCMR's 1x1 after_up_layer conv with its bias
-                y = _conv_pm(u, (a["w"],), 1, 0)
-                u = ops.bias_act(y, a["b"], relu=False, out=y)
-            outs.append(u)
+        first, down, conv2, ups = self._prepared(x.dtype, x.device)
+        skips = [first(x)]
+        for blocks in down:
+            skips.append(_run(blocks, skips[-1]))
+        outs = [conv2(skips.pop())]
+        for blocks, after in ups:  # each on cat[2x resize(coarser), skip]: e3, e2, e1
+            u = _run(blocks, ops.upsample2x_concat(outs[-1], skips.pop()))
+            outs.append(u if after is None else after(u))
         return outs
 
     forward = _no_forward

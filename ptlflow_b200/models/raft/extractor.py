@@ -5,6 +5,7 @@ from __future__ import annotations
 
 import os
 import threading
+from typing import List, NamedTuple, Optional
 
 import torch
 import torch.nn as nn
@@ -76,26 +77,9 @@ class BottleneckBlock(nn.Module):
         return self.relu(x + y)
 
 
-def _fold(conv: nn.Conv2d, norm: nn.Module, dtype, device):
-    """(weight, bias) of ``conv`` in channels_last storage; an eval-mode BatchNorm that follows is folded in
-    (y = s * conv(x) + t  ->  weight * s, bias * s + t).  Instance norm / identity leave the conv as is."""
-    w = conv.weight.detach().to(device=device, dtype=torch.float32)
-    b = conv.bias.detach().to(device=device, dtype=torch.float32) if conv.bias is not None else torch.zeros(w.shape[0], device=device)
-    if isinstance(norm, nn.BatchNorm2d):
-        s = norm.weight.detach().float().to(device) / torch.sqrt(norm.running_var.detach().float().to(device) + norm.eps)
-        t = norm.bias.detach().float().to(device) - norm.running_mean.detach().float().to(device) * s
-        w = w * s.view(-1, 1, 1, 1)
-        b = b * s + t
-    w = w.to(dtype).contiguous(memory_format=torch.channels_last)
-    b = b.contiguous()  # fp32: added by this library's kernels
-    if dtype == torch.float32:
-        return w, b
-    return w, b, b.to(dtype)  # + the storage-type copy cuDNN's fused bias + ReLU epilogue wants (cast once, not per forward)
-
-
 _NATIVE_CONV1 = bool(int(os.environ.get("PFB_NATIVE_CONV1", "1")))
 _NATIVE_CONV2 = bool(int(os.environ.get("PFB_NATIVE_CONV2", "1")))
-# the residual blocks' 3x3 stride-1 convolutions on pfb_enc_conv3x3 (read at every forward: tools/time_encoder_convs.py
+# the residual blocks' 3x3 stride-1 convolutions on pfb_enc_conv3x3 (read at every call: tools/time_encoder_convs.py
 # switches it to compare both paths in one process)
 _NATIVE_ENC_CONV = bool(int(os.environ.get("PFB_NATIVE_ENC_CONV", "1")))
 # (Cin, Cout) of eligible layers that stay on cuDNN unless the kernel also takes their residual join: at 96 output channels
@@ -106,13 +90,12 @@ _CUDNN_FUSED_RELU = bool(int(os.environ.get("PFB_CUDNN_FUSED_RELU", "1")))
 _prep_lock = threading.Lock()
 
 
-def _conv_pm(x: torch.Tensor, wb, stride: int, padding: int) -> torch.Tensor:
-    """cuDNN convolution on a pixel-major tensor [N,H,W,C] -> [N,H',W',C'] (channels_last in and out, no copies)."""
-    # no bias here: PyTorch would add it as a separate broadcast kernel; it is folded into pfb_bias_act (batch / no norm)
-    # and is mathematically irrelevant in front of an instance norm (a per-channel constant is removed by the mean)
-    y = F.conv2d(x.permute(0, 3, 1, 2), wb[0], None, stride=stride, padding=padding)
-    y = y.permute(0, 2, 3, 1)
-    return y if y.is_contiguous() else y.contiguous()
+def _norm_kind(norm: Optional[nn.Module]) -> str:
+    if isinstance(norm, nn.InstanceNorm2d):
+        return "instance"
+    if isinstance(norm, nn.GroupNorm):
+        return "group"
+    return "batch" if isinstance(norm, nn.BatchNorm2d) else "none"
 
 
 def enc_conv_eligible(conv: nn.Conv2d, dtype: torch.dtype, fused_residual: bool = False) -> bool:
@@ -125,11 +108,152 @@ def enc_conv_eligible(conv: nn.Conv2d, dtype: torch.dtype, fused_residual: bool 
             and ops.enc_conv3x3_supported(conv.in_channels, conv.out_channels, dtype))
 
 
+def route_conv(conv: nn.Conv2d, norm: str, relu: bool, residual: bool, dtype: torch.dtype, native: Optional[str] = None) -> str:
+    """The kernel that runs an encoder convolution followed by ``norm`` ('instance', 'group', 'batch' (folded) or 'none'), ReLU
+    and the residual join, in this storage type.  ``native``: the library kernel the encoder offers the layer ('first_conv7x7s2'
+    for the 7x7 stride-2 first convolution, 'enc_conv3x3' for a residual block's convolutions, 'conv2d' for the 1x1 output
+    projection, None for cuDNN only); it is taken where the layer is that kernel's.  Else the cuDNN route:
+    'cudnn_convolution_relu' (cuDNN's bias + ReLU epilogue), or a cuDNN convolution and the norm pass 'instance_norm_act',
+    'group_norm_act' or 'bias_act'."""
+    half = dtype in (torch.float16, torch.bfloat16)
+    geometry = (tuple(conv.kernel_size), tuple(conv.stride), tuple(conv.padding), tuple(conv.dilation), conv.groups)
+    if native == "first_conv7x7s2" and _NATIVE_CONV1 and half and tuple(conv.weight.shape) == (64, 3, 7, 7) \
+            and geometry == ((7, 7), (2, 2), (3, 3), (1, 1), 1):
+        return native
+    # its epilogues: none (the instance norm follows), bias + ReLU (+ the residual join)
+    if (native == "enc_conv3x3" and relu and norm != "group"
+            and enc_conv_eligible(conv, dtype, fused_residual=residual and norm != "instance")):
+        return native
+    # cuDNN picked an sm_80 kernel without shared-memory staging for the projection (50 us per encoder, ncu launch list r02f),
+    # and its bias needed a pass of its own
+    if (native == "conv2d" and _NATIVE_CONV2 and half and geometry[:3] == ((1, 1), (1, 1), (0, 0)) and norm == "none"
+            and not relu and not residual and conv.in_channels % 64 == 0 and conv.out_channels % 32 == 0 and conv.out_channels <= 1024):
+        return native
+    if norm in ("instance", "group"):
+        return norm + "_norm_act"
+    if _CUDNN_FUSED_RELU and relu and not residual and half:
+        return "cudnn_convolution_relu"
+    return "bias_act"
+
+
+def _conv_pm(x: torch.Tensor, weight: torch.Tensor, stride, padding) -> torch.Tensor:
+    """cuDNN convolution on a pixel-major tensor [N,H,W,C] -> [N,H',W',C'] (channels_last in and out, no copies)."""
+    y = F.conv2d(x.permute(0, 3, 1, 2), weight, None, stride=stride, padding=padding)
+    y = y.permute(0, 2, 3, 1)
+    return y if y.is_contiguous() else y.contiguous()
+
+
+class _EncConv:
+    """One encoder convolution with the norm, ReLU and residual join that follow it, planned once per storage type and device:
+    ``route`` names the kernel (route_conv), ``cudnn_route`` the cuDNN route that runs where the input does not suit it.
+
+    Operands: ``weight``, the filter in the storage type (channels_last) with an eval-mode batch norm folded in (y = s * conv(x)
+    + t -> weight * s, bias * s + t); ``bias`` fp32, added by this library's kernels (or ignored in front of an instance norm,
+    whose mean removes it); ``bias_storage``, its storage-type copy for cuDNN's fused epilogue; the group norm's affine;
+    ``packed``, the library kernel's weights.  ``conv`` is the module it was planned from."""
+
+    def __init__(self, conv: nn.Conv2d, norm: Optional[nn.Module], dtype: torch.dtype, device, relu: bool = True,
+                 residual: bool = False, native: Optional[str] = None) -> None:
+        self.conv, self.relu, self.residual = conv, relu, residual
+        self.norm = _norm_kind(norm)
+        self.route = route_conv(conv, self.norm, relu, residual, dtype, native)
+        self.cudnn_route = route_conv(conv, self.norm, relu, residual, dtype)
+        self.stride, self.padding = tuple(conv.stride), tuple(conv.padding)
+        w = conv.weight.detach().to(device=device, dtype=torch.float32)
+        b = conv.bias.detach().to(device=device, dtype=torch.float32) if conv.bias is not None else torch.zeros(w.shape[0], device=device)
+        if self.norm == "batch":
+            s = norm.weight.detach().float().to(device) / torch.sqrt(norm.running_var.detach().float().to(device) + norm.eps)
+            t = norm.bias.detach().float().to(device) - norm.running_mean.detach().float().to(device) * s
+            w = w * s.view(-1, 1, 1, 1)
+            b = b * s + t
+        self.weight = w.to(dtype).contiguous(memory_format=torch.channels_last)
+        self.bias = b.contiguous()
+        # cast once, not per call
+        self.bias_storage = self.bias.to(dtype) if self.cudnn_route == "cudnn_convolution_relu" else None
+        if self.norm == "group":
+            self.gamma = norm.weight.detach().to(device=device, dtype=torch.float32).contiguous()
+            self.beta = norm.bias.detach().to(device=device, dtype=torch.float32).contiguous()
+            self.group, self.eps = conv.out_channels // norm.num_groups, float(norm.eps)
+        if self.route == "first_conv7x7s2":
+            self.packed = ops.pack_first_conv(w, dtype)
+        elif self.route == "enc_conv3x3":  # from the fp32 fold, rounded to the storage type once, as the cuDNN filter
+            self.packed = ops.PackedConv([ops.ConvWeights(w)], dtype, device, src_channels=[conv.in_channels])
+        elif self.route == "conv2d":  # the bias goes into the kernel's epilogue
+            self.packed = ops.PackedConv([conv], dtype, device, src_channels=[conv.in_channels])
+        self._padded = {}  # frame channel count -> the filter zero-padded to it
+
+    def __call__(self, x: torch.Tensor, residual: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """x [N,H,W,Cin] pixel-major -> [N,H',W',Cout]; ``residual`` (when the step takes the join) [N,H',W',Cout]."""
+        if self.route == "first_conv7x7s2" and x.shape[-1] == 4 and x.shape[1] % 2 == 0 and x.shape[2] % 2 == 0 and x.is_contiguous():
+            if self.norm in ("instance", "group"):  # the norm's per-(image, channel) sums come out of the kernel's epilogue
+                ws = ops.instance_norm_workspace((x.shape[0], 0, 0, 64), x.device)
+                y = ops.first_conv7x7s2(x, self.packed, None, relu=False, stats_ws=ws)
+                return self._norm_act(y, stats_ws=ws)
+            return ops.first_conv7x7s2(x, self.packed, self.bias, relu=self.relu)
+        if (self.route == "enc_conv3x3" and _NATIVE_ENC_CONV and x.is_contiguous()
+                and (residual is None or residual.is_contiguous())):
+            if self.norm == "instance":
+                return self._norm_act(ops.enc_conv3x3(x, self.packed), residual)
+            epi = _lib.ENC_CONV_BIAS_RELU if residual is None else _lib.ENC_CONV_BIAS_RELU_RESIDUAL
+            return ops.enc_conv3x3(x, self.packed, epi, bias=self.bias, residual=residual)
+        if self.route == "conv2d" and x.is_contiguous():
+            out = torch.empty(x.shape[:3] + (self.packed.Cout,), dtype=x.dtype, device=x.device)
+            return ops.conv2d([x], self.packed, out, epilogue=_lib.EPI_LINEAR)
+        w = self.weight
+        if x.shape[-1] != w.shape[1]:  # frames carry zero channels beyond RGB (8-byte pixels): pad the filter to match
+            if x.shape[-1] not in self._padded:
+                wp = torch.zeros((w.shape[0], x.shape[-1]) + tuple(w.shape[2:]), dtype=w.dtype, device=w.device)
+                wp[:, : w.shape[1]] = w
+                self._padded[x.shape[-1]] = wp.contiguous(memory_format=torch.channels_last)
+            w = self._padded[x.shape[-1]]
+        if self.cudnn_route == "cudnn_convolution_relu":
+            y = torch.cudnn_convolution_relu(x.permute(0, 3, 1, 2), w, self.bias_storage, self.stride, self.padding, (1, 1), 1)
+            y = y.permute(0, 2, 3, 1)
+            return y if y.is_contiguous() else y.contiguous()
+        # no bias in the convolution: PyTorch would add it as a broadcast kernel of its own
+        return self._norm_act(_conv_pm(x, w, self.stride, self.padding), residual)
+
+    def _norm_act(self, y: torch.Tensor, residual: Optional[torch.Tensor] = None, stats_ws: Optional[torch.Tensor] = None):
+        """The norm, ReLU and residual join on the convolution's output y, in place."""
+        if self.norm == "instance":
+            if stats_ws is not None:
+                return ops.instance_norm_apply(y, stats_ws, relu=self.relu, out=y)
+            return ops.instance_norm_act(y, relu=self.relu, residual=residual, out=y)
+        if self.norm == "group":  # the bias joins the statistics: a bias that differs within a group is not removed by its mean
+            return ops.group_norm_act(y, self.gamma, self.beta, self.group, bias=self.bias, relu=self.relu, residual=residual,
+                                      eps=self.eps, out=y, stats_ws=stats_ws)
+        return ops.bias_act(y, self.bias, relu=self.relu, residual=residual, out=y)
+
+
+class _Block(NamedTuple):
+    """A residual block's steps: ``down`` the shortcut's convolution (None: identity), ``convs`` the branch in order; the one
+    with ``residual`` set takes the join."""
+    down: Optional[_EncConv]
+    convs: List[_EncConv]
+
+
+def _block(down: Optional[nn.Sequential], convs, dtype, device, native: Optional[str] = None, join: bool = True) -> _Block:
+    """``down``: Sequential(1x1 convolution, norm) or None; ``convs``: the branch's (convolution, norm) pairs, each followed by
+    ReLU; the last takes the residual join when ``join``."""
+    last = len(convs) - 1
+    return _Block(None if down is None else _EncConv(down[0], down[1], dtype, device, relu=False),
+                  [_EncConv(c, n, dtype, device, residual=join and i == last, native=native) for i, (c, n) in enumerate(convs)])
+
+
+def _run(blocks, x: torch.Tensor) -> torch.Tensor:
+    for down, convs in blocks:
+        xs = x if down is None else down(x)
+        for step in convs:
+            x = step(x, xs if step.residual else None)
+    return x
+
+
 class _Encoder(nn.Module):
     block = ResidualBlock
     widths = (64, 64, 96, 128)
     strides = (1, 2, 2)  # of layer1..3: output at 1/8
     project_shortcut = False  # ResidualBlock(project=True) in every block
+    enc_conv3x3 = True  # the residual blocks' stride-1 3x3 convolutions on pfb_enc_conv3x3 where route_conv allows
 
     def __init__(self, output_dim: int = 128, norm_fn: str = "batch", dropout: float = 0.0) -> None:
         super().__init__()
@@ -154,7 +278,7 @@ class _Encoder(nn.Module):
         kw = {"project": True} if self.project_shortcut else {}
         return nn.Sequential(self.block(cin, cout, self.norm_fn, stride=stride, **kw), self.block(cout, cout, self.norm_fn, stride=1, **kw))
 
-    # ---- inference path: cuDNN convs + this library's fused norm / activation / residual kernels ----
+    # ---- inference path: planned convolutions (_EncConv) on cuDNN and this library's kernels ----
     def _signature(self, dtype, device):
         return (dtype, str(device)) + tuple((p.data_ptr(), p._version) for p in self.parameters()) + \
             tuple((b.data_ptr(), b._version) for b in self.buffers())
@@ -168,47 +292,27 @@ class _Encoder(nn.Module):
             cache = getattr(self, "_prep_cache", None)
             if cache is not None and cache[0] == sig:
                 return cache[1]
-            return self._prepare_locked(sig, dtype, device)
+            plan = self._plan(dtype, device)
+            # the fold / pack kernels ran on this thread's stream: finish them before other streams can see the cache
+            torch.cuda.current_stream(device).synchronize()
+            self._prep_cache = (sig, plan)
+            return plan
 
-    def _prepare_locked(self, sig, dtype, device):
-        prep = {"conv1": _fold(self.conv1, self.norm1, dtype, device), "conv2": _fold(self.conv2, nn.Identity(), dtype, device), "blocks": []}
-        for layer in (self.layer1, self.layer2, self.layer3):
-            for blk in layer:
-                e = {"stride": blk.conv2.stride[0] if isinstance(blk, BottleneckBlock) else blk.conv1.stride[0]}
-                names = ("conv1", "conv2", "conv3") if isinstance(blk, BottleneckBlock) else ("conv1", "conv2")
-                for i, nme in enumerate(names, start=1):
-                    e[nme] = _fold(getattr(blk, nme), getattr(blk, f"norm{i}"), dtype, device)
-                if blk.downsample is not None:
-                    e["down"] = _fold(blk.downsample[0], blk.downsample[1], dtype, device)
-                prep["blocks"].append(e)
-        if (_NATIVE_CONV1 and tuple(self.conv1.weight.shape) == (64, 3, 7, 7) and dtype in (torch.float16, torch.bfloat16)
-                and self.norm_fn in ("instance", "batch", "none")):
-            folded = _fold(self.conv1, self.norm1, torch.float32, device)
-            prep["conv1_native"] = (ops.pack_first_conv(folded[0], dtype), folded[1])
-        # the output projection (1x1, w3 -> output_dim) on this library's wgmma implicit-GEMM kernel with the bias in its
-        # epilogue: cuDNN picked an sm_80 kernel without shared-memory staging for it (50 us per encoder, ncu launch list r02f)
-        # and the bias needed a pass of its own
-        c2 = self.conv2
-        if (_NATIVE_CONV2 and dtype in (torch.float16, torch.bfloat16) and tuple(c2.kernel_size) == (1, 1) and c2.in_channels % 64 == 0
-                and c2.out_channels % 32 == 0 and c2.out_channels <= 1024):
-            prep["conv2_native"] = ops.PackedConv([c2], dtype, device, src_channels=[c2.in_channels])
-        # the residual blocks' 3x3 stride-1 convolutions on pfb_enc_conv3x3 (output channels on the MMA's M dimension): packed
-        # from the folded fp32 weights (rounded to the storage type once, as _fold does for cuDNN), with the fp32 bias.  Packed
-        # whatever PFB_NATIVE_ENC_CONV says: forward_pm reads the switch at every call
-        if dtype in (torch.float16, torch.bfloat16):
-            blocks = [blk for layer in (self.layer1, self.layer2, self.layer3) for blk in layer]
-            for e, blk in zip(prep["blocks"], blocks):
-                if not isinstance(blk, ResidualBlock):
-                    continue
-                for nme, norm in (("conv1", blk.norm1), ("conv2", blk.norm2)):
-                    conv = getattr(blk, nme)
-                    if enc_conv_eligible(conv, dtype, fused_residual=nme == "conv2" and self.norm_fn != "instance"):
-                        w, b = _fold(conv, norm, torch.float32, device)
-                        e[nme + "_enc"] = (ops.PackedConv([ops.ConvWeights(w)], dtype, device, src_channels=[conv.in_channels]), b)
-        # the fold / pack kernels ran on this thread's stream: finish them before other streams can see the cache
-        torch.cuda.current_stream(device).synchronize()
-        self._prep_cache = (sig, prep)
-        return prep
+    def _layers(self):
+        """((first convolution, its norm), [(shortcut or None, [(convolution, norm), ...]) per block], output projection)."""
+        blocks = []
+        for blk in (*self.layer1, *self.layer2, *self.layer3):
+            convs = [(blk.conv1, blk.norm1), (blk.conv2, blk.norm2)]
+            blocks.append((blk.downsample, convs + [(blk.conv3, blk.norm3)] if isinstance(blk, BottleneckBlock) else convs))
+        return (self.conv1, self.norm1), blocks, self.conv2
+
+    def _plan(self, dtype, device):
+        """(first convolution, output projection, blocks) as steps."""
+        (conv1, norm1), blocks, proj = self._layers()
+        native = "enc_conv3x3" if self.enc_conv3x3 else None
+        return (_EncConv(conv1, norm1, dtype, device, native="first_conv7x7s2"),
+                _EncConv(proj, None, dtype, device, relu=False, native="conv2d"),
+                [_block(down, convs, dtype, device, native) for down, convs in blocks])
 
     def forward_pm(self, x: torch.Tensor) -> torch.Tensor:
         """x: pixel-major frames [N,H,W,3] on CUDA -> features [N,H/8,W/8,C] (H/4 with strides (1, 2, 1)) (eval semantics of
@@ -216,66 +320,8 @@ class _Encoder(nn.Module):
         (+ residual join) is one fused pass (pfb_instance_norm_act) instead of five PyTorch kernels."""
         if self.norm_fn not in ("instance", "batch", "none"):
             return ops.to_pixel_major(self.forward(x.permute(0, 3, 1, 2)))
-        inst = self.norm_fn == "instance"
-        prep = self._prepared(x.dtype, x.device)
-
-        def conv_act(x, wb, stride, padding, relu=True, residual=None, native=None):
-            if (native is not None and _NATIVE_ENC_CONV and relu and x.is_contiguous()
-                    and (residual is None or residual.is_contiguous())):
-                packed, bias = native
-                if inst:  # the instance norm removes the bias
-                    y = ops.enc_conv3x3(x, packed)
-                    return ops.instance_norm_act(y, relu=True, residual=residual, out=y)
-                epi = _lib.ENC_CONV_BIAS_RELU if residual is None else _lib.ENC_CONV_BIAS_RELU_RESIDUAL
-                return ops.enc_conv3x3(x, packed, epi, bias=bias, residual=residual)
-            if _CUDNN_FUSED_RELU and not inst and relu and residual is None and x.dtype != torch.float32:
-                bh = wb[2] if len(wb) > 2 else wb[1].to(x.dtype)
-                y = torch.cudnn_convolution_relu(x.permute(0, 3, 1, 2), wb[0], bh, (stride, stride), (padding, padding), (1, 1), 1)
-                y = y.permute(0, 2, 3, 1)
-                return y if y.is_contiguous() else y.contiguous()
-            y = _conv_pm(x, wb, stride, padding)
-            if inst:
-                return ops.instance_norm_act(y, relu=relu, residual=residual, out=y)
-            return ops.bias_act(y, wb[1], relu=relu, residual=residual, out=y)
-
-        c1 = prep["conv1"]
-        native_c1 = ("conv1_native" in prep and x.shape[-1] == 4 and tuple(self.conv1.weight.shape) == (64, 3, 7, 7) and x.dtype in (torch.float16, torch.bfloat16)
-                     and x.shape[1] % 2 == 0 and x.shape[2] % 2 == 0)
-        if native_c1:
-            # wgmma first convolution (csrc/first_conv.cu): statistics of the instance norm come out of its epilogue,
-            # bias + ReLU of the folded batch norm are applied in it
-            wpack, bias = prep["conv1_native"]
-            if inst:
-                ws = ops.instance_norm_workspace((x.shape[0], 0, 0, 64), x.device)
-                y = ops.first_conv7x7s2(x, wpack, None, relu=False, stats_ws=ws)
-                x = ops.instance_norm_apply(y, ws, relu=True, out=y)
-            else:
-                x = ops.first_conv7x7s2(x, wpack, bias, relu=True)
-        elif x.shape[-1] != c1[0].shape[1]:  # frames carry zero channels beyond RGB (8-byte pixels): pad the filter to match
-            key = ("conv1_pad", x.shape[-1])
-            if key not in prep:
-                w = torch.zeros((c1[0].shape[0], x.shape[-1]) + tuple(c1[0].shape[2:]), dtype=c1[0].dtype, device=c1[0].device)
-                w[:, : c1[0].shape[1]] = c1[0]
-                prep[key] = (w.contiguous(memory_format=torch.channels_last), c1[1])
-            c1 = prep[key]
-        if not native_c1:
-            x = conv_act(x, c1, 2, 3)
-        for e in prep["blocks"]:
-            s = e["stride"]
-            xs = conv_act(x, e["down"], s, 0, relu=False) if "down" in e else x
-            if "conv3" in e:  # bottleneck: 1x1 -> 3x3 (stride) -> 1x1
-                y = conv_act(x, e["conv1"], 1, 0)
-                y = conv_act(y, e["conv2"], s, 1)
-                x = conv_act(y, e["conv3"], 1, 0, relu=True, residual=xs)
-            else:  # residual: 3x3 (stride) -> 3x3
-                y = conv_act(x, e["conv1"], s, 1, native=e.get("conv1_enc"))
-                x = conv_act(y, e["conv2"], 1, 1, relu=True, residual=xs, native=e.get("conv2_enc"))
-        if "conv2_native" in prep and x.is_contiguous():
-            packed = prep["conv2_native"]
-            out = torch.empty(x.shape[:3] + (packed.Cout,), dtype=x.dtype, device=x.device)
-            return ops.conv2d([x], packed, out, epilogue=_lib.EPI_LINEAR)
-        y = _conv_pm(x, prep["conv2"], 1, 0)
-        return ops.bias_act(y, prep["conv2"][1], relu=False, out=y)
+        first, proj, blocks = self._prepared(x.dtype, x.device)
+        return proj(_run(blocks, first(x)))
 
     def forward(self, x):
         """Accepts one tensor or a list/tuple of two (processed as one batch: instance norm is
@@ -300,3 +346,4 @@ class BasicEncoder(_Encoder):
 class SmallEncoder(_Encoder):
     block = BottleneckBlock
     widths = (32, 32, 64, 96)
+    enc_conv3x3 = False  # the bottlenecks stay on cuDNN

@@ -22,7 +22,7 @@ import torch.nn as nn
 from ... import _lib, ops
 from ...engine import SEARaftEngine
 from ...utils.registry import register_model, trainable
-from ..raft.extractor import _NATIVE_CONV1, _NATIVE_CONV2, _Encoder, _fold
+from ..raft.extractor import _Encoder
 from ..raft.raft import RAFT
 from ..raft.update import BasicMotionEncoder, _no_forward
 
@@ -51,6 +51,8 @@ class ResNetFPN(_Encoder):
     """sea_raft/extractor.py:6-116 with BatchNorm: conv1 7x7 / 2 -> bn1 -> ReLU -> three stages of BasicBlocks (1/2, 1/4, 1/8) ->
     final_conv 1x1.  Inference through _Encoder.forward_pm: every BatchNorm folded into its convolution (eval mode)."""
 
+    enc_conv3x3 = False  # its stride-1 3x3 layers stay on cuDNN, the 64 -> 64 and 128 -> 128 ones pfb_enc_conv3x3 supports included
+
     def __init__(self, block_dims: Sequence[int], initial_dim: int, pretrain: str, input_dim: int = 3, output_dim: int = 256) -> None:
         nn.Module.__init__(self)
         self.norm_fn = "batch"
@@ -74,26 +76,9 @@ class ResNetFPN(_Encoder):
         self.in_planes = dim
         return nn.Sequential(*layers)
 
-    def _prepare_locked(self, sig, dtype, device):
-        prep = {"conv1": _fold(self.conv1, self.bn1, dtype, device), "conv2": _fold(self.final_conv, nn.Identity(), dtype, device),
-                "blocks": []}
-        for layer in (self.layer1, self.layer2, self.layer3):
-            for blk in layer:
-                e = {"stride": blk.conv1.stride[0], "conv1": _fold(blk.conv1, blk.bn1, dtype, device),
-                     "conv2": _fold(blk.conv2, blk.bn2, dtype, device)}
-                if blk.downsample is not None:
-                    e["down"] = _fold(blk.downsample[0], blk.downsample[1], dtype, device)
-                prep["blocks"].append(e)
-        half = dtype in (torch.float16, torch.bfloat16)
-        if _NATIVE_CONV1 and half and tuple(self.conv1.weight.shape) == (64, 3, 7, 7):
-            folded = _fold(self.conv1, self.bn1, torch.float32, device)
-            prep["conv1_native"] = (ops.pack_first_conv(folded[0], dtype), folded[1])
-        fc = self.final_conv
-        if _NATIVE_CONV2 and half and fc.in_channels % 64 == 0 and fc.out_channels % 32 == 0 and fc.out_channels <= 1024:
-            prep["conv2_native"] = ops.PackedConv([fc], dtype, device, src_channels=[fc.in_channels])
-        torch.cuda.current_stream(device).synchronize()  # the fold / pack kernels finish before other streams see the cache
-        self._prep_cache = (sig, prep)
-        return prep
+    def _layers(self):
+        blocks = [(blk.downsample, [(blk.conv1, blk.bn1), (blk.conv2, blk.bn2)]) for blk in (*self.layer1, *self.layer2, *self.layer3)]
+        return (self.conv1, self.bn1), blocks, self.final_conv
 
     forward = _no_forward
 

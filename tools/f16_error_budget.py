@@ -44,7 +44,7 @@ def forward(sd, images, rnd: Rounder, variant="raft", iters=12, alternate_corr=F
     assert not small
     radius = r_default if corr_radius is None else corr_radius
     sd = {k: v.float() for k, v in sd.items() if v.is_floating_point()}
-    # weights as stored by the kernels: f16 weights, fp32 biases; batch norm folded in fp32 first (extractor._fold)
+    # weights as stored by the kernels: f16 weights, fp32 biases; batch norm folded in fp32 first (extractor._EncConv)
     sdw = {}
     for k, v in sd.items():
         if v.dim() == 4:

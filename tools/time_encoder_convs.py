@@ -1,6 +1,6 @@
 #!/usr/bin/env python
 """The encoders' stride-1 3x3 convolutions of the bench workload (RAFT, 1024x436 padded to 440, 8 pairs, f16): cuDNN as
-_Encoder.forward_pm calls it against pfb_enc_conv3x3, in one process.
+the encoders' planned convolutions (_EncConv in models/raft/extractor.py) call it against pfb_enc_conv3x3, in one process.
 
   1. one eager fnet + cnet pass per path under torch.profiler (CUDA activities): device time per kernel;
   2. every eligible layer shape timed with CUDA events, 50 launches per sample, the two paths alternating, with TFLOP/s,
@@ -99,38 +99,36 @@ def main():
 
     # ---- 2. per layer: CUDA events, the two paths alternating ----
     extractor._NATIVE_ENC_CONV = True
-    fprep = model.fnet._prepared(dt, torch.device(dev))
-    cprep = model.cnet._prepared(dt, torch.device(dev))
-    # (name, images, grid, block index, conv, kind, layers of this kind per encoder pass)
+    fblocks = model.fnet._prepared(dt, torch.device(dev))[2]
+    cblocks = model.cnet._prepared(dt, torch.device(dev))[2]
+    # (name, images, grid, the second block's conv1 or conv2 step, kind, layers of this kind per encoder pass)
     specs = []
-    for lname, (hh, ww), blocks in (("layer1", (220, 512), (0, 1)), ("layer2", (110, 256), (2, 3)), ("layer3", (55, 128), (4, 5))):
+    for lname, (hh, ww), blk in (("layer1", (220, 512), 1), ("layer2", (110, 256), 3), ("layer3", (55, 128), 5)):
         n_conv1 = 2 if lname == "layer1" else 1  # conv1 of layer2's and layer3's first block is strided
-        specs.append((lname, "fnet", 2 * B, (hh, ww), fprep["blocks"][blocks[1]], "conv1", "linear", n_conv1 + 2))
-        specs.append((lname, "cnet", B, (hh, ww), cprep["blocks"][blocks[1]], "conv1", "bias_relu", n_conv1))
-        specs.append((lname, "cnet", B, (hh, ww), cprep["blocks"][blocks[1]], "conv2", "bias_relu_residual", 2))
+        specs.append((lname, "fnet", 2 * B, (hh, ww), fblocks[blk].convs[0], "linear", n_conv1 + 2))
+        specs.append((lname, "cnet", B, (hh, ww), cblocks[blk].convs[0], "bias_relu", n_conv1))
+        specs.append((lname, "cnet", B, (hh, ww), cblocks[blk].convs[1], "bias_relu_residual", 2))
     layers = []
     ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     with torch.no_grad():
-        for lname, enc, nb, (hh, ww), e, cname, kind, per_pass in specs:
-            wb = e[cname]
-            routed = cname + "_enc" in e
-            if routed:
-                packed, bias = e[cname + "_enc"]
-            else:  # a layer the dispatch leaves on cuDNN: packed here from the same storage-rounded weights
-                packed = ops.PackedConv([ops.ConvWeights(wb[0].float())], dt, dev, src_channels=[wb[0].shape[1]])
-                bias = wb[1]
+        for lname, enc, nb, (hh, ww), step, kind, per_pass in specs:
+            routed = step.route == "enc_conv3x3"
+            # a layer the plan leaves on cuDNN: packed here from the same storage-rounded weights
+            packed = step.packed if routed else ops.PackedConv([ops.ConvWeights(step.weight.float())], dt, dev,
+                                                               src_channels=[step.weight.shape[1]])
+            bias = step.bias
             cin, cout = packed.Cin, packed.Cout
             x = (torch.randn(nb, hh, ww, cin, device=dev) * 0.5).relu().to(dt)
             r = (torch.randn(nb, hh, ww, cout, device=dev) * 0.5).relu().to(dt)
 
             def cudnn():
                 if kind == "linear":
-                    return extractor._conv_pm(x, wb, 1, 1)
+                    return extractor._conv_pm(x, step.weight, 1, 1)
                 if kind == "bias_relu":
-                    y = torch.cudnn_convolution_relu(x.permute(0, 3, 1, 2), wb[0], wb[2], (1, 1), (1, 1), (1, 1), 1)
+                    y = torch.cudnn_convolution_relu(x.permute(0, 3, 1, 2), step.weight, step.bias_storage, (1, 1), (1, 1), (1, 1), 1)
                     return y.permute(0, 2, 3, 1)
-                y = extractor._conv_pm(x, wb, 1, 1)
-                return ops.bias_act(y, wb[1], relu=True, residual=r, out=y)
+                y = extractor._conv_pm(x, step.weight, 1, 1)
+                return ops.bias_act(y, step.bias, relu=True, residual=r, out=y)
 
             def native():
                 if kind == "linear":
