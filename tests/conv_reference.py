@@ -69,13 +69,14 @@ def q(t: Tensor, dtype: torch.dtype) -> Tensor:
 
 
 def conv_terms(xs: Sequence[Tensor], weight: Tensor, bias: Optional[Tensor] = None, addend: Optional[Tensor] = None,
-               per_sample: bool = False) -> Tuple[Tensor, Tensor, int]:
+               per_sample: bool = False, stride: int = 1) -> Tuple[Tensor, Tensor, int]:
     """Pre-activation and magnitude sum of a convolution, float64, pixel-major.
 
     xs: the sources [B,H,W,Ci] (float64, storage-rounded), concatenated along channels.  weight: [Cout, sum Ci, KH, KW], or
     with ``per_sample`` [B, Cout, sum Ci] (1x1, one matrix per sample).  bias [Cout] or addend [B,H,W,Cout] (instead of the
-    bias).  Returns (acc, S, n): acc = conv + bias / addend and S = conv(|x|, |w|) + |bias| / |addend|, both [B,H,W,Cout], and
-    n, the number of terms each output adds."""
+    bias).  ``stride``: of the convolution, with the same zero padding KH // 2, KW // 2 (the encoders' 7x7 stride-2 conv1).
+    Returns (acc, S, n): acc = conv + bias / addend and S = conv(|x|, |w|) + |bias| / |addend|, both [B,Ho,Wo,Cout], and n,
+    the number of terms each output adds."""
     x = torch.cat([t.double() for t in xs], -1)
     w = weight.double()
     if per_sample:
@@ -85,8 +86,8 @@ def conv_terms(xs: Sequence[Tensor], weight: Tensor, bias: Optional[Tensor] = No
     else:
         kh, kw = w.shape[2], w.shape[3]
         xn = x.permute(0, 3, 1, 2)
-        acc = F.conv2d(xn, w, padding=(kh // 2, kw // 2)).permute(0, 2, 3, 1)
-        S = F.conv2d(xn.abs(), w.abs(), padding=(kh // 2, kw // 2)).permute(0, 2, 3, 1)
+        acc = F.conv2d(xn, w, padding=(kh // 2, kw // 2), stride=stride).permute(0, 2, 3, 1)
+        S = F.conv2d(xn.abs(), w.abs(), padding=(kh // 2, kw // 2), stride=stride).permute(0, 2, 3, 1)
         n = kh * kw * w.shape[1]
     if addend is not None:
         acc, S = acc + addend.double(), S + addend.double().abs()
