@@ -90,6 +90,9 @@ class RaftBuffers(C.Structure):
 PFB_SK_MAX_DW = 8
 SK_CONVC1, SK_CONVC2, SK_CONVF2, SK_CONV, SK_GRU, SK_FLOW_HEAD, SK_BLOCKS = range(7)
 KERNEL_CLASSES = 15  # PFB_KERNEL_CLASSES (12 = depthwise convolution, 13 = depthwise convolution + LayerNorm, 14 = 1D attention)
+# pfb_profile_collect's classes by index, in the header's order
+KERNEL_CLASS_NAMES = ("volume", "pool", "lookup", "onthefly", "conv", "upsample", "misc", "enc_affine", "enc_stats", "enc_conv1",
+                      "flowconv", "gather", "depthwise", "dw_layernorm", "attn1d")
 ATTN1D_CORR, ATTN1D_ATTN = 1, 2  # pfb_attn1d modes
 ATTN1D_MAX_L = 1024  # PFB_ATTN1D_MAX_L
 

@@ -36,6 +36,15 @@ def test_header_symbols_are_exported_and_bound(lib):
     assert sorted(_lib.SIGNATURES) == names
 
 
+def test_kernel_class_names_match_the_header():
+    """One name per profiler class: a class added to the header without a name here would drop out of every split."""
+    from ptlflow_b200 import _lib
+
+    declared = int(re.search(r"#define\s+PFB_KERNEL_CLASSES\s+(\d+)", open(HEADER).read()).group(1))
+    assert len(_lib.KERNEL_CLASS_NAMES) == _lib.KERNEL_CLASSES == declared
+    assert len(set(_lib.KERNEL_CLASS_NAMES)) == declared
+
+
 def test_version_and_error_channel(lib):
     assert lib.pfb_version() >= 100
     rc = lib.pfb_corr_lookup(None, None, None, 1, 8, 8, 4, 4, 0, 0, 0, 324, None)

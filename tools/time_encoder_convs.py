@@ -14,36 +14,18 @@ The full result (every sample, the profiler's kernel table) goes to --out, by de
 system's temporary directory; the summary is printed.
 """
 import argparse
-import ctypes as C
 import json
 import os
 import statistics
-import subprocess
-import sys
 import tempfile
 from argparse import Namespace
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import torch
 
+import timing  # (puts the repository root on sys.path)
 import ptlflow_b200 as pb
 from ptlflow_b200 import _lib, ops
 from ptlflow_b200.models.raft import extractor
-
-PEAK_TFLOPS, PEAK_TBS = 989.0, 3.35  # H100 SXM data sheet: dense f16 tensor, HBM3
-KC_NAMES = ["volume", "pool", "lookup", "onthefly", "conv", "upsample", "misc", "enc_affine", "enc_stats", "enc_conv1", "flowconv",
-            "gather", "depthwise", "dw_layernorm"]
-
-
-def card():
-    info = {"name": torch.cuda.get_device_name(0)}
-    try:
-        q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True,
-                           text=True, timeout=30).stdout.strip().splitlines()[0]
-        info["nvidia_smi"] = q
-    except (OSError, IndexError, subprocess.SubprocessError) as e:
-        info["nvidia_smi"] = f"unavailable: {e}"
-    return info
 
 
 def main():
@@ -62,7 +44,7 @@ def main():
     images = torch.rand(B, 2, 3, H, W, device=dev).to(dt)
     frames = torch.zeros(2 * B, 440, 1024, 4, device=dev, dtype=dt)
     frames[..., :3] = torch.rand(2 * B, 440, 1024, 3, device=dev).to(dt) * 2 - 1
-    res = {"card": card(), "workload": "raft 1024x436 (440 padded), 8 pairs, f16"}
+    res = {"card": timing.card(), "workload": "raft 1024x436 (440 padded), 8 pairs, f16"}
 
     def encoders():
         f = model.fnet.forward_pm(frames)
@@ -109,7 +91,6 @@ def main():
         specs.append((lname, "cnet", B, (hh, ww), cblocks[blk].convs[0], "bias_relu", n_conv1))
         specs.append((lname, "cnet", B, (hh, ww), cblocks[blk].convs[1], "bias_relu_residual", 2))
     layers = []
-    ev0, ev1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
     with torch.no_grad():
         for lname, enc, nb, (hh, ww), step, kind, per_pass in specs:
             routed = step.route == "enc_conv3x3"
@@ -143,25 +124,17 @@ def main():
                 cudnn(); native()
             for _ in range(a.rounds):
                 for path, fn in (("cudnn", cudnn), ("native", native)):
-                    torch.cuda.synchronize()
-                    ev0.record()
-                    for _ in range(a.launches):
-                        fn()
-                    ev1.record()
-                    ev1.synchronize()
-                    t[path].append(ev0.elapsed_time(ev1) * 1e3 / a.launches)
+                    t[path].append(timing.events_ms(fn, a.launches, 0) * 1e3)
             flop = 2.0 * nb * hh * ww * cout * cin * 9
             nbytes = 2.0 * nb * hh * ww * (cin + cout + (cout if kind == "bias_relu_residual" else 0))
             row = {"layer": lname, "encoder": enc, "images": nb, "grid": [hh, ww], "cin": cin, "cout": cout, "epilogue": kind,
                    "per_pass": per_pass, "routed_to_enc_conv": routed, "max_abs_diff": diff}
             for path in ("cudnn", "native"):
                 us = statistics.median(t[path])
-                row[path] = {"us": round(us, 2), "tflops": round(flop / us * 1e-6, 1), "gbs": round(nbytes / us * 1e-3, 1),
-                             "share_of_peak": round(max(flop / (PEAK_TFLOPS * 1e12), nbytes / (PEAK_TBS * 1e12)) / (us * 1e-6), 3),
-                             "samples_us": [round(v, 2) for v in t[path]]}
+                row[path] = {"us": round(us, 2), **timing.bound_share(us * 1e-3, flop, nbytes), "samples_us": [round(v, 2) for v in t[path]]}
             layers.append(row)
             print(f"{lname} {enc} {kind:20s} {nb:2d}x{hh}x{ww} {cin}->{cout}: cudnn {row['cudnn']['us']:8.1f} us "
-                  f"({row['cudnn']['tflops']:6.1f} TFLOP/s)  native {row['native']['us']:8.1f} us ({row['native']['tflops']:6.1f} TFLOP/s)"
+                  f"({row['cudnn']['tflop_per_s']:6.1f} TFLOP/s)  native {row['native']['us']:8.1f} us ({row['native']['tflop_per_s']:6.1f} TFLOP/s)"
                   f"  x{per_pass}/pass  max|diff| {diff:.3g}", flush=True)
     res["layers"] = layers
     for path in ("cudnn", "native"):
@@ -172,25 +145,15 @@ def main():
           f"as dispatched {res['dispatch_stride1_ms_per_step']} ms", flush=True)
 
     # ---- 3. eager per-class split of whole steps (one stream, no fork) ----
-    lib = _lib.load()
     res["eager_steps"] = {}
     with torch.no_grad():
         model.use_cuda_graph = False
         model.fork_encoders = model.fork_flow = False
         for native in (False, True, False, True):
             extractor._NATIVE_ENC_CONV = native
-            model({"images": images})
-            torch.cuda.synchronize()
-            lib.pfb_profile_enable(1)
-            ev0.record()
-            for _ in range(a.steps):
-                model({"images": images})
-            ev1.record()
-            ms_arr, n_arr = (C.c_double * 16)(), (C.c_ulonglong * 16)()
-            _lib.check(lib.pfb_profile_collect(ms_arr, n_arr, 16), "profile_collect")
-            lib.pfb_profile_enable(0)
-            step = ev0.elapsed_time(ev1) / a.steps
-            split = {KC_NAMES[k]: round(ms_arr[k] / a.steps, 3) for k in range(len(KC_NAMES)) if n_arr[k]}
+            step = timing.events_ms(lambda: model({"images": images}), a.steps, 1)
+            classes = timing.class_split(lambda: [model({"images": images}) for _ in range(a.steps)])
+            split = {k: round(v["ms"] / a.steps, 3) for k, v in classes.items()}
             key = "native" if native else "cudnn"
             res["eager_steps"].setdefault(key, []).append({"ms_per_step": round(step, 3), "classes_ms_per_step": split})
             print(f"eager step ({key}): {step:.3f} ms; {split}", flush=True)
