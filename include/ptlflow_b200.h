@@ -52,7 +52,7 @@ typedef enum {
 #define PFB_MAX_LEVELS 8
 #define PFB_MAX_SRC 4
 
-PFB_API int pfb_version(void);
+PFB_API int pfb_version(void); /* 101: pfb_raft_buffers gained agg_score (callers built for 100 pass a shorter struct) */
 PFB_API const char* pfb_last_error(void);
 /* sm major*10+minor of the current device, or negative status. */
 PFB_API int pfb_device_arch(void);
@@ -407,7 +407,9 @@ typedef struct {
   size_t workspace_bytes;
   const void* attention;      /* gma: softmax attention [heads, B, H*W, H*W] dtype, head-major (pfb_softmax_rows or
                                  pfb_attention_softmax_relpos) */
-  float agg_gamma;            /* gma: Aggregate.gamma */
+  float agg_gamma;            /* gma: Aggregate.gamma; craft: the aggregator's input_skip_coeff */
+  const float* agg_score;     /* craft: the aggregator's feat2score weight fp32 [128]: motion_global = pfb_craft_mode_aggregate of the
+                                 heads' attn @ v (no project); NULL for gma */
 } pfb_raft_buffers;
 
 PFB_API size_t pfb_raft_workspace_bytes(const pfb_raft_cfg* cfg);
@@ -750,6 +752,49 @@ PFB_API int pfb_shift_pack(const void* fmap1, const void* f1, const float* a1, c
  * pfb_corr_volume_build_tiled (levels 1..4, pyramid[l] sized by pfb_corr_level_bytes_tiled(B, H, W, H, W, l)): wgmma over 104
  * K chunks of 64, the B tiles read as boxes of b_pad shifted by delta_l.  Kernel class 0 (volume). */
 PFB_API int pfb_shift_volume_tiled(const void* a_pack, const void* b_pad, void* const* pyramid, int B, int H, int W, int levels,
+                                   pfb_dtype dtype, pfb_stream stream);
+
+/* ------------------------------------------------------------------------------------
+ * a23: CRAFT (ptlflow/models/craft/craft.py, setrans.py, corr.py): cross-attention with M modes (M <= 4), a (2R+1)^2 sliding
+ * position bias (R <= 15) and the batch-global clamp of CrossAttFeatTrans.  Per-mode logits are head-major [M, B, N, N] (N = H*W,
+ * query row i, key column j; (qy, qx) = divmod(i, W), (ky, kx) = divmod(j, W)), as pfb_corr_volume_build gives them for
+ * head-major q / k.  bias: fp32 [(2R+1)^2], already times the position weight; the bias of (i, j) is
+ * bias[(ky - qy + R) * (2R+1) + (kx - qx + R)] when |ky - qy| <= R and |kx - qx| <= R, else 0.  flag: int on the device, 1 when
+ * the clamp applies, so the decision never reaches the host.
+ * ---------------------------------------------------------------------------------- */
+/* *flag = 1 if any of the n values of x exceeds clip, else 0 (it zeroes *flag first).  Kernel class 6. */
+PFB_API int pfb_craft_clamp_flag(const void* x, size_t n, float clip, int* flag, pfb_dtype dtype, pfb_stream stream);
+/* In place on logits [rows, N], rows a multiple of N, grid at most 200 x 200:
+ *   attn[r, j] = softmax_j((flag ? clamp(logit, -clip, clip) : logit) + bias(i, j) - (mask_radius > 0 and
+ *                max(|ky - qy|, |kx - qx|) > mask_radius ? 1e9 : 0)),   i = r % N,
+ * in fp32, with the row in shared memory (the row machinery of pfb_attention_softmax_relpos).  Kernel class 6. */
+PFB_API int pfb_craft_window_softmax(void* logits, size_t rows, int H, int W, const float* bias, int R, int mask_radius,
+                                     const int* flag, float clip, pfb_dtype dtype, pfb_stream stream);
+/* LearnedSoftAggregate over M modes, the input skip and the LayerNorm of ExpandedFeatTrans (setrans.py:320-341, 465-468), one warp per
+ * pixel p < P:  y_m = feat[p, m F .. m F + F),  pi = softmax_m(<w, y_m>) (feat2score's bias cancels),
+ *   out[p] = LayerNorm_eps=1e-12(coeff skip[p] + sum_m pi_m y_m), no affine.
+ * F = 128 or 256; feat, skip and out are pixel-major with the given strides (elements) and offsets; out may be feat (M = 1, in
+ * place).  Kernel class 6. */
+PFB_API int pfb_craft_mode_aggregate(const void* feat, int feat_stride, int M, int F, const float* w, float coeff, const void* skip,
+                                     int skip_stride, int skip_offset, void* out, int out_stride, int out_offset, int P, pfb_dtype dtype,
+                                     pfb_stream stream);
+/* The inter-frame volume's level 0 [B*N, H, W] (corr.py:202-218 with do_corr_global_norm) from the per-mode scores [M, B, N, N]:
+ *   s_m = (flag ? clamp(score_m, -clip, clip) : score_m) + bias(i, j),   v = sum_m softmax_m(a s_m) s_m (M = 1: v = s_0),
+ *   level0[b] = (v - mean_b) / sqrt(var_b + 1e-12) over the N^2 values of sample b.
+ * v stays fp32 in the workspace until it is normalised; the statistics are fp64 per-CTA partials summed in a fixed order, so
+ * repeated runs are bit-identical.  Kernel class 6. */
+PFB_API size_t pfb_craft_volume_workspace_bytes(int B, int H, int W);
+PFB_API int pfb_craft_volume_norm(const void* scores, int M, float a, const float* bias, int R, const int* flag, float clip, void* level0,
+                                  void* workspace, size_t workspace_bytes, int B, int H, int W, pfb_dtype dtype, pfb_stream stream);
+/* The same level 0 and its pooled levels as the tiled pyramid of pfb_corr_volume_build_tiled (f16 / bf16, levels 1..4, pyramid[l] sized
+ * by pfb_corr_level_bytes_tiled(B, H, W, H, W, l)), fused on wgmma: q1 = LN(fmap1) Wq^T + b and k2 = LN(fmap2') Wq^T + b, pixel-major
+ * [B, H, W, 256] (mode m = channels m 256/M ..), 16-byte aligned; M in {1, 2, 4}.  Three passes over the K = 256 GEMM: the clamp flag
+ * (it zeroes *flag first), the per-sample statistics (fp64 per-CTA partials, summed in a fixed order), and the normalised values
+ * through the tiled epilogue.  The mode mix runs on the accumulators in fp32; nothing is rounded to the storage type before the
+ * normalisation.  Kernel class 0 (volume). */
+PFB_API size_t pfb_craft_volume_tiled_workspace_bytes(int B, int H, int W);
+PFB_API int pfb_craft_volume_tiled(const void* q1, const void* k2, int M, float a, const float* bias, int R, int* flag, float clip,
+                                   void* const* pyramid, void* workspace, size_t workspace_bytes, int B, int H, int W, int levels,
                                    pfb_dtype dtype, pfb_stream stream);
 
 /* ------------------------------------------------------------------------------------

@@ -82,7 +82,7 @@ class RaftBuffers(C.Structure):
         ("pyramid", C.POINTER(C.c_void_p)), ("fmap1", C.c_void_p), ("net", C.c_void_p), ("inp", C.c_void_p),
         ("coords", C.c_void_p), ("flow_up", C.c_void_p), ("flow_small", C.c_void_p),
         ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
-        ("attention", C.c_void_p), ("agg_gamma", C.c_float),
+        ("attention", C.c_void_p), ("agg_gamma", C.c_float), ("agg_score", C.c_void_p),
     ]
 
 
@@ -239,6 +239,14 @@ SIGNATURES = {
     "pfb_local_aggregate": (_I, [_P, _P, _P, C.c_float, _P, _I, _I, _I, _I, _S]),
     "pfb_shift_pack": (_I, [_P, _P, _P, _P, _P, C.c_float, _P, _P, _P, _I, _I, _I, _I, _S]),
     "pfb_shift_volume_tiled": (_I, [_P, _P, _PP, _I, _I, _I, _I, _I, _S]),
+    # CRAFT (a23)
+    "pfb_craft_clamp_flag": (_I, [_P, C.c_size_t, C.c_float, _P, _I, _S]),
+    "pfb_craft_window_softmax": (_I, [_P, C.c_size_t, _I, _I, _P, _I, _I, _P, C.c_float, _I, _S]),
+    "pfb_craft_mode_aggregate": (_I, [_P, _I, _I, _I, _P, C.c_float, _P, _I, _I, _P, _I, _I, _I, _I, _S]),
+    "pfb_craft_volume_workspace_bytes": (C.c_size_t, [_I, _I, _I]),
+    "pfb_craft_volume_norm": (_I, [_P, _I, C.c_float, _P, _I, _P, C.c_float, _P, _P, C.c_size_t, _I, _I, _I, _I, _S]),
+    "pfb_craft_volume_tiled_workspace_bytes": (C.c_size_t, [_I, _I, _I]),
+    "pfb_craft_volume_tiled": (_I, [_P, _P, _I, C.c_float, _P, _I, _P, C.c_float, _PP, _P, C.c_size_t, _I, _I, _I, _I, _I, _S]),
 }
 
 

@@ -5,6 +5,7 @@
 #include <atomic>
 
 #include "common.cuh"
+#include "softmax_row.cuh"
 
 namespace pfb {
 
@@ -259,34 +260,15 @@ __global__ void __launch_bounds__(256) softmax_rows_kernel(T* __restrict__ x, in
   for (int c = threadIdx.x; c < cols; c += blockDim.x) row[c] = from_f32<T>(expf(to_f32(row[c]) - m) * inv);
 }
 
-constexpr int kRelposThreads = 256;
-
-template <bool MAX>
-__device__ __forceinline__ float relpos_block_reduce(float v, float* red) {
-  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-  for (int o = 16; o > 0; o >>= 1) {
-    const float w = __shfl_xor_sync(0xffffffffu, v, o);
-    v = MAX ? fmaxf(v, w) : v + w;
-  }
-  if (lane == 0) red[warp] = v;
-  __syncthreads();
-  v = red[0];
-  for (int i = 1; i < kRelposThreads / 32; ++i) v = MAX ? fmaxf(v, red[i]) : v + red[i];
-  __syncthreads();
-  return v;
-}
-
 // GMA attention with the relative-position term (gma_utils.py:6-30, 62-74): one CTA per row r = (head, b, query i = x*W + y),
 // logit[u*W + v] = C[r][u*W + v] (or 0 without content) + Th[r][u - x + P - 1] + Tw[r][v - y + P - 1], softmax over the row in
-// fp32.  The row lives in shared memory between the passes, so HBM sees one read of C and one write of attn; the row's H + W
-// table entries are staged in shared memory too.  VEC: rows of a multiple of 16 bytes, moved with 16-byte loads / stores.
+// fp32 (softmax_row_smem).  The row's H + W table entries are staged in shared memory behind the row.
 template <typename T, bool VEC>
-__global__ void __launch_bounds__(kRelposThreads) attention_softmax_relpos_kernel(const T* __restrict__ logits, const float* __restrict__ th_tab,
-                                                                                  const float* __restrict__ tw_tab, size_t tstride,
-                                                                                  T* __restrict__ attn, int H, int W, int P) {
-  constexpr int EV = VEC ? 16 / (int)sizeof(T) : 1;
+__global__ void __launch_bounds__(kRowThreads) attention_softmax_relpos_kernel(const T* __restrict__ logits, const float* __restrict__ th_tab,
+                                                                               const float* __restrict__ tw_tab, size_t tstride,
+                                                                               T* __restrict__ attn, int H, int W, int P) {
   extern __shared__ __align__(16) float srow[];  // [N] row, then th [H], tw [W]
-  __shared__ float red[kRelposThreads / 32];
+  __shared__ float red[kRowThreads / 32];
   const int N = H * W;
   float* th = srow + N;
   float* tw = th + H;
@@ -294,70 +276,11 @@ __global__ void __launch_bounds__(kRelposThreads) attention_softmax_relpos_kerne
   const int i = (int)(r % (size_t)N), x = i / W, y = i - x * W;
   const float* thr = th_tab + r * tstride + (P - 1 - x);
   const float* twr = tw_tab + r * tstride + (P - 1 - y);
-  for (int u = threadIdx.x; u < H; u += kRelposThreads) th[u] = thr[u];
-  for (int v = threadIdx.x; v < W; v += kRelposThreads) tw[v] = twr[v];
+  for (int u = threadIdx.x; u < H; u += kRowThreads) th[u] = thr[u];
+  for (int v = threadIdx.x; v < W; v += kRowThreads) tw[v] = twr[v];
   __syncthreads();
-  const T* lrow = logits ? logits + r * N : nullptr;
-  T* arow = attn + r * N;
-  const int nvec = N / EV;
-
-  float m = -INFINITY;
-  for (int c = threadIdx.x; c < nvec; c += kRelposThreads) {
-    const int j0 = c * EV;
-    float f[EV];
-    if (lrow) {
-      if constexpr (VEC) {
-        const uint4 raw = *reinterpret_cast<const uint4*>(lrow + j0);
-        const T* e = reinterpret_cast<const T*>(&raw);
-#pragma unroll
-        for (int k = 0; k < EV; ++k) f[k] = to_f32(e[k]);
-      } else {
-        f[0] = to_f32(lrow[j0]);
-      }
-    } else {
-#pragma unroll
-      for (int k = 0; k < EV; ++k) f[k] = 0.f;
-    }
-    int u = j0 / W, v = j0 - u * W;
-#pragma unroll
-    for (int k = 0; k < EV; ++k) {
-      f[k] += th[u] + tw[v];
-      m = fmaxf(m, f[k]);
-      if (++v == W) { v = 0; ++u; }
-    }
-#pragma unroll
-    for (int k = 0; k < EV; k += 4 > EV ? EV : 4) {
-      if constexpr (EV >= 4) *reinterpret_cast<float4*>(srow + j0 + k) = make_float4(f[k], f[k + 1], f[k + 2], f[k + 3]);
-      else srow[j0 + k] = f[k];
-    }
-  }
-  m = relpos_block_reduce<true>(m, red);
-
-  float sum = 0.f;  // every thread revisits the entries it wrote: no barrier needed before this pass
-  for (int c = threadIdx.x; c < nvec; c += kRelposThreads) {
-    const int j0 = c * EV;
-#pragma unroll
-    for (int k = 0; k < EV; ++k) {
-      const float e = __expf(srow[j0 + k] - m);
-      srow[j0 + k] = e;
-      sum += e;
-    }
-  }
-  sum = relpos_block_reduce<false>(sum, red);
-  const float inv = 1.f / sum;
-
-  for (int c = threadIdx.x; c < nvec; c += kRelposThreads) {
-    const int j0 = c * EV;
-    if constexpr (VEC) {
-      uint4 raw;
-      T* e = reinterpret_cast<T*>(&raw);
-#pragma unroll
-      for (int k = 0; k < EV; ++k) e[k] = from_f32<T>(srow[j0 + k] * inv);
-      *reinterpret_cast<uint4*>(arow + j0) = raw;
-    } else {
-      arow[j0] = from_f32<T>(srow[j0] * inv);
-    }
-  }
+  softmax_row_smem<T, VEC>(logits ? logits + r * N : nullptr, attn + r * N, N, W, srow, red,
+                           [&](float f, int u, int v) { return f + (th[u] + tw[v]); });
 }
 
 // [B][HW][C] -> [B][C][HW_pad], zero fill for hw >= HW (32x32 smem tile transpose)
@@ -389,7 +312,7 @@ int launch_flow_from_coords(const float* coords, float* flow, int B, int H, int 
 
 using namespace pfb;
 
-extern "C" PFB_API int pfb_version(void) { return 100; }
+extern "C" PFB_API int pfb_version(void) { return 101; }
 extern "C" PFB_API const char* pfb_last_error(void) { return g_err; }
 
 extern "C" PFB_API int pfb_device_arch(void) {
@@ -551,7 +474,7 @@ static int launch_relpos_softmax(const void* logits, const float* th, const floa
     PFB_CUDA(cudaFuncSetAttribute(attention_softmax_relpos_kernel<T, VEC>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
     attr_done.fetch_or(1ull << (dev & 63), std::memory_order_release);
   }
-  attention_softmax_relpos_kernel<T, VEC><<<(unsigned)rows, kRelposThreads, smem, s>>>((const T*)logits, th, tw, tstride, (T*)attn, H, W, P);
+  attention_softmax_relpos_kernel<T, VEC><<<(unsigned)rows, kRowThreads, smem, s>>>((const T*)logits, th, tw, tstride, (T*)attn, H, W, P);
   return PFB_OK;
 }
 

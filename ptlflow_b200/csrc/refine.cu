@@ -141,7 +141,7 @@ static int heads_of(const pfb_raft_cfg* c) { return c->num_heads > 0 ? c->num_he
 
 int gma_aggregate(const pfb_raft_cfg* c, const pfb_layer& agg_v, const pfb_layer& agg_proj, const void* attention_ptr, float gamma,
                   void* motion, int motion_stride, int motion_offset, int out_offset, void* vbuf_ptr, void* vT_ptr, void* agg_ptr, int n_pad,
-                  cudaStream_t s) {
+                  cudaStream_t s, const float* mode_score) {
   PFB_CHECK_ARG(attention_ptr, "gma: null attention");
   const int N = c->H * c->W, heads = heads_of(c), vdim = heads * 128;
   const size_t es = dtype_size(c->dtype);
@@ -151,7 +151,9 @@ int gma_aggregate(const pfb_raft_cfg* c, const pfb_layer& agg_v, const pfb_layer
   // one head: attn @ v goes straight into the AXPY epilogue.  Several heads (gma_utils.py:101-111): every head's attn @ v
   // lands in its 128 columns of `agg`, then project (heads*128 -> 128) carries the AXPY epilogue.
   char* agg = heads > 1 ? reinterpret_cast<char*>(agg_ptr) : nullptr;
-  PFB_CHECK_ARG(heads == 1 || (agg_proj.weight && agg_proj.Cin == vdim),
+  // CRAFT (mode_score): the heads are the aggregator's modes, and pfb_craft_mode_aggregate of [motion | the heads' attn @ v] replaces
+  // project + AXPY (setrans.py:423-471); one mode's attn @ v lands in the motion_global columns and is aggregated there in place
+  PFB_CHECK_ARG(heads == 1 || mode_score || (agg_proj.weight && agg_proj.Cin == vdim),
                 "gma: num_heads=%d needs the Aggregate.project layer (%d -> 128)", heads, vdim);
   PFB_CHECK_ARG(agg_v.weight && agg_v.Cin == 128, "gma: Aggregate.to_v layer missing");
   {  // v = to_v(motion)
@@ -181,6 +183,7 @@ int gma_aggregate(const pfb_raft_cfg* c, const pfb_layer& agg_v, const pfb_layer
     const pfb_conv_src a = src_of(attention + ((size_t)h * c->B + b0) * N * N * es, N, N);
     if (heads > 1) return launch_conv(c, s, v, {a}, {PFB_EPI_LINEAR, agg + (size_t)b0 * N * vdim * es, vdim, h * 128}, e);
     char* mrow = reinterpret_cast<char*>(motion) + (size_t)b0 * N * motion_stride * es;
+    if (mode_score) return launch_conv(c, s, v, {a}, {PFB_EPI_LINEAR, mrow, motion_stride, out_offset}, e);
     e.aux_h = mrow + (size_t)motion_offset * es;
     e.hidden = motion_stride;
     return launch_conv(c, s, v, {a}, {PFB_EPI_AXPY, mrow, motion_stride, out_offset, gamma}, e);
@@ -188,6 +191,14 @@ int gma_aggregate(const pfb_raft_cfg* c, const pfb_layer& agg_v, const pfb_layer
   for (int h = 0; h < heads; ++h) {
     if (tensor_path && env_batched) PFB_TRY(attn_v(h, -1));
     else for (int b = 0; b < c->B; ++b) PFB_TRY(attn_v(h, b));
+  }
+  if (mode_score) {
+    const int P = c->B * N;
+    return heads > 1 ? pfb_craft_mode_aggregate(agg, vdim, heads, 128, mode_score, gamma, motion, motion_stride, motion_offset, motion,
+                                                motion_stride, out_offset, P, c->dtype, (pfb_stream)s)
+                     : pfb_craft_mode_aggregate(reinterpret_cast<char*>(motion) + (size_t)out_offset * es, motion_stride, 1, 128, mode_score,
+                                                gamma, motion, motion_stride, motion_offset, motion, motion_stride, out_offset, P, c->dtype,
+                                                (pfb_stream)s);
   }
   if (heads > 1) {  // motion_global = motion + gamma * project(out)   gma_utils.py:108-111
     pfb_layer proj = agg_proj;
@@ -442,7 +453,7 @@ static int update_iter(const Ctx& x, const void* corr_ext, void* mask_out) {
   // ---- gma: motion_global = motion + gamma * (attention @ to_v(motion))   gma_utils.py:101-113, gma/update.py:149 ----
   if (sp.aggregate == AGG_GMA)
     PFB_TRY(gma_aggregate(c, L[PFB_L_AGG_V], L[PFB_L_AGG_PROJ], x.b->attention, x.b->agg_gamma, motion, ws.c_motion, 0, 128,
-                          x.at(ws.off_vbuf), x.at(ws.off_vT), x.at(ws.off_agg), ws.n_pad, x.s));
+                          x.at(ws.off_vbuf), x.at(ws.off_vT), x.at(ws.off_agg), ws.n_pad, x.s, x.b->agg_score));
   // ---- ccmr: motion_global = aggregator(global_context, motion)   ccmr/update.py:156-161 ----
   if (sp.aggregate == AGG_CCMR) PFB_TRY(ccmr_aggregate(c, x.ccmr, motion, ws.c_motion, x.ccmr_base, x.s));
 

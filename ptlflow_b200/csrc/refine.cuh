@@ -99,7 +99,7 @@ int mask_head(const pfb_raft_cfg* c, cudaStream_t s, const ConvExtras& e, const 
 // out_offset .. +127.  vbuf [P][heads*128], vT [B][heads*128][n_pad], agg (heads > 1) [P][heads*128]: scratch of the storage type.
 int gma_aggregate(const pfb_raft_cfg* c, const pfb_layer& agg_v, const pfb_layer& agg_proj, const void* attention, float gamma,
                   void* motion, int motion_stride, int motion_offset, int out_offset, void* vbuf, void* vT, void* agg, int n_pad,
-                  cudaStream_t s);
+                  cudaStream_t s, const float* mode_score = nullptr);
 
 // The arguments of one scale of ms_raft_plus / ccmr: iters >= 1, corr_scale >= 0, next_coords or flow_up, and for the last scale
 // an output window inside the (2 << upflow2)-times grid and, with flow_small, at least 16 pixels per side

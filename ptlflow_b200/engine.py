@@ -58,6 +58,7 @@ class RaftEngine:
         self.corr_levels, self.corr_radius = corr_levels, corr_radius
         self.dtype, self.device, self.impl = dtype, device, impl
         self.agg_gamma, self.num_heads = 0.0, 1
+        self.agg_score: Optional[torch.Tensor] = None  # craft: the aggregator's feat2score weight (pfb_raft_buffers.agg_score)
         self.signature = None  # what the model built this engine for (RAFT._get_engine)
         self._keep: List[object] = []  # everything the weight structs point into
         self._workspaces: Dict[int, Tuple] = {}
@@ -233,7 +234,8 @@ class RaftEngine:
         """``symbol(cfg, weights, buffers, *args, stream)`` on the current stream of the engine's device."""
         pyr = ptr_array(pyramid) if pyramid is not None else None
         buf = _lib.RaftBuffers(C.cast(pyr, C.POINTER(C.c_void_p)) if pyr is not None else None, _ptr(fmap1), net.data_ptr(), inp.data_ptr(),
-                               coords.data_ptr(), _ptr(flow_up), _ptr(flow_small), ws.data_ptr(), ws.numel(), _ptr(attention), self.agg_gamma)
+                               coords.data_ptr(), _ptr(flow_up), _ptr(flow_small), ws.data_ptr(), ws.numel(), _ptr(attention), self.agg_gamma,
+                               _ptr(self.agg_score))
         with torch.cuda.device(self.device):
             check(getattr(load(), symbol)(C.byref(cfg), C.byref(weights), C.byref(buf), *args, stream_ptr(self.device)), symbol[4:])
 
@@ -702,3 +704,129 @@ class LLAFlowEngine(RaftEngine):
         if tiled:
             return ops.shift_volume_tiled(a, b, self.corr_levels), 1
         return ops.corr_volume_build_ex(a, b, self.corr_levels, scale=1.0, impl=1), 0
+
+
+class CRAFTEngine(RaftEngine):
+    """CRAFT (craft.py:57-376): GMA's loop (PFB_VARIANT_GMA) with the intra-frame modes as its heads, and the three cross-attention
+    sites of setrans.py.  The aggregator (ExpandedFeatTrans: first_linear, feat_softaggr, input_skip_coeff) rides on GMA's multi-head
+    aggregate: first_linear is to_v, each mode's attn @ v lands in its 128 columns, and pfb_craft_mode_aggregate (agg_score =
+    feat2score, agg_gamma = input_skip_coeff) replaces project + AXPY.  Each attention's q / k projections are packed per mode as 1x1
+    layers with head-major outputs (the intra-frame 32-channel modes zero-padded to 64, which leaves every dot product unchanged)."""
+
+    def _pack(self, update_block: torch.nn.Module, attention_module=None, f2_trans=None, corr_trans=None) -> _lib.RaftWeights:
+        w = super()._pack(update_block, attention_module)
+        self.f2 = self._pack_setrans(f2_trans)
+        self.corr = self._pack_setrans(corr_trans) if corr_trans is not None else None
+        if corr_trans is not None:  # the shared q = k projection of all modes at once (the fused volume's operands)
+            lin = corr_trans.setrans.query
+            self.corr_qk = ops.PackedConv([ConvWeights(lin.weight.detach()[:, :, None, None], lin.bias)], self.dtype, self.device,
+                                          src_channels=[lin.weight.shape[1]])
+        ft = f2_trans.setrans.out_trans
+        self.f2_v = ops.PackedConv([ConvWeights(ft.first_linear.weight.detach()[:, :, None, None])], self.dtype, self.device, src_channels=[256])
+        self.f2_score = ft.feat_softaggr.feat2score.weight.detach().to(self.device, torch.float32).reshape(-1).contiguous()
+        self.f2_coeff = float(ft.input_skip_coeff.detach().float().cpu().item())
+        return w
+
+    def _pack_attention(self, agg: torch.nn.Module, attention_module: torch.nn.Module):
+        self.num_heads = agg.num_modes
+        to_v = ops.PackedConv([ConvWeights(agg.first_linear.weight.detach()[:, :, None, None])], self.dtype, self.device, src_channels=[128])
+        self.agg_gamma = float(agg.input_skip_coeff.detach().float().cpu().item())
+        self.agg_score = agg.feat_softaggr.feat2score.weight.detach().to(self.device, torch.float32).reshape(-1).contiguous()
+        self.att = self._pack_setrans(attention_module)
+        return to_v, None
+
+    def _pack_setrans(self, mod: torch.nn.Module) -> dict:
+        """A SelfAttVisPosTrans / TransCorrBlock: per mode the q and k 1x1 layers (K = mode width padded to a multiple of 64, zero rows),
+        the weighted window bias fp32 [(2R+1)^2], the mode count and width, the position weight and the scalar of attn_softaggr."""
+        st = mod.setrans
+        M, cin = st.num_modes, st.query.weight.shape[1]
+        d = cin // M
+        dp = _align(d, 64)
+
+        def per_mode(lin: torch.nn.Linear):
+            out = []
+            for m in range(M):
+                wm = torch.zeros((dp, cin), dtype=lin.weight.dtype, device=lin.weight.device)
+                wm[:d] = lin.weight.detach()[m * d:(m + 1) * d]
+                b = None
+                if lin.bias is not None:
+                    b = torch.zeros(dp, dtype=lin.bias.dtype, device=lin.bias.device)
+                    b[:d] = lin.bias.detach()[m * d:(m + 1) * d]
+                out.append(ops.PackedConv([ConvWeights(wm[:, :, None, None].contiguous(), b)], self.dtype, self.device, src_channels=[cin]))
+            return out
+
+        bias = (st.pos_code_weight * mod.vispos_encoder.pos_coder.biases.detach().double()).float().to(self.device).reshape(-1).contiguous()
+        soft = getattr(st, "attn_softaggr", None)
+        return dict(q=per_mode(st.query), k=per_mode(st.key), M=M, d=d, dp=dp, R=mod.vispos_encoder.pos_coder.R, bias=bias,
+                    a=float(soft.feat2score.weight.detach().float().cpu().item()) if soft is not None else 0.0)
+
+    def _scores(self, sp: dict, x1: torch.Tensor, x2: torch.Tensor, impl: int) -> torch.Tensor:
+        """Head-major per-mode scores [M*B*N, N] = <q_m(x1), k_m(x2)> / sqrt(d)."""
+        B, H, W, _ = x1.shape
+        M, dp = sp["M"], sp["dp"]
+        q = torch.empty((M, B, H, W, dp), dtype=x1.dtype, device=x1.device)
+        k = torch.empty_like(q)
+        for m in range(M):
+            ops.conv2d([x1], sp["q"][m], q[m], impl=impl)
+            ops.conv2d([x2], sp["k"][m], k[m], impl=impl)
+        return ops.corr_volume_build_ex(q.view(M * B, H, W, dp), k.view(M * B, H, W, dp), 1, scale=sp["d"] ** -0.5, impl=impl)[0].view(
+            M * B * H * W, H * W)
+
+    def attention_probs(self, sp: dict, xn: torch.Tensor, mask_radius: int, impl: int) -> torch.Tensor:
+        """CrossAttFeatTrans's softmax probabilities of the normalised tokens xn with themselves (setrans.py:578-648), head-major
+        [M*B*N, N]."""
+        _, H, W, _ = xn.shape
+        logits = self._scores(sp, xn, xn, impl)
+        return ops.craft_window_softmax(logits, H, W, sp["bias"], sp["R"], ops.craft_clamp_flag(logits), mask_radius)
+
+    def attend_values(self, attn: torch.Tensor, v: torch.Tensor, F_: int, impl: int = 0) -> torch.Tensor:
+        """out[b, i, m F + c] = sum_j attn[m, b, i, j] v[b, j, m F + c]: per mode a 1x1 GEMM over the N attention columns whose weights
+        are the sample's v, as the loop's GMA aggregate runs it (one launch for all samples on wgmma, via v's transpose)."""
+        B, H, W, MF = v.shape
+        M, N = MF // F_, H * W
+        out = torch.empty_like(v)
+        a = attn.view(M, B, H, W, N)
+        tensor = v.dtype != torch.float32 and impl != 1 and N % 8 == 0
+        vT = ops.transpose_pm(v.view(B, N, MF), _align(N, 64)) if tensor else None
+        zero_bias = torch.zeros(128, dtype=torch.float32, device=v.device)
+        for c0 in range(0, MF, 128):  # 128 output columns per GEMM, as for GMA's heads; weight rows strided by M F
+            src = a[c0 // F_]
+            if tensor:
+                layer = ops.PerSampleWeights(v[0].view(N, MF)[:, c0:], zero_bias, 128, MF, v.dtype, vT[0, c0:], vT.shape[-1], 128)
+                ops.conv2d([src], layer, out, out_offset=c0, impl=2, w_rows_per_sample=MF)
+            else:
+                for b in range(B):
+                    layer = ops.PerSampleWeights(v[b].view(N, MF)[:, c0:], zero_bias, 128, MF, v.dtype)
+                    ops.conv2d([src[b:b + 1]], layer, out[b:b + 1], out_offset=c0, impl=impl)
+        return out
+
+    def f2_transform(self, fmap2: torch.Tensor, mask_radius: int = -1, impl: int = 0) -> torch.Tensor:
+        """SelfAttVisPosTrans "F2 transformer" (setrans.py:656-710, 346-471): LN(coeff x + soft-aggregate_m(P_m @ V_m)), x = LN(fmap2)."""
+        x = ops.layernorm(fmap2, eps=1e-12)
+        attn = self.attention_probs(self.f2, x, mask_radius, impl)
+        v = ops.conv2d([x], self.f2_v, torch.empty(x.shape[:3] + (self.f2_v.Cout,), dtype=x.dtype, device=x.device), impl=impl)
+        y = self.attend_values(attn, v, 256, impl)
+        return ops.craft_mode_aggregate(y, self.f2["M"], self.f2_score, self.f2_coeff, x)
+
+    def craft_volume(self, fmap1: torch.Tensor, fmap2t: torch.Tensor, impl: int = 0):
+        """(pyramid, layout) of TransCorrBlock.update (corr.py:157-218): the fused wgmma volume into the tiled pyramid (layout 1) where
+        RaftEngine's volume_tiled holds for fmap1 and the modes are 64-channel multiples, else the materialised route (dense, layout 0)."""
+        sp = self.corr
+        if self.volume_tiled(fmap1, impl) and sp["d"] % 64 == 0:
+            q1 = ops.conv2d([ops.layernorm(fmap1, eps=1e-12)], self.corr_qk, torch.empty_like(fmap1), impl=impl)
+            k2 = ops.conv2d([ops.layernorm(fmap2t, eps=1e-12)], self.corr_qk, torch.empty_like(fmap2t), impl=impl)
+            return ops.craft_volume_tiled(q1, k2, sp["M"], sp["a"], sp["bias"], sp["R"], self.corr_levels), 1
+        return self.craft_volume_dense(fmap1, fmap2t, impl), 0
+
+    def craft_volume_dense(self, fmap1: torch.Tensor, fmap2t: torch.Tensor, impl: int = 0) -> List[torch.Tensor]:
+        """TransCorrBlock.update (corr.py:157-218): the globally normalised mode mix of LN(fmap1) against LN(fmap2'), and RAFT's
+        avg-pool pyramid (dense, layout 0)."""
+        B, H, W, _ = fmap1.shape
+        sp = self.corr
+        scores = self._scores(sp, ops.layernorm(fmap1, eps=1e-12), ops.layernorm(fmap2t, eps=1e-12), impl)
+        level = ops.craft_volume_norm(scores, sp["M"], B, H, W, sp["a"], sp["bias"], sp["R"], ops.craft_clamp_flag(scores))
+        pyr = [level]
+        for _ in range(self.corr_levels - 1):
+            q, h, w = pyr[-1].shape
+            pyr.append(ops.avg_pool2x2(pyr[-1].view(q, h, w, 1)).view(q, h // 2, w // 2))
+        return pyr

@@ -1113,3 +1113,128 @@ def shift_volume_tiled(a_pack: torch.Tensor, b_pad: torch.Tensor, levels: int = 
         check(lib.pfb_shift_volume_tiled(a_pack.data_ptr(), b_pad.data_ptr(), ptr_array(pyr), B, H, W, levels, dtype_code(a_pack.dtype),
                                          stream_ptr(a_pack.device)), "shift_volume_tiled")
     return pyr
+
+
+# ------------------------------------------------------------------------------------------
+# CRAFT (include/ptlflow_b200.h, a23)
+# ------------------------------------------------------------------------------------------
+ATTN_CLIP = 100.0  # SETransConfig.attn_clip (setrans.py:102)
+
+
+def craft_clamp_flag(x: torch.Tensor, clip: float = ATTN_CLIP) -> torch.Tensor:
+    """int32 [1] on the device: 1 when any value of ``x`` exceeds ``clip`` (the clamp decision of setrans.py:601-612, taken over
+    every sample and mode of the call without a host synchronisation)."""
+    require_cuda(x, "x")
+    flag = torch.empty(1, dtype=torch.int32, device=x.device)
+    with torch.cuda.device(x.device):
+        check(load().pfb_craft_clamp_flag(x.data_ptr(), x.numel(), float(clip), flag.data_ptr(), dtype_code(x.dtype), stream_ptr(x.device)),
+              "craft_clamp_flag")
+    return flag
+
+
+def _bias_table(bias: torch.Tensor, R: int) -> torch.Tensor:
+    if bias.dtype != torch.float32 or not bias.is_cuda or bias.numel() != (2 * R + 1) ** 2 or not bias.is_contiguous():
+        raise RuntimeError(f"craft: the position bias must be a contiguous fp32 CUDA tensor of (2R+1)^2 = {(2 * R + 1) ** 2} values")
+    return bias
+
+
+def craft_window_softmax(logits: torch.Tensor, H: int, W: int, bias: torch.Tensor, R: int, flag: torch.Tensor, mask_radius: int = -1,
+                         clip: float = ATTN_CLIP) -> torch.Tensor:
+    """In place on the head-major logits [rows, H*W]: clamp (when ``flag``), add the weighted window ``bias`` (fp32 [(2R+1)^2]) and the
+    optional -1e9 outside the Chebyshev ``mask_radius``, then the row softmax (setrans.py:601-640)."""
+    require_cuda(logits, "logits")
+    rows = logits.shape[0]
+    if logits.dim() != 2 or logits.shape[1] != H * W or not logits.is_contiguous():
+        raise RuntimeError(f"craft_window_softmax: logits must be contiguous [rows, {H * W}]")
+    with torch.cuda.device(logits.device):
+        check(load().pfb_craft_window_softmax(logits.data_ptr(), rows, H, W, _bias_table(bias, R).data_ptr(), R, int(mask_radius),
+                                              flag.data_ptr(), float(clip), dtype_code(logits.dtype), stream_ptr(logits.device)),
+              "craft_window_softmax")
+    return logits
+
+
+def craft_mode_aggregate(feat: torch.Tensor, M: int, w: torch.Tensor, coeff: float, skip: torch.Tensor, out: Optional[torch.Tensor] = None,
+                         out_offset: int = 0) -> torch.Tensor:
+    """LayerNorm(coeff skip + sum_m softmax_m(<w, y_m>) y_m) per pixel (setrans.py:320-341, 465-468): feat [..., M*F] pixel-major,
+    skip [..., F], w fp32 [F]; writes ``out`` [..., >= out_offset + F] (a new [..., F] tensor by default)."""
+    require_cuda(feat, "feat"); require_cuda(skip, "skip")
+    F_ = skip.shape[-1]
+    P = skip.numel() // F_
+    if feat.shape[-1] < M * F_ or feat.numel() // feat.shape[-1] != P or w.dtype != torch.float32 or w.numel() != F_:
+        raise RuntimeError("craft_mode_aggregate: feat [..., M*F], skip [..., F] and fp32 w [F] must agree")
+    if out is None:
+        out = torch.empty_like(skip)
+    with torch.cuda.device(feat.device):
+        check(load().pfb_craft_mode_aggregate(feat.data_ptr(), feat.shape[-1], M, F_, w.data_ptr(), float(coeff), skip.data_ptr(), F_, 0,
+                                              out.data_ptr(), out.shape[-1], out_offset, P, dtype_code(feat.dtype), stream_ptr(feat.device)),
+              "craft_mode_aggregate")
+    return out
+
+
+def craft_volume_norm(scores: torch.Tensor, M: int, B: int, H: int, W: int, a: float, bias: torch.Tensor, R: int, flag: torch.Tensor,
+                      clip: float = ATTN_CLIP) -> torch.Tensor:
+    """Level 0 [B*H*W, H, W] of CRAFT's volume from the head-major per-mode scores [M*B*N, N]: clamp, bias, the mode mix
+    sum_m softmax_m(a s_m) s_m and the LayerNorm over each sample's N^2 values (corr.py:202-218)."""
+    require_cuda(scores, "scores")
+    N = H * W
+    if scores.shape != (M * B * N, N) or not scores.is_contiguous():
+        raise RuntimeError(f"craft_volume_norm: scores must be contiguous [{M * B * N}, {N}]")
+    lib = load()
+    ws = _scratch(("craft_volume", B, H, W), -(-lib.pfb_craft_volume_workspace_bytes(B, H, W) // 8), scores.device)  # fp64 elements
+    level0 = torch.empty((B * N, H, W), dtype=scores.dtype, device=scores.device)
+    with torch.cuda.device(scores.device):
+        check(lib.pfb_craft_volume_norm(scores.data_ptr(), M, float(a), _bias_table(bias, R).data_ptr(), R, flag.data_ptr(), float(clip),
+                                        level0.data_ptr(), ws.data_ptr(), ws.numel() * 8, B, H, W, dtype_code(scores.dtype),
+                                        stream_ptr(scores.device)), "craft_volume_norm")
+    return level0
+
+
+def transpose_pm(x: torch.Tensor, n_pad: int) -> torch.Tensor:
+    """x [B, HW, C] -> [B, C, n_pad] (zero columns from HW on): the K-major operand of a per-sample-weight 1x1 GEMM."""
+    require_cuda(x, "x")
+    B, HW, Cc = x.shape
+    out = torch.empty((B, Cc, n_pad), dtype=x.dtype, device=x.device)
+    with torch.cuda.device(x.device):
+        check(load().pfb_transpose_pm(x.data_ptr(), out.data_ptr(), B, HW, Cc, n_pad, dtype_code(x.dtype), stream_ptr(x.device)), "transpose_pm")
+    return out
+
+
+def craft_volume_tiled(q1: torch.Tensor, k2: torch.Tensor, M: int, a: float, bias: torch.Tensor, R: int, levels: int = 4,
+                       clip: float = ATTN_CLIP) -> List[torch.Tensor]:
+    """CRAFT's inter-frame volume fused on wgmma: q1 / k2 f16 / bf16 [B,H,W,256] (the shared projection of LN(fmap1) / LN(fmap2'))
+    -> the tiled pyramid (layout of corr_volume_build_tiled) of the clamped, biased, mode-mixed and globally normalised scores."""
+    require_cuda(q1, "q1"); require_cuda(k2, "k2")
+    B, H, W, Cc = q1.shape
+    if k2.shape != q1.shape or k2.dtype != q1.dtype or Cc != 256 or not (q1.is_contiguous() and k2.is_contiguous()):
+        raise RuntimeError("craft_volume_tiled: q1 / k2 must be contiguous [B,H,W,256] of one dtype")
+    lib = load()
+    pyr = []
+    for l in range(levels):
+        nbytes = lib.pfb_corr_level_bytes_tiled(B, H, W, H, W, l)
+        if nbytes == 0:
+            raise RuntimeError(f"craft_volume_tiled: {H}x{W} grid too small for {levels} levels")
+        pyr.append(torch.empty((B * H * W, nbytes // (2 * B * H * W)), dtype=q1.dtype, device=q1.device))
+    ws = _scratch(("craft_volume_tiled", B, H, W), -(-lib.pfb_craft_volume_tiled_workspace_bytes(B, H, W) // 8), q1.device)
+    flag = torch.empty(1, dtype=torch.int32, device=q1.device)
+    with torch.cuda.device(q1.device):
+        check(lib.pfb_craft_volume_tiled(q1.data_ptr(), k2.data_ptr(), M, float(a), _bias_table(bias, R).data_ptr(), R, flag.data_ptr(),
+                                         float(clip), ptr_array(pyr), ws.data_ptr(), ws.numel() * 8, B, H, W, levels, dtype_code(q1.dtype),
+                                         stream_ptr(q1.device)), "craft_volume_tiled")
+    return pyr
+
+
+class PerSampleWeights(NamedTuple):
+    """A 1x1 layer of ``Cout`` outputs whose weights are one sample's value matrix (GMA's and CRAFT's attn @ v): ``weight`` the SIMT
+    layout [Cin][Cout_pad] with Cout_pad = the row stride of v, ``weight_k`` the K-major rows of v's transpose (wgmma) or None.
+    conv2d reads it as it reads a PackedConv."""
+
+    weight: torch.Tensor
+    bias: torch.Tensor
+    Cout: int
+    Cout_pad: int
+    dtype: torch.dtype
+    weight_k: Optional[torch.Tensor] = None
+    Cin_pad: int = 0
+    Cout_pad_k: int = 0
+    KH: int = 1
+    KW: int = 1

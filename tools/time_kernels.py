@@ -129,6 +129,44 @@ def shift_volume_tiled(dtype, pairs, levels=4):
     return lambda: ops.shift_volume_tiled(A, Bp, levels), 2.0 * n * n * ops.LLA_K * pairs, 0
 
 
+def craft_volume_tiled(dtype, pairs, modes=4, levels=4):
+    """CRAFT's fused inter-frame volume (clamp flag, statistics and the normalised tiled pyramid: three passes over the K = 256
+    GEMM) at the 1024x436 grid.  FLOP = 3 x 2 N^2 256 per pair."""
+    from ptlflow_b200 import ops
+
+    (h8, w8), g = GRID, _gen()
+    q1, k2 = (torch.randn(pairs, h8, w8, 256, device="cuda", generator=g).to(DTYPES[dtype]) for _ in range(2))
+    bias = torch.randn(225, device="cuda", generator=g)
+    n = h8 * w8
+    return lambda: ops.craft_volume_tiled(q1, k2, modes, 0.5, bias, 7, levels), 3 * 2.0 * n * n * 256 * pairs, 0
+
+
+def craft_window_softmax(modes, pairs, dtype="bf16"):
+    """CRAFT's windowed-bias attention softmax over modes x pairs rows of N at the 1024x436 grid, in place.  Bytes: the logits read
+    and the probabilities written."""
+    from ptlflow_b200 import ops
+
+    (h8, w8), g = GRID, _gen()
+    n = h8 * w8
+    x = torch.randn(modes * pairs * n, n, device="cuda", generator=g).to(DTYPES[dtype])
+    bias = torch.randn(225, device="cuda", generator=g)
+    flag = ops.craft_clamp_flag(x)
+    return lambda: ops.craft_window_softmax(x, h8, w8, bias, 7, flag), 0, 2 * x.numel() * x.element_size()
+
+
+def craft_mode_aggregate(F, modes, pairs, dtype="bf16"):
+    """CRAFT's mode soft-aggregate + skip + LayerNorm at the 1024x436 grid (F = 256: the f2 transformer, 128: the loop's
+    aggregator).  Bytes: the modes' features and the skip read, the result written."""
+    from ptlflow_b200 import ops
+
+    (h8, w8), g = GRID, _gen()
+    feat = torch.randn(pairs, h8, w8, modes * F, device="cuda", generator=g).to(DTYPES[dtype])
+    skip = torch.randn(pairs, h8, w8, F, device="cuda", generator=g).to(DTYPES[dtype])
+    w = torch.randn(F, device="cuda", generator=g)
+    out = torch.empty_like(skip)
+    return lambda: ops.craft_mode_aggregate(feat, modes, w, 1.0, skip, out), 0, (feat.numel() + 2 * skip.numel()) * feat.element_size()
+
+
 class Case(NamedTuple):
     build: Callable  # (**variant) -> (fn, flop, nbytes)
     variants: list
@@ -153,6 +191,9 @@ CASES = {
     "knn_topk": Case(knn_topk, [dict(grid=grid, dtype=d) for grid in ((56, 128), (112, 256)) for d in ("bf16", "fp32")], 10),
     "sparse_lookup": Case(sparse_lookup, [{}], 100),
     "shift_volume_tiled": Case(shift_volume_tiled, [dict(dtype=d, pairs=b) for d in ("bf16", "f16") for b in (1, 4)], 10),
+    "craft_volume_tiled": Case(craft_volume_tiled, [dict(dtype=d, pairs=b) for d in ("bf16", "f16") for b in (1, 4)], 10),
+    "craft_window_softmax": Case(craft_window_softmax, [dict(modes=4, pairs=b) for b in (1, 4)], 10),
+    "craft_mode_aggregate": Case(craft_mode_aggregate, [dict(F=f, modes=4, pairs=b) for f in (128, 256) for b in (1, 4)], 50),
 }
 
 
