@@ -798,6 +798,30 @@ PFB_API int pfb_craft_volume_tiled(const void* q1, const void* k2, int M, float 
                                    pfb_dtype dtype, pfb_stream stream);
 
 /* ------------------------------------------------------------------------------------
+ * a24: SplatFlow (ptlflow/models/splatflow/splatflow.py, softsplat.py): the last motion features of pair (0, 1), forward-splatted
+ * by that pair's flow, are a fixed extra GRU input of pair (1, 2).  The loop is pfb_raft_refine with variant PFB_VARIANT_GMA and
+ * context_dim = 256: buf->inp is [inp | mf_t], and the GRU layers take [h | inp | mf_t | motion | motion_global].
+ * ---------------------------------------------------------------------------------- */
+/* Where the loop's motion buffer lies in the workspace of `cfg` (host only, no device needed): byte offset and channel stride
+ * (elements of the storage type per pixel).  Channels 0..125 hold the last iteration's relu(conv) of the motion encoder, 126..127
+ * the flow that iteration started from, once pfb_raft_refine has returned (in stream order); nothing after the motion encoder of
+ * the last iteration writes them.  Fails for a cfg the pfb_raft_* entry points refuse. */
+PFB_API int pfb_raft_workspace_motion(const pfb_raft_cfg* cfg, size_t* offset, int* channel_stride);
+/* The "average" forward splat of softsplat.py:10-60, 435-468 (reference arithmetic, summation order aside):
+ *   src [B,H,W,src_stride] storage type, channels src_offset .. +C-1;  flow fp32 [B,2,H,W] (u, v);
+ *   for each source pixel (x, y) the target (x + u, y + v) in fp32 and the bilinear weights of its four floor / floor + 1 corners
+ *   in fp32; each fp32 product value * weight is added into an fp64 accumulator at every corner inside the image (the others are
+ *   dropped), and so is the weight itself (the ones channel);
+ *   dst[p, dst_offset + c] = float(acc[p, c]) / n in fp32, n = float(acc[p, C]), or 1 where that is exactly 0; one rounding to the
+ *   storage type.  dst [B,H,W,dst_stride].
+ * The fp64 atomics make the result independent of the order of the additions unless a sum needs more than 53 bits.
+ * workspace: pfb_softsplat_workspace_bytes(B, H, W, C), cleared with cudaMemsetAsync inside the call.  Kernel class 6. */
+PFB_API size_t pfb_softsplat_workspace_bytes(int B, int H, int W, int C);
+PFB_API int pfb_softsplat_average(const void* src, int src_stride, int src_offset, const float* flow, void* dst, int dst_stride,
+                                  int dst_offset, void* workspace, size_t workspace_bytes, int B, int H, int W, int C, pfb_dtype dtype,
+                                  pfb_stream stream);
+
+/* ------------------------------------------------------------------------------------
  * Encoder-side kernels (SURVEY.md section 8(f) rank 1: the callers either side of the path).
  * The first 7x7 convolution and the residual blocks' stride-1 3x3 convolutions of BasicEncoder (extractor.py:122-267)
  * run here, the strided, 1x1 and bottleneck convolutions in cuDNN; pre-processing, instance norm + ReLU (+ residual)
@@ -809,6 +833,10 @@ PFB_API int pfb_craft_volume_tiled(const void* q1, const void* k2, int M, float 
  * raft.py:127-135, base_model.py:206-246 */
 PFB_API int pfb_preprocess_frames(const void* images, void* out, int B, int H, int W, int Hp, int Wp, int pad_top,
                                   int pad_left, int out_channels, pfb_dtype dtype, pfb_stream stream);
+/* The same for images [B,T,3,H,W] (T frames per sample): the first F <= T frames of every sample into out [F*B,Hp,Wp,out_channels],
+ * frame-major (all frames 0, then all frames 1, ...).  T = F = 2 is pfb_preprocess_frames. */
+PFB_API int pfb_preprocess_frames_ex(const void* images, void* out, int B, int T, int F, int H, int W, int Hp, int Wp, int pad_top,
+                                     int pad_left, int out_channels, pfb_dtype dtype, pfb_stream stream);
 /* y = act(IN(x)) or, with residual, y = relu(residual + act(IN(x)));  x, y, residual: [B,H,W,C].
  * IN = nn.InstanceNorm2d defaults (no affine, biased variance, eps).   extractor.py:29-31,52-58 */
 PFB_API size_t pfb_instance_norm_workspace_bytes(int B, int C);

@@ -176,6 +176,7 @@ SIGNATURES = {
     "pfb_raft_workspace_bytes": (C.c_size_t, [C.POINTER(RaftCfg)]),
     "pfb_raft_refine": (_I, [C.POINTER(RaftCfg), C.POINTER(RaftWeights), C.POINTER(RaftBuffers), _S]),
     "pfb_preprocess_frames": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
+    "pfb_preprocess_frames_ex": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
     "pfb_instance_norm_workspace_bytes": (C.c_size_t, [_I, _I]),
     "pfb_instance_norm_act": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, C.c_float, _I, _I, _S]),
     "pfb_instance_norm_apply": (_I, [_P, _P, _P, _P, _I, _I, _I, _I, C.c_float, _I, _I, _S]),
@@ -247,6 +248,9 @@ SIGNATURES = {
     "pfb_craft_volume_norm": (_I, [_P, _I, C.c_float, _P, _I, _P, C.c_float, _P, _P, C.c_size_t, _I, _I, _I, _I, _S]),
     "pfb_craft_volume_tiled_workspace_bytes": (C.c_size_t, [_I, _I, _I]),
     "pfb_craft_volume_tiled": (_I, [_P, _P, _I, C.c_float, _P, _I, _P, C.c_float, _PP, _P, C.c_size_t, _I, _I, _I, _I, _I, _S]),
+    "pfb_raft_workspace_motion": (_I, [C.POINTER(RaftCfg), C.POINTER(C.c_size_t), C.POINTER(C.c_int)]),
+    "pfb_softsplat_workspace_bytes": (C.c_size_t, [_I, _I, _I, _I]),
+    "pfb_softsplat_average": (_I, [_P, _I, _I, _P, _P, _I, _I, _P, C.c_size_t, _I, _I, _I, _I, _I, _S]),
 }
 
 

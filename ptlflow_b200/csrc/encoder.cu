@@ -15,10 +15,10 @@
 namespace pfb {
 
 template <typename T>
-__global__ void preprocess_frames_kernel(const T* __restrict__ img, T* __restrict__ out, int B, int H, int W, int Hp,
+__global__ void preprocess_frames_kernel(const T* __restrict__ img, T* __restrict__ out, int B, int T_in, int F, int H, int W, int Hp,
                                          int Wp, int pad_top, int pad_left, int OC) {
-  // out: [2B][Hp][Wp][OC], frame-major (all first frames, then all second frames); channels >= 3 are zero
-  const size_t total = (size_t)2 * B * Hp * Wp;
+  // out: [F*B][Hp][Wp][OC], frame-major (all first frames, then all second frames, ...); channels >= 3 are zero
+  const size_t total = (size_t)F * B * Hp * Wp;
   for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
     int x = (int)(idx % Wp);
     size_t t = idx / Wp;
@@ -28,7 +28,7 @@ __global__ void preprocess_frames_kernel(const T* __restrict__ img, T* __restric
     int sy = y - pad_top, sx = x - pad_left;
     sy = sy < 0 ? 0 : (sy >= H ? H - 1 : sy);
     sx = sx < 0 ? 0 : (sx >= W ? W - 1 : sx);
-    const T* src = img + (((size_t)b * 2 + f) * 3) * H * W + (size_t)sy * W + sx;
+    const T* src = img + (((size_t)b * T_in + f) * 3) * H * W + (size_t)sy * W + sx;
     T* o = out + idx * OC;
 #pragma unroll
     for (int c = 0; c < 3; ++c) {  // output channel c (RGB) <- input channel 2-c (BGR)
@@ -42,10 +42,11 @@ __global__ void preprocess_frames_kernel(const T* __restrict__ img, T* __restric
 // fast path: 4-channel output, no horizontal padding, W % 8 == 0 -> a thread turns 8 pixels (3 x 16-byte plane loads)
 // into 8 x 8-byte pixels (4 x 16-byte stores); rows are still replicate-padded vertically
 template <typename T>
-__global__ void preprocess_frames_vec8_kernel(const T* __restrict__ img, T* __restrict__ out, int B, int H, int W, int Hp, int pad_top) {
+__global__ void preprocess_frames_vec8_kernel(const T* __restrict__ img, T* __restrict__ out, int B, int T_in, int F, int H, int W, int Hp,
+                                              int pad_top) {
   static_assert(sizeof(T) == 2, "16-byte vectors of 2-byte elements");
   const int W8 = W / 8;
-  const size_t total = (size_t)2 * B * Hp * W8;
+  const size_t total = (size_t)F * B * Hp * W8;
   for (size_t idx = blockIdx.x * (size_t)blockDim.x + threadIdx.x; idx < total; idx += (size_t)gridDim.x * blockDim.x) {
     const int x8 = (int)(idx % W8);
     size_t t = idx / W8;
@@ -54,7 +55,7 @@ __global__ void preprocess_frames_vec8_kernel(const T* __restrict__ img, T* __re
     const int f = n / B, b = n - f * B;
     int sy = y - pad_top;
     sy = sy < 0 ? 0 : (sy >= H ? H - 1 : sy);
-    const T* src = img + (((size_t)b * 2 + f) * 3) * H * W + (size_t)sy * W + 8 * x8;
+    const T* src = img + (((size_t)b * T_in + f) * 3) * H * W + (size_t)sy * W + 8 * x8;
     uint4 pl[3];
 #pragma unroll
     for (int c = 0; c < 3; ++c) pl[c] = __ldg(reinterpret_cast<const uint4*>(src + (size_t)(2 - c) * H * W));  // RGB <- BGR planes
@@ -353,30 +354,39 @@ __global__ void __launch_bounds__(256) inorm_fused_kernel(const T* __restrict__ 
 
 using namespace pfb;
 
-extern "C" PFB_API int pfb_preprocess_frames(const void* images, void* out, int B, int H, int W, int Hp, int Wp, int pad_top,
-                                             int pad_left, int out_channels, pfb_dtype dtype, pfb_stream stream) {
+extern "C" PFB_API int pfb_preprocess_frames_ex(const void* images, void* out, int B, int T, int F, int H, int W, int Hp, int Wp, int pad_top,
+                                                int pad_left, int out_channels, pfb_dtype dtype, pfb_stream stream) {
   PFB_CHECK_ARG(images && out, "preprocess_frames: null pointer");
   PFB_CHECK_ARG(out_channels >= 3 && out_channels <= 16, "preprocess_frames: out_channels=%d (3..16)", out_channels);
+  PFB_CHECK_ARG(F >= 1 && T >= F, "preprocess_frames: %d of %d frames", F, T);
   PFB_CHECK_ARG(dtype_ok(dtype) && B > 0 && H > 0 && W > 0 && Hp >= H && Wp >= W && pad_top >= 0 && pad_left >= 0 &&
                     pad_top + H <= Hp && pad_left + W <= Wp,
                 "preprocess_frames: bad geometry %dx%d -> %dx%d (+%d,+%d)", H, W, Hp, Wp, pad_top, pad_left);
   cudaStream_t s = as_stream(stream);
-  size_t total = (size_t)2 * B * Hp * Wp;
+  size_t total = (size_t)F * B * Hp * Wp;
   unsigned blocks = (unsigned)std::min<size_t>(ceil_div_sz(total, 256), (size_t)sm_count() * 16);
   ProfScope prof(KC_MISC, s);
   if (dtype != PFB_F32 && out_channels == 4 && pad_left == 0 && Wp == W && W % 8 == 0 &&
       ((reinterpret_cast<uintptr_t>(images) | reinterpret_cast<uintptr_t>(out)) & 15) == 0 && ((size_t)H * W) % 8 == 0) {
     blocks = (unsigned)std::min<size_t>(ceil_div_sz(total / 8, 256), (size_t)sm_count() * 16);
-    if (dtype == PFB_F16) preprocess_frames_vec8_kernel<__half><<<blocks, 256, 0, s>>>((const __half*)images, (__half*)out, B, H, W, Hp, pad_top);
-    else preprocess_frames_vec8_kernel<__nv_bfloat16><<<blocks, 256, 0, s>>>((const __nv_bfloat16*)images, (__nv_bfloat16*)out, B, H, W, Hp, pad_top);
+    if (dtype == PFB_F16)
+      preprocess_frames_vec8_kernel<__half><<<blocks, 256, 0, s>>>((const __half*)images, (__half*)out, B, T, F, H, W, Hp, pad_top);
+    else
+      preprocess_frames_vec8_kernel<__nv_bfloat16><<<blocks, 256, 0, s>>>((const __nv_bfloat16*)images, (__nv_bfloat16*)out, B, T, F, H, W,
+                                                                          Hp, pad_top);
     PFB_LAUNCH_CHECK();
     return PFB_OK;
   }
-  PFB_DISPATCH_DTYPE(dtype, T, {
-    preprocess_frames_kernel<T><<<blocks, 256, 0, s>>>((const T*)images, (T*)out, B, H, W, Hp, Wp, pad_top, pad_left, out_channels);
+  PFB_DISPATCH_DTYPE(dtype, T_, {
+    preprocess_frames_kernel<T_><<<blocks, 256, 0, s>>>((const T_*)images, (T_*)out, B, T, F, H, W, Hp, Wp, pad_top, pad_left, out_channels);
   });
   PFB_LAUNCH_CHECK();
   return PFB_OK;
+}
+
+extern "C" PFB_API int pfb_preprocess_frames(const void* images, void* out, int B, int H, int W, int Hp, int Wp, int pad_top,
+                                             int pad_left, int out_channels, pfb_dtype dtype, pfb_stream stream) {
+  return pfb_preprocess_frames_ex(images, out, B, 2, 2, H, W, Hp, Wp, pad_top, pad_left, out_channels, dtype, stream);
 }
 
 extern "C" PFB_API size_t pfb_instance_norm_workspace_bytes(int B, int C) {

@@ -333,7 +333,10 @@ static int check_cfg(const pfb_raft_cfg* c, LoopFamily family) {
     case LOOKUP_PYRAMID: break;
   }
   PFB_CHECK_ARG(c->num_heads >= 0 && c->num_heads <= 64 && (sp->aggregate == AGG_GMA || heads_of(c) == 1), "%s: num_heads=%d", name, c->num_heads);
-  if (!sp->small) PFB_CHECK_ARG(c->hidden_dim == 128 && c->context_dim == 128, "%s: the update block expects hidden=context=128", name);
+  // gma also takes a 256-channel static GRU input: SplatFlow's [inp | mf_t] (a24); the context split handles any context width
+  if (!sp->small)
+    PFB_CHECK_ARG(c->hidden_dim == 128 && (c->context_dim == 128 || (c->variant == PFB_VARIANT_GMA && c->context_dim == 256)),
+                  "%s: the update block expects hidden=context=128 (gma: context 128 or 256)", name);
   else PFB_CHECK_ARG(c->hidden_dim == 96 && c->context_dim == 64, "raft_small: SmallUpdateBlock expects hidden=96 context=64");
   return PFB_OK;
 }
@@ -525,6 +528,15 @@ static int update_iter_once(Ctx& x, const void* corr, void* mask_out) {
 }
 
 extern "C" PFB_API size_t pfb_raft_workspace_bytes(const pfb_raft_cfg* cfg) { return workspace_bytes(cfg, FAMILY_RAFT); }
+
+extern "C" PFB_API int pfb_raft_workspace_motion(const pfb_raft_cfg* cfg, size_t* offset, int* channel_stride) {
+  PFB_CHECK_ARG(offset && channel_stride, "raft_workspace_motion: null output");
+  PFB_TRY(check_cfg(cfg, FAMILY_RAFT));
+  const Workspace w = plan(cfg);
+  *offset = w.off_motion;
+  *channel_stride = w.c_motion;
+  return PFB_OK;
+}
 
 extern "C" PFB_API int pfb_raft_update_iter(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf,
                                     const void* corr, void* mask_out, pfb_stream stream) {

@@ -830,3 +830,54 @@ class CRAFTEngine(RaftEngine):
             q, h, w = pyr[-1].shape
             pyr.append(ops.avg_pool2x2(pyr[-1].view(q, h, w, 1)).view(q, h // 2, w // 2))
         return pyr
+
+
+class SplatFlowEngine(RaftEngine):
+    """SplatFlow (splatflow.py:86-154, update.py:82-123): GMA's loop (PFB_VARIANT_GMA, one head) run once per frame pair, with two
+    weight sets.  ``weights``: the two-frame set, GMA's packing of encoder, gru, flow_head, mask and aggregator (context 128).
+    ``three_frame``: the same engine for pair (1, 2) of three frames, whose static GRU input is [inp | mf_t] (context 256): gru_sp with
+    its input columns permuted from the reference's [h | inp | mf | mf_s | mf_t] to [h | inp | mf_t | mf | mf_s], so that the loop's
+    context split evaluates the inp and mf_t terms once per forward, plus flow_head_sp and mask_sp.  Its encoder and aggregator
+    layers are the two-frame set's structs: the shared weights are resident once."""
+
+    def _pack(self, update_block: torch.nn.Module, attention_module: Optional[torch.nn.Module] = None) -> _lib.RaftWeights:
+        import copy
+        from types import SimpleNamespace
+
+        ub = update_block
+        w2 = super()._pack(ub, attention_module)
+        layers2 = self.layers
+        hd = self.hidden_dim
+        perm = torch.cat([torch.arange(2 * hd), torch.arange(4 * hd, 5 * hd), torch.arange(2 * hd, 4 * hd)]).to(ub.gru_sp.convz1.weight.device)
+
+        def permuted(conv):
+            return SimpleNamespace(weight=conv.weight.detach()[:, perm].contiguous(), bias=conv.bias, in_channels=conv.in_channels)
+
+        g = ub.gru_sp
+        gru_sp = SimpleNamespace(**{n: permuted(getattr(g, n)) for n in ("convz1", "convr1", "convq1", "convz2", "convr2", "convq2")})
+        view = SimpleNamespace(encoder=ub.encoder, gru=gru_sp, flow_head=ub.flow_head_sp, mask=ub.mask_sp, aggregator=ub.aggregator)
+        three = copy.copy(self)
+        three.context_dim = 2 * self.context_dim
+        w3 = RaftEngine._pack(three, view, attention_module)
+        for k in (_lib.L_CONVC1, _lib.L_CONVC2, _lib.L_CONVF1, _lib.L_CONVF2, _lib.L_CONV, _lib.L_CONVC2F2, _lib.L_AGG_V, _lib.L_AGG_PROJ):
+            if k in layers2:
+                three.layers[k] = layers2[k]
+                w3.layers[k] = w2.layers[k]
+            else:
+                three.layers.pop(k, None)
+        three.weights = w3
+        self.three_frame = three
+        self.layers = layers2
+        return w2
+
+    def motion_features(self, B: int, H: int, W: int, scratch: Optional[dict] = None) -> torch.Tensor:
+        """The loop's motion buffer as a pixel-major view [B,H,W,stride] of the workspace that refine(.., scratch) used for this grid:
+        channels 0..127 are mf, the motion features of the last iteration (pfb_raft_workspace_motion); read them before the next call
+        of the loop on this workspace."""
+        cfg = self.make_cfg(B, H, W, 1, (8 * H, 8 * W), (0, 0), False, 0)
+        off, stride = C.c_size_t(), C.c_int()
+        check(load().pfb_raft_workspace_motion(C.byref(cfg), C.byref(off), C.byref(stride)), "raft_workspace_motion")
+        ws = self.workspace(cfg, scratch)
+        es = torch.empty((), dtype=self.dtype).element_size()
+        n = B * H * W * stride.value * es
+        return ws[off.value: off.value + n].view(self.dtype).view(B, H, W, stride.value)

@@ -488,18 +488,50 @@ def context_split(cnet: torch.Tensor, hidden: int, context: int):
 # ------------------------------------------------------------------------------------------
 # encoder-side kernels
 # ------------------------------------------------------------------------------------------
-def preprocess_frames(images: torch.Tensor, padded_hw, pad_top_left, out_channels: int = 3) -> torch.Tensor:
+def preprocess_frames(images: torch.Tensor, padded_hw, pad_top_left, out_channels: int = 3, frames: Optional[int] = None) -> torch.Tensor:
     """images [B,2,3,H,W] (BGR, [0,1]) -> [2B,Hp,Wp,out_channels] pixel-major RGB in [-1,1] (extra channels zero),
-    replicate padded; frame-major."""
+    replicate padded; frame-major.  With ``frames``: images [B,T,3,H,W], T >= frames, and the first ``frames`` frames of every
+    sample -> [frames*B,Hp,Wp,out_channels]."""
     require_cuda(images, "images")
-    B, two, three, H, W = images.shape
-    if two != 2 or three != 3:
-        raise RuntimeError("preprocess_frames: expected images of shape [B,2,3,H,W]")
+    B, T, three, H, W = images.shape
+    if frames is None and T != 2 or three != 3 or frames is not None and not 1 <= frames <= T:
+        raise RuntimeError("preprocess_frames: expected images of shape [B,2,3,H,W], or [B,T,3,H,W] with T >= frames")
     Hp, Wp = padded_hw
-    out = torch.empty((2 * B, Hp, Wp, out_channels), dtype=images.dtype, device=images.device)
+    F_ = 2 if frames is None else frames
+    out = torch.empty((F_ * B, Hp, Wp, out_channels), dtype=images.dtype, device=images.device)
     with torch.cuda.device(images.device):
-        check(load().pfb_preprocess_frames(images.data_ptr(), out.data_ptr(), B, H, W, Hp, Wp, pad_top_left[0], pad_top_left[1],
-                                           out_channels, dtype_code(images.dtype), stream_ptr(images.device)), "preprocess_frames")
+        if frames is None:
+            rc = load().pfb_preprocess_frames(images.data_ptr(), out.data_ptr(), B, H, W, Hp, Wp, pad_top_left[0], pad_top_left[1],
+                                              out_channels, dtype_code(images.dtype), stream_ptr(images.device))
+        else:
+            rc = load().pfb_preprocess_frames_ex(images.data_ptr(), out.data_ptr(), B, T, F_, H, W, Hp, Wp, pad_top_left[0], pad_top_left[1],
+                                                 out_channels, dtype_code(images.dtype), stream_ptr(images.device))
+        check(rc, "preprocess_frames")
+    return out
+
+
+def softsplat_average(src: torch.Tensor, flow: torch.Tensor, out: Optional[torch.Tensor] = None, channels: Optional[int] = None,
+                      src_offset: int = 0, out_offset: int = 0) -> torch.Tensor:
+    """The "average" forward splat of softsplat.py (pfb_softsplat_average): channels ``src_offset ..`` of the pixel-major src
+    [B,H,W,S] moved by flow fp32 [B,2,H,W], normalised by the splatted ones channel, into channels ``out_offset ..`` of out
+    [B,H,W,O] (a new [B,H,W,channels] tensor when out is None).  The fp64 accumulator is scratch of this call (a CUDA graph brings
+    its own through scratch_scope)."""
+    require_cuda(src, "src")
+    B, H, W, S = src.shape
+    C = channels if channels is not None else S - src_offset
+    if out is None:
+        out = torch.empty((B, H, W, C), dtype=src.dtype, device=src.device)
+    require_cuda(out, "out")
+    fl = flow.contiguous()
+    if tuple(fl.shape) != (B, 2, H, W) or fl.dtype != torch.float32 or out.dtype != src.dtype or tuple(out.shape[:3]) != (B, H, W):
+        raise RuntimeError("softsplat_average: expected flow fp32 [B,2,H,W] and out [B,H,W,*] of src's dtype")
+    lib = load()
+    nbytes = lib.pfb_softsplat_workspace_bytes(B, H, W, C)
+    ws = _scratch(("softsplat", str(src.device), B, H, W, C), (nbytes + 7) // 8, src.device)
+    with torch.cuda.device(src.device):
+        check(lib.pfb_softsplat_average(src.data_ptr(), S, src_offset, fl.data_ptr(), out.data_ptr(), out.shape[3], out_offset,
+                                        ws.data_ptr(), ws.numel() * 8, B, H, W, C, dtype_code(src.dtype), stream_ptr(src.device)),
+              "softsplat_average")
     return out
 
 

@@ -167,6 +167,21 @@ def craft_mode_aggregate(F, modes, pairs, dtype="bf16"):
     return lambda: ops.craft_mode_aggregate(feat, modes, w, 1.0, skip, out), 0, (feat.numel() + 2 * skip.numel()) * feat.element_size()
 
 
+def softsplat_average(pairs, dtype="bf16", channels=128):
+    """SplatFlow's average splat of the 128 motion channels (stride 256, as in the loop's motion buffer) into the mf_t columns of a
+    256-channel buffer at the 1024x436 grid, by a random flow of a few px.  Bytes: source and flow read, the fp64 accumulator
+    (channels + 1) cleared, added into and read once, the result written."""
+    from ptlflow_b200 import ops
+
+    (H, W), g = GRID, _gen(7)
+    src = torch.randn(pairs, H, W, 2 * channels, device="cuda", generator=g).to(DTYPES[dtype])
+    flow = 4 * torch.randn(pairs, 2, H, W, device="cuda", generator=g)
+    out = torch.empty_like(src)
+    P, es = pairs * H * W, src.element_size()
+    nbytes = 2 * P * channels * es + P * 2 * 4 + 3 * P * (channels + 1) * 8
+    return lambda: ops.softsplat_average(src, flow, out=out, channels=channels, out_offset=channels), 0, nbytes
+
+
 class Case(NamedTuple):
     build: Callable  # (**variant) -> (fn, flop, nbytes)
     variants: list
@@ -194,6 +209,7 @@ CASES = {
     "craft_volume_tiled": Case(craft_volume_tiled, [dict(dtype=d, pairs=b) for d in ("bf16", "f16") for b in (1, 4)], 10),
     "craft_window_softmax": Case(craft_window_softmax, [dict(modes=4, pairs=b) for b in (1, 4)], 10),
     "craft_mode_aggregate": Case(craft_mode_aggregate, [dict(F=f, modes=4, pairs=b) for f in (128, 256) for b in (1, 4)], 50),
+    "softsplat_average": Case(softsplat_average, [dict(pairs=b, dtype=d) for d in ("bf16", "f16") for b in (1, 4)], 50),
 }
 
 
