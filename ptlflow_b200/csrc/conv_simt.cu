@@ -305,7 +305,8 @@ extern "C" PFB_API int pfb_conv2d(const pfb_conv_params* p, pfb_stream stream) {
       PFB_CHECK_ARG(p->aux_h && p->aux_z && p->hidden > 0 && p->Cout == p->hidden, "conv2d: GRU_Q needs aux_h, aux_z and Cout == hidden");
       break;
     case PFB_EPI_FLOW:
-      PFB_CHECK_ARG(p->coords && p->Cout == 2, "conv2d: FLOW epilogue needs coords and Cout == 2");
+      PFB_CHECK_ARG(p->coords && p->Cout == 2 && p->out_offset >= 0 && p->out_stride >= p->out_offset + 2,
+                    "conv2d: FLOW epilogue needs coords, Cout == 2 and an output window with stride >= offset + 2");
       break;
     case PFB_EPI_RELU_APPEND_FLOW:
     case PFB_EPI_LINEAR_APPEND_FLOW:

@@ -22,7 +22,8 @@ template <typename T, int KH, int KW>
 __global__ void __launch_bounds__(256) conv_cout2_flow_kernel(const T* __restrict__ x, int stride, int offset, int Cin,
                                                               int B, int H, int W, const T* __restrict__ wk,
                                                               int Cout_pad_k, int Cin_pad, const float* __restrict__ bias,
-                                                              float* __restrict__ coords, float* __restrict__ flow_out) {
+                                                              float* __restrict__ coords, float* __restrict__ flow_out,
+                                                              int out_stride, int out_offset) {
   extern __shared__ __align__(16) uint8_t sm_raw[];
   T* sw = reinterpret_cast<T*>(sm_raw);  // [tap][2][Cin]
   constexpr int TAPS = KH * KW;
@@ -71,8 +72,8 @@ __global__ void __launch_bounds__(256) conv_cout2_flow_kernel(const T* __restric
       const float c1 = coords[2 * (size_t)p + 1] + a1 + b1;
       coords[2 * (size_t)p] = c0;
       coords[2 * (size_t)p + 1] = c1;
-      flow_out[2 * (size_t)p] = c0 - (float)px;
-      flow_out[2 * (size_t)p + 1] = c1 - (float)py;
+      flow_out[(size_t)p * out_stride + out_offset] = c0 - (float)px;
+      flow_out[(size_t)p * out_stride + out_offset + 1] = c1 - (float)py;
     }
   }
 }
@@ -214,11 +215,12 @@ int conv_cout2_flow(const pfb_conv_params* p, cudaStream_t s) {
   if (p->dtype == PFB_F16)
     conv_cout2_flow_kernel<__half, 3, 3><<<blocks, 256, smem, s>>>((const __half*)x.ptr, x.stride, x.offset, x.channels, p->B, p->H, p->W,
                                                                    (const __half*)p->weight_k, p->Cout_pad_k, p->Cin_pad, p->bias,
-                                                                   p->coords, (float*)p->out);
+                                                                   p->coords, (float*)p->out, p->out_stride, p->out_offset);
   else
     conv_cout2_flow_kernel<__nv_bfloat16, 3, 3><<<blocks, 256, smem, s>>>((const __nv_bfloat16*)x.ptr, x.stride, x.offset, x.channels, p->B,
                                                                           p->H, p->W, (const __nv_bfloat16*)p->weight_k, p->Cout_pad_k,
-                                                                          p->Cin_pad, p->bias, p->coords, (float*)p->out);
+                                                                          p->Cin_pad, p->bias, p->coords, (float*)p->out, p->out_stride,
+                                                                          p->out_offset);
   PFB_LAUNCH_CHECK();
   return PFB_OK;
 }

@@ -22,6 +22,12 @@ Bound.  For every output element
   * rho_out is half an ulp of the output type relative to the value (2^-11 f16, 2^-8 bf16, 2^-24 fp32) and eta_out half
     the smallest subnormal (2^-25 f16, 2^-134 bf16, 2^-150 fp32): the one rounding of the fp32 result to storage.  The
     factor (1 + rho_out) is there because the value that is rounded is the fp32 result, not ref.
+  * FLOW (fp32 coordinates and flow, Cout 2): coords_out = c + acc and flow = coords_out - (x, y), from the stored
+    coordinates c.  On top of E_acc come the fp32 roundings of the coordinate add, at most 2^-23 * |coords_out| (two
+    roundings of 2^-24: the warp kernel adds the coordinates before the bias, so one intermediate sum is coordinate-sized
+    as well; its |bias| part is one of the spare terms), and for the flow one more, 2^-24 * |flow|, of the grid
+    subtraction.  Both outputs are fp32 already: no storage rounding.  flow_reference.py shows that the tensor-core
+    route (per-tap GEMM + gather) stays inside the same E_acc.
   * L_epi is the epilogue's Lipschitz factor in the accumulator: |scale| (LINEAR, LINEAR_F32, AXPY), 1 (RELU, the
     APPEND_FLOW channels), max |gelu'| = Phi(sqrt 2) + sqrt 2 * phi(sqrt 2) < 1.13 (GELU, RESIDUAL_GELU; times
     1.13 * |1 + post_w| for the second step), 1/4 (sigmoid: z), |h| / 4 (r * h), |z| (tanh' <= 1: GRU_Q).
@@ -102,13 +108,23 @@ def gelu64(x: Tensor) -> Tensor:
 
 def epilogue(epi: int, acc: Tensor, S: Tensor, n: int, dtype: torch.dtype, *, scale: float = 1.0, h: Optional[Tensor] = None,
              z: Optional[Tensor] = None, hidden: int = 0, residual: Optional[Tensor] = None, post_w: Optional[Tensor] = None,
-             post_b: Optional[Tensor] = None, flow: Optional[Tensor] = None) -> Dict[str, Tuple[Tensor, Tensor]]:
-    """The epilogue in float64 and its bound: {"out": (ref, bound)} (+ "z" for GRU_ZR), each [B,H,W,C].  ``dtype`` is the
-    output's storage type (fp32 for LINEAR_F32).  h / z: [B,H,W,hidden] (GRU; AXPY reads h as its residual), residual
-    [B,H,W,Cout] (the operand's channels already selected), post_w / post_b [Cout], flow [B,H,W,2]; all float64 of the stored
-    values."""
+             post_b: Optional[Tensor] = None, flow: Optional[Tensor] = None,
+             coords: Optional[Tensor] = None) -> Dict[str, Tuple[Tensor, Tensor]]:
+    """The epilogue in float64 and its bound: {"out": (ref, bound)} (+ "z" for GRU_ZR, + "coords" for FLOW), each [B,H,W,C].
+    ``dtype`` is the output's storage type (fp32 for LINEAR_F32 and FLOW).  h / z: [B,H,W,hidden] (GRU; AXPY reads h as its
+    residual), residual [B,H,W,Cout] (the operand's channels already selected), post_w / post_b [Cout], flow [B,H,W,2],
+    coords [B,H,W,2] (FLOW: the coordinates before the update); all float64 of the stored values."""
     rho, eta = RHO[dtype], ETA[dtype]
     E = (n + C_SPARE) * U * S
+    if epi == FLOW:
+        B, H, W, _ = acc.shape
+        ys, xs = torch.meshgrid(torch.arange(H, dtype=torch.float64, device=acc.device),
+                                torch.arange(W, dtype=torch.float64, device=acc.device), indexing="ij")
+        grid = torch.stack([xs, ys], -1).expand(B, H, W, 2)
+        c_out = coords.double().to(acc.device) + acc
+        e_c = E + 2.0 ** -23 * c_out.abs()
+        f = c_out - grid
+        return {"coords": (c_out, e_c), "out": (f, e_c + 2.0 ** -24 * f.abs())}
 
     def pair(ref, err):
         return ref, rho * ref.abs() + (1.0 + rho) * err + eta
