@@ -52,7 +52,8 @@ typedef enum {
 #define PFB_MAX_LEVELS 8
 #define PFB_MAX_SRC 4
 
-PFB_API int pfb_version(void); /* 101: pfb_raft_buffers gained agg_score (callers built for 100 pass a shorter struct) */
+PFB_API int pfb_version(void); /* 102: pfb_raft_buffers gained pool_min_side (101: agg_score); the library reads every field of the
+                                 struct, so callers must be built against this header */
 PFB_API const char* pfb_last_error(void);
 /* sm major*10+minor of the current device, or negative status. */
 PFB_API int pfb_device_arch(void);
@@ -100,6 +101,14 @@ PFB_API int pfb_corr_lookup_ex(void* const* pyramid, const int* level_h, const i
                                int H, int W, int levels, int radius, pfb_dtype dtype, pfb_dtype out_dtype, int out_nchw,
                                int out_stride, pfb_stream stream);
 
+/* The level sizes of a pyramid of `levels` levels over an H x W target grid (host only, no device needed).  pool_min_side = 0:
+ * level l is (H >> l) x (W >> l), every level 2x2-pooled from the one before (RAFT).  pool_min_side = m > 0: level l is the 2x2
+ * pooling of level l-1 only while the smaller side of level l-1 exceeds m, otherwise level l repeats level l-1 (LCV's pyramid with
+ * m = 2r+1, ptlflow/models/lcv/corr_lcv.py:44-50).  Either way the distinct levels are the first n levels of RAFT's pyramid, and
+ * level l >= n is level n-1 again, still sampled at coords / 2^l.  Writes level_h[0..levels-1], level_w[0..levels-1]; returns n
+ * (1..levels), or a negative status for bad arguments.  Sizes may reach 0 only with pool_min_side = 0. */
+PFB_API int pfb_corr_level_sizes(int H, int W, int levels, int pool_min_side, int* level_h, int* level_w);
+
 /* ------------------------------------------------------------------------------------
  * a1 + a2 + a3 on the TILED pyramid (f16 / bf16 storage; what pfb_raft_refine uses with cfg.volume_layout = 1).
  * Level l of query q is ceil(h_l/4) x ceil(w_l/8) tiles of 4 rows x 8 columns (64 bytes = one DRAM access granule);
@@ -115,6 +124,13 @@ PFB_API int pfb_corr_volume_build_tiled(const void* fmap1, const void* fmap2, vo
                                         int W2, int C, int levels, float scale, pfb_dtype dtype, pfb_stream stream);
 PFB_API int pfb_corr_lookup_tiled(void* const* pyramid, const float* coords, void* out, int B, int H1, int W1, int H2, int W2,
                                   int levels, int radius, pfb_dtype dtype, int out_stride, pfb_stream stream);
+/* Same with explicit level sizes (level_h[l] x level_w[l] instead of H2>>l x W2>>l; both NULL: pfb_corr_lookup_tiled), as
+ * pfb_corr_lookup_ex: a pyramid whose levels stop pooling (pfb_corr_level_sizes) passes the last distinct level's pointer and sizes
+ * again for every repeated level; level l is still sampled at coords / 2^l.  pyramid[l] holds level_h[l] x level_w[l] maps in
+ * the tiled layout (pfb_corr_level_bytes_tiled of that size). */
+PFB_API int pfb_corr_lookup_tiled_ex(void* const* pyramid, const int* level_h, const int* level_w, const float* coords, void* out, int B,
+                                     int H1, int W1, int H2, int W2, int levels, int radius, pfb_dtype dtype, int out_stride,
+                                     pfb_stream stream);
 
 /* ------------------------------------------------------------------------------------
  * a4: on-the-fly correlation + lookup (no 4D volume)
@@ -410,9 +426,14 @@ typedef struct {
   float agg_gamma;            /* gma: Aggregate.gamma; craft: the aggregator's input_skip_coeff */
   const float* agg_score;     /* craft: the aggregator's feat2score weight fp32 [128]: motion_global = pfb_craft_mode_aggregate of the
                                  heads' attn @ v (no project); NULL for gma */
+  int pool_min_side;          /* how the pyramid's levels were sized (pfb_corr_level_sizes of the cfg's grid): 0 = RAFT's pyramid;
+                                 m > 0 = levels stop pooling once the smaller side is <= m (lcv: 2r+1), the repeated levels passed
+                                 as the same pointer again.  Materialised pyramids only (not alternate_corr). */
 } pfb_raft_buffers;
 
 PFB_API size_t pfb_raft_workspace_bytes(const pfb_raft_cfg* cfg);
+/* The same for a pyramid sized with pool_min_side (pfb_raft_buffers.pool_min_side): its grid needs no empty level under that rule. */
+PFB_API size_t pfb_raft_workspace_bytes_ex(const pfb_raft_cfg* cfg, int pool_min_side);
 /* Runs cfg->iters refinement iterations followed by the final upsample.  Only the last
  * iteration evaluates the mask head (raft.py:192 returns only the last prediction in eval). */
 PFB_API int pfb_raft_refine(const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf,

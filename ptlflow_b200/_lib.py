@@ -82,7 +82,7 @@ class RaftBuffers(C.Structure):
         ("pyramid", C.POINTER(C.c_void_p)), ("fmap1", C.c_void_p), ("net", C.c_void_p), ("inp", C.c_void_p),
         ("coords", C.c_void_p), ("flow_up", C.c_void_p), ("flow_small", C.c_void_p),
         ("workspace", C.c_void_p), ("workspace_bytes", C.c_size_t),
-        ("attention", C.c_void_p), ("agg_gamma", C.c_float), ("agg_score", C.c_void_p),
+        ("attention", C.c_void_p), ("agg_gamma", C.c_float), ("agg_score", C.c_void_p), ("pool_min_side", C.c_int),
     ]
 
 
@@ -154,6 +154,8 @@ SIGNATURES = {
     "pfb_corr_level_bytes_tiled": (C.c_size_t, [_I, _I, _I, _I, _I, _I]),
     "pfb_corr_volume_build_tiled": (_I, [_P, _P, _PP, _I, _I, _I, _I, _I, _I, _I, C.c_float, _I, _S]),
     "pfb_corr_lookup_tiled": (_I, [_PP, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
+    "pfb_corr_lookup_tiled_ex": (_I, [_PP, C.POINTER(C.c_int), C.POINTER(C.c_int), _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
+    "pfb_corr_level_sizes": (_I, [_I, _I, _I, _I, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "pfb_corr_lookup_onthefly": (_I, [_P, _PP, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
     "pfb_corr_lookup_onthefly_tc_workspace_bytes": (C.c_size_t, [_I, _I, _I]),
     "pfb_corr_lookup_onthefly_tc": (_I, [_P, _PP, _P, _P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
@@ -174,6 +176,7 @@ SIGNATURES = {
     "pfb_init_coords": (_I, [_P, _P, _I, _I, _I, _S]),
     "pfb_forward_interpolate": (_I, [_P, _P, _I, _I, _I, _S]),
     "pfb_raft_workspace_bytes": (C.c_size_t, [C.POINTER(RaftCfg)]),
+    "pfb_raft_workspace_bytes_ex": (C.c_size_t, [C.POINTER(RaftCfg), C.c_int]),
     "pfb_raft_refine": (_I, [C.POINTER(RaftCfg), C.POINTER(RaftWeights), C.POINTER(RaftBuffers), _S]),
     "pfb_preprocess_frames": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _S]),
     "pfb_preprocess_frames_ex": (_I, [_P, _P, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _I, _S]),

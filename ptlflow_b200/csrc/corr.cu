@@ -452,6 +452,24 @@ static int launch_lookup_t(const LevelTable& lv, const float* coords, void* out,
   return PFB_OK;
 }
 
+extern "C" PFB_API int pfb_corr_level_sizes(int H, int W, int levels, int pool_min_side, int* level_h, int* level_w) {
+  PFB_CHECK_ARG(level_h && level_w, "corr_level_sizes: null output");
+  PFB_CHECK_ARG(H > 0 && W > 0, "corr_level_sizes: bad grid %dx%d", H, W);
+  PFB_CHECK_ARG(levels >= 1 && levels <= PFB_MAX_LEVELS, "corr_level_sizes: levels=%d out of range", levels);
+  PFB_CHECK_ARG(pool_min_side >= 0, "corr_level_sizes: pool_min_side=%d", pool_min_side);
+  int distinct = 1;
+  level_h[0] = H;
+  level_w[0] = W;
+  for (int l = 1; l < levels; ++l) {
+    const int ph = level_h[l - 1], pw = level_w[l - 1];
+    const bool pool = pool_min_side == 0 || (ph < pw ? ph : pw) > pool_min_side;
+    level_h[l] = pool ? ph / 2 : ph;
+    level_w[l] = pool ? pw / 2 : pw;
+    distinct += pool;
+  }
+  return distinct;
+}
+
 extern "C" PFB_API int pfb_corr_lookup(void* const* pyramid, const float* coords, void* out, int B, int H, int W,
                                int levels, int radius, pfb_dtype dtype, pfb_dtype out_dtype, int out_nchw,
                                int out_stride, pfb_stream stream) {

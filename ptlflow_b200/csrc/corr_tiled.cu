@@ -208,7 +208,14 @@ extern "C" PFB_API size_t pfb_corr_level_bytes_tiled(int B, int H1, int W1, int 
 
 extern "C" PFB_API int pfb_corr_lookup_tiled(void* const* pyramid, const float* coords, void* out, int B, int H, int W, int H2, int W2,
                                              int levels, int radius, pfb_dtype dtype, int out_stride, pfb_stream stream) {
+  return pfb_corr_lookup_tiled_ex(pyramid, nullptr, nullptr, coords, out, B, H, W, H2, W2, levels, radius, dtype, out_stride, stream);
+}
+
+extern "C" PFB_API int pfb_corr_lookup_tiled_ex(void* const* pyramid, const int* level_h, const int* level_w, const float* coords, void* out,
+                                                int B, int H, int W, int H2, int W2, int levels, int radius, pfb_dtype dtype, int out_stride,
+                                                pfb_stream stream) {
   PFB_CHECK_ARG(pyramid && coords && out, "corr_lookup_tiled: null pointer");
+  PFB_CHECK_ARG((level_h == nullptr) == (level_w == nullptr), "corr_lookup_tiled: level_h and level_w come together");
   PFB_CHECK_ARG(dtype == PFB_F16 || dtype == PFB_BF16, "corr_lookup_tiled: the tiled pyramid is f16 / bf16 only");
   PFB_CHECK_ARG(B > 0 && H > 0 && W > 0 && H2 > 0 && W2 > 0, "corr_lookup_tiled: bad shape");
   PFB_CHECK_ARG(levels >= 1 && levels <= 4, "corr_lookup_tiled: levels=%d out of range (1..4)", levels);
@@ -219,8 +226,8 @@ extern "C" PFB_API int pfb_corr_lookup_tiled(void* const* pyramid, const float* 
   for (int l = 0; l < levels; ++l) {
     PFB_CHECK_ARG(pyramid[l] && (reinterpret_cast<uintptr_t>(pyramid[l]) & 15) == 0, "corr_lookup_tiled: pyramid[%d] null or not 16-byte aligned", l);
     lv.ptr[l] = pyramid[l];
-    lv.h[l] = H2 >> l;
-    lv.w[l] = W2 >> l;
+    lv.h[l] = level_h ? level_h[l] : H2 >> l;
+    lv.w[l] = level_w ? level_w[l] : W2 >> l;
     PFB_CHECK_ARG(lv.h[l] >= 1 && lv.w[l] >= 1, "corr_lookup_tiled: level %d is empty", l);
     lv.tiles_x[l] = tiled_tiles_x(lv.w[l]);
     lv.map_elems[l] = (unsigned)(tiled_tiles_y(lv.h[l]) * lv.tiles_x[l] * 32);

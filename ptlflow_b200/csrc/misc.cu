@@ -312,7 +312,7 @@ int launch_flow_from_coords(const float* coords, float* flow, int B, int H, int 
 
 using namespace pfb;
 
-extern "C" PFB_API int pfb_version(void) { return 101; }
+extern "C" PFB_API int pfb_version(void) { return 102; }
 extern "C" PFB_API const char* pfb_last_error(void) { return g_err; }
 
 extern "C" PFB_API int pfb_device_arch(void) {

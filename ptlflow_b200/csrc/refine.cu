@@ -36,15 +36,18 @@ int launch_conv(const pfb_raft_cfg* c, cudaStream_t s, const pfb_layer& L, std::
   return pfb_conv2d(&p, (pfb_stream)s);
 }
 
-int check_loop_cfg(const pfb_raft_cfg* c, const char* name, bool levels_fit_grid, int max_radius) {
+int check_loop_cfg(const pfb_raft_cfg* c, const char* name, bool levels_fit_grid, int max_radius, int pool_min_side) {
   PFB_CHECK_ARG(c, "%s: null cfg", name);
   PFB_CHECK_ARG(dtype_ok(c->dtype), "%s: bad dtype %d", name, (int)c->dtype);
   PFB_CHECK_ARG(c->B > 0 && c->H > 0 && c->W > 0, "%s: bad grid %dx%dx%d", name, c->B, c->H, c->W);
   PFB_CHECK_ARG(c->corr_levels >= 1 && c->corr_levels <= PFB_MAX_LEVELS && c->corr_radius >= 0 && c->corr_radius <= max_radius,
                 "%s: corr_levels=%d corr_radius=%d", name, c->corr_levels, c->corr_radius);
-  if (levels_fit_grid)
-    PFB_CHECK_ARG((c->H >> (c->corr_levels - 1)) >= 1 && (c->W >> (c->corr_levels - 1)) >= 1, "%s: %dx%d grid too small for %d levels",
-                  name, c->H, c->W, c->corr_levels);
+  if (levels_fit_grid) {
+    int lh[PFB_MAX_LEVELS], lw[PFB_MAX_LEVELS];
+    PFB_TRY(pfb_corr_level_sizes(c->H, c->W, c->corr_levels, pool_min_side, lh, lw) > 0 ? PFB_OK : PFB_ERR_ARG);
+    PFB_CHECK_ARG(lh[c->corr_levels - 1] >= 1 && lw[c->corr_levels - 1] >= 1, "%s: %dx%d grid too small for %d levels", name, c->H, c->W,
+                  c->corr_levels);
+  }
   PFB_CHECK_ARG(c->iters >= 0, "%s: iters=%d", name, c->iters);
   PFB_CHECK_ARG(c->volume_layout == 0 || (c->volume_layout == 1 && c->dtype != PFB_F32 && !c->alternate_corr && c->corr_levels <= 4),
                 "%s: volume_layout=%d needs f16/bf16, a materialised pyramid and <= 4 levels", name, c->volume_layout);
@@ -58,6 +61,8 @@ int check_loop_buffers(const pfb_raft_cfg* c, const pfb_raft_buffers* buf, bool 
     PFB_CHECK_ARG(buf->pyramid, "%s: null pyramid", name);
     PFB_CHECK_ARG(!c->alternate_corr || (buf->fmap1 && c->feat_dim > 0), "%s: alternate_corr needs fmap1 and feat_dim", name);
   }
+  PFB_CHECK_ARG(buf->pool_min_side >= 0 && (buf->pool_min_side == 0 || !c->alternate_corr),
+                "%s: pool_min_side=%d (positive values describe a materialised pyramid)", name, buf->pool_min_side);
   PFB_CHECK_ARG(buf->workspace_bytes >= need, "%s: workspace %zu bytes < required %zu", name, buf->workspace_bytes, need);
   return PFB_OK;
 }
@@ -75,7 +80,7 @@ int copy_wide_state(const pfb_raft_cfg* c, const pfb_raft_buffers* buf, void* X,
 }
 
 int raft_lookup(const pfb_raft_cfg* c, void* const* pyramid, const void* fmap1, const float* coords, void* out, int out_stride,
-                void* flags, cudaStream_t s, float scale) {
+                void* flags, cudaStream_t s, float scale, int pool_min_side) {
   if (c->alternate_corr) {
     static const int env_tc = getenv("PFB_ONTHEFLY_TC") ? atoi(getenv("PFB_ONTHEFLY_TC")) : 1;
     if (env_tc && c->impl != 1 && corr_onthefly_umma_supported(c->B, c->H, c->W, c->feat_dim, c->corr_levels, c->corr_radius, c->dtype, out_stride))
@@ -86,11 +91,15 @@ int raft_lookup(const pfb_raft_cfg* c, void* const* pyramid, const void* fmap1, 
     return pfb_corr_lookup_onthefly_ex(fmap1, pyramid, coords, out, c->B, c->H, c->W,
                                        c->feat_dim, c->corr_levels, c->corr_radius, scale, c->dtype, c->dtype, 0,
                                        out_stride, (pfb_stream)s);
+  // RAFT's pyramid (pool_min_side = 0) keeps the lookups' own H >> l sizes; a pyramid that stops pooling passes them explicitly
+  int lh[PFB_MAX_LEVELS], lw[PFB_MAX_LEVELS];
+  const bool sized = pool_min_side > 0;
+  if (sized && pfb_corr_level_sizes(c->H, c->W, c->corr_levels, pool_min_side, lh, lw) < 1) return PFB_ERR_ARG;
   if (c->volume_layout == 1)
-    return pfb_corr_lookup_tiled(pyramid, coords, out, c->B, c->H, c->W, c->H, c->W, c->corr_levels,
-                                 c->corr_radius, c->dtype, out_stride, (pfb_stream)s);
-  return pfb_corr_lookup(pyramid, coords, out, c->B, c->H, c->W, c->corr_levels,
-                         c->corr_radius, c->dtype, c->dtype, 0, out_stride, (pfb_stream)s);
+    return pfb_corr_lookup_tiled_ex(pyramid, sized ? lh : nullptr, sized ? lw : nullptr, coords, out, c->B, c->H, c->W, c->H, c->W,
+                                    c->corr_levels, c->corr_radius, c->dtype, out_stride, (pfb_stream)s);
+  return pfb_corr_lookup_ex(pyramid, sized ? lh : nullptr, sized ? lw : nullptr, coords, out, c->B, c->H, c->W, c->corr_levels,
+                            c->corr_radius, c->dtype, c->dtype, 0, out_stride, (pfb_stream)s);
 }
 
 int motion_encoder(const pfb_raft_cfg* c, cudaStream_t s, const ConvExtras& e, const MotionLayers& L, const MotionBuffers& m,
@@ -308,12 +317,15 @@ static Workspace plan(const pfb_raft_cfg* c) {
   return w;
 }
 
-static int check_cfg(const pfb_raft_cfg* c, LoopFamily family) {
+// buf: the buffers of a run (or of pfb_raft_workspace_bytes_ex), whose pool_min_side sizes the pyramid levels that must not be empty;
+// NULL checks them as RAFT's pyramid sizes them
+static int check_cfg(const pfb_raft_cfg* c, LoopFamily family, const pfb_raft_buffers* buf = nullptr) {
   const char* name = kFamilyName[family];
   PFB_CHECK_ARG(c, "%s: null cfg", name);
   const LoopSpec* sp = loop_spec(c->variant);
   PFB_CHECK_ARG(sp && sp->family == family, "%s: variant=%d is not a loop of the pfb_%s_* entry points", name, c->variant, name);
-  PFB_TRY(check_loop_cfg(c, name, sp->lookup != LOOKUP_SPARSE, sp->lookup == LOOKUP_1D ? 64 : 15));
+  const int pool_min_side = buf && buf->pool_min_side > 0 ? buf->pool_min_side : 0;
+  PFB_TRY(check_loop_cfg(c, name, sp->lookup != LOOKUP_SPARSE, sp->lookup == LOOKUP_1D ? 64 : 15, pool_min_side));
   switch (sp->lookup) {
     case LOOKUP_SPARSE:  // 5 levels of 9 x 9 bins (scv.py:245-260) over a table of feat_dim = num_k matches per query
       PFB_CHECK_ARG(c->corr_levels == 5 && c->corr_radius == 4 && !c->alternate_corr && c->volume_layout == 0 && c->feat_dim >= 1 &&
@@ -425,7 +437,7 @@ static int lookup(const Ctx& x) {
     return pfb_corr1d_lookup(x.b->pyramid[0], x.b->pyramid[1], x.b->coords, x.at(x.ws.off_corr), x.c->B, x.c->H, x.c->W, x.c->corr_radius,
                              x.c->dtype, x.ws.corr_stride, (pfb_stream)x.s);
   PFB_TRY(raft_lookup(x.c, x.b->pyramid, x.b->fmap1, x.b->coords, x.at(x.ws.off_corr), x.ws.corr_stride, x.at(x.ws.off_flags), x.s,
-                      x.corr_scale));
+                      x.corr_scale, x.b->pool_min_side));
   if (x.sp->lookup != LOOKUP_STRIP) return PFB_OK;
   // csflow: the 4D lookup above wrote planes 0 .. L K^2 - 1 and zero-filled the rest; the strip taps follow (a20)
   const int L = x.c->corr_levels, K = 2 * x.c->corr_radius + 1;
@@ -496,7 +508,7 @@ static int update_iter(const Ctx& x, const void* corr_ext, void* mask_out) {
 
 static int make_ctx(Ctx& x, const pfb_raft_cfg* cfg, const pfb_raft_weights* w, const pfb_raft_buffers* buf,
                     cudaStream_t s, bool need_pyramid, LoopFamily family) {
-  PFB_TRY(check_cfg(cfg, family));
+  PFB_TRY(check_cfg(cfg, family, buf));
   const char* name = kFamilyName[family];
   PFB_CHECK_ARG(w, "%s: null weights", name);
   x.c = cfg; x.sp = loop_spec(cfg->variant); x.w = w; x.b = buf; x.s = s;
@@ -513,8 +525,8 @@ static int make_ctx(Ctx& x, const pfb_raft_cfg* cfg, const pfb_raft_weights* w, 
 using namespace pfb;
 
 // the workspace of the msraft / ccmr / raft entry points (ccmr's holds its XCiT plan after the loop's); 0 for a cfg they refuse
-static size_t workspace_bytes(const pfb_raft_cfg* cfg, LoopFamily family) {
-  if (check_cfg(cfg, family) != PFB_OK) return 0;
+static size_t workspace_bytes(const pfb_raft_cfg* cfg, LoopFamily family, const pfb_raft_buffers* buf = nullptr) {
+  if (check_cfg(cfg, family, buf) != PFB_OK) return 0;
   return plan(cfg).total + (family == FAMILY_CCMR ? ccmr_plan(cfg).total : 0);
 }
 
@@ -528,6 +540,13 @@ static int update_iter_once(Ctx& x, const void* corr, void* mask_out) {
 }
 
 extern "C" PFB_API size_t pfb_raft_workspace_bytes(const pfb_raft_cfg* cfg) { return workspace_bytes(cfg, FAMILY_RAFT); }
+
+extern "C" PFB_API size_t pfb_raft_workspace_bytes_ex(const pfb_raft_cfg* cfg, int pool_min_side) {
+  if (pool_min_side < 0) return 0;
+  pfb_raft_buffers buf{};
+  buf.pool_min_side = pool_min_side;
+  return workspace_bytes(cfg, FAMILY_RAFT, &buf);
+}
 
 extern "C" PFB_API int pfb_raft_workspace_motion(const pfb_raft_cfg* cfg, size_t* offset, int* channel_stride) {
   PFB_CHECK_ARG(offset && channel_stride, "raft_workspace_motion: null output");

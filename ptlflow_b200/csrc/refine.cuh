@@ -54,8 +54,9 @@ int launch_conv(const pfb_raft_cfg* c, cudaStream_t s, const pfb_layer& L, std::
                 const ConvExtras& e = ConvExtras());
 
 // The rules every loop's cfg follows (dtype, grid, levels / radius <= max_radius, volume_layout, iters >= 0); with `levels_fit_grid`
-// the coarsest pyramid level must keep at least one pixel.  name: the entry point family, for the messages.
-int check_loop_cfg(const pfb_raft_cfg* c, const char* name, bool levels_fit_grid = true, int max_radius = 15);
+// the coarsest pyramid level (sized by pfb_corr_level_sizes with pool_min_side) must keep at least one pixel.  name: the entry point
+// family, for the messages.
+int check_loop_cfg(const pfb_raft_cfg* c, const char* name, bool levels_fit_grid = true, int max_radius = 15, int pool_min_side = 0);
 // The state buffers, the pyramid (and fmap1 for alternate_corr) when the call looks up, and a workspace of at least `need` bytes
 int check_loop_buffers(const pfb_raft_cfg* c, const pfb_raft_buffers* buf, bool need_pyramid, size_t need, const char* name);
 
@@ -68,8 +69,9 @@ int launch_flow_from_coords(const float* coords, float* flow, int B, int H, int 
 // The multi-scale lookup of the loop configured by `c` (dense, tiled or on-the-fly pyramid, as pfb_raft_refine picks it) into
 // out [B,H,W,out_stride] (storage type); flags: the on-the-fly tensor-core lookup's per-query workspace (alternate_corr only).
 // scale: the on-the-fly lookup's scale, 0 = 1/sqrt(feat_dim) (ms_raft_plus passes the real C when its rows carry zero channels).
+// pool_min_side: pfb_raft_buffers.pool_min_side, the rule that sized the materialised pyramid's levels (pfb_corr_level_sizes).
 int raft_lookup(const pfb_raft_cfg* c, void* const* pyramid, const void* fmap1, const float* coords, void* out, int out_stride,
-                void* flags, cudaStream_t s, float scale = 0.f);
+                void* flags, cudaStream_t s, float scale = 0.f, int pool_min_side = 0);
 
 // RAFT's motion encoder (update.py:76-112): relu(conv([relu(convc2(relu(convc1(corr)))) | relu(convf2(relu(convf1(flow))))])) and
 // the flow (e.flow) into `out` (RELU_APPEND_FLOW).  convc2 == NULL: SmallMotionEncoder, convc1 writes the correlation columns of

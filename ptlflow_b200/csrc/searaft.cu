@@ -154,7 +154,8 @@ int make_ctx(SrCtx& x, const pfb_raft_cfg* cfg, const pfb_searaft_weights* w, co
 }
 
 int lookup(const SrCtx& x) {
-  return raft_lookup(x.c, x.b->pyramid, x.b->fmap1, x.b->coords, x.at(x.ws.off_corr), x.ws.corr_stride, x.at(x.ws.off_flags), x.s);
+  return raft_lookup(x.c, x.b->pyramid, x.b->fmap1, x.b->coords, x.at(x.ws.off_corr), x.ws.corr_stride, x.at(x.ws.off_flags), x.s, 0.f,
+                     x.b->pool_min_side);
 }
 
 }  // namespace

@@ -189,7 +189,8 @@ int begin(const SkCtx& x, bool lookup_buffer) {
 int finish(const SkCtx& x) { return copy_wide_state(x.c, x.b, x.at(x.ws.off_x), kX, false, x.s); }  // the final hidden state
 
 int lookup(const SkCtx& x) {
-  return raft_lookup(x.c, x.b->pyramid, x.b->fmap1, x.b->coords, x.at(x.ws.off_corr), x.ws.corr_stride, x.at(x.ws.off_flags), x.s);
+  return raft_lookup(x.c, x.b->pyramid, x.b->fmap1, x.b->coords, x.at(x.ws.off_corr), x.ws.corr_stride, x.at(x.ws.off_flags), x.s, 0.f,
+                     x.b->pool_min_side);
 }
 
 }  // namespace

@@ -9,6 +9,7 @@ from __future__ import annotations
 import ctypes as C
 import math
 import os
+import warnings
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import torch
@@ -59,6 +60,7 @@ class RaftEngine:
         self.dtype, self.device, self.impl = dtype, device, impl
         self.agg_gamma, self.num_heads = 0.0, 1
         self.agg_score: Optional[torch.Tensor] = None  # craft: the aggregator's feat2score weight (pfb_raft_buffers.agg_score)
+        self.pool_min_side = 0  # how build_volume sizes the pyramid's levels (pfb_raft_buffers.pool_min_side; lcv: 2r+1)
         self.signature = None  # what the model built this engine for (RAFT._get_engine)
         self._keep: List[object] = []  # everything the weight structs point into
         self._workspaces: Dict[int, Tuple] = {}
@@ -235,7 +237,7 @@ class RaftEngine:
         pyr = ptr_array(pyramid) if pyramid is not None else None
         buf = _lib.RaftBuffers(C.cast(pyr, C.POINTER(C.c_void_p)) if pyr is not None else None, _ptr(fmap1), net.data_ptr(), inp.data_ptr(),
                                coords.data_ptr(), _ptr(flow_up), _ptr(flow_small), ws.data_ptr(), ws.numel(), _ptr(attention), self.agg_gamma,
-                               _ptr(self.agg_score))
+                               _ptr(self.agg_score), self.pool_min_side)
         with torch.cuda.device(self.device):
             check(getattr(load(), symbol)(C.byref(cfg), C.byref(weights), C.byref(buf), *args, stream_ptr(self.device)), symbol[4:])
 
@@ -830,6 +832,64 @@ class CRAFTEngine(RaftEngine):
             q, h, w = pyr[-1].shape
             pyr.append(ops.avg_pool2x2(pyr[-1].view(q, h, w, 1)).view(q, h // 2, w // 2))
         return pyr
+
+
+# The largest learned diagonal entry an f16 LCV engine takes without a warning.  The volume's values are <f1^T W, f2> / sqrt(C), up to
+# max(D) times RAFT's: measured on an H100 with the fnet features of a smooth 436x1024 pair, max |volume| is 71168 at D = 199 (f16
+# overflows past 65504) and 22.9k at D = 64, a factor 2.9 below the f16 maximum (DESIGN.md section 5, LCV).
+LCV_F16_MAX_D = 64.0
+
+
+def lcv_bilinear_form(corr_block: torch.nn.Module) -> torch.Tensor:
+    """W = P^T D P of LearnableCorrBlock (lcv/corr_lcv.py:19-31) in fp64: S = (triu(raw_P) - triu(raw_P)^T) / 2, P = (I + S)(I - S)^-1
+    (Cayley), t = atan(raw_D) 2 / pi, D = diag((1 + t) / (1 - t)).  I is the block's ``eye`` buffer, as the reference reads it."""
+    eye = corr_block.eye.detach().double()
+    up = torch.triu(corr_block.raw_P.detach().double())
+    S = (up - up.t()) / 2
+    P = (eye + S) @ torch.inverse(eye - S)
+    t = torch.atan(corr_block.raw_D.detach().double()) * 2 / math.pi
+    return P.t() @ torch.diag((1 + t) / (1 - t)) @ P
+
+
+class LCVEngine(RaftEngine):
+    """LCV (lcv_raft.py:41-221, corr_lcv.py): RAFT's or raft_small's loop (VARIANT_RAFT / VARIANT_RAFT_SMALL) over the learned volume
+    f1^T W f2 / sqrt(C) and a pyramid that stops pooling once a level's smaller side is <= 2r+1.  W / sqrt(C) is folded in fp64 once
+    per parameter version (the model keys the engine on the corr_block parameters) and applied to fmap1 as a 1x1 layer; the distinct
+    levels are built with scale 1 by the volume builders and the repeated ones alias the last of them (pool_min_side tells the
+    lookup their sizes)."""
+
+    def _pack(self, update_block: torch.nn.Module, corr_block: Optional[torch.nn.Module] = None) -> _lib.RaftWeights:
+        w = super()._pack(update_block)
+        c = corr_block.raw_D.shape[0]
+        W = lcv_bilinear_form(corr_block)
+        d_max = float(torch.linalg.eigvalsh((W + W.t()) / 2).max())  # max(D): W = P^T D P with P orthogonal
+        if self.dtype == torch.float16 and d_max > LCV_F16_MAX_D:
+            warnings.warn(f"lcv: the learned diagonal reaches D = {d_max:.0f}, and the f16 correlation volume holds values up to D times "
+                          f"RAFT's; above D = {LCV_F16_MAX_D} it can exceed the f16 range (inf in the pyramid, NaN flow). Run this model in "
+                          "bfloat16 or float32.", RuntimeWarning, stacklevel=2)
+        wf = W / math.sqrt(c)
+        # the 1x1 layer's out[j] = sum_i W'[j, i] f1[i] is (f1^T W)[j] for W' = W^T
+        self.learned = ops.PackedConv([ConvWeights(wf.t().float()[:, :, None, None].contiguous())], self.dtype, self.device, src_channels=[c])
+        self.pool_min_side = 2 * self.corr_radius + 1
+        return w
+
+    def _new_workspace(self, cfg: _lib.RaftCfg) -> torch.Tensor:
+        # grids whose RAFT pyramid would have an empty level (a 4x4 grid) are valid here
+        nbytes = load().pfb_raft_workspace_bytes_ex(C.byref(cfg), self.pool_min_side)
+        if nbytes == 0:
+            check(-1, "raft_workspace_bytes_ex")
+        return torch.empty(nbytes, dtype=torch.uint8, device=self.device)
+
+    def build_volume(self, fmap1: torch.Tensor, fmap2: torch.Tensor, impl: int = 0):
+        """(the corr_levels levels of compute_cost_volume, of which the repeated ones are the same tensor, its layout)."""
+        B, H, W, _ = fmap1.shape
+        _, distinct = ops.corr_level_sizes(H, W, self.corr_levels, self.pool_min_side)
+        f1w = ops.conv2d([fmap1], self.learned, torch.empty_like(fmap1), impl=impl)
+        if self.volume_tiled(fmap1, impl):
+            pyr, layout = ops.corr_volume_build_tiled(f1w, fmap2, distinct, scale=1.0), 1
+        else:
+            pyr, layout = ops.corr_volume_build_ex(f1w, fmap2, distinct, scale=1.0, impl=impl), 0
+        return pyr + [pyr[-1]] * (self.corr_levels - distinct), layout
 
 
 class SplatFlowEngine(RaftEngine):

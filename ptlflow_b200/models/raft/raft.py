@@ -124,6 +124,7 @@ class RAFT(BaseModel):
     }
     _variant = _lib.VARIANT_RAFT  # pfb_raft_cfg.variant
     _engine_cls = RaftEngine  # packs the update block and runs its loop (SKFlow brings its own)
+    _encoder_cls = BasicEncoder  # fnet and cnet (LCV brings encoders that take BGR frames)
 
     def __init__(self, corr_levels: int = 4, corr_radius: int = 4, dropout: float = 0.0, gamma: float = 0.8,
                  max_flow: float = 400, iters: int = 32, alternate_corr: bool = False, **kwargs) -> None:
@@ -162,8 +163,8 @@ class RAFT(BaseModel):
 
     def _build_networks(self) -> None:
         self.hidden_dim = self.context_dim = 128
-        self.fnet = BasicEncoder(output_dim=256, norm_fn="instance", dropout=self.dropout)
-        self.cnet = BasicEncoder(output_dim=self.hidden_dim + self.context_dim, norm_fn="batch", dropout=self.dropout)
+        self.fnet = self._encoder_cls(output_dim=256, norm_fn="instance", dropout=self.dropout)
+        self.cnet = self._encoder_cls(output_dim=self.hidden_dim + self.context_dim, norm_fn="batch", dropout=self.dropout)
         self.update_block = BasicUpdateBlock(self.corr_levels, self.corr_radius, hidden_dim=self.hidden_dim)
 
     def freeze_bn(self) -> None:
@@ -446,6 +447,7 @@ class RAFTSmall(RAFT):
         "things": "https://github.com/hmorimitsu/ptlflow/releases/download/weights1/raft_small-things-b7d9f997.ckpt"
     }
     _variant = _lib.VARIANT_RAFT_SMALL
+    _encoder_cls = SmallEncoder
 
     def __init__(self, corr_levels: int = 4, corr_radius: int = 3, dropout: float = 0.0, gamma: float = 0.8,
                  max_flow: float = 400, iters: int = 32, alternate_corr: bool = False, **kwargs) -> None:
@@ -454,8 +456,8 @@ class RAFTSmall(RAFT):
 
     def _build_networks(self) -> None:
         self.hidden_dim, self.context_dim = 96, 64
-        self.fnet = SmallEncoder(output_dim=128, norm_fn="instance", dropout=self.dropout)
-        self.cnet = SmallEncoder(output_dim=self.hidden_dim + self.context_dim, norm_fn="none", dropout=self.dropout)
+        self.fnet = self._encoder_cls(output_dim=128, norm_fn="instance", dropout=self.dropout)
+        self.cnet = self._encoder_cls(output_dim=self.hidden_dim + self.context_dim, norm_fn="none", dropout=self.dropout)
         self.update_block = SmallUpdateBlock(self.corr_levels, self.corr_radius, hidden_dim=self.hidden_dim)
 
 

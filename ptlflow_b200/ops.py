@@ -10,7 +10,7 @@ from __future__ import annotations
 import contextlib
 import ctypes as C
 import threading
-from typing import List, NamedTuple, Optional, Sequence
+from typing import List, NamedTuple, Optional, Sequence, Tuple
 
 import torch
 
@@ -108,8 +108,10 @@ def untile_level(level: torch.Tensor, h: int, w: int) -> torch.Tensor:
     return v[:, :h, :w].contiguous()
 
 
-def corr_lookup_tiled(pyramid: Sequence[torch.Tensor], coords: torch.Tensor, radius: int, targets_hw, out_stride: Optional[int] = None) -> torch.Tensor:
-    """coords fp32 [B,H1,W1,2] -> [B,H1,W1,out_stride] in the pyramid's dtype (pixel-major, the refinement loop's layout)."""
+def corr_lookup_tiled(pyramid: Sequence[torch.Tensor], coords: torch.Tensor, radius: int, targets_hw, out_stride: Optional[int] = None,
+                      level_hw=None) -> torch.Tensor:
+    """coords fp32 [B,H1,W1,2] -> [B,H1,W1,out_stride] in the pyramid's dtype (pixel-major, the refinement loop's layout).
+    ``level_hw``: explicit (h, w) per level (pfb_corr_lookup_tiled_ex), e.g. the repeated levels of corr_level_sizes."""
     require_cuda(coords, "coords")
     if coords.dtype != torch.float32:
         raise RuntimeError("corr_lookup_tiled: coords must be float32 [B,H,W,2]")
@@ -119,9 +121,26 @@ def corr_lookup_tiled(pyramid: Sequence[torch.Tensor], coords: torch.Tensor, rad
     stride = (planes + 7) // 8 * 8 if out_stride is None else out_stride
     out = torch.empty((B, H, W, stride), dtype=pyramid[0].dtype, device=coords.device)
     with torch.cuda.device(coords.device):
-        check(load().pfb_corr_lookup_tiled(ptr_array(pyramid), coords.data_ptr(), out.data_ptr(), B, H, W, targets_hw[0], targets_hw[1], L,
-                                           radius, dtype_code(pyramid[0].dtype), stride, stream_ptr(coords.device)), "corr_lookup_tiled")
+        if level_hw is None:
+            check(load().pfb_corr_lookup_tiled(ptr_array(pyramid), coords.data_ptr(), out.data_ptr(), B, H, W, targets_hw[0], targets_hw[1],
+                                               L, radius, dtype_code(pyramid[0].dtype), stride, stream_ptr(coords.device)), "corr_lookup_tiled")
+        else:
+            lh = (C.c_int * L)(*[int(h) for h, _ in level_hw])
+            lw = (C.c_int * L)(*[int(w) for _, w in level_hw])
+            check(load().pfb_corr_lookup_tiled_ex(ptr_array(pyramid), lh, lw, coords.data_ptr(), out.data_ptr(), B, H, W, targets_hw[0],
+                                                  targets_hw[1], L, radius, dtype_code(pyramid[0].dtype), stride, stream_ptr(coords.device)),
+                  "corr_lookup_tiled_ex")
     return out
+
+
+def corr_level_sizes(H: int, W: int, levels: int, pool_min_side: int = 0) -> Tuple[List[Tuple[int, int]], int]:
+    """([(h, w) per level], number of distinct levels) of a pyramid over an H x W grid (pfb_corr_level_sizes, host only): RAFT's
+    floor-halved levels for pool_min_side = 0; for m > 0 a level stops pooling once the smaller side of the one before is <= m, and
+    the distinct levels are the first ones, the rest repeat the last of them."""
+    lh, lw = (C.c_int * max(levels, 1))(), (C.c_int * max(levels, 1))()
+    n = load().pfb_corr_level_sizes(int(H), int(W), int(levels), int(pool_min_side), lh, lw)
+    check(min(n, 0), "corr_level_sizes")
+    return [(lh[l], lw[l]) for l in range(levels)], n
 
 
 # ------------------------------------------------------------------------------------------
